@@ -2,11 +2,14 @@
 // Reference behaviour: crates/hypercube/src/logup_gkr/{prover.rs:70-215, execution.rs:13-382, logup_poly.rs:71-552, cpu.rs:76-226};
 // GPU twin it replaces: sp1-gpu/crates/logup_gkr + sys/lib/logup_gkr/{first_layer,execution,round,lookahead}.cu.
 // HOW (results identical):
-//  * the circuit is kept as ONE fraction sequence per (chip, interaction) and level, F_l[j] (numerator EF, denominator EF),
+//  * the circuit is kept as ONE fraction sequence per (chip, interaction) and level, F_l[j] (numerator EF, denominator EF;
+//    level 0 keeps its numerators, the multiplicities, in the base field: 20 B per entry instead of 32),
 //    F_{l+1}[j] = F_l[2j] (+) F_l[2j+1]; the reference's four arrays of a layer are the parity classes of F_l
 //    (numerator_0 = even entries, numerator_1 = odd entries), so no transposition or re-layout is needed between levels;
-//  * every sumcheck round of a layer is one launch over ALL chips (work items are looked up in a small prefix table),
-//    fused as "fix the previous variable + accumulate the next round's three sums";
+//    levels 0, 1 and 2 come out of one pass over the trace;
+//  * every sumcheck round of a layer is one launch over ALL chips (work items are looked up in a small prefix table);
+//    rounds 0 and 1 are summed in one pass over the fraction sequence and fixed together in a second one, the later row
+//    rounds are fused as "fix the previous variable + accumulate the next round's three sums";
 //  * once a layer's row variables are exhausted the remaining (interaction) variables range over <= 2^v <= a few
 //    thousand values, which the host transcript driver folds directly.
 #include "ctx.cuh"
@@ -54,39 +57,93 @@ __device__ __forceinline__ int find_job(const JobTable& t, uint64_t w) {
 __device__ __forceinline__ Ext ldE(const uint32_t* p, uint64_t i) { return kb::ext_load(p + 4 * i); }
 __device__ __forceinline__ void stE(uint32_t* p, uint64_t i, const Ext& e) { kb::ext_store(p + 4 * i, e); }
 
-// ---- level 0: per (chip, interaction k, row r) fraction from the trace (execution.rs:13-36, 114-252) -----------------------
+// ---- levels 0 and 1: per (chip, interaction k, row r) fraction from the trace (execution.rs:13-36, 114-252) -----------------
 // q = a / b for work indices that almost always fit 32 bits: the 64-bit division (~60 instructions) only when needed
 __device__ __forceinline__ uint32_t div_small(uint64_t a, uint64_t b) {
     return ((a | b) >> 32) ? (uint32_t)(a / b) : (uint32_t)a / (uint32_t)b;
 }
 
-__global__ void __launch_bounds__(256) gkr_first_level_kernel(const uint32_t* __restrict__ main, const uint32_t* __restrict__ prep, uint64_t h,
-                                                              const InterDev* __restrict__ inter, uint32_t I, const VColDev* __restrict__ vcols,
-                                                              const TermDev* __restrict__ terms, Ext alpha, const uint32_t* __restrict__ betas,
-                                                              uint32_t* __restrict__ num, uint32_t* __restrict__ den) {
-    uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= h * I) return;
-    const uint32_t k = div_small(t, h);
-    const uint64_t r = t - (uint64_t)k * h;
-    const InterDev in = inter[k];
-    auto apply = [&](const VColDev& v) {
-        uint32_t acc = v.constant;
-        for (uint32_t q = 0; q < v.n_terms; q++) {
-            const TermDev tm = terms[v.term_start + q];
-            const uint32_t x = __ldg((tm.source == 4 ? main : prep) + (uint64_t)tm.col * h + r);
-            acc = kb::add(acc, kb::mul(x, tm.weight));
-        }
-        return acc;
-    };
-    Ext d = kb::ext_add(alpha, kb::ext_mul_base(ldE(betas, 0), kb::from_canonical(in.arg_index)));
-    for (uint32_t j = 0; j < in.n_values; j++) d = kb::ext_add(d, kb::ext_mul_base(ldE(betas, j + 1), apply(vcols[in.vcol_start + 1 + j])));
-    uint32_t m = apply(vcols[in.vcol_start]);
-    if (!in.is_send) m = kb::neg(m);
-    stE(num, (uint64_t)k * h + r, kb::ext_from_base(m));
-    stE(den, (uint64_t)k * h + r, d);
+struct FirstSrc { const uint32_t* main; const uint32_t* prep; uint64_t off2; };  // a job's trace columns, its offset at level 2
+
+__device__ __forceinline__ void frac_add(const Ext& n0, const Ext& d0, const Ext& n1, const Ext& d1, Ext& n, Ext& d) {
+    n = kb::ext_add(kb::ext_mul(d1, n0), kb::ext_mul(d0, n1));
+    d = kb::ext_mul(d0, d1);
 }
 
-// ---- level l -> l+1: F'[j] = F[2j] (+) F[2j+1]  (missing odd entry = padding (0,1): identity) ------------------------------
+// Level 0 keeps its numerators (the multiplicities) in the base field: num0 = u32 words, den0 = EF.  A thread computes the
+// entries 4j .. 4j+3 of one (chip, k) sequence and stores them, which the layer-0 sumcheck reads, together with entries 2j, 2j+1
+// of level 1 and entry j of level 2 (num2 = nullptr: the tree has two levels).  A missing odd entry is the padding (0,1): the
+// even entry passes up unchanged.  work item = (chip, k, j), all chips in one launch; job.int_off doubles as the chip's first
+// entry in `inter`.
+__global__ void __launch_bounds__(256) gkr_first_level_kernel(JobTable jobs, const FirstSrc* __restrict__ src, const InterDev* __restrict__ inter,
+                                                              const VColDev* __restrict__ vcols, const TermDev* __restrict__ terms, Ext alpha,
+                                                              const uint32_t* __restrict__ betas, uint32_t* __restrict__ num0, uint32_t* __restrict__ den0,
+                                                              uint32_t* __restrict__ num1, uint32_t* __restrict__ den1, uint32_t* __restrict__ num2,
+                                                              uint32_t* __restrict__ den2) {
+    const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= jobs.total) return;
+    const int jx = find_job(jobs, w);
+    const ChipJob& c = jobs.j[jx];
+    const uint64_t lw = w - c.work_start, h = c.rows_in;
+    const uint32_t len1 = (c.rows_in + 1) / 2, len2 = (len1 + 1) / 2;
+    const uint32_t k = div_small(lw, len2), j = (uint32_t)(lw - (uint64_t)k * len2);
+    const InterDev in = inter[c.int_off + k];
+    const FirstSrc s = src[jx];
+    const uint64_t r0 = 4ull * j;
+    const uint32_t nv = (uint32_t)(h - r0 < 4 ? h - r0 : 4);  // entries of level 0 this thread holds (1..4)
+    auto apply = [&](const VColDev& v, uint32_t (&a)[4]) {  // the virtual column at rows r0 .. r0 + nv - 1
+#pragma unroll
+        for (int t = 0; t < 4; t++) a[t] = v.constant;
+        for (uint32_t q = 0; q < v.n_terms; q++) {
+            const TermDev tm = terms[v.term_start + q];
+            const uint32_t* col = (tm.source == 4 ? s.main : s.prep) + (uint64_t)tm.col * h + r0;
+#pragma unroll
+            for (int t = 0; t < 4; t++)
+                if (t < nv) a[t] = kb::add(a[t], kb::mul(__ldg(col + t), tm.weight));
+        }
+    };
+    Ext d[4];
+    d[0] = kb::ext_add(alpha, kb::ext_mul_base(ldE(betas, 0), kb::from_canonical(in.arg_index)));
+#pragma unroll
+    for (int t = 1; t < 4; t++) d[t] = d[0];
+    uint32_t x[4];
+    for (uint32_t q = 0; q < in.n_values; q++) {
+        apply(vcols[in.vcol_start + 1 + q], x);
+        const Ext b = ldE(betas, q + 1);
+#pragma unroll
+        for (int t = 0; t < 4; t++) d[t] = kb::ext_add(d[t], kb::ext_mul_base(b, x[t]));
+    }
+    uint32_t m[4];
+    apply(vcols[in.vcol_start], m);
+    if (!in.is_send) {
+#pragma unroll
+        for (int t = 0; t < 4; t++) m[t] = kb::neg(m[t]);
+    }
+    const uint64_t o0 = c.in_off + (uint64_t)k * h + r0, o1 = c.out_off + (uint64_t)k * len1 + 2 * j;
+#pragma unroll
+    for (int t = 0; t < 4; t++)
+        if (t < nv) { num0[o0 + t] = m[t]; stE(den0, o0 + t, d[t]); }
+    Ext n1[2], d1[2];  // level 1 entries 2j, 2j+1 (the second one exists when nv > 2)
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+        if (2 * e + 1 < nv) {
+            n1[e] = kb::ext_add(kb::ext_mul_base(d[2 * e + 1], m[2 * e]), kb::ext_mul_base(d[2 * e], m[2 * e + 1]));
+            d1[e] = kb::ext_mul(d[2 * e], d[2 * e + 1]);
+        } else {
+            n1[e] = kb::ext_from_base(m[2 * e]); d1[e] = d[2 * e];
+        }
+    }
+    stE(num1, o1, n1[0]); stE(den1, o1, d1[0]);
+    if (nv > 2) { stE(num1, o1 + 1, n1[1]); stE(den1, o1 + 1, d1[1]); }
+    if (num2) {
+        Ext n2 = n1[0], d2 = d1[0];
+        if (nv > 2) frac_add(n1[0], d1[0], n1[1], d1[1], n2, d2);
+        const uint64_t o2 = s.off2 + (uint64_t)k * len2 + j;
+        stE(num2, o2, n2); stE(den2, o2, d2);
+    }
+}
+
+// ---- level l -> l+1 (l >= 2): F'[j] = F[2j] (+) F[2j+1]  (missing odd entry = padding (0,1): identity) ---------------------
 __global__ void __launch_bounds__(256) gkr_level_kernel(JobTable jobs, const uint32_t* __restrict__ num, const uint32_t* __restrict__ den,
                                                         uint32_t* __restrict__ num_o, uint32_t* __restrict__ den_o) {
     uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -99,23 +156,43 @@ __global__ void __launch_bounds__(256) gkr_level_kernel(JobTable jobs, const uin
     const uint64_t base = c.in_off + (uint64_t)k * c.rows_in;
     Ext n0 = ldE(num, base + 2 * j), d0 = ldE(den, base + 2 * j);
     Ext n = n0, d = d0;
-    if (2 * j + 1 < c.rows_in) {
-        Ext n1 = ldE(num, base + 2 * j + 1), d1 = ldE(den, base + 2 * j + 1);
-        n = kb::ext_add(kb::ext_mul(d1, n0), kb::ext_mul(d0, n1));
-        d = kb::ext_mul(d0, d1);
-    }
+    if (2 * j + 1 < c.rows_in) frac_add(n0, d0, ldE(num, base + 2 * j + 1), ldE(den, base + 2 * j + 1), n, d);
     stE(num_o, c.out_off + (uint64_t)k * len_o + j, n);
     stE(den_o, c.out_off + (uint64_t)k * len_o + j, d);
 }
 
-// the four layer arrays seen through a fraction sequence F (length len): row i -> (n0,d0) = F[2i], (n1,d1) = F[2i+1]
-struct Row4 { Ext n0, d0, n1, d1; };
-__device__ __forceinline__ Row4 row_from_seq(const uint32_t* num, const uint32_t* den, uint64_t base, uint32_t len, uint32_t i) {
-    Row4 r;
-    r.n0 = kb::ext_zero(); r.n1 = kb::ext_zero(); r.d0 = kb::ext_one(); r.d1 = kb::ext_one();
-    if (2 * i < len) { r.n0 = ldE(num, base + 2 * i); r.d0 = ldE(den, base + 2 * i); }
-    if (2 * i + 1 < len) { r.n1 = ldE(num, base + 2 * i + 1); r.d1 = ldE(den, base + 2 * i + 1); }
+// The four layer arrays seen through a fraction sequence F (length len): row i -> (n0,d0) = F[2i], (n1,d1) = F[2i+1].
+// N = numerator type: uint32_t (level 0, base field) or Ext; the overloads below keep one source for both.
+template <class N> struct RowT { N n0, n1; Ext d0, d1; };
+using Row4 = RowT<Ext>;
+__device__ __forceinline__ void ld_num(const uint32_t* p, uint64_t i, uint32_t& x) { x = p[i]; }
+__device__ __forceinline__ void ld_num(const uint32_t* p, uint64_t i, Ext& x) { x = ldE(p, i); }
+__device__ __forceinline__ uint32_t nadd(uint32_t a, uint32_t b) { return kb::add(a, b); }
+__device__ __forceinline__ Ext nadd(const Ext& a, const Ext& b) { return kb::ext_add(a, b); }
+__device__ __forceinline__ uint32_t nsub(uint32_t a, uint32_t b) { return kb::sub(a, b); }
+__device__ __forceinline__ Ext nsub(const Ext& a, const Ext& b) { return kb::ext_sub(a, b); }
+__device__ __forceinline__ Ext nmul(const Ext& d, uint32_t n) { return kb::ext_mul_base(d, n); }  // 4 products
+__device__ __forceinline__ Ext nmul(const Ext& d, const Ext& n) { return kb::ext_mul(d, n); }     // 16 products
+__device__ __forceinline__ Ext nfix(uint32_t x, uint32_t y, const Ext& a) { return kb::ext_add(kb::ext_from_base(x), kb::ext_mul_base(a, kb::sub(y, x))); }
+__device__ __forceinline__ Ext nfix(const Ext& x, const Ext& y, const Ext& a) { return kb::ext_add(x, kb::ext_mul(a, kb::ext_sub(y, x))); }
+
+template <class N>
+__device__ __forceinline__ RowT<N> row_from_seq(const uint32_t* num, const uint32_t* den, uint64_t base, uint32_t len, uint32_t i) {
+    RowT<N> r;
+    r.n0 = N{}; r.n1 = N{}; r.d0 = kb::ext_one(); r.d1 = kb::ext_one();
+    if (2 * i < len) { ld_num(num, base + 2 * i, r.n0); r.d0 = ldE(den, base + 2 * i); }
+    if (2 * i + 1 < len) { ld_num(num, base + 2 * i + 1, r.n1); r.d1 = ldE(den, base + 2 * i + 1); }
     return r;
+}
+template <class N> __device__ __forceinline__ RowT<N> row_add(const RowT<N>& x, const RowT<N>& y) {
+    return RowT<N>{nadd(x.n0, y.n0), nadd(x.n1, y.n1), kb::ext_add(x.d0, y.d0), kb::ext_add(x.d1, y.d1)};
+}
+template <class N> __device__ __forceinline__ RowT<N> row_sub(const RowT<N>& x, const RowT<N>& y) {
+    return RowT<N>{nsub(x.n0, y.n0), nsub(x.n1, y.n1), kb::ext_sub(x.d0, y.d0), kb::ext_sub(x.d1, y.d1)};
+}
+// the layer's summand lambda (n0 d1 + n1 d0) + d0 d1: a quadratic form in the row
+template <class N> __device__ __forceinline__ Ext row_poly(const RowT<N>& x, const Ext& lambda) {
+    return kb::ext_add(kb::ext_mul(lambda, kb::ext_add(nmul(x.d1, x.n0), nmul(x.d0, x.n1))), kb::ext_mul(x.d0, x.d1));
 }
 // working layout of a chip (after the first fix): [4][I][rows] EF = n0 | d0 | n1 | d1
 __device__ __forceinline__ Row4 row_from_work(const uint32_t* a, uint64_t base, uint32_t I, uint32_t rows, uint32_t k, uint32_t i) {
@@ -127,102 +204,158 @@ __device__ __forceinline__ Row4 row_from_work(const uint32_t* a, uint64_t base, 
     }
     return r;
 }
-__device__ __forceinline__ Row4 fix_rows(const Row4& x, const Row4& y, const Ext& a) {
+template <class N> __device__ __forceinline__ Row4 fix_rows(const RowT<N>& x, const RowT<N>& y, const Ext& a) {
     Row4 r;
-    r.n0 = kb::ext_add(x.n0, kb::ext_mul(a, kb::ext_sub(y.n0, x.n0)));
+    r.n0 = nfix(x.n0, y.n0, a);
     r.d0 = kb::ext_add(x.d0, kb::ext_mul(a, kb::ext_sub(y.d0, x.d0)));
-    r.n1 = kb::ext_add(x.n1, kb::ext_mul(a, kb::ext_sub(y.n1, x.n1)));
+    r.n1 = nfix(x.n1, y.n1, a);
     r.d1 = kb::ext_add(x.d1, kb::ext_mul(a, kb::ext_sub(y.d1, x.d1)));
     return r;
 }
 // contributions of the row pair (x = row 2i, y = row 2i+1) to (eval_0, eval_half, eq_sum)   logup_poly.rs:330-505
 __device__ __forceinline__ void pair_sums(const Row4& x, const Row4& y, const Ext& e, const Ext& er0, const Ext& er1, const Ext& lambda,
                                           Ext& s0, Ext& sh, Ext& se) {
-    Ext t0 = kb::ext_add(kb::ext_mul(lambda, kb::ext_add(kb::ext_mul(x.d0, x.n1), kb::ext_mul(x.d1, x.n0))), kb::ext_mul(x.d0, x.d1));
-    Ext D0 = kb::ext_add(x.d0, y.d0), D1 = kb::ext_add(x.d1, y.d1), N0 = kb::ext_add(x.n0, y.n0), N1 = kb::ext_add(x.n1, y.n1);
-    Ext th = kb::ext_add(kb::ext_mul(lambda, kb::ext_add(kb::ext_mul(D0, N1), kb::ext_mul(D1, N0))), kb::ext_mul(D0, D1));
+    const Ext t0 = row_poly(x, lambda), th = row_poly(row_add(x, y), lambda);
     const Ext ee0 = kb::ext_mul(e, er0), ees = kb::ext_mul(e, kb::ext_add(er0, er1));  // shared by the three sums
     s0 = kb::ext_add(s0, kb::ext_mul(ee0, t0));
     sh = kb::ext_add(sh, kb::ext_mul(ees, th));
     se = kb::ext_add(se, ees);
 }
 
-__device__ __forceinline__ void block_reduce3(Ext a, Ext b, Ext c, uint32_t* __restrict__ partial, const Mail& mail) {
+// NE extension sums per block -> partial[block][4 NE] (the mailbox payload: the host transcript polls the flag, ctx.cuh)
+template <int NE>
+__device__ __forceinline__ void block_reduce(const Ext (&v)[NE], uint32_t* __restrict__ partial, const Mail& mail) {
     // warp shuffles + one barrier (these kernels are latency-bound on the upper layers: a shared-memory tree costs 8 barriers)
-    __shared__ uint32_t red[12][8];
+    __shared__ uint32_t red[4 * NE][8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t w[12];
 #pragma unroll
-    for (int l = 0; l < 4; l++) { w[l] = a.c[l]; w[4 + l] = b.c[l]; w[8 + l] = c.c[l]; }
+    for (int k = 0; k < 4 * NE; k++) {
+        uint32_t x = v[k / 4].c[k % 4];
 #pragma unroll
-    for (int k = 0; k < 12; k++) {
-        uint32_t v = w[k];
-#pragma unroll
-        for (int sft = 16; sft > 0; sft >>= 1) v = kb::add(v, __shfl_down_sync(0xffffffffu, v, sft));
-        if (lane == 0) red[k][warp] = v;
+        for (int sft = 16; sft > 0; sft >>= 1) x = kb::add(x, __shfl_down_sync(0xffffffffu, x, sft));
+        if (lane == 0) red[k][warp] = x;
     }
     __syncthreads();
-    if (threadIdx.x < 12) {
-        uint32_t v = 0;
-        for (int q = 0; q < (int)(blockDim.x >> 5); q++) v = kb::add(v, red[threadIdx.x][q]);
-        partial[blockIdx.x * 12 + threadIdx.x] = v;
+    if (threadIdx.x < 4 * NE) {
+        uint32_t x = 0;
+        for (int q = 0; q < (int)(blockDim.x >> 5); q++) x = kb::add(x, red[threadIdx.x][q]);
+        partial[blockIdx.x * 4 * NE + threadIdx.x] = x;
     }
-    sp1_mail_done(mail);  // `partial` is the mailbox payload: the host transcript polls the flag (ctx.cuh)
+    sp1_mail_done(mail);
 }
 
-// round 0 of a layer: sums straight from the fraction sequence. work item = (chip, k, row pair i)
-__global__ void __launch_bounds__(256) gkr_sum_seq_kernel(JobTable jobs, const uint32_t* __restrict__ num, const uint32_t* __restrict__ den,
-                                                          const uint32_t* __restrict__ eq_int, const uint32_t* __restrict__ eq_row, Ext lambda,
-                                                          uint32_t* __restrict__ partial, Mail mail) {
-    Ext s0 = kb::ext_zero(), sh = kb::ext_zero(), se = kb::ext_zero();
+// Rounds 0 and 1 of a layer in one pass over its fraction sequence.  work item = (chip, k, row quad i): rows x0..x3 = 4i..4i+3.
+// The eq table is a product, E[2j + b] = P[j] (b ? last : 1 - last) with P[j] = E[2j] + E[2j+1], `last` = round 0's point
+// coordinate: round 0's eval_0 is (1 - last) sum_pairs e P q(x_even), the host applies the factor.  Binding round 0 to a, the
+// round-1 rows are x0 + a (x1 - x0), x2 + a (x3 - x2) and the eq table becomes c(a) P.  The summand q is a quadratic form, so
+// q(x + a (y - x)) = (1-a) q(x) + a q(y) + (a^2 - a) q(y - x): round 1's sums are c(a) times a quadratic in a whose
+// coefficients per sum are accumulated here; the host evaluates them at the sampled a.  With w = e P0 (first pair), v = e P1
+// (second pair), X = x0 + x2, Y = x1 + x3, the sums (EF) are
+//   0: v q(x2)   1: v q(x2 + x3)   2: w + v   3: w q(x0)   4: w q(x1)   5: w q(x0 + x1)   6..8: (w + v) q(X), q(Y), q(Y - X)
+// two = 0 (a layer with one row variable: no second pair, no round 1): sums 2, 3, 5 with w only.
+constexpr int SUM2_WORDS = 36;
+constexpr int SUM2_THREADS = 128;  // ~160 registers per thread: three 128-thread blocks per SM instead of one 256-thread block
+template <class N>
+__global__ void __launch_bounds__(SUM2_THREADS) gkr_sum2_kernel(JobTable jobs, const uint32_t* __restrict__ num, const uint32_t* __restrict__ den,
+                                                                const uint32_t* __restrict__ eq_int, const uint32_t* __restrict__ eq_row, Ext lambda,
+                                                                int two, uint32_t* __restrict__ partial, Mail mail) {
+    Ext acc[9];
+#pragma unroll
+    for (int q = 0; q < 9; q++) acc[q] = kb::ext_zero();
     for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < jobs.total; w += (uint64_t)gridDim.x * blockDim.x) {
         const ChipJob& c = jobs.j[find_job(jobs, w)];
         const uint64_t lw = w - c.work_start;
-        const uint32_t rows = (c.rows_in + 1) / 2, pairs = (rows + 1) / 2;
+        const uint32_t rows = (c.rows_in + 1) / 2, quads = (rows + 3) / 4;
+        const uint32_t k = div_small(lw, quads), i4 = 4 * (uint32_t)(lw - (uint64_t)k * quads);
+        const uint64_t base = c.in_off + (uint64_t)k * c.rows_in;
+        const Ext e = ldE(eq_int, c.int_off + k);
+        const RowT<N> x0 = row_from_seq<N>(num, den, base, c.rows_in, i4), x1 = row_from_seq<N>(num, den, base, c.rows_in, i4 + 1);
+        const Ext wt = kb::ext_mul(e, kb::ext_add(ldE(eq_row, i4), ldE(eq_row, i4 + 1)));
+        acc[2] = kb::ext_add(acc[2], wt);
+        acc[3] = kb::ext_add(acc[3], kb::ext_mul(wt, row_poly(x0, lambda)));
+        acc[5] = kb::ext_add(acc[5], kb::ext_mul(wt, row_poly(row_add(x0, x1), lambda)));
+        if (two) {  // rows <= 2^r with r >= 2: the second pair is inside the eq table (all padding past the chip's rows)
+            const RowT<N> x2 = row_from_seq<N>(num, den, base, c.rows_in, i4 + 2), x3 = row_from_seq<N>(num, den, base, c.rows_in, i4 + 3);
+            const Ext vt = kb::ext_mul(e, kb::ext_add(ldE(eq_row, i4 + 2), ldE(eq_row, i4 + 3))), wv = kb::ext_add(wt, vt);
+            acc[0] = kb::ext_add(acc[0], kb::ext_mul(vt, row_poly(x2, lambda)));
+            acc[1] = kb::ext_add(acc[1], kb::ext_mul(vt, row_poly(row_add(x2, x3), lambda)));
+            acc[2] = kb::ext_add(acc[2], vt);
+            acc[4] = kb::ext_add(acc[4], kb::ext_mul(wt, row_poly(x1, lambda)));
+            const RowT<N> X = row_add(x0, x2), Y = row_add(x1, x3);
+            acc[6] = kb::ext_add(acc[6], kb::ext_mul(wv, row_poly(X, lambda)));
+            acc[7] = kb::ext_add(acc[7], kb::ext_mul(wv, row_poly(Y, lambda)));
+            acc[8] = kb::ext_add(acc[8], kb::ext_mul(wv, row_poly(row_sub(Y, X), lambda)));
+        }
+    }
+    block_reduce<9>(acc, partial, mail);
+}
+
+// The first fix of a layer: bind round 0's variable with a0 (and, TWO, round 1's with a1) straight from the fraction sequence,
+// write the working arrays of the next round and accumulate that round's sums.  work item = (chip, k, NEW row pair i).
+template <class N, bool TWO>
+__global__ void __launch_bounds__(256) gkr_fix2_kernel(JobTable jobs, const uint32_t* __restrict__ num, const uint32_t* __restrict__ den,
+                                                       uint32_t* __restrict__ out, const uint32_t* __restrict__ eq_int,
+                                                       const uint32_t* __restrict__ eq_row_new, Ext a0, Ext a1, Ext lambda,
+                                                       uint32_t* __restrict__ partial, Mail mail) {
+    Ext s[3] = {kb::ext_zero(), kb::ext_zero(), kb::ext_zero()};
+    for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < jobs.total; w += (uint64_t)gridDim.x * blockDim.x) {
+        const ChipJob& c = jobs.j[find_job(jobs, w)];
+        const uint64_t lw = w - c.work_start;
+        const uint32_t rows = (c.rows_in + 1) / 2;
+        const uint32_t rows_new = TWO ? (rows + 3) / 4 : (rows + 1) / 2, pairs = (rows_new + 1) / 2;
         const uint32_t k = div_small(lw, pairs), i = (uint32_t)(lw - (uint64_t)k * pairs);
         const uint64_t base = c.in_off + (uint64_t)k * c.rows_in;
-        Row4 x = row_from_seq(num, den, base, c.rows_in, 2 * i), y = row_from_seq(num, den, base, c.rows_in, 2 * i + 1);
-        pair_sums(x, y, ldE(eq_int, c.int_off + k), ldE(eq_row, 2 * i), ldE(eq_row, 2 * i + 1), lambda, s0, sh, se);
+        Row4 nr[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; hh++) {
+            const uint32_t o = 2 * i + hh;  // new row index
+            if (o < rows_new) {
+                if (TWO) {  // old rows 4o .. 4o+3
+                    const Row4 lo = fix_rows(row_from_seq<N>(num, den, base, c.rows_in, 4 * o), row_from_seq<N>(num, den, base, c.rows_in, 4 * o + 1), a0);
+                    const Row4 hi = fix_rows(row_from_seq<N>(num, den, base, c.rows_in, 4 * o + 2), row_from_seq<N>(num, den, base, c.rows_in, 4 * o + 3), a0);
+                    nr[hh] = fix_rows(lo, hi, a1);
+                } else {
+                    nr[hh] = fix_rows(row_from_seq<N>(num, den, base, c.rows_in, 2 * o), row_from_seq<N>(num, den, base, c.rows_in, 2 * o + 1), a0);
+                }
+                const uint64_t st = (uint64_t)c.I * rows_new, q = c.out_off + (uint64_t)k * rows_new + o;
+                stE(out, q, nr[hh].n0); stE(out, q + st, nr[hh].d0); stE(out, q + 2 * st, nr[hh].n1); stE(out, q + 3 * st, nr[hh].d1);
+            } else {  // beyond the real rows: padding values for the sums below
+                nr[hh].n0 = kb::ext_zero(); nr[hh].n1 = kb::ext_zero(); nr[hh].d0 = kb::ext_one(); nr[hh].d1 = kb::ext_one();
+            }
+        }
+        pair_sums(nr[0], nr[1], ldE(eq_int, c.int_off + k), ldE(eq_row_new, 2 * i), ldE(eq_row_new, 2 * i + 1), lambda, s[0], s[1], s[2]);
     }
-    block_reduce3(s0, sh, se, partial, mail);
+    block_reduce<3>(s, partial, mail);
 }
 
-// fix the last row variable (input = fraction sequence or working arrays), write the working arrays of the next round and
-// accumulate that round's sums.  work item = (chip, k, NEW row pair i): new rows 2i, 2i+1 come from old rows 4i .. 4i+3.
-template <bool FROM_SEQ>
-__global__ void __launch_bounds__(256) gkr_fix_sum_kernel(JobTable jobs, const uint32_t* __restrict__ in_a, const uint32_t* __restrict__ in_b,
-                                                          uint32_t* __restrict__ out, const uint32_t* __restrict__ eq_int,
-                                                          const uint32_t* __restrict__ eq_row_new, Ext alpha, Ext lambda, uint32_t* __restrict__ partial,
-                                                          Mail mail) {
-    Ext s0 = kb::ext_zero(), sh = kb::ext_zero(), se = kb::ext_zero();
+// the later row rounds: fix the last row variable of the working arrays, write the halved arrays and accumulate the next
+// round's sums.  work item = (chip, k, NEW row pair i): new rows 2i, 2i+1 come from old rows 4i .. 4i+3.
+__global__ void __launch_bounds__(256) gkr_fix_sum_kernel(JobTable jobs, const uint32_t* __restrict__ in, uint32_t* __restrict__ out,
+                                                          const uint32_t* __restrict__ eq_int, const uint32_t* __restrict__ eq_row_new, Ext alpha,
+                                                          Ext lambda, uint32_t* __restrict__ partial, Mail mail) {
+    Ext s[3] = {kb::ext_zero(), kb::ext_zero(), kb::ext_zero()};
     for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < jobs.total; w += (uint64_t)gridDim.x * blockDim.x) {
         const ChipJob& c = jobs.j[find_job(jobs, w)];
         const uint64_t lw = w - c.work_start;
-        const uint32_t rows_old = FROM_SEQ ? (c.rows_in + 1) / 2 : c.rows_in;
+        const uint32_t rows_old = c.rows_in;
         const uint32_t rows_new = (rows_old + 1) / 2, pairs = (rows_new + 1) / 2;
         const uint32_t k = div_small(lw, pairs), i = (uint32_t)(lw - (uint64_t)k * pairs);
         Row4 nr[2];
 #pragma unroll
         for (int hh = 0; hh < 2; hh++) {
             const uint32_t o = 2 * i + hh;  // new row index; old rows 2o, 2o+1
-            Row4 x, y;
-            if (FROM_SEQ) {
-                const uint64_t base = c.in_off + (uint64_t)k * c.rows_in;
-                x = row_from_seq(in_a, in_b, base, c.rows_in, 2 * o); y = row_from_seq(in_a, in_b, base, c.rows_in, 2 * o + 1);
-            } else {
-                x = row_from_work(in_a, c.in_off, c.I, rows_old, k, 2 * o); y = row_from_work(in_a, c.in_off, c.I, rows_old, k, 2 * o + 1);
-            }
+            const Row4 x = row_from_work(in, c.in_off, c.I, rows_old, k, 2 * o), y = row_from_work(in, c.in_off, c.I, rows_old, k, 2 * o + 1);
             nr[hh] = fix_rows(x, y, alpha);
             if (o < rows_new) {
-                const uint64_t s = (uint64_t)c.I * rows_new, q = c.out_off + (uint64_t)k * rows_new + o;
-                stE(out, q, nr[hh].n0); stE(out, q + s, nr[hh].d0); stE(out, q + 2 * s, nr[hh].n1); stE(out, q + 3 * s, nr[hh].d1);
+                const uint64_t st = (uint64_t)c.I * rows_new, q = c.out_off + (uint64_t)k * rows_new + o;
+                stE(out, q, nr[hh].n0); stE(out, q + st, nr[hh].d0); stE(out, q + 2 * st, nr[hh].n1); stE(out, q + 3 * st, nr[hh].d1);
             } else {  // beyond the real rows: padding values for the sums below
                 nr[hh].n0 = kb::ext_zero(); nr[hh].n1 = kb::ext_zero(); nr[hh].d0 = kb::ext_one(); nr[hh].d1 = kb::ext_one();
             }
         }
-        pair_sums(nr[0], nr[1], ldE(eq_int, c.int_off + k), ldE(eq_row_new, 2 * i), ldE(eq_row_new, 2 * i + 1), lambda, s0, sh, se);
+        pair_sums(nr[0], nr[1], ldE(eq_int, c.int_off + k), ldE(eq_row_new, 2 * i), ldE(eq_row_new, 2 * i + 1), lambda, s[0], s[1], s[2]);
     }
-    block_reduce3(s0, sh, se, partial, mail);
+    block_reduce<3>(s, partial, mail);
 }
 
 // ---- interaction variables (logup_poly.rs:118-176 + the generic round of sumcheck/src/prover.rs) -------------------------------
@@ -277,18 +410,30 @@ __global__ void __launch_bounds__(256) gkr_inter_round_kernel(const uint32_t* __
             for (int a = 0; a < 4; a++) { stE(payload, 3 + 2 * a, v[a][0]); stE(payload, 4 + 2 * a, v[a][1]); }
         }
     }
-    block_reduce3(s0, sh, se, payload, mail);
+    const Ext sums[3] = {s0, sh, se};
+    block_reduce<3>(sums, payload, mail);
 }
 
-__global__ void gkr_eq_table_kernel(const uint32_t* __restrict__ point, int k, uint32_t* __restrict__ E) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= ((uint64_t)1 << k)) return;
-    Ext acc = kb::ext_one();
-    for (int t = 0; t < k; t++) {
-        Ext x = kb::ext_load(point + 4 * t);
-        bool bit = (j >> (k - 1 - t)) & 1;
-        acc = kb::ext_mul(acc, bit ? x : kb::ext_sub(kb::ext_one(), x));
+// E[j] = prod_t (bit (k-1-t) of j ? x_t : 1 - x_t).  The EQ_LOW_BITS low bits vary inside a block, the others do not: their
+// product is formed once per block, so a thread does EQ_LOW_BITS products instead of k.  Launched with 2^EQ_LOW_BITS threads.
+constexpr int EQ_LOW_BITS = 8;
+__global__ void __launch_bounds__(1 << EQ_LOW_BITS) gkr_eq_table_kernel(const uint32_t* __restrict__ point, int k, uint32_t* __restrict__ E) {
+    const int lo = k < EQ_LOW_BITS ? k : EQ_LOW_BITS;
+    const uint64_t j0 = (uint64_t)blockIdx.x << EQ_LOW_BITS, j = j0 + threadIdx.x;
+    auto factor = [&](uint64_t idx, int t) {
+        const Ext x = kb::ext_load(point + 4 * t);
+        return ((idx >> (k - 1 - t)) & 1) ? x : kb::ext_sub(kb::ext_one(), x);
+    };
+    __shared__ Ext high;
+    if (threadIdx.x == 0) {
+        Ext acc = kb::ext_one();
+        for (int t = 0; t < k - lo; t++) acc = kb::ext_mul(acc, factor(j0, t));
+        high = acc;
     }
+    __syncthreads();
+    if (j >= ((uint64_t)1 << k)) return;
+    Ext acc = high;
+    for (int t = k - lo; t < k; t++) acc = kb::ext_mul(acc, factor(j, t));
     kb::ext_store(E + 4 * j, acc);
 }
 // E'[j] = E[2j] + alpha (E[2j+1] - E[2j])
@@ -297,6 +442,14 @@ __global__ void gkr_fix_eq_kernel(const uint32_t* __restrict__ E, uint64_t n_out
     if (j >= n_out) return;
     Ext a = ldE(E, 2 * j), b = ldE(E, 2 * j + 1);
     stE(Eo, j, kb::ext_add(a, kb::ext_mul(alpha, kb::ext_sub(b, a))));
+}
+// E''[j] = E'[2j] + a1 (E'[2j+1] - E'[2j]) with E' = E folded by a0: two variables in one launch
+__global__ void gkr_fix_eq2_kernel(const uint32_t* __restrict__ E, uint64_t n_out, Ext a0, Ext a1, uint32_t* __restrict__ Eo) {
+    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_out) return;
+    const Ext e0 = ldE(E, 4 * j), e1 = ldE(E, 4 * j + 1), e2 = ldE(E, 4 * j + 2), e3 = ldE(E, 4 * j + 3);
+    const Ext lo = kb::ext_add(e0, kb::ext_mul(a0, kb::ext_sub(e1, e0))), hi = kb::ext_add(e2, kb::ext_mul(a0, kb::ext_sub(e3, e2)));
+    stE(Eo, j, kb::ext_add(lo, kb::ext_mul(a1, kb::ext_sub(hi, lo))));
 }
 // per-column openings of EVERY chip in two launches: out[c] = sum_{r < rows} eq[r] * col[r].
 // A block takes one chunk of OPEN_ROWS rows of one table (a chip's main or preprocessed columns), keeps its eq values in

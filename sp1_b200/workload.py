@@ -131,7 +131,8 @@ def chip_stats():
 
 # ---- full-shard synthetic machine (constraints + interactions) for bench.py and the scale tests -------------------------------
 def synthetic_machine(workload, seed=42, max_log_rows=22, scale=1.0):
-    """-> dict(names, specs [(height, groups, with_prep[, extra_cols])], blob, main_shapes [(rows, cols)], prep_shapes)
+    """-> dict(names, specs [(height, groups, with_prep[, extra_cols])], blob, main_shapes [(rows, cols)], prep_shapes,
+    interactions [per chip: number of LogUp interactions])
     chips = the core cluster's chips (CORE_CHIPS widths -> 6-column constraint groups) + the three preprocessed tables (+ the
     precompile table of the S3p / S3c workloads), in name order; heights from shard_shapes (multiples of 32), optionally scaled
     down by `scale` (CPU baseline sample).  Calibrated workloads take each chip's constraint count and interaction message
@@ -174,13 +175,14 @@ def synthetic_machine(workload, seed=42, max_log_rows=22, scale=1.0):
         words.append(cw)
         iwords.append(iw)
     blob = SA.machine_blob_with_interactions(words, iwords)
-    return _machine_dict(names, specs, blob)
+    return _machine_dict(names, specs, blob, iwords)
 
 
-def _machine_dict(names, specs, blob):
+def _machine_dict(names, specs, blob, iwords):
     main_shapes = [(s.h, 6 * s.g + (1 if s.wp else 0) + s.extra) for s in specs]
     prep_shapes = [(s.h, 1 + s.extra_prep) for s in specs if s.wp]
-    return dict(names=names, specs=specs, blob=blob, main_shapes=main_shapes, prep_shapes=prep_shapes)
+    interactions = [int(iw[0]) if len(iw) else 0 for iw in iwords]   # each chip's interaction section starts with its count
+    return dict(names=names, specs=specs, blob=blob, main_shapes=main_shapes, prep_shapes=prep_shapes, interactions=interactions)
 
 
 def _recursion_machine(workload, seed, scale):
@@ -199,4 +201,4 @@ def _recursion_machine(workload, seed, scale):
         words.append(cw)
         # recursion chips talk to the memory argument only: a few 5-value (address, extension value) messages per row
         iwords.append(SA.synth_interactions_calibrated(g, True, [5] * min(2 * g, 12)))
-    return _machine_dict(names, specs, SA.machine_blob_with_interactions(words, iwords))
+    return _machine_dict(names, specs, SA.machine_blob_with_interactions(words, iwords), iwords)

@@ -1,0 +1,179 @@
+#!/usr/bin/env python
+"""Per-kernel device times of ONE shard proven alone (torch.profiler, CUDA activities), with the modelled HBM bytes of the
+LogUp-GKR kernels computed from the shard's shapes, and the phase times the library reports for an unprofiled shard.
+usage: python tools/gkr_profile.py [--workload S2c] [--warmup 2] [--out FILE]
+
+The byte model counts the fraction-tree and working arrays only (16 B per extension element, 4 B per base element); trace
+reads of the first level and the eq tables (at most 2^21 x 16 B per layer) are left out."""
+import argparse
+import os
+import re
+import subprocess
+import sys
+from collections import defaultdict
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from sp1_b200 import workload as W  # noqa: E402
+
+
+def gkr_bytes_model(heights, inters, mlr):
+    """modelled bytes per GKR kernel name for the code as it stands: level 0 = base-field numerators + EF denominators, levels 1
+    and 2 written by the first-level pass, two row rounds summed and fixed per pass, the remaining row rounds one per pass"""
+    half = lambda x: (x + 1) // 2  # noqa: E731
+    lens = [list(heights)]
+    for _ in range(1, mlr):
+        lens.append([half(x) for x in lens[-1]])
+    S = [sum(i * x for i, x in zip(inters, ln)) for ln in lens]
+    m = defaultdict(float)
+    m["gkr_first_level_kernel"] = 20 * S[0] + 32 * S[1] + (32 * S[2] if mlr > 2 else 0)
+    for l in range(2, mlr - 1):
+        m["gkr_level_kernel"] += 32 * (S[l] + S[l + 1])
+    for l in range(mlr - 1):
+        seq = (20 if l == 0 else 32) * S[l]
+        rows = [half(x) for x in lens[l]]
+        m["gkr_sum2_kernel"] += seq
+        r = mlr - 1 - l
+        n_fix = 2 if r >= 2 else 1
+        for _ in range(n_fix):
+            rows = [half(x) for x in rows]
+        m["gkr_fix2_kernel"] += seq + 64 * sum(i * x for i, x in zip(inters, rows))
+        for _ in range(r - n_fix):
+            nxt = [half(x) for x in rows]
+            m["gkr_fix_sum_kernel"] += 64 * sum(i * (x + y) for i, x, y in zip(inters, rows, nxt))
+            rows = nxt
+    return m, S
+
+
+def previous_gkr_bytes_model(heights, inters, mlr):
+    """the same model for the pass structure this code replaced (kept for before / after tables): level 0 = EF numerators and
+    denominators written by the first-level pass and read by the level pass; each layer summed by one pass over its sequence
+    (gkr_sum_seq_kernel), then one fix per row round, the first one reading the sequence (gkr_fix_sum_kernel<true>)"""
+    half = lambda x: (x + 1) // 2  # noqa: E731
+    lens = [list(heights)]
+    for _ in range(1, mlr):
+        lens.append([half(x) for x in lens[-1]])
+    S = [sum(i * x for i, x in zip(inters, ln)) for ln in lens]
+    m = defaultdict(float)
+    m["gkr_first_level_kernel"] = 32 * S[0]
+    for l in range(mlr - 1):
+        m["gkr_level_kernel"] += 32 * (S[l] + S[l + 1])
+        m["gkr_sum_seq_kernel"] += 32 * S[l]
+        rows = [half(half(x)) for x in lens[l]]
+        m["gkr_fix_sum_kernel<true>"] += 32 * S[l] + 64 * sum(i * x for i, x in zip(inters, rows))
+        for _ in range(mlr - 2 - l):
+            nxt = [half(x) for x in rows]
+            m["gkr_fix_sum_kernel<false>"] += 64 * sum(i * (x + y) for i, x, y in zip(inters, rows, nxt))
+            rows = nxt
+    return m
+
+
+def kernel_name(n):
+    n = n.replace("(anonymous namespace)::", "")
+    n = re.sub(r"^void ", "", n)
+    return re.sub(r"\(.*", "", n)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="S2c", choices=list(W.WORKLOADS))
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--out", default=None, help="also write the table to this file")
+    args = ap.parse_args()
+
+    import numpy as np
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    from sp1_b200 import Lib
+    from sp1_b200.lib import HostChallenger
+    from sp1_b200 import synth_air as SA
+    from sp1_b200 import shards as SH
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(0)
+    params = W.params_of(args.workload)
+    lib = Lib(device=0, **params)
+    mach = W.synthetic_machine(args.workload, seed=42)
+    inters = mach["interactions"]
+    specs, names = mach["specs"], mach["names"]
+    heights = [s_[0] for s_ in specs]
+    pv0 = 12345
+    pv = ((np.array([pv0, 5, 6, 7], dtype=np.uint64) << np.uint64(32)) % np.uint64(W.P)).astype(np.uint32)
+    mains, preps = [], []
+    for i, sp in enumerate(specs):
+        m_, p_ = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, pv0, SH.shard_seed(0, 0) + i, dev, extra_cols=sp.extra, extra_prep=sp.extra_prep)
+        mains.append(m_)
+        if sp.wp:
+            preps.append(p_)
+    d_main = torch.cat(mains).contiguous()
+    d_prep = torch.cat(preps).contiguous()
+    del mains, preps
+    torch.cuda.synchronize()
+    machine = lib.machine_create(mach["blob"])
+    _, h_prep = lib.jagged_commit_dense(d_prep, [s_.h for s_ in specs if s_.wp], [1 + s_.extra_prep for s_ in specs if s_.wp])
+    chal0 = HostChallenger().st.copy()
+
+    def step():
+        st = chal0.copy()
+        lib.prove_shard(machine, h_prep, d_main, heights, names, pv, st)
+        lib.sync()
+
+    for _ in range(args.warmup):
+        step()
+    step()   # unprofiled: the library's own phase timers
+    phases = {n: lib.phase_ms(n) for n in ("gkr.circuit", "gkr.rounds", "gkr.openings", "gkr.total", "gkr.host_wait", "shard.total")}
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        step()
+        torch.cuda.synchronize()
+    tot, cnt = defaultdict(float), defaultdict(int)
+    for e in prof.events():
+        if e.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        n = kernel_name(e.name)
+        tot[n] += e.time_range.elapsed_us() / 1e3
+        cnt[n] += 1
+
+    mlr = lib.params["max_log_row_count"]
+    model, S = gkr_bytes_model(heights, inters, mlr)
+    try:
+        card = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=5).stdout.strip()
+    except Exception:
+        card = "unavailable"
+    allms = sum(tot.values())
+    lines = [f"# {args.workload}, one shard alone, card: {card}; rows x interactions at level 0 = {S[0]:.3e}",
+             f"# {sum(cnt.values())} device activities, {allms:.2f} ms of device time (serialised)",
+             f"{'kernel':40s} {'launches':>8s} {'ms':>9s} {'share':>6s} {'avg us':>9s}"]
+    for n in sorted(tot, key=lambda k: -tot[k]):
+        lines.append(f"{n:40s} {cnt[n]:8d} {tot[n]:9.3f} {100 * tot[n] / allms:5.1f}% {1e3 * tot[n] / cnt[n]:9.1f}")
+    by_base = defaultdict(float)   # template instances summed: the byte model is per kernel family
+    for n, v in tot.items():
+        if n.startswith("gkr_"):
+            by_base[re.sub(r"<.*", "", n)] += v
+    lines.append(f"{'GKR kernel family':40s} {'ms':>9s} {'model GB':>9s} {'GB/s':>7s}")
+    for n in sorted(by_base, key=lambda k: -by_base[k]):
+        gb = model.get(n, 0.0) / 1e9
+        lines.append(f"{n:40s} {by_base[n]:9.3f}" + (f" {gb:9.3f} {gb / (by_base[n] / 1e3):7.0f}" if gb else ""))
+    gkr_ms = sum(by_base.values())
+    gkr_gb = sum(model.get(n, 0.0) for n in by_base) / 1e9
+    lines.append(f"GKR kernels (gkr_*): {gkr_ms:.3f} ms ({100 * gkr_ms / allms:.1f}% of device time), modelled {gkr_gb:.2f} GB")
+    prev = previous_gkr_bytes_model(heights, inters, mlr)
+    lines.append("previous pass structure (EF level 0, one row round per pass), modelled GB: " +
+                 ", ".join(f"{k} {v / 1e9:.2f}" for k, v in prev.items()) + f"; total {sum(prev.values()) / 1e9:.2f}")
+    lines.append("phases of an unprofiled shard (ms): " + ", ".join(f"{k} {v:.3f}" for k, v in phases.items()))
+    lines.append(f"gpu_mem_used_gb {(torch.cuda.mem_get_info(dev)[1] - torch.cuda.mem_get_info(dev)[0]) / 2**30:.1f}")
+    text = "\n".join(lines)
+    print(text)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write(text + "\n")
+    lib.jagged_round_free(h_prep)
+    lib.machine_free(machine)
+    lib.close()
+
+
+if __name__ == "__main__":
+    main()
