@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 from tests import oracle_lib as O
+from tests.machines import Chip, first_diff, n_interactions, spec_machine
 from tests.test_oracle import _synth_machine_gkr
 
 pytestmark = pytest.mark.gpu
@@ -79,3 +80,145 @@ def test_logup_gkr_and_whole_shard_with_silent_chips():
             lib.jagged_round_free(prep_round)
         lib.machine_free(mach)
         lib.close()
+
+
+# ---- the benchmark's chip shapes: calibrated interactions, >= 2^10 padded interactions, looping grid-stride kernels, mlr = 2, a full
+# batch table -------------------------------------------------------------------------------------------------------------------------
+PRE = [9] * 50 + [5] * 4          # the calibrated precompile table's messages (sp1_b200.workload.synthetic_machine)
+SUM2_THREADS_TOTAL = 396 * 128    # gkr_sum2_kernel: at most 396 blocks of 128 threads (gkr_driver.inc)
+FIX_THREADS_TOTAL = 528 * 256     # gkr_fix2_kernel / gkr_fix_sum_kernel: at most 528 blocks of 256 threads
+
+
+def _upload(mains, preps):
+    import torch
+    d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
+    d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
+    torch.cuda.synchronize()
+    return d_mains, d_preps
+
+
+def _check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed, pow_bits=4):
+    rng = np.random.default_rng(seed)
+    ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
+    och = ch.clone()
+    owords = O.gkr_prove_verify(blob, heights, mains, preps, mlr, och, gkr_pow_bits=pow_bits)
+    d_mains, d_preps = _upload(mains, preps)
+    st = ch.st.copy()
+    words = lib.logup_gkr(mach, heights, d_mains, d_preps, st)
+    assert words.size == owords.size and (words == owords).all(), first_diff(words, owords, "LogUp-GKR proof")
+    assert (st == och.st).all(), "final challenger state differs from the oracle"
+
+
+def _gkr_case(spec, mlr, seed):
+    from sp1_b200 import Lib
+    blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(seed), spec)
+    lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21), gkr_pow_bits=4)
+    mach = lib.machine_create(blob)
+    _check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed + 1)
+    lib.machine_free(mach)
+    lib.close()
+    return blob, heights
+
+
+def _work_items(blob, heights, spec):
+    """(quads of gkr_sum2_kernel, pairs of gkr_fix2_kernel, pairs of the first gkr_fix_sum_kernel) on layer 0"""
+    from sp1_b200 import synth_air as SA
+    q = f2 = fs = 0
+    for c, h in zip(spec, heights):
+        c = Chip(*c)
+        I = SA.synth_interactions_calibrated(c.g, c.wp, list(c.vps))[0] if c.vps else 0
+        rows = (h + 1) // 2
+        q += I * ((rows + 3) // 4)
+        r2 = (rows + 3) // 4
+        f2 += I * ((r2 + 1) // 2)
+        r3 = (r2 + 1) // 2
+        fs += I * ((r3 + 1) // 2)
+    return q, f2, fs
+
+
+def test_logup_gkr_calibrated_ten_interaction_variables():
+    """690 interactions (2^10 padded: the interaction rounds take a second stride over 256 threads, the flatten runs over 1024 slots),
+    messages of 12 values (16 beta powers), filler columns and four preprocessed columns in the openings, an absent chip"""
+    spec = [Chip(1000, 4, False, 30, 3, 0, [12, 4, 9, 5, 1, 7, 12, 3] * 8), Chip(600, 3, True, 20, 0, 3, [9] * 54 + [12] * 100),
+            Chip(2048 + 32, 2, False, None, 0, 0, [2, 3] * 60), Chip(0, 2, True, None, 0, 2, [4] * 5)]
+    blob, _ = _gkr_case(spec, 12, 970)
+    assert 512 < n_interactions(blob) <= 1024
+
+
+def test_logup_gkr_calibrated_eleven_interaction_variables_and_looping_kernels():
+    """nine copies of the calibrated precompile table's messages at full height: 1222 interactions (2^11 padded), and enough work
+    items that gkr_sum2_kernel, gkr_fix2_kernel and gkr_fix_sum_kernel loop over their grids with jobs changing inside a block"""
+    spec = [Chip(4096, 6, i % 2 == 0, 40, 2, 2 if i % 2 == 0 else 0, PRE + [12] * 10) for i in range(9)] + [Chip(3000, 2, False, None, 0, 0, [12] * 30)]
+    blob, heights = _gkr_case(spec, 12, 980)
+    assert n_interactions(blob) > 1024
+    q, f2, fs = _work_items(blob, heights, spec)
+    assert q > SUM2_THREADS_TOTAL and f2 > FIX_THREADS_TOTAL and fs > FIX_THREADS_TOTAL, (q, f2, fs)
+
+
+MLR2_CASES = [
+    # heights 0..4 under max_log_row_count = 2: one row variable per layer, a tree of two levels
+    [Chip(4, 1, False, None, 0, 0, [12, 3]), Chip(3, 1, True, None, 0, 2, [5]), Chip(0, 1, False, None, 0, 0, [4]),
+     Chip(1, 2, False, 12, 1, 0, [4, 4]), Chip(2, 1, False, None, 0, 0, ())],
+    [Chip(2, 1, True), Chip(4, 2, False), Chip(1, 1, False)],
+]
+
+
+@pytest.mark.parametrize("case", range(len(MLR2_CASES)))
+def test_logup_gkr_and_whole_shard_two_row_variables(case):
+    """max_log_row_count = 2 is the only use of gkr_fix2_kernel<uint32_t, false>, of gkr_sum2_kernel<uint32_t> with two = 0 and of
+    gkr_first_level_kernel without level 2: LogUp-GKR alone and the whole shard"""
+    from sp1_b200 import Lib
+    from tests.machines import dense_main, shard_diff
+    mlr, log_stack = 2, 2
+    seed = 990 + case
+    blob, heights, mains, preps, pv, names = spec_machine(np.random.default_rng(seed), MLR2_CASES[case])
+    prm = dict(num_queries=4, pow_bits=3, batch_pow_bits=2, gkr_pow_bits=4)
+    lib = Lib(0, max_log_row_count=mlr, log_stacking_height=log_stack, **prm)
+    mach = lib.machine_create(blob)
+    _check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed + 1)
+    ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(seed + 2), 9))
+    och = ch.clone()
+    opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, **prm)
+    pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+    assert (pc == opc).all(), "preprocessed commitment differs from the oracle"
+    st = ch.st.copy()
+    words = lib.prove_shard(mach, prep_round, dense_main(mains), heights, names, pv, st)
+    assert words.size == owords.size and (words == owords).all(), shard_diff(words, owords)
+    assert (st == och.st).all(), "final challenger state differs from the oracle"
+    lib.jagged_round_free(prep_round)
+    lib.machine_free(mach)
+    lib.close()
+
+
+def full_table_spec(n_chips, seed, absent=True):
+    """n_chips tiny chips with varied heights (1 included, and 0 when `absent`), some with preprocessed columns or filler columns,
+    light and calibrated interactions.  With absent=False every chip takes a slot of the GKR batch table."""
+    rng = np.random.default_rng(seed)
+    heights = ([0] if absent else []) + [1, 2, 3, 32]
+    heights += [int(x) for x in rng.integers(0 if absent else 1, 33, n_chips - len(heights))]
+    spec = []
+    for k, h in enumerate(heights):
+        vps = None if k % 3 == 0 else [int(x) for x in rng.integers(1, 13, 1 + k % 4)]
+        spec.append(Chip(h, 1 + k % 2, k % 4 == 1, None, int(k % 5 == 2), 1 if k % 8 == 5 else 0, vps))
+    return spec
+
+
+def test_logup_gkr_full_batch_table_then_one_chip_too_many():
+    """96 chips with interactions fill the batch table (find_job at n = MAX_JOBS, the largest parameter block); 97 chips must be a
+    clean error, after which the same context proves a valid machine"""
+    from sp1_b200 import Lib
+    from sp1_b200.lib import Sp1B200Error
+    mlr = 5
+    lib = Lib(0, max_log_row_count=mlr, log_stacking_height=mlr, gkr_pow_bits=4)
+    blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(1001), full_table_spec(97, 1000))
+    mach = lib.machine_create(blob)
+    d_mains, d_preps = _upload(mains, preps)
+    with pytest.raises(Sp1B200Error, match="batch table"):
+        lib.logup_gkr(mach, heights, d_mains, d_preps, O.Challenger().st.copy())
+    lib.machine_free(mach)
+    for k, absent in enumerate((False, True)):
+        blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(1002 + k), full_table_spec(96, 1010 + k, absent))
+        mach = lib.machine_create(blob)
+        _check_gkr(lib, mach, blob, heights, mains, preps, mlr, 1020 + k)
+        lib.machine_free(mach)
+    lib.close()

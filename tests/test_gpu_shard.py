@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 from tests import oracle_lib as O
+from tests import machines as M
 from tests.test_oracle import SHARD_SPECS, _synth_machine_gkr
 
 pytestmark = pytest.mark.gpu
@@ -172,3 +173,113 @@ def test_setup_and_prove_shard_equals_setup_then_prove():
     lib.jagged_round_free(prep_round); lib.jagged_round_free(round2)
     lib.machine_free(mach)
     lib.close()
+
+
+# ---- the benchmark's shapes at reduced size, a full GKR batch table, and several contexts proving at once ------------------------------
+
+SMALL_PRM = dict(num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
+
+
+def _oracle_shard(inp, log_stack, mlr, seed):
+    blob, heights, mains, preps, pv, names = inp
+    ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(seed), 9))
+    och = ch.clone()
+    opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, **SMALL_PRM)
+    return ch.st.copy(), opc, owords, och.st.copy()
+
+
+def _prove_and_compare(inp, log_stack, mlr, seed):
+    from sp1_b200 import Lib
+    blob, heights, mains, preps, pv, names = inp
+    st0, opc, owords, ost = _oracle_shard(inp, log_stack, mlr, seed)
+    lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **SMALL_PRM)
+    mach = lib.machine_create(blob)
+    pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+    assert (pc == opc).all(), "preprocessed commitment differs from the oracle"
+    st = st0.copy()
+    words = lib.prove_shard(mach, prep_round, M.dense_main(mains), heights, names, pv, st)
+    assert words.size == owords.size and (words == owords).all(), M.shard_diff(words, owords)
+    assert (st == ost).all(), "final challenger state differs from the oracle"
+    lib.jagged_round_free(prep_round)
+    lib.machine_free(mach)
+    lib.close()
+
+
+@pytest.mark.parametrize("workload,mlr,log_stack", [("tinyc", 14, 12), ("tinyr", 14, 12)])
+def test_prove_shard_workload_machines_match_oracle(workload, mlr, log_stack):
+    """the calibrated core machine (36 chips, 640 interactions, a 682-column precompile table, 2.2 M cells) and the compress-shape machine
+    (recursion chips with up to 36 preprocessed columns) at full smoke size, word for word"""
+    inp = M.workload_machine(workload, seed=1300, max_log_rows=mlr)
+    assert max(inp[1]) <= 1 << mlr
+    _prove_and_compare(inp, log_stack, mlr, 1301)
+
+
+def test_prove_shard_full_batch_table():
+    """96 chips, the most the LogUp-GKR batch table takes (tests/test_gpu_gkr.py checks that 97 is an error): every phase of the shard
+    proof at that chip count, with tiny heights (0 and 1 included)"""
+    from tests.test_gpu_gkr import full_table_spec
+    inp = M.spec_machine(np.random.default_rng(1311), full_table_spec(96, 1321, absent=True))
+    _prove_and_compare(inp, 5, 5, 1330)
+
+
+def test_concurrent_contexts_prove_their_own_shards():
+    """four contexts on four host threads, as bench.py runs its in-flight provers: each has its own machine and preprocessed commit and
+    proves a different shard (own heights and trace seed) twice, so that pooled memory is reused.  Every proof and final challenger
+    state must equal the oracle's proof of that context's own input."""
+    import threading
+    import torch
+    from sp1_b200 import Lib
+    # (machine, max_log_row_count, log_stacking_height): two compress-shape shards of different heights (machine seeds 42 and 44) and
+    # two calibrated core-like shards
+    jobs = [(M.workload_machine("tinyr", seed=1400, max_log_rows=12, scale=0.25, machine_seed=42), 12, 10),
+            (M.workload_machine("tinyr", seed=1401, max_log_rows=12, scale=0.25, machine_seed=44), 12, 10),
+            (M.spec_machine(np.random.default_rng(1402), [M.Chip(1000, 4, False, 30, 3, 0, [12, 4, 9, 5] * 4), M.Chip(0, 2, False, None, 0, 0, [4]),
+                                                          M.Chip(700, 3, True, 20, 0, 3, [9] * 10), M.Chip(96, 1, False, None, 0, 0, None)]), 10, 9),
+            (M.spec_machine(np.random.default_rng(1403), [M.Chip(512, 4, False, 30, 3, 0, [12, 4, 9, 5] * 4), M.Chip(33, 2, False, None, 0, 0, [4]),
+                                                          M.Chip(1024, 3, True, 20, 0, 3, [9] * 10), M.Chip(0, 1, False, None, 0, 0, None)]), 10, 9)]
+    inputs = [inp for inp, _, _ in jobs]
+    assert len({tuple(x[1]) for x in inputs}) == len(inputs), "every context must prove a shard of its own heights"
+    oracle = [_oracle_shard(inp, ls, mlr, 1410 + k) for k, (inp, mlr, ls) in enumerate(jobs)]
+    ctxs = []
+    for (blob, heights, mains, preps, pv, names), mlr, ls in jobs:
+        lib = Lib(0, log_stacking_height=ls, max_log_row_count=mlr, **SMALL_PRM)
+        mach = lib.machine_create(blob)
+        pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+        ctxs.append((lib, mach, pc, prep_round))
+    # half the contexts read their trace from device memory, half through the double-buffered upload slots from pinned host memory
+    dense = [M.dense_main(inp[2]) for inp in inputs]
+    d_dense = [torch.from_numpy(d.view(np.int32)).cuda() if k % 2 == 0 else torch.from_numpy(d.view(np.int32)).pin_memory()
+               for k, d in enumerate(dense)]
+    torch.cuda.synchronize()
+    results = [[None, None] for _ in jobs]
+    errors = []
+    start = threading.Barrier(len(jobs))
+
+    def run(k):
+        try:
+            lib, mach, _, prep_round = ctxs[k]
+            blob, heights, mains, preps, pv, names = inputs[k]
+            start.wait()
+            for rep in range(2):
+                src = d_dense[k] if k % 2 == 0 else lib.upload_begin(d_dense[k], rep)
+                st = oracle[k][0].copy()
+                words = lib.prove_shard(mach, prep_round, src, heights, names, pv, st)
+                results[k][rep] = (words, st)
+        except Exception as e:  # reported below, on the main thread
+            errors.append((k, e))
+
+    ths = [threading.Thread(target=run, args=(k,)) for k in range(len(jobs))]
+    for t in ths:
+        t.start()
+    for t in ths:
+        t.join()
+    assert not errors, errors
+    for k, (_, opc, owords, ost) in enumerate(oracle):
+        assert (ctxs[k][2] == opc).all(), f"context {k}: preprocessed commitment differs from the oracle"
+        for rep, (words, st) in enumerate(results[k]):
+            assert words.size == owords.size and (words == owords).all(), f"context {k}, proof {rep}: " + M.shard_diff(words, owords)
+            assert (st == ost).all(), f"context {k}, proof {rep}: final challenger state differs from the oracle"
+    for lib, mach, _, prep_round in ctxs:
+        lib.jagged_round_free(prep_round)
+        lib.machine_free(mach)
+        lib.close()

@@ -359,3 +359,43 @@ def test_logup_gkr_roundtrip_with_silent_chips(spec, silent, mlr):
     words = O.gkr_prove_verify(blob, heights, mains, preps, mlr, c1, gkr_pow_bits=4)
     c2 = ch.clone()
     assert (O.gkr_prove_verify(blob, heights, mains, preps, mlr, c2, gkr_pow_bits=4) == words).all()
+
+
+# ---- the benchmark's chip shapes at reduced size (calibrated constraints and interactions, filler and extra preprocessed columns) ----
+@pytest.mark.parametrize("workload,mlr,log_stack", [("tinyc", 14, 12), ("tinyr", 12, 10)])
+def test_workload_shard_roundtrip_and_tamper(workload, mlr, log_stack):
+    """a calibrated core shard (36 chips, 640 interactions, messages of up to 12 values, a 682-column precompile table) and a
+    compress-shape shard (recursion chips with up to 36 preprocessed columns), both at a quarter of their size: the restated verifier
+    accepts the oracle's proof and ends in the prover's state, and rejects it after one flipped bit in the LogUp-GKR or zerocheck section"""
+    from tests import machines as M
+    blob, heights, mains, preps, pv, names = M.workload_machine(workload, seed=71, max_log_rows=mlr, scale=0.25)
+    assert max(heights) <= 1 << mlr
+    prm = dict(num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
+    ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(72), 9))
+    c1 = ch.clone()
+    pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, c1, **prm)
+    n_sec = int(words[0])
+    lens = [int(x) for x in words[1:1 + n_sec]]
+    assert n_sec == 5 and words.size == 1 + n_sec + sum(lens)
+    v = ch.clone()
+    assert O.verify_shard(blob, heights, names, log_stack, mlr, v, pc, words, **prm) == 0
+    assert (v.st == c1.st).all()
+    for sec in (1, 2):   # LogUp-GKR, zerocheck
+        off = 1 + n_sec + sum(lens[:sec]) + lens[sec] // 2
+        bad = words.copy(); bad[off] ^= 1
+        assert O.verify_shard(blob, heights, names, log_stack, mlr, ch.clone(), pc, bad, **prm) != 0, sec
+
+
+def test_logup_gkr_roundtrip_calibrated_interactions():
+    """calibrated interactions (synth_interactions_calibrated): a 12-value message (four beta-power bits), constant-1 and column
+    multiplicities, 3-term linear combinations, filler columns and three further preprocessed columns"""
+    from tests.machines import Chip, n_interactions, spec_machine
+    rng = np.random.default_rng(54)
+    blob, heights, mains, preps, pv, _ = spec_machine(rng, [Chip(40, 2, False, 12, 3, 0, [12, 4, 9]), Chip(17, 1, True, None, 0, 3, [5, 12]),
+                                                            Chip(0, 1, False, None, 0, 0, [1]), Chip(64, 3, False, 20, 0, 0, [2, 11, 7, 3])])
+    assert n_interactions(blob) == 2 * (3 + 2 + 1 + 4) + 2
+    ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
+    c1 = ch.clone()
+    words = O.gkr_prove_verify(blob, heights, mains, preps, 6, c1, gkr_pow_bits=4)
+    c2 = ch.clone()
+    assert (O.gkr_prove_verify(blob, heights, mains, preps, 6, c2, gkr_pow_bits=4) == words).all() and (c1.st == c2.st).all()
