@@ -5,9 +5,9 @@
 // jagged_eval/{sumcheck_poly.rs,sumcheck_sum_as_poly.rs,eval_sumcheck_prover.rs}; the GPU twins it replaces:
 // sp1-gpu/crates/{jagged_sumcheck,jagged_assist} + sys/lib/{jagged_sumcheck,jagged_assist}/*.cu.
 // HOW (results identical): the dense buffers of all rounds form one virtual long vector (no restacking copy);
-// each sumcheck round after the first runs as ONE fused kernel (fix the previous variable + accumulate the next
-// round's sums) so the folded vectors are written once and read once; the branching-program sumcheck evaluates all
-// (column, node) pairs of a round in one launch.
+// the first K <= 5 rounds are summed straight from the base-field trace, then each round runs as ONE fused kernel (fix the
+// previous variable + accumulate the next round's sums) so the folded vectors are written once and read once; the
+// branching-program sumcheck evaluates all (column, node) pairs of a round in one launch.
 #include "ctx.cuh"
 #include "challenger.cuh"
 #include "hostfield.hpp"
@@ -192,82 +192,155 @@ __global__ void __launch_bounds__(256) hadamard_fold0_kernel(SegTable base, cons
     block_reduce2(s0, sh, partial, mail);
 }
 
-// ---- round 0 without the materialised little polynomial ("factored" path) -------------------------------------------------------
-// ext[i] = col_eq[c(i)] * row_eq[i - prefix[c]] is a product of two small tables (2^11 and 2^22 entries), so when every column
-// start is even (all heights even: the reference pads heights to multiples of 32, crates/hypercube/src/util.rs:57) a pair (2j, 2j+1)
-// lies in one column and
-//   sum_j ext[2j] b[2j]                       = sum_c col_eq[c] * sum_{j in c} row_eq[r_j] b[2j]
-//   sum_j (ext[2j]+ext[2j+1]) (b[2j]+b[2j+1]) = sum_c col_eq[c] * sum_{j in c} (row_eq[r_j]+row_eq[r_j+1]) (b[2j]+b[2j+1])
-// with base-field b: the inner sums cost EF x F products only and the 2^log_m-entry EF polynomial (4.3 GB for a 2^22-cycle shard) is
-// never written or read.  Every warp walks a contiguous span of pairs, lanes keep running sums for their current column and
-// multiply by col_eq[c] only when the column changes.  The fold by alpha keeps the product form:
-//   ext'[o] = col_eq[c(2o)] * row_eq'[(2o - prefix[c]) / 2],   row_eq'[k] = row_eq[2k] + alpha (row_eq[2k+1] - row_eq[2k]).
+// ---- rounds 0 .. K-1 summed straight from the base-field trace ("aligned" path) -----------------------------------------------
+// ext[i] = col_eq[c(i)] * row_eq[i - prefix[c]].  When 2^K divides every column prefix sum (the reference pads trace heights to
+// multiples of 32, crates/hypercube/src/util.rs:57), every aligned block of 2^(r+1) <= 2^K entries lies in one column, and after
+// r folds by alpha_0 .. alpha_{r-1} both sides of the sumcheck stay in closed form over the base-field trace b:
+//   dense_r[o] = sum_{t < 2^r} w_r[t] b[o 2^r + t],            w_r[t] = prod_{s < r} (bit s of t ? alpha_s : 1 - alpha_s)
+//   ext_r[o]   = col_eq[c] * row_eq_r[(o 2^r - prefix[c]) >> r],  row_eq_r[k] = sum_t w_r[t] row_eq[k 2^r + t].
+// row_eq = eq(z_row high bits) (x) eq(z_row low JK_LOW bits), so row_eq_r = eq_hi (x) L_r with L_r[u] = sum_t w_r[t] eq_lo[u 2^r + t]
+// a table of at most 2^JK_LOW entries that each block builds in shared memory.  A round r < K is then one read-only pass over the
+// trace: per block of 2^(r+1) words, two EF x F weighted sums (lazy 64-bit accumulation) and two products with the L_r table; the
+// factor col_eq[c] * eq_hi[h] is applied once per (column, high row bits) run of a lane.  After round K-1 one pass writes the
+// level-K dense and eq arrays (2^(log_m - K) EF entries each) and sums round K; hadamard_fold_kernel takes it from there.
+// K = 0 (some column starts at an odd index) keeps the materialised path above.
+constexpr int JK_MAX = 5;   // rounds summed from the trace at most (K = 4 measured slower on S2c, DESIGN.md §3.5)
+constexpr int JK_LOW = 10;  // low row bits of the eq_lo factor (the shared tables: 2 x 2^9 EF for round 0)
+struct JWeights { Ext w[1 << JK_MAX]; };  // w_r[t], t < 2^r
+
 __device__ __forceinline__ uint32_t jp_column(const uint64_t* __restrict__ prefix, uint32_t ncols, uint32_t c, uint64_t i) {
     while (c + 1 < ncols && prefix[c + 1] <= i) c++;
     return c;
 }
-__global__ void __launch_bounds__(256) row_eq_fold_kernel(const uint32_t* __restrict__ row_eq, Ext alpha, uint64_t n_out, uint32_t* __restrict__ out) {
-    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= n_out) return;
-    const Ext a = kb::ext_load(row_eq + 8 * k), b = kb::ext_load(row_eq + 8 * k + 4);
-    kb::ext_store(out + 4 * k, kb::ext_add(a, kb::ext_mul(alpha, kb::ext_sub(b, a))));
+// pointer to word i of the virtual vector (i < the last segment end); the caller's aligned block lies inside one segment
+__device__ __forceinline__ const uint32_t* seg_ptr(const SegTable& t, uint64_t i) {
+    int s = 0;
+    uint64_t start = 0;
+    while (s + 1 < t.n && i >= t.end[s]) { start = t.end[s]; s++; }
+    return t.ptr[s] + (i - start);
 }
-__global__ void __launch_bounds__(256) hadamard_sum0_fused_kernel(SegTable base, const uint64_t* __restrict__ prefix, uint32_t ncols,
-                                                                  const uint32_t* __restrict__ start, const uint32_t* __restrict__ col_eq,
-                                                                  const uint32_t* __restrict__ row_eq, uint64_t npairs_real, uint64_t span,
-                                                                  uint32_t* __restrict__ partial, Mail mail) {
+template <int NW>
+__device__ __forceinline__ void load_words(const uint32_t* p, uint32_t* b) {  // p aligned to 4 * min(NW, 4) bytes
+    if constexpr (NW == 1) {
+        b[0] = __ldg(p);
+    } else if constexpr (NW == 2) {
+        const uint2 v = __ldg(reinterpret_cast<const uint2*>(p)); b[0] = v.x; b[1] = v.y;
+    } else {
+#pragma unroll
+        for (int k = 0; k < NW / 4; k++) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(p) + k);
+            b[4 * k] = v.x; b[4 * k + 1] = v.y; b[4 * k + 2] = v.z; b[4 * k + 3] = v.w;
+        }
+    }
+}
+// sum_{t < NW} w[t] b[t]: up to four products (< 4 (p-1)^2 < 2 p 2^32) per 64-bit limb accumulator before one reduction
+template <int NW>
+__device__ __forceinline__ Ext wdot(const Ext* w, const uint32_t* b) {
+    Ext r = kb::ext_zero();
+#pragma unroll
+    for (int t0 = 0; t0 < NW; t0 += 4) {
+        uint64_t a[4] = {0, 0, 0, 0};
+#pragma unroll
+        for (int t = t0; t < t0 + 4 && t < NW; t++)
+#pragma unroll
+            for (int l = 0; l < 4; l++) a[l] += (uint64_t)b[t] * w[t].c[l];
+#pragma unroll
+        for (int l = 0; l < 4; l++) r.c[l] = kb::add(r.c[l], kb::monty_reduce2(a[l]));
+    }
+    return r;
+}
+// L_r[u] = sum_{t < 2^r} w[t] eq_lo[u 2^r + t]
+template <int R>
+__device__ __forceinline__ Ext folded_eq_lo(const JWeights& W, const uint32_t* __restrict__ eq_lo, uint32_t u) {
+    Ext acc = kb::ext_zero();
+#pragma unroll
+    for (int t = 0; t < (1 << R); t++) acc = kb::ext_add(acc, kb::ext_mul(W.w[t], kb::ext_load(eq_lo + 4 * ((u << R) + t))));
+    return acc;
+}
+
+// round R < K: s0 = sum_j ext_R[2j] dense_R[2j], sh = sum_j (ext_R[2j] + ext_R[2j+1]) (dense_R[2j] + dense_R[2j+1]) over the
+// nblk blocks of 2^(R+1) words of the real area; each warp walks a contiguous span of blocks (a multiple of 32)
+template <int R>
+__global__ void __launch_bounds__(256) jagged_round_kernel(SegTable base, const uint64_t* __restrict__ prefix, uint32_t ncols,
+                                                           const uint32_t* __restrict__ start, const uint32_t* __restrict__ col_eq,
+                                                           const uint32_t* __restrict__ eq_hi, const uint32_t* __restrict__ eq_lo, int lb,
+                                                           JWeights W, uint64_t nblk, uint64_t span, uint32_t* __restrict__ partial, Mail mail) {
+    constexpr int NB = 2 << R;  // words per block
+    __shared__ Ext tA[1 << (JK_LOW - 1)], tB[1 << (JK_LOW - 1)];  // tA[q] = L_R[2q], tB[q] = L_R[2q] + L_R[2q+1]
+    for (uint32_t q = threadIdx.x; q < (1u << (lb - R - 1)); q += blockDim.x) {
+        const Ext l0 = folded_eq_lo<R>(W, eq_lo, 2 * q), l1 = folded_eq_lo<R>(W, eq_lo, 2 * q + 1);
+        tA[q] = l0; tB[q] = kb::ext_add(l0, l1);
+    }
+    __syncthreads();
     Ext s0 = kb::ext_zero(), sh = kb::ext_zero();
     Ext t0 = kb::ext_zero(), th = kb::ext_zero();
     const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
-    const uint64_t j_begin = warp * span, j_end = min(j_begin + span, npairs_real);
+    const uint64_t j_begin = warp * span, j_end = min(j_begin + span, nblk);
+    const uint64_t lomask = (1ull << lb) - 1;
     uint32_t c = 0xffffffffu;
+    uint64_t h = 0;
+    auto flush = [&]() {
+        const Ext f = kb::ext_mul(kb::ext_load(col_eq + 4 * c), kb::ext_load(eq_hi + 4 * h));
+        s0 = kb::ext_add(s0, kb::ext_mul(f, t0)); sh = kb::ext_add(sh, kb::ext_mul(f, th));
+        t0 = kb::ext_zero(); th = kb::ext_zero();
+    };
     for (uint64_t j = j_begin + lane; j < j_end; j += 32) {
-        const uint64_t i = 2 * j;
+        const uint64_t i = j * NB;
         const uint32_t cn = jp_column(prefix, ncols, c == 0xffffffffu ? start[i >> JP_SHIFT] : c, i);
-        if (cn != c) {
-            if (c != 0xffffffffu) {
-                const Ext ce = kb::ext_load(col_eq + 4 * c);
-                s0 = kb::ext_add(s0, kb::ext_mul(ce, t0)); sh = kb::ext_add(sh, kb::ext_mul(ce, th));
-                t0 = kb::ext_zero(); th = kb::ext_zero();
-            }
-            c = cn;
+        const uint64_t rho = i - prefix[cn], hn = rho >> lb;
+        if (cn != c || hn != h) {
+            if (c != 0xffffffffu) flush();
+            c = cn; h = hn;
         }
-        const uint32_t b0 = seg_load(base, i), b1 = seg_load(base, i + 1);
-        const uint64_t r = i - prefix[c];
-        const Ext e0 = kb::ext_load(row_eq + 4 * r), e1 = kb::ext_load(row_eq + 4 * r + 4);
-        t0 = kb::ext_add(t0, kb::ext_mul_base(e0, b0));
-        th = kb::ext_add(th, kb::ext_mul_base(kb::ext_add(e0, e1), kb::add(b0, b1)));
+        uint32_t b[NB];
+        load_words<NB>(seg_ptr(base, i), b);
+        const uint32_t q = (uint32_t)((rho & lomask) >> (R + 1));
+        if constexpr (R == 0) {
+            t0 = kb::ext_add(t0, kb::ext_mul_base(tA[q], b[0]));
+            th = kb::ext_add(th, kb::ext_mul_base(tB[q], kb::add(b[0], b[1])));
+        } else {
+            const Ext d0 = wdot<(1 << R)>(W.w, b), d1 = wdot<(1 << R)>(W.w, b + (1 << R));
+            t0 = kb::ext_add(t0, kb::ext_mul(tA[q], d0));
+            th = kb::ext_add(th, kb::ext_mul(tB[q], kb::ext_add(d0, d1)));
+        }
     }
-    if (c != 0xffffffffu) {
-        const Ext ce = kb::ext_load(col_eq + 4 * c);
-        s0 = kb::ext_add(s0, kb::ext_mul(ce, t0)); sh = kb::ext_add(sh, kb::ext_mul(ce, th));
-    }
+    if (c != 0xffffffffu) flush();
     block_reduce2(s0, sh, partial, mail);
 }
-// fix the last variable of round 0 in product form and accumulate round-1 sums; roweq2 = row_eq folded by alpha (row_eq_fold_kernel)
-__global__ void __launch_bounds__(256) hadamard_fold0_fused_kernel(SegTable base, const uint64_t* __restrict__ prefix, uint32_t ncols,
-                                                                   const uint32_t* __restrict__ start, const uint32_t* __restrict__ col_eq,
-                                                                   const uint32_t* __restrict__ roweq2, uint64_t area, uint64_t nout_pairs, Ext alpha,
-                                                                   uint32_t* __restrict__ base_out, uint32_t* __restrict__ ext_out,
-                                                                   uint32_t* __restrict__ partial, uint64_t nout, Mail mail) {
+
+// fix alpha_{K-1}: write level K (dense_K, ext_K: nout = 2^(log_m - K) EF entries each, zero beyond the real area) and sum round K
+template <int K>
+__global__ void __launch_bounds__(256) jagged_fold_to_kernel(SegTable base, const uint64_t* __restrict__ prefix, uint32_t ncols,
+                                                             const uint32_t* __restrict__ start, const uint32_t* __restrict__ col_eq,
+                                                             const uint32_t* __restrict__ eq_hi, const uint32_t* __restrict__ eq_lo, int lb,
+                                                             JWeights W, uint64_t area, uint64_t nout_pairs, uint32_t* __restrict__ base_out,
+                                                             uint32_t* __restrict__ ext_out, uint32_t* __restrict__ partial, uint64_t nout, Mail mail) {
+    constexpr int NW = 1 << K;  // words per level-K entry
+    __shared__ Ext tL[1 << (JK_LOW - 1)];  // L_K[u], u < 2^(lb - K)
+    for (uint32_t u = threadIdx.x; u < (1u << (lb - K)); u += blockDim.x) tL[u] = folded_eq_lo<K>(W, eq_lo, u);
+    __syncthreads();
+    const uint64_t lomask = (1ull << lb) - 1;
     Ext s0 = kb::ext_zero(), sh = kb::ext_zero();
     for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nout_pairs; j += (uint64_t)gridDim.x * blockDim.x) {
         Ext nb[2], ne[2];
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const uint64_t o = 2 * j + h;  // output index; inputs 2o, 2o+1
+        for (int hh = 0; hh < 2; hh++) {
+            const uint64_t o = 2 * j + hh, i = o * NW;
+            nb[hh] = kb::ext_zero(); ne[hh] = kb::ext_zero();
             if (o < nout) {
-                const uint64_t i = 2 * o;
-                const uint32_t b0 = seg_load(base, i), b1 = seg_load(base, i + 1);
-                nb[h] = kb::ext_add(kb::ext_from_base(b0), kb::ext_mul_base(alpha, kb::sub(b1, b0)));
                 if (i < area) {
+                    uint32_t b[NW];
+                    load_words<NW>(seg_ptr(base, i), b);
+                    nb[hh] = wdot<NW>(W.w, b);
                     const uint32_t c = jp_column(prefix, ncols, start[i >> JP_SHIFT], i);
-                    ne[h] = kb::ext_mul(kb::ext_load(col_eq + 4 * c), kb::ext_load(roweq2 + 4 * ((i - prefix[c]) >> 1)));
-                } else ne[h] = kb::ext_zero();
-                kb::ext_store(base_out + 4 * o, nb[h]);
-                kb::ext_store(ext_out + 4 * o, ne[h]);
-            } else { nb[h] = kb::ext_zero(); ne[h] = kb::ext_zero(); }
+                    const uint64_t rho = i - prefix[c];
+                    ne[hh] = kb::ext_mul(kb::ext_mul(kb::ext_load(col_eq + 4 * c), kb::ext_load(eq_hi + 4 * (rho >> lb))),
+                                         tL[(rho & lomask) >> K]);
+                }
+                kb::ext_store(base_out + 4 * o, nb[hh]);
+                kb::ext_store(ext_out + 4 * o, ne[hh]);
+            }
         }
         s0 = kb::ext_add(s0, kb::ext_mul(ne[0], nb[0]));
         sh = kb::ext_add(sh, kb::ext_mul(kb::ext_add(ne[0], ne[1]), kb::ext_add(nb[0], nb[1])));
@@ -684,19 +757,35 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     E4 claim;
     for (size_t i = 0; i < column_claims.size(); i++) claim = claim + col_eq_full[i] * column_claims[i];
 
-    // device tables: col_eq (over last log2_ceil(ncols) coords of z_col == all of z_col), row_eq, prefix sums
-    uint32_t *d_coleq, *d_zrow, *d_roweq, *d_ext, *d_ext2, *d_b, *d_b2, *d_partial;
+    // K = the rounds summed straight from the base-field trace (see jagged_round_kernel): every aligned 2^K block must lie in one
+    // column (2^K divides every prefix sum), in one segment (K <= log_stacking_height) and in one run of 2^lb rows (K <= lb); round
+    // K must still exist (K <= log_m - 1).  K = 0 materialises the little polynomial (odd column starts).
+    const int lb = (int)std::min<uint32_t>(JK_LOW, mlr);
+    uint32_t K = std::min<uint32_t>({(uint32_t)JK_MAX, ls, lm ? lm - 1 : 0, (uint32_t)lb});
+    for (uint64_t p : prefix)
+        if (p) K = std::min<uint32_t>(K, (uint32_t)__builtin_ctzll(p));
+    const uint64_t area = prefix.back();
+
+    // device tables: col_eq (over last log2_ceil(ncols) coords of z_col == all of z_col), the row eq table(s), prefix sums
+    uint32_t *d_coleq, *d_zrow, *d_roweq = nullptr, *d_eqhi = nullptr, *d_eqlo = nullptr, *d_ext, *d_ext2, *d_b, *d_b2, *d_partial;
     uint64_t* d_prefix;
     SP1_TRY(mem.alloc((void**)&d_coleq, col_eq_full.size() * 16));
     SP1_CUDA(cudaMemcpyAsync(d_coleq, col_eq_full.data(), col_eq_full.size() * 16, cudaMemcpyHostToDevice, st));
     SP1_TRY(mem.alloc((void**)&d_zrow, mlr * 16));
     SP1_CUDA(cudaMemcpyAsync(d_zrow, h_z_row, mlr * 16, cudaMemcpyHostToDevice, st));
-    SP1_TRY(mem.alloc((void**)&d_roweq, ((size_t)16) << mlr));
-    SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << mlr), 256, 0, d_zrow, (int)mlr, d_roweq);
+    if (K) {  // row_eq = eq_hi (x) eq_lo: z_row[0 .. mlr-lb) is the high (most significant) part
+        SP1_TRY(mem.alloc((void**)&d_eqhi, ((size_t)16) << (mlr - lb)));
+        SP1_TRY(mem.alloc((void**)&d_eqlo, ((size_t)16) << lb));
+        SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << (mlr - lb)), 256, 0, d_zrow, (int)(mlr - lb), d_eqhi);
+        SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << lb), 256, 0, d_zrow + 4 * (mlr - lb), lb, d_eqlo);
+    } else {
+        SP1_TRY(mem.alloc((void**)&d_roweq, ((size_t)16) << mlr));
+        SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << mlr), 256, 0, d_zrow, (int)mlr, d_roweq);
+    }
     SP1_TRY(mem.alloc((void**)&d_prefix, prefix.size() * 8));
     SP1_CUDA(cudaMemcpyAsync(d_prefix, prefix.data(), prefix.size() * 8, cudaMemcpyHostToDevice, st));
     // start[b] = last column with prefix <= b << JP_SHIFT (two-pointer walk over the blocks of the real area)
-    std::vector<uint32_t> jp_start((size_t)((prefix.back() >> JP_SHIFT) + 1));
+    std::vector<uint32_t> jp_start((size_t)((area >> JP_SHIFT) + 1));
     {
         uint32_t c = 0;
         for (size_t b = 0; b < jp_start.size(); b++) {
@@ -708,26 +797,24 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     uint32_t* d_jp_start;
     SP1_TRY(mem.alloc((void**)&d_jp_start, jp_start.size() * 4));
     SP1_CUDA(cudaMemcpyAsync(d_jp_start, jp_start.data(), jp_start.size() * 4, cudaMemcpyHostToDevice, st));
-    // factored round 0 (no materialised little polynomial) whenever every column starts at an even index
-    bool factored = lm >= 2;
-    for (uint64_t p : prefix) factored = factored && (p & 1) == 0;
-    { static const bool off = [] { const char* e = getenv("SP1B200_JAGGED_MATERIALISE"); return e && e[0] == '1'; }(); if (off) factored = false; }
-    uint32_t* d_roweq2 = nullptr;
-    if (factored) {
-        SP1_TRY(mem.alloc((void**)&d_ext, (N / 4 + 1) * 16));          // only from round 2 on
-        SP1_TRY(mem.alloc((void**)&d_roweq2, ((size_t)16) << (mlr - 1)));
+    // working arrays: level K (written by the fold pass after round K-1) and level K+1; later levels reuse them in turn
+    if (K) {
+        SP1_TRY(mem.alloc((void**)&d_b, (N >> K) * 16));
+        SP1_TRY(mem.alloc((void**)&d_ext, (N >> K) * 16));
+        SP1_TRY(mem.alloc((void**)&d_b2, ((N >> (K + 1)) + 1) * 16));
+        SP1_TRY(mem.alloc((void**)&d_ext2, ((N >> (K + 1)) + 1) * 16));
     } else {
         SP1_TRY(mem.alloc((void**)&d_ext, N * 16));
+        SP1_TRY(mem.alloc((void**)&d_ext2, (N / 2) * 16));
+        SP1_TRY(mem.alloc((void**)&d_b, (N / 2) * 16));
+        SP1_TRY(mem.alloc((void**)&d_b2, (N / 4 + 1) * 16));
     }
-    SP1_TRY(mem.alloc((void**)&d_ext2, (N / 2) * 16));
-    SP1_TRY(mem.alloc((void**)&d_b, (N / 2) * 16));
-    SP1_TRY(mem.alloc((void**)&d_b2, (N / 4 + 1) * 16));
     const unsigned MAXB = 132 * 8;  // eight blocks per SM of an H100
     static_assert(132 * 8 * 8 + 16 <= SP1_MAIL_WORDS, "round partials must fit the mailbox payload");
     d_partial = sp1b200_mail_dev(ctx);  // the round kernels post their block partials straight into the mailbox
     {
         PhaseTimer t(ctx, "jagged.little_poly");
-        if (!factored) SP1_LAUNCH(ctx, jagged_poly_kernel, blocks_for(N), 256, 0, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, d_roweq, N, d_ext);
+        if (!K) SP1_LAUNCH(ctx, jagged_poly_kernel, blocks_for(N), 256, 0, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, d_roweq, N, d_ext);
         t.stop();
     }
     SegTable seg{};
@@ -740,7 +827,33 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     E4 round_claim = claim;
     PhaseTimer t_sc(ctx, "jagged.sumcheck");
     auto grid_for = [&](uint64_t n) { unsigned g = blocks_for(n); return g > MAXB ? MAXB : (g ? g : 1u); };
-    uint32_t *cur_b = nullptr, *cur_e = d_ext, *nxt_b = d_b, *nxt_e = d_ext2;
+    std::vector<E4> w{E4::one()};  // w_r (see jagged_round_kernel): the weights of the 2^r trace words behind one level-r entry
+    JWeights dw{};
+    auto load_weights = [&]() { for (size_t t = 0; t < w.size(); t++) for (int l = 0; l < 4; l++) dw.w[t].c[l] = w[t].c[l]; };
+    // round R < K from the trace; contiguous span of blocks per warp (multiple of 32), over the real area only
+    auto launch_round = [&](uint32_t R, const Mail& mail, unsigned& g) -> sp1b200_err {
+        const uint64_t nblk = area >> (R + 1);
+        g = grid_for(nblk);
+        const uint64_t warps = (uint64_t)g * 8, span = std::max<uint64_t>((((nblk + warps - 1) / warps) + 31) / 32 * 32, 32);
+#define SP1_JROUND(r) case r: SP1_LAUNCH(ctx, jagged_round_kernel<r>, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, \
+                                         d_eqhi, d_eqlo, lb, dw, nblk, span, d_partial, mail); break;
+        switch (R) { SP1_JROUND(0) SP1_JROUND(1) SP1_JROUND(2) SP1_JROUND(3) SP1_JROUND(4)
+                     default: return sp1b200_set_error("jagged_prove: internal: trace round %u", R); }
+#undef SP1_JROUND
+        static_assert(JK_MAX == 5, "one jagged_round_kernel instance per round below JK_MAX");
+        return nullptr;
+    };
+    auto launch_fold_to = [&](const Mail& mail, uint32_t* out_b, uint32_t* out_e, unsigned& g) -> sp1b200_err {
+        const uint64_t nout = N >> K, nout_pairs = nout / 2;
+        g = grid_for(nout_pairs);
+#define SP1_JFOLD(k) case k: SP1_LAUNCH(ctx, jagged_fold_to_kernel<k>, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, \
+                                        d_eqhi, d_eqlo, lb, dw, area, nout_pairs, out_b, out_e, d_partial, nout, mail); break;
+        switch (K) { SP1_JFOLD(1) SP1_JFOLD(2) SP1_JFOLD(3) SP1_JFOLD(4) SP1_JFOLD(5)
+                     default: return sp1b200_set_error("jagged_prove: internal: fold to level %u", K); }
+#undef SP1_JFOLD
+        return nullptr;
+    };
+    uint32_t *cur_b = nullptr, *cur_e = d_ext, *nxt_b = d_b, *nxt_e = K ? d_ext : d_ext2;
     unsigned prev_g = 0;
     uint32_t prev_seq = 0;
     for (uint32_t rd = 0; rd < lm; rd++) {
@@ -748,20 +861,17 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         E4 e0, eh;
         unsigned g;
         if (rd == 0) {
-            g = grid_for(n / 2);
             const Mail mail = sp1b200_mail_next(ctx);
-            if (factored) {
-                // contiguous span of pairs per warp (multiple of 32), over the real area only (beyond it the polynomial is zero)
-                const uint64_t pairs_real = prefix.back() / 2, warps = (uint64_t)g * 8;
-                const uint64_t span = (((pairs_real + warps - 1) / warps) + 31) / 32 * 32;
-                SP1_LAUNCH(ctx, hadamard_sum0_fused_kernel, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, d_roweq, pairs_real,
-                           span ? span : 32, d_partial, mail);
+            if (K) {
+                load_weights();
+                SP1_TRY(launch_round(0, mail, g));
             } else {
+                g = grid_for(n / 2);
                 SP1_LAUNCH(ctx, hadamard_sum0_kernel, g, 256, 0, seg, cur_e, n / 2, d_partial, mail);
             }
             SP1_TRY(sum_mail(ctx, mail.seq, g, e0, eh));
         } else {
-            SP1_TRY(sum_mail(ctx, prev_seq, prev_g, e0, eh));  // accumulated by the previous fold launch
+            SP1_TRY(sum_mail(ctx, prev_seq, prev_g, e0, eh));  // accumulated by the previous launch
         }
         E4 e1 = round_claim - e0;
         E4 c[3];
@@ -776,18 +886,24 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         // fix the variable; the same launch accumulates the next round's sums (unless this was the last round)
         const uint64_t nout = n / 2;
         Ext da{{alpha.c[0], alpha.c[1], alpha.c[2], alpha.c[3]}};
-        g = grid_for((nout + 1) / 2);
         const Mail mail = sp1b200_mail_next(ctx); prev_seq = mail.seq;
-        if (rd == 0) {
-            if (factored) {
-                SP1_LAUNCH(ctx, row_eq_fold_kernel, blocks_for((uint64_t)1 << (mlr - 1)), 256, 0, d_roweq, da, (uint64_t)1 << (mlr - 1), d_roweq2);
-                SP1_LAUNCH(ctx, hadamard_fold0_fused_kernel, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, d_roweq2, prefix.back(),
-                           (nout + 1) / 2, da, nxt_b, nxt_e, d_partial, nout, mail);
-            } else {
-                SP1_LAUNCH(ctx, hadamard_fold0_kernel, g, 256, 0, seg, cur_e, (nout + 1) / 2, da, nxt_b, nxt_e, d_partial, nout, mail);
-            }
-            cur_b = nxt_b; cur_e = nxt_e; nxt_b = d_b2; nxt_e = d_ext;  // d_ext is free again (materialised path) / sized for round 2 on
+        if (rd < K) {  // w_{rd+1}[t] = w_rd[t mod 2^rd] * (bit rd of t ? alpha : 1 - alpha)
+            const size_t m = w.size();
+            w.resize(2 * m);
+            for (size_t t = 0; t < m; t++) { w[m + t] = w[t] * alpha; w[t] = w[t] * (E4::one() - alpha); }
+            load_weights();
+        }
+        if (rd + 1 < K) {
+            SP1_TRY(launch_round(rd + 1, mail, g));
+        } else if (K && rd + 1 == K) {
+            SP1_TRY(launch_fold_to(mail, nxt_b, nxt_e, g));
+            cur_b = nxt_b; cur_e = nxt_e; nxt_b = d_b2; nxt_e = d_ext2;
+        } else if (rd == 0) {
+            g = grid_for((nout + 1) / 2);
+            SP1_LAUNCH(ctx, hadamard_fold0_kernel, g, 256, 0, seg, cur_e, (nout + 1) / 2, da, nxt_b, nxt_e, d_partial, nout, mail);
+            cur_b = nxt_b; cur_e = nxt_e; nxt_b = d_b2; nxt_e = d_ext;  // d_ext (the materialised polynomial) is free again
         } else {
+            g = grid_for((nout + 1) / 2);
             SP1_LAUNCH(ctx, hadamard_fold_kernel, g, 256, 0, cur_b, cur_e, (nout + 1) / 2, da, nxt_b, nxt_e, d_partial, nout, mail);
             std::swap(cur_b, nxt_b); std::swap(cur_e, nxt_e);
         }

@@ -1,10 +1,12 @@
 #!/usr/bin/env python
 """Per-kernel device times of ONE shard proven alone (torch.profiler, CUDA activities), with the modelled HBM bytes of the
-LogUp-GKR kernels computed from the shard's shapes, and the phase times the library reports for an unprofiled shard.
+LogUp-GKR and jagged-sumcheck kernels computed from the shard's shapes, and the phase times the library reports for an
+unprofiled shard.
 usage: python tools/gkr_profile.py [--workload S2c] [--warmup 2] [--out FILE]
 
-The byte model counts the fraction-tree and working arrays only (16 B per extension element, 4 B per base element); trace
-reads of the first level and the eq tables (at most 2^21 x 16 B per layer) are left out."""
+The GKR byte model counts the fraction-tree and working arrays only (16 B per extension element, 4 B per base element); trace
+reads of the first level and the eq tables (at most 2^21 x 16 B per layer) are left out.  The jagged model counts the trace
+reads (4 B per cell of the stacked area) and the extension-field working arrays; the eq tables and L2 re-reads are left out."""
 import argparse
 import os
 import re
@@ -69,6 +71,60 @@ def previous_gkr_bytes_model(heights, inters, mlr):
     return m
 
 
+JK_MAX, JK_LOW = 5, 10  # csrc/jagged.cu
+
+
+def jagged_layout(rounds_heights, ls, mlr):
+    """rounds_heights: per jagged round the column heights -> (area, log_m, K) as sp1b200_jagged_prove sees them: each round
+    padded to a multiple of 2^ls with dummy columns (sp1b200_jagged_commit), K = the rounds summed straight from the trace"""
+    S, R = 1 << ls, 1 << mlr
+    heights = []
+    for hs in rounds_heights:
+        area = sum(hs)
+        added = max(-(-area // S) * S, S) - area
+        added_cols = max(-(-added // R), 1)
+        heights += list(hs) + [R] * (added_cols - 1) + [added - (added_cols - 1) * R]
+    total = sum(heights)
+    lm = (total - 1).bit_length()
+    k = min(JK_MAX, ls, lm - 1, min(JK_LOW, mlr))
+    p = 0
+    for h in heights:
+        p += h
+        if p:
+            k = min(k, (p & -p).bit_length() - 1)
+    return total, lm, k
+
+
+def jagged_bytes_model(area, lm, k):
+    """modelled bytes per jagged-sumcheck kernel for the code as it stands: rounds 0 .. k-1 each one read of the trace, one pass
+    that reads it again and writes the level-k dense and eq arrays, then one fix-and-sum pass per round on EF arrays"""
+    m = defaultdict(float)
+    N = 1 << lm
+    if k == 0:
+        m["jagged_poly_kernel"] = 16 * N
+        m["hadamard_sum0_kernel"] = 4 * area + 16 * N
+        m["hadamard_fold0_kernel"] = 4 * area + 16 * N + 32 * (N >> 1)
+        first = 1
+    else:
+        m["jagged_round_kernel"] = k * 4 * area
+        m["jagged_fold_to_kernel"] = 4 * area + 32 * (N >> k)
+        first = k
+    m["hadamard_fold_kernel"] = sum(32 * (N >> r) + 32 * (N >> (r + 1)) for r in range(first, lm))
+    return m
+
+
+def previous_jagged_bytes_model(area, lm, mlr):
+    """the same model for the pass structure this code replaced: round 0 from the trace, then row_eq folded by alpha_0 and one
+    pass writing the level-1 dense and eq arrays (4.3 GB at log_m = 28), then one fix-and-sum pass per round"""
+    N = 1 << lm
+    m = defaultdict(float)
+    m["hadamard_sum0_fused_kernel"] = 4 * area
+    m["row_eq_fold_kernel"] = 16 * (1 << mlr) + 16 * (1 << (mlr - 1))
+    m["hadamard_fold0_fused_kernel"] = 4 * area + 32 * (N >> 1)
+    m["hadamard_fold_kernel"] = sum(32 * (N >> r) + 32 * (N >> (r + 1)) for r in range(1, lm))
+    return m
+
+
 def kernel_name(n):
     n = n.replace("(anonymous namespace)::", "")
     n = re.sub(r"^void ", "", n)
@@ -101,8 +157,13 @@ def main():
     pv0 = 12345
     pv = ((np.array([pv0, 5, 6, 7], dtype=np.uint64) << np.uint64(32)) % np.uint64(W.P)).astype(np.uint32)
     mains, preps = [], []
+    prep_heights, main_heights = [], []
     for i, sp in enumerate(specs):
         m_, p_ = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, pv0, SH.shard_seed(0, 0) + i, dev, extra_cols=sp.extra, extra_prep=sp.extra_prep)
+        if sp.h:
+            main_heights += [sp.h] * (m_.numel() // sp.h)
+            if sp.wp:
+                prep_heights += [sp.h] * (p_.numel() // sp.h)
         mains.append(m_)
         if sp.wp:
             preps.append(p_)
@@ -122,7 +183,8 @@ def main():
     for _ in range(args.warmup):
         step()
     step()   # unprofiled: the library's own phase timers
-    phases = {n: lib.phase_ms(n) for n in ("gkr.circuit", "gkr.rounds", "gkr.openings", "gkr.total", "gkr.host_wait", "shard.total")}
+    phases = {n: lib.phase_ms(n) for n in ("gkr.circuit", "gkr.rounds", "gkr.openings", "gkr.total", "gkr.host_wait",
+                                            "jagged.sumcheck", "jagged.total", "shard.total")}
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         step()
@@ -162,6 +224,25 @@ def main():
     prev = previous_gkr_bytes_model(heights, inters, mlr)
     lines.append("previous pass structure (EF level 0, one row round per pass), modelled GB: " +
                  ", ".join(f"{k} {v / 1e9:.2f}" for k, v in prev.items()) + f"; total {sum(prev.values()) / 1e9:.2f}")
+    area, lm, k = jagged_layout([prep_heights, main_heights], lib.params["log_stacking_height"], mlr)
+    jmodel = jagged_bytes_model(area, lm, k)
+    jprev = previous_jagged_bytes_model(area, lm, mlr)
+    jmeasured = jprev if "hadamard_sum0_fused_kernel" in tot else jmodel   # a library built before the trace rounds
+    jfam = defaultdict(float)   # the jagged sumcheck and the PCS passes over the same trace
+    for n, v in tot.items():
+        b = re.sub(r"<.*", "", n)
+        if b.startswith(("hadamard_", "jagged_", "row_eq_fold")) or b in ("column_evals_kernel", "batch_columns_kernel", "eq_table_kernel"):
+            jfam[b] += v
+    lines.append(f"{'jagged kernel family':40s} {'ms':>9s} {'model GB':>9s} {'GB/s':>7s}   (area {area / 1e6:.1f} M cells, log_m {lm}, "
+                 f"K = {k} rounds from the trace)")
+    for n in sorted(jfam, key=lambda x: -jfam[x]):
+        gb = (jmeasured.get(n) or (4 * area if n in ("column_evals_kernel", "batch_columns_kernel") else 0.0)) / 1e9
+        lines.append(f"{n:40s} {jfam[n]:9.3f}" + (f" {gb:9.3f} {gb / (jfam[n] / 1e3):7.0f}" if gb else ""))
+    hj = [n for n in jfam if n in jmodel or n in jprev]
+    lines.append(f"jagged sumcheck kernels: {sum(jfam[n] for n in hj):.3f} ms, modelled {sum(jmeasured.values()) / 1e9:.2f} GB "
+                 "(column_evals / batch_columns: trace bytes only)")
+    lines.append("previous jagged pass structure (round 0 from the trace, level 1 materialised), modelled GB: " +
+                 ", ".join(f"{n} {v / 1e9:.2f}" for n, v in jprev.items()) + f"; total {sum(jprev.values()) / 1e9:.2f}")
     lines.append("phases of an unprofiled shard (ms): " + ", ".join(f"{k} {v:.3f}" for k, v in phases.items()))
     lines.append(f"gpu_mem_used_gb {(torch.cuda.mem_get_info(dev)[1] - torch.cuda.mem_get_info(dev)[0]) / 2**30:.1f}")
     text = "\n".join(lines)
