@@ -50,6 +50,18 @@ inline uint32_t* sp1b200_mail_dev(sp1b200_ctx* c) { return c->d_mail + SP1_MAIL_
 inline const uint32_t* sp1b200_mail_host(sp1b200_ctx* c) { return c->h_mail + SP1_MAIL_HDR; }
 extern "C" sp1b200_err sp1b200_mail_wait(sp1b200_ctx* c, uint32_t seq);
 
+// device-level internals shared between translation units (C++ linkage: they stay inside the library)
+sp1b200_err sp1b200_init_tables(sp1b200_ctx* ctx);                                                        // ntt.cu
+sp1b200_err sp1b200_rs_encode_device(sp1b200_ctx* ctx, const uint32_t* d_msg, uint64_t ncols, uint32_t log_h, uint32_t log_blowup,
+                                     uint32_t* d_out);                                                    // ntt.cu
+sp1b200_err sp1b200_permute_device(sp1b200_ctx* ctx, uint32_t* d_states, uint64_t n);                      // merkle.cu
+sp1b200_err sp1b200_merkle_commit_device(sp1b200_ctx* ctx, const uint32_t* d_mat, uint64_t width, uint32_t log_h, uint32_t* d_layers,
+                                         uint32_t* d_root_commit16);                                      // merkle.cu
+sp1b200_err sp1b200_merkle_tree_from_leaves_device(sp1b200_ctx* ctx, uint32_t* d_layers, uint32_t log_h, uint32_t width,
+                                                   uint32_t* d_root_commit16);                            // merkle.cu
+sp1b200_err sp1b200_fri_tree_device(sp1b200_ctx* ctx, const uint32_t* d_cw, uint64_t m, uint32_t* d_layers, uint32_t log_leaves,
+                                    uint32_t* d_root_commit16, Mail mail);                                // merkle.cu
+
 #ifdef __CUDACC__
 // Last step of a posting kernel, called by EVERY thread after the block's payload words were stored through the device
 // alias: the last block to arrive publishes the sequence number (system-scope release) and re-arms the counter.

@@ -16,6 +16,7 @@
 #include "challenger.cuh"
 #include "hostfield.hpp"
 #include "kb31.cuh"
+#include "sumcheck.cuh"
 #include <algorithm>
 #include <memory>
 #include <vector>
@@ -222,28 +223,6 @@ __device__ __forceinline__ void pair_sums(const Row4& x, const Row4& y, const Ex
     se = kb::ext_add(se, ees);
 }
 
-// NE extension sums per block -> partial[block][4 NE] (the mailbox payload: the host transcript polls the flag, ctx.cuh)
-template <int NE>
-__device__ __forceinline__ void block_reduce(const Ext (&v)[NE], uint32_t* __restrict__ partial, const Mail& mail) {
-    // warp shuffles + one barrier (these kernels are latency-bound on the upper layers: a shared-memory tree costs 8 barriers)
-    __shared__ uint32_t red[4 * NE][8];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < 4 * NE; k++) {
-        uint32_t x = v[k / 4].c[k % 4];
-#pragma unroll
-        for (int sft = 16; sft > 0; sft >>= 1) x = kb::add(x, __shfl_down_sync(0xffffffffu, x, sft));
-        if (lane == 0) red[k][warp] = x;
-    }
-    __syncthreads();
-    if (threadIdx.x < 4 * NE) {
-        uint32_t x = 0;
-        for (int q = 0; q < (int)(blockDim.x >> 5); q++) x = kb::add(x, red[threadIdx.x][q]);
-        partial[blockIdx.x * 4 * NE + threadIdx.x] = x;
-    }
-    sp1_mail_done(mail);
-}
-
 // Rounds 0 and 1 of a layer in one pass over its fraction sequence.  work item = (chip, k, row quad i): rows x0..x3 = 4i..4i+3.
 // The eq table is a product, E[2j + b] = P[j] (b ? last : 1 - last) with P[j] = E[2j] + E[2j+1], `last` = round 0's point
 // coordinate: round 0's eval_0 is (1 - last) sum_pairs e P q(x_even), the host applies the factor.  Binding round 0 to a, the
@@ -414,28 +393,6 @@ __global__ void __launch_bounds__(256) gkr_inter_round_kernel(const uint32_t* __
     block_reduce<3>(sums, payload, mail);
 }
 
-// E[j] = prod_t (bit (k-1-t) of j ? x_t : 1 - x_t).  The EQ_LOW_BITS low bits vary inside a block, the others do not: their
-// product is formed once per block, so a thread does EQ_LOW_BITS products instead of k.  Launched with 2^EQ_LOW_BITS threads.
-constexpr int EQ_LOW_BITS = 8;
-__global__ void __launch_bounds__(1 << EQ_LOW_BITS) gkr_eq_table_kernel(const uint32_t* __restrict__ point, int k, uint32_t* __restrict__ E) {
-    const int lo = k < EQ_LOW_BITS ? k : EQ_LOW_BITS;
-    const uint64_t j0 = (uint64_t)blockIdx.x << EQ_LOW_BITS, j = j0 + threadIdx.x;
-    auto factor = [&](uint64_t idx, int t) {
-        const Ext x = kb::ext_load(point + 4 * t);
-        return ((idx >> (k - 1 - t)) & 1) ? x : kb::ext_sub(kb::ext_one(), x);
-    };
-    __shared__ Ext high;
-    if (threadIdx.x == 0) {
-        Ext acc = kb::ext_one();
-        for (int t = 0; t < k - lo; t++) acc = kb::ext_mul(acc, factor(j0, t));
-        high = acc;
-    }
-    __syncthreads();
-    if (j >= ((uint64_t)1 << k)) return;
-    Ext acc = high;
-    for (int t = k - lo; t < k; t++) acc = kb::ext_mul(acc, factor(j, t));
-    kb::ext_store(E + 4 * j, acc);
-}
 // E'[j] = E[2j] + alpha (E[2j+1] - E[2j])
 __global__ void gkr_fix_eq_kernel(const uint32_t* __restrict__ E, uint64_t n_out, Ext alpha, uint32_t* __restrict__ Eo) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -522,16 +479,6 @@ __global__ void __launch_bounds__(256) gkr_open_reduce_kernel(const OpenJob* __r
         out[(uint64_t)job.out_col * 4 + t] = v;
     }
 }
-
-struct DevFree {
-    sp1b200_ctx* ctx; std::vector<void*> ptrs;
-    explicit DevFree(sp1b200_ctx* c) : ctx(c) {}
-    ~DevFree() { for (void* p : ptrs) cudaFreeAsync(p, ctx->stream); }
-    sp1b200_err alloc(void** p, size_t bytes) { SP1_CUDA(cudaMallocFromPoolAsync(p, bytes ? bytes : 4, ctx->pool, ctx->stream)); ptrs.push_back(*p); return nullptr; }
-};
-inline unsigned blocks_for(uint64_t n, unsigned bs = 256) { return (unsigned)((n + bs - 1) / bs); }
-
-inline Ext toExt(const E4& e) { return Ext{{e.c[0], e.c[1], e.c[2], e.c[3]}}; }
 
 // every read is bounds-checked against the end of the blob and every column against the chip's widths: a blob exported for another
 // chip set must become an error, not an out-of-bounds read on host or device

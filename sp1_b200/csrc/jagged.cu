@@ -12,16 +12,10 @@
 #include "challenger.cuh"
 #include "hostfield.hpp"
 #include "kb31.cuh"
+#include "sumcheck.cuh"
 #include <algorithm>
 #include <memory>
 #include <vector>
-
-struct sp1b200_commit;
-extern "C" sp1b200_err sp1b200_stacked_commit(sp1b200_ctx*, const uint32_t*, uint64_t, int, uint32_t*, sp1b200_commit**);
-extern "C" void sp1b200_commit_free(sp1b200_ctx*, sp1b200_commit*);
-extern "C" sp1b200_err sp1b200_stacked_prove(sp1b200_ctx*, sp1b200_commit* const*, uint32_t, const uint32_t*, uint32_t, const uint32_t*,
-                                             uint32_t*, uint32_t*, uint64_t, uint64_t*);
-void host_poseidon2_permute(uint32_t* s16);
 
 #include "pcs.cuh"
 
@@ -49,32 +43,6 @@ void host_compress(const uint32_t* l, const uint32_t* r, uint32_t* out8) {
     for (int j = 0; j < 8; j++) out8[j] = st[j];
 }
 
-struct DevFree {
-    sp1b200_ctx* ctx;
-    std::vector<void*> ptrs;
-    explicit DevFree(sp1b200_ctx* c) : ctx(c) {}
-    ~DevFree() { for (void* p : ptrs) cudaFreeAsync(p, ctx->stream); }
-    sp1b200_err alloc(void** p, size_t bytes) {
-        SP1_CUDA(cudaMallocFromPoolAsync(p, bytes ? bytes : 4, ctx->pool, ctx->stream));
-        ptrs.push_back(*p);
-        return nullptr;
-    }
-};
-inline unsigned blocks_for(uint64_t n, unsigned bs = 256) { return (unsigned)((n + bs - 1) / bs); }
-
-// E[j] = prod_t (j_t ? x_t : 1 - x_t), point[0] <-> MSB of j
-__global__ void eq_table_kernel(const uint32_t* __restrict__ point, int k, uint32_t* __restrict__ E) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= ((uint64_t)1 << k)) return;
-    Ext acc = kb::ext_one();
-    for (int t = 0; t < k; t++) {
-        Ext x = kb::ext_load(point + 4 * t);
-        bool bit = (j >> (k - 1 - t)) & 1;
-        acc = kb::ext_mul(acc, bit ? x : kb::ext_sub(kb::ext_one(), x));
-    }
-    kb::ext_store(E + 4 * j, acc);
-}
-
 // per-column claims: out[c] = sum_{r < rows} row_eq[r] * col[r]   (one block per column)
 __global__ void __launch_bounds__(256) column_claims_kernel(const uint32_t* __restrict__ dense, const uint64_t* __restrict__ col_start,
                                                             const uint64_t* __restrict__ col_rows, const uint32_t* __restrict__ row_eq,
@@ -89,15 +57,8 @@ __global__ void __launch_bounds__(256) column_claims_kernel(const uint32_t* __re
         a0 = kb::add(a0, kb::mul(x, v.x)); a1 = kb::add(a1, kb::mul(x, v.y));
         a2 = kb::add(a2, kb::mul(x, v.z)); a3 = kb::add(a3, kb::mul(x, v.w));
     }
-    __shared__ uint32_t red[4][256];
-    red[0][threadIdx.x] = a0; red[1][threadIdx.x] = a1; red[2][threadIdx.x] = a2; red[3][threadIdx.x] = a3;
-    __syncthreads();
-    for (int s = 128; s > 0; s >>= 1) {
-        if ((int)threadIdx.x < s)
-            for (int l = 0; l < 4; l++) red[l][threadIdx.x] = kb::add(red[l][threadIdx.x], red[l][threadIdx.x + s]);
-        __syncthreads();
-    }
-    if (threadIdx.x < 4) out[c * 4 + threadIdx.x] = red[threadIdx.x][0];
+    const Ext v[1] = {Ext{{a0, a1, a2, a3}}};
+    block_reduce<1>(v, out, Mail{});  // -> out[c * 4 ..]
 }
 
 // jagged little polynomial: ext[i] = col_eq[c(i)] * row_eq[i - prefix[c(i)]] for i < prefix[ncols], else 0.
@@ -131,29 +92,6 @@ __device__ __forceinline__ uint32_t seg_load(const SegTable& t, uint64_t i) {
     return 0;
 }
 
-__device__ __forceinline__ void block_reduce2(Ext a, Ext b, uint32_t* __restrict__ partial, const Mail& mail) {
-    // warp shuffles + one barrier (the late rounds are latency-bound)
-    __shared__ uint32_t red[8][8];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t w[8];
-#pragma unroll
-    for (int l = 0; l < 4; l++) { w[l] = a.c[l]; w[4 + l] = b.c[l]; }
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        uint32_t v = w[k];
-#pragma unroll
-        for (int sft = 16; sft > 0; sft >>= 1) v = kb::add(v, __shfl_down_sync(0xffffffffu, v, sft));
-        if (lane == 0) red[k][warp] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < 8) {
-        uint32_t v = 0;
-        for (int q = 0; q < (int)(blockDim.x >> 5); q++) v = kb::add(v, red[threadIdx.x][q]);
-        partial[blockIdx.x * 8 + threadIdx.x] = v;
-    }
-    sp1_mail_done(mail);  // `partial` is the mailbox payload (ctx.cuh): the host transcript polls instead of copy + synchronise
-}
-
 // round 0: sum_j ext[2j]*base[2j]  and  sum_j (ext[2j]+ext[2j+1]) * (base[2j]+base[2j+1])   (base in F)
 __global__ void __launch_bounds__(256) hadamard_sum0_kernel(SegTable base, const uint32_t* __restrict__ ext, uint64_t npairs,
                                                             uint32_t* __restrict__ partial, Mail mail) {
@@ -164,7 +102,7 @@ __global__ void __launch_bounds__(256) hadamard_sum0_kernel(SegTable base, const
         s0 = kb::ext_add(s0, kb::ext_mul_base(e0, b0));
         sh = kb::ext_add(sh, kb::ext_mul_base(kb::ext_add(e0, e1), kb::add(b0, b1)));
     }
-    block_reduce2(s0, sh, partial, mail);
+    block_reduce<2>({s0, sh}, partial, mail);
 }
 
 // fix the last variable of round 0 (base F -> EF) and accumulate round-1 sums
@@ -189,7 +127,7 @@ __global__ void __launch_bounds__(256) hadamard_fold0_kernel(SegTable base, cons
         s0 = kb::ext_add(s0, kb::ext_mul(ne[0], nb[0]));
         sh = kb::ext_add(sh, kb::ext_mul(kb::ext_add(ne[0], ne[1]), kb::ext_add(nb[0], nb[1])));
     }
-    block_reduce2(s0, sh, partial, mail);
+    block_reduce<2>({s0, sh}, partial, mail);
 }
 
 // ---- rounds 0 .. K-1 summed straight from the base-field trace ("aligned" path) -----------------------------------------------
@@ -306,7 +244,7 @@ __global__ void __launch_bounds__(256) jagged_round_kernel(SegTable base, const 
         }
     }
     if (c != 0xffffffffu) flush();
-    block_reduce2(s0, sh, partial, mail);
+    block_reduce<2>({s0, sh}, partial, mail);
 }
 
 // fix alpha_{K-1}: write level K (dense_K, ext_K: nout = 2^(log_m - K) EF entries each, zero beyond the real area) and sum round K
@@ -345,7 +283,7 @@ __global__ void __launch_bounds__(256) jagged_fold_to_kernel(SegTable base, cons
         s0 = kb::ext_add(s0, kb::ext_mul(ne[0], nb[0]));
         sh = kb::ext_add(sh, kb::ext_mul(kb::ext_add(ne[0], ne[1]), kb::ext_add(nb[0], nb[1])));
     }
-    block_reduce2(s0, sh, partial, mail);
+    block_reduce<2>({s0, sh}, partial, mail);
 }
 
 // rounds >= 1: fix the last variable (EF -> EF) and accumulate the next round's sums
@@ -371,7 +309,7 @@ __global__ void __launch_bounds__(256) hadamard_fold_kernel(const uint32_t* __re
         s0 = kb::ext_add(s0, kb::ext_mul(ne[0], nb[0]));
         sh = kb::ext_add(sh, kb::ext_mul(kb::ext_add(ne[0], ne[1]), kb::ext_add(nb[0], nb[1])));
     }
-    block_reduce2(s0, sh, partial, mail);
+    block_reduce<2>({s0, sh}, partial, mail);
 }
 
 // ---- branching program (slop/crates/jagged/src/poly.rs:136-175, 384-470) ---------------------------------------
@@ -384,82 +322,6 @@ __device__ __forceinline__ int bp_transition(int row_bit, int index_bit, int cur
     return (s >> 1) + 2 * new_cmp;
 }
 
-// One thread per (merged prefix sum k, node in {0, 1/2}).  Point of thread (k, node), big-endian, length dim = 2*(lm+1):
-//   [ bits[k][0 .. split) , lambda , rhos[0 .. round) ]   with split = dim - round - 1
-// left half = "prefix_sum", right half = "next_prefix_sum"; layer l reads the l-th least significant coordinate of each.
-// ri_eq: per layer the 4 values eq((z_row_l, z_index_l), (a, b)) for (a,b) = 00,01,10,11  (shared by all threads).
-// has_lambda == 0: the point is the boolean prefix sums themselves (split == dim): full evaluation, weight zc only.
-__global__ void __launch_bounds__(128) bp_round_kernel(const uint8_t* __restrict__ bits, uint32_t nk, uint32_t dim, uint32_t split,
-                                                       int has_lambda, const uint32_t* __restrict__ rhos, const uint32_t* __restrict__ ri_eq,
-                                                       const uint32_t* __restrict__ zc, const uint32_t* __restrict__ inter, Ext half,
-                                                       uint32_t* __restrict__ partial) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    Ext v = kb::ext_zero();
-    const uint32_t k = t >> 1, node = t & 1;
-    const uint32_t hl = dim / 2;  // lm + 1
-    if (k < nk && (has_lambda || node == 0)) {
-        const uint8_t* b = bits + (size_t)k * dim;
-        auto coord = [&](uint32_t pos) -> Ext {  // pos in [0, dim)
-            if (pos < split) return b[pos] ? kb::ext_one() : kb::ext_zero();
-            if (has_lambda && pos == split) return node ? half : kb::ext_zero();
-            return kb::ext_load(rhos + 4 * (pos - split - 1));
-        };
-        Ext res[4] = {kb::ext_zero(), kb::ext_zero(), kb::ext_one(), kb::ext_zero()};  // success = carry 0, cmp 1
-        for (int layer = (int)hl; layer >= 0; layer--) {
-            // num_vars = hl (z_index has lm+1 coordinates); layer == hl reads beyond every point -> all coordinates 0
-            Ext cur = kb::ext_zero(), nxt = kb::ext_zero();
-            Ext r00 = kb::ext_one(), r01 = kb::ext_zero(), r10 = kb::ext_zero(), r11 = kb::ext_zero();
-            if ((uint32_t)layer < hl) {
-                cur = coord(hl - 1 - layer);
-                nxt = coord(dim - 1 - layer);
-                const uint32_t* e = ri_eq + (size_t)layer * 16;
-                r00 = kb::ext_load(e); r01 = kb::ext_load(e + 4); r10 = kb::ext_load(e + 8); r11 = kb::ext_load(e + 12);
-            }
-            // eq over (cur, next): c00, c01, c10, c11
-            Ext cn = kb::ext_mul(cur, nxt);
-            Ext c11 = cn, c10 = kb::ext_sub(cur, cn), c01 = kb::ext_sub(nxt, cn);
-            Ext c00 = kb::ext_sub(kb::ext_sub(kb::ext_one(), cur), c01);
-            const Ext ri[4] = {r00, r01, r10, r11};
-            const Ext cc[4] = {c00, c01, c10, c11};
-            Ext nres[4];
-#pragma unroll
-            for (int st = 0; st < 4; st++) {
-                Ext acc = kb::ext_zero();
-#pragma unroll
-                for (int a = 0; a < 4; a++) {      // (row_bit, index_bit)
-                    Ext inner = kb::ext_zero();
-                    bool any = false;
-#pragma unroll
-                    for (int c = 0; c < 4; c++) {  // (cur_bit, next_bit)
-                        int o = bp_transition(a >> 1, a & 1, c >> 1, c & 1, st);
-                        if (o >= 0) { inner = kb::ext_add(inner, kb::ext_mul(cc[c], res[o])); any = true; }
-                    }
-                    if (any) acc = kb::ext_add(acc, kb::ext_mul(ri[a], inner));
-                }
-                nres[st] = acc;
-            }
-#pragma unroll
-            for (int st = 0; st < 4; st++) res[st] = nres[st];
-        }
-        // eq factor of this round's variable and the accumulated one
-        v = kb::ext_mul(kb::ext_load(zc + 4 * k), res[0]);
-        if (has_lambda) {
-            Ext eqv = node ? half : (b[split] ? kb::ext_zero() : kb::ext_one());
-            v = kb::ext_mul(v, kb::ext_mul(kb::ext_load(inter + 4 * k), eqv));
-        }
-    }
-    // block reduce: node 0 -> y_0, node 1 -> y_half
-    __shared__ uint32_t red[4][128];
-    for (int l = 0; l < 4; l++) red[l][threadIdx.x] = v.c[l];
-    __syncthreads();
-    for (int s = 64; s >= 2; s >>= 1) {  // keep parity (node) separate: stop at 2
-        if ((int)threadIdx.x < s)
-            for (int l = 0; l < 4; l++) red[l][threadIdx.x] = kb::add(red[l][threadIdx.x], red[l][threadIdx.x + s]);
-        __syncthreads();
-    }
-    if (threadIdx.x < 8) partial[blockIdx.x * 8 + threadIdx.x] = red[threadIdx.x & 3][threadIdx.x >> 2];
-}
-
 // ---- prefix / suffix form of the same evaluation -----------------------------------------------------------------
 // The evaluation is  e0^T M_0 M_1 ... M_hl init  with one 4x4 transfer matrix per layer, M_l = M(cur_l, next_l).  In sumcheck
 // round r only ONE layer holds the free variable: layers above it still see the column's boolean prefix-sum bits (and, in
@@ -469,6 +331,7 @@ __global__ void __launch_bounds__(128) bp_round_kernel(const uint8_t* __restrict
 //   P_k    = e0^T M_0 ... M_{layer-1}   (prefix row vector, one vector-matrix product per round: bp_update_kernel)
 // i.e. two small products per (column, node) and round instead of hl+1 (the reference keeps the same prefix/suffix states,
 // sp1-gpu/crates/sys/lib/jagged_assist).  Every product is exact field arithmetic, so the round polynomials are unchanged.
+// ri_eq: per layer the 4 values eq((z_row_l, z_index_l), (a, b)) for (a, b) = 00, 01, 10, 11 (shared by all columns)
 struct BpMat { Ext ri[4], cc[4]; };
 __device__ __forceinline__ void bp_layer_coeffs(const uint32_t* __restrict__ ri_eq, uint32_t layer, uint32_t hl, const Ext& cur, const Ext& nxt, BpMat& m) {
     if (layer < hl) {
@@ -479,7 +342,7 @@ __device__ __forceinline__ void bp_layer_coeffs(const uint32_t* __restrict__ ri_
     m.cc[3] = cn; m.cc[2] = kb::ext_sub(cur, cn); m.cc[1] = kb::ext_sub(nxt, cn);
     m.cc[0] = kb::ext_sub(kb::ext_sub(kb::ext_one(), cur), m.cc[1]);
 }
-// out = M res   (column form; same accumulation order as bp_round_kernel)
+// out = M res   (column form)
 __device__ __forceinline__ void bp_apply(const BpMat& m, const Ext res[4], Ext out[4]) {
 #pragma unroll
     for (int st = 0; st < 4; st++) {
@@ -541,11 +404,11 @@ __global__ void __launch_bounds__(128) bp_suffix_kernel(const uint8_t* __restric
     }
 }
 // round r: thread (k, node) -> zc[k] * inter[k] * eq(lambda, bit) * P_k . M_layer(lambda_node) . T_k[layer+1]
-__global__ void __launch_bounds__(128) bp_round2_kernel(const uint8_t* __restrict__ bits, uint32_t nk, uint32_t dim, uint32_t round,
-                                                        const uint32_t* __restrict__ rho_by_pos, const uint32_t* __restrict__ ri_eq,
-                                                        const uint32_t* __restrict__ zc, const uint32_t* __restrict__ inter,
-                                                        const uint32_t* __restrict__ P, const uint32_t* __restrict__ T, Ext half,
-                                                        uint32_t* __restrict__ partial, Mail mail) {
+__global__ void __launch_bounds__(128) bp_round_kernel(const uint8_t* __restrict__ bits, uint32_t nk, uint32_t dim, uint32_t round,
+                                                       const uint32_t* __restrict__ rho_by_pos, const uint32_t* __restrict__ ri_eq,
+                                                       const uint32_t* __restrict__ zc, const uint32_t* __restrict__ inter,
+                                                       const uint32_t* __restrict__ P, const uint32_t* __restrict__ T, Ext half,
+                                                       uint32_t* __restrict__ partial, Mail mail) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     Ext v = kb::ext_zero();
     const uint32_t k = t >> 1, node = t & 1;
@@ -569,16 +432,8 @@ __global__ void __launch_bounds__(128) bp_round2_kernel(const uint8_t* __restric
         const Ext eqv = node ? half : (b[split] ? kb::ext_zero() : kb::ext_one());
         v = kb::ext_mul(kb::ext_mul(kb::ext_load(zc + 4 * k), val), kb::ext_mul(kb::ext_load(inter + 4 * k), eqv));
     }
-    __shared__ uint32_t red[4][128];
-    for (int l = 0; l < 4; l++) red[l][threadIdx.x] = v.c[l];
-    __syncthreads();
-    for (int s = 64; s >= 2; s >>= 1) {  // keep parity (node) separate: stop at 2
-        if ((int)threadIdx.x < s)
-            for (int l = 0; l < 4; l++) red[l][threadIdx.x] = kb::add(red[l][threadIdx.x], red[l][threadIdx.x + s]);
-        __syncthreads();
-    }
-    if (threadIdx.x < 8) partial[blockIdx.x * 8 + threadIdx.x] = red[threadIdx.x & 3][threadIdx.x >> 2];
-    sp1_mail_done(mail);
+    // node 0 -> y_0, node 1 -> y_half: partial[block] = (y_0 limbs, y_half limbs)
+    block_reduce<2>({node ? kb::ext_zero() : v, node ? v : kb::ext_zero()}, partial, mail);
 }
 // after round r's challenge: bind position split = dim-1-r: rho_by_pos, inter[k] *= eq(alpha, bit), P_k <- P_k M_layer(bound)
 // (at the switch to the second half P_k restarts at e0^T: the caller rebuilds T with the bound next-coordinates first)
@@ -614,23 +469,6 @@ inline void interp_0_1_half(const E4& y0, const E4& y1, const E4& yh, E4 c[3]) {
     c[2] = (y1 + y0) * two - yh * four;
 }
 inline E4 eval3(const E4 c[3], const E4& x) { return (c[2] * x + c[1]) * x + c[0]; }
-
-sp1b200_err sum_partials(sp1b200_ctx* ctx, const uint32_t* d_partial, unsigned nblk, E4& a, E4& b) {
-    std::vector<uint32_t> h((size_t)nblk * 8);
-    SP1_CUDA(cudaMemcpyAsync(h.data(), d_partial, h.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    SP1_CUDA(cudaStreamSynchronize(ctx->stream));
-    a = E4(); b = E4();
-    for (unsigned k = 0; k < nblk; k++) { a = a + E4::load(&h[8 * k]); b = b + E4::load(&h[8 * k + 4]); }
-    return nullptr;
-}
-// same sums from the mailbox payload of the posting kernel with sequence number `seq` (8 words per block)
-sp1b200_err sum_mail(sp1b200_ctx* ctx, uint32_t seq, unsigned nblk, E4& a, E4& b) {
-    SP1_TRY(sp1b200_mail_wait(ctx, seq));
-    const uint32_t* h = sp1b200_mail_host(ctx);
-    a = E4(); b = E4();
-    for (unsigned k = 0; k < nblk; k++) { a = a + E4::load(&h[8 * k]); b = b + E4::load(&h[8 * k + 4]); }
-    return nullptr;
-}
 
 }  // namespace
 
@@ -703,7 +541,7 @@ sp1b200_err sp1b200_jagged_column_claims(sp1b200_ctx* ctx, const sp1b200_jagged_
     SP1_CUDA(cudaMemcpyAsync(d_z, h_z_row, mlr * 16, cudaMemcpyHostToDevice, ctx->stream));
     SP1_CUDA(cudaMemcpyAsync(d_start, start.data(), nc * 8, cudaMemcpyHostToDevice, ctx->stream));
     SP1_CUDA(cudaMemcpyAsync(d_rows, nrows.data(), nc * 8, cudaMemcpyHostToDevice, ctx->stream));
-    SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << mlr), 256, 0, d_z, (int)mlr, d_eq);
+    SP1_TRY(launch_eq_table(ctx, d_z, (int)mlr, d_eq));
     SP1_LAUNCH(ctx, column_claims_kernel, (unsigned)nc, 256, 0, r->d_dense, d_start, d_rows, d_eq, d_out);
     SP1_CUDA(cudaMemcpyAsync(h_out, d_out, nc * 16, cudaMemcpyDeviceToHost, ctx->stream));
     SP1_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -776,11 +614,11 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     if (K) {  // row_eq = eq_hi (x) eq_lo: z_row[0 .. mlr-lb) is the high (most significant) part
         SP1_TRY(mem.alloc((void**)&d_eqhi, ((size_t)16) << (mlr - lb)));
         SP1_TRY(mem.alloc((void**)&d_eqlo, ((size_t)16) << lb));
-        SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << (mlr - lb)), 256, 0, d_zrow, (int)(mlr - lb), d_eqhi);
-        SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << lb), 256, 0, d_zrow + 4 * (mlr - lb), lb, d_eqlo);
+        SP1_TRY(launch_eq_table(ctx, d_zrow, (int)(mlr - lb), d_eqhi));
+        SP1_TRY(launch_eq_table(ctx, d_zrow + 4 * (mlr - lb), lb, d_eqlo));
     } else {
         SP1_TRY(mem.alloc((void**)&d_roweq, ((size_t)16) << mlr));
-        SP1_LAUNCH(ctx, eq_table_kernel, blocks_for((uint64_t)1 << mlr), 256, 0, d_zrow, (int)mlr, d_roweq);
+        SP1_TRY(launch_eq_table(ctx, d_zrow, (int)mlr, d_roweq));
     }
     SP1_TRY(mem.alloc((void**)&d_prefix, prefix.size() * 8));
     SP1_CUDA(cudaMemcpyAsync(d_prefix, prefix.data(), prefix.size() * 8, cudaMemcpyHostToDevice, st));
@@ -858,7 +696,8 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     uint32_t prev_seq = 0;
     for (uint32_t rd = 0; rd < lm; rd++) {
         const uint64_t n = N >> rd;  // current length
-        E4 e0, eh;
+        E4 s2[2];  // eval_0, eval_half
+        E4 &e0 = s2[0], &eh = s2[1];
         unsigned g;
         if (rd == 0) {
             const Mail mail = sp1b200_mail_next(ctx);
@@ -869,9 +708,9 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
                 g = grid_for(n / 2);
                 SP1_LAUNCH(ctx, hadamard_sum0_kernel, g, 256, 0, seg, cur_e, n / 2, d_partial, mail);
             }
-            SP1_TRY(sum_mail(ctx, mail.seq, g, e0, eh));
+            SP1_TRY(sum_mail_partials(ctx, mail.seq, g, s2));
         } else {
-            SP1_TRY(sum_mail(ctx, prev_seq, prev_g, e0, eh));  // accumulated by the previous launch
+            SP1_TRY(sum_mail_partials(ctx, prev_seq, prev_g, s2));  // accumulated by the previous launch
         }
         E4 e1 = round_claim - e0;
         E4 c[3];
@@ -885,7 +724,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         round_claim = eval3(c, alpha);
         // fix the variable; the same launch accumulates the next round's sums (unless this was the last round)
         const uint64_t nout = n / 2;
-        Ext da{{alpha.c[0], alpha.c[1], alpha.c[2], alpha.c[3]}};
+        const Ext da = to_ext(alpha);
         const Mail mail = sp1b200_mail_next(ctx); prev_seq = mail.seq;
         if (rd < K) {  // w_{rd+1}[t] = w_rd[t mod 2^rd] * (bit rd of t ? alpha : 1 - alpha)
             const size_t m = w.size();
@@ -944,12 +783,11 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             E4 e11 = p, e10 = zr - p, e01 = zi - p, e00 = one - zr - e01;
             e00.store(&ri[l * 16]); e01.store(&ri[l * 16 + 4]); e10.store(&ri[l * 16 + 8]); e11.store(&ri[l * 16 + 12]);
         }
-        uint8_t* d_bits; uint32_t *d_ri, *d_zc, *d_inter, *d_rhos, *d_part;
+        uint8_t* d_bits; uint32_t *d_ri, *d_zc, *d_inter, *d_part;
         SP1_TRY(mem.alloc((void**)&d_bits, bits.size()));
         SP1_TRY(mem.alloc((void**)&d_ri, ri.size() * 4));
         SP1_TRY(mem.alloc((void**)&d_zc, (size_t)nk * 16));
         SP1_TRY(mem.alloc((void**)&d_inter, (size_t)nk * 16));
-        SP1_TRY(mem.alloc((void**)&d_rhos, (size_t)dim * 16));
         const unsigned nblk = (2 * nk + 127) / 128;
         SP1_TRY(mem.alloc((void**)&d_part, (size_t)nblk * 32));
         SP1_CUDA(cudaMemcpyAsync(d_bits, bits.data(), bits.size(), cudaMemcpyHostToDevice, st));
@@ -957,15 +795,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         SP1_CUDA(cudaMemcpyAsync(d_zc, zc.data(), (size_t)nk * 16, cudaMemcpyHostToDevice, st));
         std::vector<E4> ones(nk, E4::one());
         SP1_CUDA(cudaMemcpyAsync(d_inter, ones.data(), (size_t)nk * 16, cudaMemcpyHostToDevice, st));
-        const E4 half = E4::from_base(hf::inv(hf::to_monty(2)));
-        Ext dhalf{{half.c[0], 0, 0, 0}};
-        // claimed sum = full evaluation at the boolean prefix sums (full_jagged_little_polynomial_evaluation, poly.rs:183-232)
-        E4 dummy;
-        SP1_LAUNCH(ctx, bp_round_kernel, nblk, 128, 0, d_bits, nk, dim, dim, 0, d_rhos, d_ri, d_zc, d_inter, dhalf, d_part);
-        SP1_TRY(sum_partials(ctx, d_part, nblk, je_claimed, dummy));
-        ch.observe_n(je_claimed.c, 4);
-        E4 cl = je_claimed;
-        je_words.push_back(dim);
+        const Ext dhalf = to_ext(E4::from_base(hf::inv(hf::to_monty(2))));
         // prefix / suffix states (see bp_suffix_kernel): T for the first half now, rebuilt once when the second half starts
         uint32_t *d_T, *d_P, *d_rho_pos;
         SP1_TRY(mem.alloc((void**)&d_T, (size_t)(hl + 2) * nk * 64));
@@ -978,15 +808,27 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             SP1_CUDA(cudaMemsetAsync(d_rho_pos, 0, (size_t)dim * 16, st));
         }
         SP1_LAUNCH(ctx, bp_suffix_kernel, blocks_for(nk, 128), 128, 0, d_bits, nk, dim, 0, d_rho_pos, d_ri, d_T);
+        // claimed sum = full evaluation at the boolean prefix sums (full_jagged_little_polynomial_evaluation, poly.rs:183-232):
+        // the first-half suffix table at layer 0 holds it per column, je_claimed = sum_k zc[k] T_k[0][state 0]
+        {
+            std::vector<E4> t0((size_t)nk * 4);  // layer 0 of T: [nk][4 states]
+            SP1_CUDA(cudaMemcpyAsync(t0.data(), d_T, t0.size() * 16, cudaMemcpyDeviceToHost, st));
+            SP1_CUDA(cudaStreamSynchronize(st));
+            for (uint32_t k = 0; k < nk; k++) je_claimed = je_claimed + zc[k] * t0[4 * k];
+        }
+        ch.observe_n(je_claimed.c, 4);
+        E4 cl = je_claimed;
+        je_words.push_back(dim);
         const bool bp_mail = (size_t)nblk * 8 <= SP1_MAIL_WORDS;  // otherwise fall back to copy + synchronise
         for (uint32_t round = 0; round < dim; round++) {
             if (round == hl) SP1_LAUNCH(ctx, bp_suffix_kernel, blocks_for(nk, 128), 128, 0, d_bits, nk, dim, 1, d_rho_pos, d_ri, d_T);
             const Mail mail = sp1b200_mail_next(ctx);
-            SP1_LAUNCH(ctx, bp_round2_kernel, nblk, 128, 0, d_bits, nk, dim, round, d_rho_pos, d_ri, d_zc, d_inter, d_P, d_T, dhalf,
+            SP1_LAUNCH(ctx, bp_round_kernel, nblk, 128, 0, d_bits, nk, dim, round, d_rho_pos, d_ri, d_zc, d_inter, d_P, d_T, dhalf,
                        bp_mail ? sp1b200_mail_dev(ctx) : d_part, bp_mail ? mail : Mail{nullptr, nullptr, 0});
-            E4 y0, yh;
-            if (bp_mail) SP1_TRY(sum_mail(ctx, mail.seq, nblk, y0, yh));
-            else SP1_TRY(sum_partials(ctx, d_part, nblk, y0, yh));
+            E4 y[2];
+            if (bp_mail) SP1_TRY(sum_mail_partials(ctx, mail.seq, nblk, y));
+            else SP1_TRY(sum_device_partials(ctx, d_part, nblk, y));
+            const E4 &y0 = y[0], &yh = y[1];
             E4 y1 = cl - y0;
             E4 c[3];
             interp_0_1_half(y0, y1, yh, c);
@@ -996,7 +838,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             E4 alpha; ch.sample_ext(alpha.c);
             rhos.insert(rhos.begin(), alpha);
             cl = eval3(c, alpha);
-            Ext da{{alpha.c[0], alpha.c[1], alpha.c[2], alpha.c[3]}};
+            const Ext da = to_ext(alpha);
             SP1_LAUNCH(ctx, bp_update_kernel, blocks_for(nk, 128), 128, 0, d_bits, nk, dim, round, da, d_rho_pos, d_ri, d_inter, d_P);
         }
         je_eval = cl;

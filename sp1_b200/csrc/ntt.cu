@@ -16,14 +16,9 @@
 #include "ctx.cuh"
 #include <cstdlib>
 #include "kb31.cuh"
+#include "sumcheck.cuh"
 
 namespace {
-
-__device__ __forceinline__ uint32_t root_pow(const uint32_t* __restrict__ TH, const uint32_t* __restrict__ TL, uint32_t e) {
-    uint32_t hi = __ldg(TH + (e >> 12));
-    uint32_t lo = e & 4095u;
-    return lo ? kb::mul(hi, __ldg(TL + lo)) : hi;
-}
 
 __global__ void init_tables_kernel(uint32_t* TH, uint32_t* TL) {
     // w = 3^127 generates the 2^24-th roots (sppark/ntt/parameters/koala_bear.h:5-36, checked in tests)

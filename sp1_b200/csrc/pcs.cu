@@ -13,14 +13,10 @@
 #include "hostfield.hpp"
 #include "kb31.cuh"
 #include "poseidon2.cuh"
+#include "sumcheck.cuh"
 #include <array>
 #include <memory>
 #include <vector>
-
-sp1b200_err sp1b200_rs_encode_device(sp1b200_ctx*, const uint32_t*, uint64_t, uint32_t, uint32_t, uint32_t*);
-sp1b200_err sp1b200_merkle_commit_device(sp1b200_ctx*, const uint32_t*, uint64_t, uint32_t, uint32_t*, uint32_t*);
-sp1b200_err sp1b200_merkle_tree_from_leaves_device(sp1b200_ctx*, uint32_t*, uint32_t, uint32_t, uint32_t*);
-sp1b200_err sp1b200_fri_tree_device(sp1b200_ctx*, const uint32_t*, uint64_t, uint32_t*, uint32_t, uint32_t*, Mail);
 
 struct sp1b200_commit {
     uint64_t ncols = 0;
@@ -35,26 +31,6 @@ struct sp1b200_commit {
 namespace {
 
 using kb::Ext;
-
-__device__ __forceinline__ uint32_t root_pow(const uint32_t* __restrict__ TH, const uint32_t* __restrict__ TL, uint32_t e) {
-    uint32_t hi = __ldg(TH + (e >> 12));
-    uint32_t lo = e & 4095u;
-    return lo ? kb::mul(hi, __ldg(TL + lo)) : hi;
-}
-
-// E[j] = prod_t (j_t ? x_t : 1 - x_t), point[0] <-> MSB of j
-__global__ void eq_table_kernel(const uint32_t* __restrict__ point, int k, uint32_t* __restrict__ E) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= ((uint64_t)1 << k)) return;
-    Ext acc = kb::ext_one();
-    for (int t = 0; t < k; t++) {
-        Ext x = kb::ext_load(point + 4 * t);
-        bool bit = (j >> (k - 1 - t)) & 1;
-        Ext f = bit ? x : kb::ext_sub(kb::ext_one(), x);
-        acc = kb::ext_mul(acc, f);
-    }
-    kb::ext_store(E + 4 * j, acc);
-}
 
 // out[i] (+)= sum_c coeff[c] * cols[c][i]   ; out as Ext AoS [h]
 __global__ void __launch_bounds__(256) batch_columns_kernel(const uint32_t* __restrict__ cols, uint64_t ncols, uint64_t h,
@@ -102,15 +78,8 @@ __global__ void __launch_bounds__(256) column_evals_kernel(const uint32_t* __res
         a0 = kb::add(a0, kb::mul(x, v.x)); a1 = kb::add(a1, kb::mul(x, v.y));
         a2 = kb::add(a2, kb::mul(x, v.z)); a3 = kb::add(a3, kb::mul(x, v.w));
     }
-    __shared__ uint32_t red[4][256];
-    red[0][threadIdx.x] = a0; red[1][threadIdx.x] = a1; red[2][threadIdx.x] = a2; red[3][threadIdx.x] = a3;
-    __syncthreads();
-    for (int s = 128; s > 0; s >>= 1) {
-        if ((int)threadIdx.x < s)
-            for (int l = 0; l < 4; l++) red[l][threadIdx.x] = kb::add(red[l][threadIdx.x], red[l][threadIdx.x + s]);
-        __syncthreads();
-    }
-    if (threadIdx.x < 4) partial[(c * slices + sl) * 4 + threadIdx.x] = red[threadIdx.x][0];
+    const Ext v[1] = {Ext{{a0, a1, a2, a3}}};
+    block_reduce<1>(v, partial + c * slices * 4, Mail{});  // -> partial[(c * slices + sl) * 4 ..]
 }
 
 // out[c] = sum_sl partial[c][sl]
@@ -140,22 +109,8 @@ __global__ void __launch_bounds__(256) dot_even_kernel(const uint32_t* __restric
         Ext m = kb::ext_load(mle + 8 * j);
         acc = kb::ext_add(acc, kb::ext_mul(e, m));
     }
-    __shared__ uint32_t red[4][256];
-    for (int l = 0; l < 4; l++) red[l][threadIdx.x] = acc.c[l];
-    __syncthreads();
-    for (int s = 128; s > 0; s >>= 1) {
-        if ((int)threadIdx.x < s)
-            for (int l = 0; l < 4; l++) red[l][threadIdx.x] = kb::add(red[l][threadIdx.x], red[l][threadIdx.x + s]);
-        __syncthreads();
-    }
-    if (threadIdx.x < 4) partial[blockIdx.x * 4 + threadIdx.x] = red[threadIdx.x][0];
-}
-
-// E'[j] = E[2j] + E[2j+1]  (drops the last coordinate of the eq point)
-__global__ void halve_eq_kernel(const uint32_t* __restrict__ E, uint64_t n_out, uint32_t* __restrict__ Eo) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n_out) return;
-    kb::ext_store(Eo + 4 * j, kb::ext_add(kb::ext_load(E + 8 * j), kb::ext_load(E + 8 * j + 4)));
+    const Ext v[1] = {acc};
+    block_reduce<1>(v, partial, Mail{});
 }
 
 // mle'[j] = mle[2j] + beta * mle[2j+1]
@@ -218,20 +173,6 @@ __global__ void gather_fri_values_kernel(const uint32_t* __restrict__ cw, uint64
     uint32_t q = t >> 3, w = t & 7;
     out[t] = cw[(w & 3) * m + 2 * (uint64_t)idx[q] + (w >> 2)];
 }
-
-struct DevFree {
-    sp1b200_ctx* ctx;
-    std::vector<void*> ptrs;
-    explicit DevFree(sp1b200_ctx* c) : ctx(c) {}
-    ~DevFree() { for (void* p : ptrs) cudaFreeAsync(p, ctx->stream); }
-    sp1b200_err alloc(void** p, size_t bytes) {
-        SP1_CUDA(cudaMallocFromPoolAsync(p, bytes ? bytes : 4, ctx->pool, ctx->stream));
-        ptrs.push_back(*p);
-        return nullptr;
-    }
-};
-
-inline unsigned blocks_for(uint64_t n, unsigned bs = 256) { return (unsigned)((n + bs - 1) / bs); }
 
 }  // namespace
 
@@ -313,7 +254,7 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
     SP1_TRY(mem.alloc((void**)&d_E, h * 16));
     SP1_TRY(mem.alloc((void**)&d_E2, (h / 2) * 16));
     PhaseTimer t_all(ctx, "open.total");
-    SP1_LAUNCH(ctx, eq_table_kernel, blocks_for(h), 256, 0, d_point, (int)log_h, d_E);
+    SP1_TRY(launch_eq_table(ctx, d_point, (int)log_h, d_E));
 
     // ---- stacked layer: per-column evaluations at the stack point (batch_evaluations) -------------------------
     uint64_t total_cols = 0;
@@ -405,7 +346,7 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         const E4 last = point.back();
         point.pop_back();
         // E for the remaining point: halve (E_{k} -> E_{k-1})
-        SP1_LAUNCH(ctx, halve_eq_kernel, blocks_for(n_cur / 2), 256, 0, cur_E, n_cur / 2, nxt_E);
+        SP1_TRY(launch_halve_eq(ctx, cur_E, n_cur / 2, nxt_E));
         std::swap(cur_E, nxt_E);
         unsigned nblk = (unsigned)((n_cur / 2 + 255) / 256);
         if (nblk > 1024) nblk = 1024;
@@ -420,9 +361,9 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         const uint32_t* mh = sp1b200_mail_host(ctx);
         uint32_t rc[16];
         memcpy(rc, mh, 64);
-        std::vector<uint32_t> parts(mh + 16, mh + 16 + (size_t)nblk * 4);
-        E4 zero_val;
-        for (unsigned k = 0; k < nblk; k++) zero_val = zero_val + E4::load(&parts[4 * k]);
+        E4 zv[1];
+        sum_partials(mh + 16, nblk, zv);
+        const E4 zero_val = zv[0];
         E4 one_val = (claim - zero_val) * hf::inv(last) + zero_val;
         uni.insert(uni.end(), zero_val.c, zero_val.c + 4);
         uni.insert(uni.end(), one_val.c, one_val.c + 4);
@@ -431,9 +372,7 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         fri_commits.insert(fri_commits.end(), rc + 8, rc + 16);
         memcpy(fri_roots[r].data(), rc, 32);
         E4 beta; ch.sample_ext(beta.c);
-        Ext dbeta{{beta.c[0], beta.c[1], beta.c[2], beta.c[3]}};
-        E4 bh = beta * half;
-        Ext dbh{{bh.c[0], bh.c[1], bh.c[2], bh.c[3]}};
+        const Ext dbeta = to_ext(beta), dbh = to_ext(beta * half);
         SP1_LAUNCH(ctx, fold_codeword_kernel, blocks_for(m_cur / 2), 256, 0, cw_ptr[r], (int)(log_h + b - r), dbh, half, ctx->d_TH,
                    ctx->d_TL, cw_ptr[r + 1]);
         SP1_LAUNCH(ctx, fold_mle_kernel, blocks_for(n_cur / 2), 256, 0, cur_mle, n_cur / 2, dbeta, nxt_mle);

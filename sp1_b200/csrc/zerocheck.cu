@@ -20,6 +20,7 @@
 
 #include "machine.cuh"
 #include "zc_lower.hpp"
+#include "sumcheck.cuh"
 
 namespace {
 
@@ -315,23 +316,6 @@ __global__ void __launch_bounds__(256) zc_batch0_kernel(const ZcFixJob* __restri
     kb::ext_store(job.out + 4 * i, kb::ext_add(sa, kb::ext_mul(alpha, sd)));
 }
 
-__global__ void zc_eq_table_kernel(const uint32_t* __restrict__ point, int k, uint32_t* __restrict__ E) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= ((uint64_t)1 << k)) return;
-    Ext acc = kb::ext_one();
-    for (int t = 0; t < k; t++) {
-        Ext x = kb::ext_load(point + 4 * t);
-        bool bit = (j >> (k - 1 - t)) & 1;
-        acc = kb::ext_mul(acc, bit ? x : kb::ext_sub(kb::ext_one(), x));
-    }
-    kb::ext_store(E + 4 * j, acc);
-}
-__global__ void zc_halve_eq_kernel(const uint32_t* __restrict__ E, uint64_t n_out, uint32_t* __restrict__ Eo) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n_out) return;
-    kb::ext_store(Eo + 4 * j, kb::ext_add(kb::ext_load(E + 8 * j), kb::ext_load(E + 8 * j + 4)));
-}
-
 // host interpreter on the all-zero row (padded_row_adjustment, shard.rs:520-537): Σ powers[alpha_idx] * reg
 E4 host_eval_zero_row(const HostProg& p, const uint32_t* pv, const std::vector<E4>& powers, uint32_t n_regs) {
     std::vector<uint32_t> regs(n_regs ? n_regs : 1, 0);
@@ -360,14 +344,6 @@ struct VGeq {
     }
     E4 at(uint64_t idx) const { return idx < threshold ? E4() : (idx == threshold ? eq_c + geq_c : geq_c); }
 };
-
-struct DevFree {
-    sp1b200_ctx* ctx; std::vector<void*> ptrs;
-    explicit DevFree(sp1b200_ctx* c) : ctx(c) {}
-    ~DevFree() { for (void* p : ptrs) cudaFreeAsync(p, ctx->stream); }
-    sp1b200_err alloc(void** p, size_t bytes) { SP1_CUDA(cudaMallocFromPoolAsync(p, bytes ? bytes : 4, ctx->pool, ctx->stream)); ptrs.push_back(*p); return nullptr; }
-};
-inline unsigned blocks_for(uint64_t n, unsigned bs = 256) { return (unsigned)((n + bs - 1) / bs); }
 
 }  // namespace
 
@@ -557,7 +533,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
     SP1_CUDA(cudaMemcpyAsync(d_point, h_gkr_point, mlr * 16, cudaMemcpyHostToDevice, st));
     SP1_TRY(mem.alloc((void**)&d_E[0], ((size_t)16 << (mlr - 1))));
     SP1_TRY(mem.alloc((void**)&d_E[1], ((size_t)16 << (mlr > 1 ? mlr - 2 : 0))));
-    SP1_LAUNCH(ctx, zc_eq_table_kernel, blocks_for((uint64_t)1 << (mlr - 1)), 256, 0, d_point, (int)mlr - 1, d_E[0]);
+    SP1_TRY(launch_eq_table(ctx, d_point, (int)mlr - 1, d_E[0]));
     int ecur = 0;
 
     // ---- the whole launch plan is known up front (heights halve deterministically): job tables of every round, one upload ----
@@ -757,7 +733,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         for (auto& c : rlc) words.insert(words.end(), c.c, c.c + 4);
         E4 a; ch.sample_ext(a.c);
         point.insert(point.begin(), a);
-        const Ext da{{a.c[0], a.c[1], a.c[2], a.c[3]}};
+        const Ext da = to_ext(a);
         if (R.fix_jobs) {
             if (rd == 0) {
                 SP1_LAUNCH(ctx, zc_fix_kernel<uint32_t>, R.fix_blocks, 256, 0, d_fjobs + R.fix0, (int)R.fix_jobs, da);
@@ -778,7 +754,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         }
         if (rd + 1 < mlr) {
             const uint64_t n_out = (uint64_t)1 << (mlr - 2 - rd);
-            SP1_LAUNCH(ctx, zc_halve_eq_kernel, blocks_for(n_out), 256, 0, d_E[ecur], n_out, d_E[ecur ^ 1]);
+            SP1_TRY(launch_halve_eq(ctx, d_E[ecur], n_out, d_E[ecur ^ 1]));
             ecur ^= 1;
         }
     }

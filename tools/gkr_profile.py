@@ -48,29 +48,6 @@ def gkr_bytes_model(heights, inters, mlr):
     return m, S
 
 
-def previous_gkr_bytes_model(heights, inters, mlr):
-    """the same model for the pass structure this code replaced (kept for before / after tables): level 0 = EF numerators and
-    denominators written by the first-level pass and read by the level pass; each layer summed by one pass over its sequence
-    (gkr_sum_seq_kernel), then one fix per row round, the first one reading the sequence (gkr_fix_sum_kernel<true>)"""
-    half = lambda x: (x + 1) // 2  # noqa: E731
-    lens = [list(heights)]
-    for _ in range(1, mlr):
-        lens.append([half(x) for x in lens[-1]])
-    S = [sum(i * x for i, x in zip(inters, ln)) for ln in lens]
-    m = defaultdict(float)
-    m["gkr_first_level_kernel"] = 32 * S[0]
-    for l in range(mlr - 1):
-        m["gkr_level_kernel"] += 32 * (S[l] + S[l + 1])
-        m["gkr_sum_seq_kernel"] += 32 * S[l]
-        rows = [half(half(x)) for x in lens[l]]
-        m["gkr_fix_sum_kernel<true>"] += 32 * S[l] + 64 * sum(i * x for i, x in zip(inters, rows))
-        for _ in range(mlr - 2 - l):
-            nxt = [half(x) for x in rows]
-            m["gkr_fix_sum_kernel<false>"] += 64 * sum(i * (x + y) for i, x, y in zip(inters, rows, nxt))
-            rows = nxt
-    return m
-
-
 JK_MAX, JK_LOW = 5, 10  # csrc/jagged.cu
 
 
@@ -110,18 +87,6 @@ def jagged_bytes_model(area, lm, k):
         m["jagged_fold_to_kernel"] = 4 * area + 32 * (N >> k)
         first = k
     m["hadamard_fold_kernel"] = sum(32 * (N >> r) + 32 * (N >> (r + 1)) for r in range(first, lm))
-    return m
-
-
-def previous_jagged_bytes_model(area, lm, mlr):
-    """the same model for the pass structure this code replaced: round 0 from the trace, then row_eq folded by alpha_0 and one
-    pass writing the level-1 dense and eq arrays (4.3 GB at log_m = 28), then one fix-and-sum pass per round"""
-    N = 1 << lm
-    m = defaultdict(float)
-    m["hadamard_sum0_fused_kernel"] = 4 * area
-    m["row_eq_fold_kernel"] = 16 * (1 << mlr) + 16 * (1 << (mlr - 1))
-    m["hadamard_fold0_fused_kernel"] = 4 * area + 32 * (N >> 1)
-    m["hadamard_fold_kernel"] = sum(32 * (N >> r) + 32 * (N >> (r + 1)) for r in range(1, lm))
     return m
 
 
@@ -221,28 +186,24 @@ def main():
     gkr_ms = sum(by_base.values())
     gkr_gb = sum(model.get(n, 0.0) for n in by_base) / 1e9
     lines.append(f"GKR kernels (gkr_*): {gkr_ms:.3f} ms ({100 * gkr_ms / allms:.1f}% of device time), modelled {gkr_gb:.2f} GB")
-    prev = previous_gkr_bytes_model(heights, inters, mlr)
-    lines.append("previous pass structure (EF level 0, one row round per pass), modelled GB: " +
-                 ", ".join(f"{k} {v / 1e9:.2f}" for k, v in prev.items()) + f"; total {sum(prev.values()) / 1e9:.2f}")
     area, lm, k = jagged_layout([prep_heights, main_heights], lib.params["log_stacking_height"], mlr)
     jmodel = jagged_bytes_model(area, lm, k)
-    jprev = previous_jagged_bytes_model(area, lm, mlr)
-    jmeasured = jprev if "hadamard_sum0_fused_kernel" in tot else jmodel   # a library built before the trace rounds
     jfam = defaultdict(float)   # the jagged sumcheck and the PCS passes over the same trace
     for n, v in tot.items():
         b = re.sub(r"<.*", "", n)
-        if b.startswith(("hadamard_", "jagged_", "row_eq_fold")) or b in ("column_evals_kernel", "batch_columns_kernel", "eq_table_kernel"):
+        if b.startswith(("hadamard_", "jagged_")) or b in ("column_evals_kernel", "batch_columns_kernel"):
             jfam[b] += v
     lines.append(f"{'jagged kernel family':40s} {'ms':>9s} {'model GB':>9s} {'GB/s':>7s}   (area {area / 1e6:.1f} M cells, log_m {lm}, "
                  f"K = {k} rounds from the trace)")
     for n in sorted(jfam, key=lambda x: -jfam[x]):
-        gb = (jmeasured.get(n) or (4 * area if n in ("column_evals_kernel", "batch_columns_kernel") else 0.0)) / 1e9
+        gb = (jmodel.get(n) or (4 * area if n in ("column_evals_kernel", "batch_columns_kernel") else 0.0)) / 1e9
         lines.append(f"{n:40s} {jfam[n]:9.3f}" + (f" {gb:9.3f} {gb / (jfam[n] / 1e3):7.0f}" if gb else ""))
-    hj = [n for n in jfam if n in jmodel or n in jprev]
-    lines.append(f"jagged sumcheck kernels: {sum(jfam[n] for n in hj):.3f} ms, modelled {sum(jmeasured.values()) / 1e9:.2f} GB "
+    hj = [n for n in jfam if n in jmodel]
+    lines.append(f"jagged sumcheck kernels: {sum(jfam[n] for n in hj):.3f} ms, modelled {sum(jmodel.values()) / 1e9:.2f} GB "
                  "(column_evals / batch_columns: trace bytes only)")
-    lines.append("previous jagged pass structure (round 0 from the trace, level 1 materialised), modelled GB: " +
-                 ", ".join(f"{n} {v / 1e9:.2f}" for n, v in jprev.items()) + f"; total {sum(jprev.values()) / 1e9:.2f}")
+    # the eq tables every sumcheck and PCS driver shares (sumcheck.cu)
+    for n in ("eq_table_kernel", "halve_eq_kernel"):
+        lines.append(f"shared {n:33s} {tot.get(n, 0.0):9.3f} ms in {cnt.get(n, 0)} launches")
     lines.append("phases of an unprofiled shard (ms): " + ", ".join(f"{k} {v:.3f}" for k, v in phases.items()))
     lines.append(f"gpu_mem_used_gb {(torch.cuda.mem_get_info(dev)[1] - torch.cuda.mem_get_info(dev)[0]) / 2**30:.1f}")
     text = "\n".join(lines)
