@@ -297,6 +297,16 @@ int64_t orc_jagged_prove_verify(const uint32_t* const* dense, uint32_t n_rounds,
     return (int64_t)o.size();
 }
 
+// tests only: z_col (4 words each, written when it fits in cap entries) and the Hadamard sumcheck claim of this thread's last jagged prove.
+// Returns the length of z_col.
+uint32_t orc_jagged_last_inputs(uint32_t* z_col_out, uint32_t cap, uint32_t* claim4) {
+    const JaggedProveInputs& in = jagged_last_inputs();
+    if (in.z_col.size() <= cap)
+        for (size_t i = 0; i < in.z_col.size(); i++) for (int k = 0; k < 4; k++) z_col_out[4 * i + k] = in.z_col[i].c[k].v;
+    for (int k = 0; k < 4; k++) claim4[k] = in.claim.c[k].v;
+    return (uint32_t)in.z_col.size();
+}
+
 
 }  // extern "C"
 

@@ -293,6 +293,11 @@ struct JaggedProof {
     unsigned max_log_rows = 0, log_m = 0;
 };
 
+// The transcript-derived inputs of the last jagged_prove on this thread: z_col and the Hadamard sumcheck's claim.  Tests read them to
+// rerun the sumcheck rounds on the reference's own kernels.
+struct JaggedProveInputs { std::vector<EF> z_col; EF claim; };
+static inline JaggedProveInputs& jagged_last_inputs() { static thread_local JaggedProveInputs v; return v; }
+
 // JaggedProver::prove_trusted_evaluations (jagged/src/prover.rs:162-328).  claims[r] = per-column evaluations at
 // z_row of every (real or empty) table column of round r, in table order.
 static inline JaggedProof jagged_prove(const std::vector<EF>& z_row, const std::vector<std::vector<EF>>& claims,
@@ -334,6 +339,7 @@ static inline JaggedProof jagged_prove(const std::vector<EF>& z_row, const std::
         return col_eq[c] * row_eq[idx - jp.prefix[c]];
     };
     EF claim = mle_eval(column_claims.data(), column_claims.size(), z_col);
+    jagged_last_inputs() = {z_col, claim};
     JaggedProof pf;
     pf.sumcheck.claimed_sum = claim;
     EF half = EF(F::two().inv()), quarter = EF(F::from_canonical(4).inv());

@@ -8,6 +8,7 @@
 // reference host code uses (cited per function).  Only thin `__global__` wrappers that call the reference's device
 // classes (kb31_t, kb31_extension_t, poseidon2::KoalaBearHasher, DuplexChallenger) are defined here; no algorithm is.
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -22,6 +23,8 @@
 #include "mle/mle.cuh"
 #include "logup_gkr/tracegen.cuh"
 #include "zerocheck/sequential.cuh"
+#include "jagged_sumcheck/jagged_sumcheck.cuh"
+#include "tracegen/jagged_tracegen/jagged.cuh"
 #include "runtime/exception.cuh"
 
 // sys/include/ntt/sppark.cuh (definitions live in lib/ntt/sppark.cu; prototypes restated: sys/src/dft.rs:5-50)
@@ -147,6 +150,21 @@ struct Ext4Raw {
     uint32_t v[4];
 };
 static_assert(sizeof(Ext4Raw) == sizeof(kb31_extension_t) && alignof(Ext4Raw) == alignof(kb31_extension_t), "ext layout");
+
+// device buffers owned by one launcher call: freed when it returns, on the error paths too
+struct DevScope {
+    std::vector<void*> bufs;
+    cudaError_t alloc(void** d, size_t bytes) {
+        cudaError_t e = cudaMalloc(d, bytes ? bytes : 8);
+        if (e == cudaSuccess) bufs.push_back(*d);
+        return e;
+    }
+    void release(void* p) {
+        for (auto& b : bufs)
+            if (b == p) { cudaFree(b); b = nullptr; }
+    }
+    ~DevScope() { for (void* b : bufs) if (b) cudaFree(b); }
+};
 
 struct DevChallenger {
     uint32_t* d_words = nullptr;  // 16 + 8 + 16 (the device duplexing writes WIDTH words into output_buffer)
@@ -515,6 +533,129 @@ const char* ref_zerocheck_node_sums(const uint32_t* h_instrs, uint32_t n_instrs,
     for (void* p : {(void*)st.instrs, (void*)st.leaves, (void*)st.consts, (void*)st.publics, (void*)st.assert_regs, (void*)st.assert_alphas, d_trace, d_pv, d_ap,
                     d_E, d_lambda, d_gkr, d_disp, d_st, d_lay, d_part, d_out})
         cudaFree(p);
+    return nullptr;
+}
+
+// ---- jagged Hadamard sumcheck: the reference's round kernels -------------------------------------------------------------------------
+// DeviceTensor::sum_dim(1) over a [rows x n_blocks] tensor of per-block partials, with the reference's kb31_extension_t addition
+__global__ void ref_sum_rows_kernel(const kb31_extension_t* partials, uint32_t rows, uint32_t n_blocks, kb31_extension_t* out) {
+    if (blockIdx.x || threadIdx.x >= rows) return;
+    kb31_extension_t acc = kb31_extension_t::zero();
+    for (uint32_t b = 0; b < n_blocks; b++) acc += partials[(size_t)threadIdx.x * n_blocks + b];
+    out[threadIdx.x] = acc;
+}
+
+extern "C" void* padded_hadamard_fix_and_sum();
+extern "C" void* mle_fix_last_variable_koala_bear_ext_ext_zero_padding();
+
+// jagged_sumcheck (sp1-gpu/crates/jagged_sumcheck/src/sumcheck.rs:233-355) with the challenges supplied instead of sampled: challenges[r]
+// is the challenge of round r, counted from 0 (alpha_1 = challenges[0], alpha_2 = challenges[1]).  The JaggedMle<JaggedSumcheckData>
+// argument is built as JaggedTraceMle::from_chip_layout builds it (sp1-gpu/crates/utils/src/traces.rs:294-350): startIndices[c] = the first
+// dense PAIR of column c (n_cols + 1 entries), colIndex[j] = the column of dense pair j; col_heights are element counts.
+// Raw outputs, ext (4 words) each:
+//   grid8    jaggedTwoRoundSumAsPoly (sumcheck.rs:103-136), block 256, grid ceil(height / (256 * 32 * 2)), height = dense_len / 2:
+//            h(0,0) h(0,1) 4h(0,1/2) h(1,0) 4h(1,1/2) 4h(1/2,0) 4h(1/2,1) 16h(1/2,1/2)
+//   r2       jaggedTwoRoundFixAndSum(alpha_1, alpha_2) (sumcheck.rs:141-209), grid ceil(height / (256 * 32 * 4)): eval_0, 4 eval_1/2 of round 2
+//   rounds   paddedHadamardFixAndSum for r = 3 .. log_m - 1 with alpha = challenges[r - 1] (sumcheck.rs:313-336 -> hadamard.rs:131-177),
+//            grid ceil(output_height / 256): eval_0, 4 eval_1/2 of round r
+//   pq       mle_fix_last_variable_koala_bear_ext_ext_zero_padding of p, then of q, with challenges[log_m - 1] (sumcheck.rs:338-352 ->
+//            hadamard.rs:82-128): p_eval, q_eval
+//   stacked  p right after the fold of round log_stacking_height (sumcheck.rs:326-328): dense_len >> log_stacking_height entries
+const char* ref_jagged_sumcheck(const uint32_t* h_dense, uint64_t dense_len, const uint64_t* col_heights, uint32_t n_cols, const uint32_t* h_eq_row,
+                                uint64_t eq_row_len, const uint32_t* h_eq_col, uint64_t eq_col_len, const uint32_t* challenges, uint32_t log_m,
+                                uint32_t log_stacking_height, uint32_t* out_grid8, uint32_t* out_r2, uint32_t* out_rounds, uint32_t* out_pq,
+                                uint32_t* out_stacked) {
+    // the kernels' preconditions (sumcheck.rs:107, 150, 247-248; jagged_sumcheck.cu:32-34, 106-107).  The kernels read eqZRow[2 rowIdx + 1] and
+    // eqZCol[colIdx] unchecked, and the stacked snapshot exists only when log_stacking_height < log_m and holds whole stacked columns.
+    if (log_m < 3 || log_stacking_height < 3 || log_stacking_height >= log_m)
+        return "ref_jagged_sumcheck: need 3 <= log_stacking_height < log_m";
+    if (dense_len % 8 || dense_len > (1ull << log_m) || dense_len <= (1ull << (log_m - 1))) return "ref_jagged_sumcheck: dense_len";
+    if (dense_len % (1ull << log_stacking_height)) return "ref_jagged_sumcheck: dense_len must be a multiple of 2^log_stacking_height";
+    if (n_cols > eq_col_len) return "ref_jagged_sumcheck: more columns than eq_z_col entries";
+    std::vector<uint32_t> col_index(dense_len / 2), start(n_cols + 1, 0);
+    size_t cnt = 0;
+    for (uint32_t c = 0; c < n_cols; c++) {
+        const size_t half = col_heights[c] / 2;
+        if (col_heights[c] % 16) return "ref_jagged_sumcheck: column heights must be multiples of 16";
+        if (col_heights[c] > eq_row_len) return "ref_jagged_sumcheck: a column is taller than eq_z_row";
+        if (cnt + half > col_index.size()) return "ref_jagged_sumcheck: the columns overrun the dense data";
+        std::fill(col_index.begin() + cnt, col_index.begin() + cnt + half, c);
+        cnt += half;
+        start[c + 1] = start[c] + (uint32_t)half;
+    }
+    if (cnt != col_index.size()) return "ref_jagged_sumcheck: the columns do not cover the dense data";
+    DevScope mem;   // every device buffer below is freed on every return
+    auto up = [&](const void* h, size_t bytes, void** d) -> cudaError_t {
+        cudaError_t e = mem.alloc(d, bytes);
+        if (e == cudaSuccess && bytes) e = cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice);
+        return e;
+    };
+    auto ext = [&](uint32_t r) { Ext4Raw a; memcpy(&a, challenges + 4 * r, 16); return a; };
+    const size_t E = sizeof(kb31_extension_t), BLOCK = 256, STRIDE = 32, smem = (BLOCK / STRIDE) * E, height = dense_len / 2;
+    void *d_dense, *d_col, *d_start, *d_eq_row, *d_eq_col, *d_part, *d_sum, *d_p, *d_q;
+    RCHK(up(h_dense, dense_len * 4, &d_dense));
+    RCHK(up(col_index.data(), col_index.size() * 4, &d_col));
+    RCHK(up(start.data(), start.size() * 4, &d_start));
+    RCHK(up(h_eq_row, eq_row_len * E, &d_eq_row));
+    RCHK(up(h_eq_col, eq_col_len * E, &d_eq_col));
+    const size_t g1 = (height + BLOCK * STRIDE * 2 - 1) / (BLOCK * STRIDE * 2), g2 = (height + BLOCK * STRIDE * 4 - 1) / (BLOCK * STRIDE * 4);
+    const size_t max_blocks = std::max(8 * g1, (height / 2 + BLOCK - 1) / BLOCK * 2);
+    RCHK(mem.alloc(&d_part, max_blocks * E));
+    RCHK(mem.alloc(&d_sum, 8 * E));
+    RCHK(mem.alloc(&d_p, (height / 2 + 1) * E));
+    RCHK(mem.alloc(&d_q, (height / 2 + 1) * E));
+    JaggedMle<JaggedSumcheckData> mle;
+    mle.colIndex = (uint32_t*)d_col;
+    mle.startIndices = (uint32_t*)d_start;
+    mle.denseData.base = (felt_t*)d_dense;
+    mle.denseData.eqZCol = (ext_t*)d_eq_col;
+    mle.denseData.eqZRow = (ext_t*)d_eq_row;
+    mle.denseData.height = height;
+    auto sum_rows = [&](uint32_t rows, size_t n_blocks, uint32_t* out) -> cudaError_t {
+        ref_sum_rows_kernel<<<1, 32>>>((const kb31_extension_t*)d_part, rows, (uint32_t)n_blocks, (kb31_extension_t*)d_sum);
+        cudaError_t e = cudaGetLastError();
+        return e == cudaSuccess ? cudaMemcpy(out, d_sum, rows * E, cudaMemcpyDeviceToHost) : e;
+    };
+    {
+        void* args[] = {&d_part, &mle};
+        RCHK(cudaLaunchKernel(jagged_two_round_sum_as_poly(), dim3((unsigned)g1), dim3((unsigned)BLOCK), args, smem, 0));
+        RCHK(sum_rows(8, g1, out_grid8));
+    }
+    {
+        Ext4Raw a1 = ext(0), a2 = ext(1);
+        void* args[] = {&d_part, &mle, &d_p, &d_q, &a1, &a2};
+        RCHK(cudaLaunchKernel(jagged_two_round_fix_and_sum(), dim3((unsigned)g2), dim3((unsigned)BLOCK), args, smem, 0));
+        RCHK(sum_rows(2, g2, out_r2));
+    }
+    size_t len = height / 2;
+    for (uint32_t r = 3; r < log_m; r++) {
+        // paddedHadamardFixAndSum stores output pairs (2i, 2i + 1) for i < ceil(out_len / 2): one entry of slack for an odd out_len
+        const size_t out_len = (len + 1) / 2, g = (out_len + BLOCK - 1) / BLOCK, hsmem = (BLOCK / 32) * E;
+        void *d_p2, *d_q2;
+        RCHK(mem.alloc(&d_p2, (out_len + 1) * E));
+        RCHK(mem.alloc(&d_q2, (out_len + 1) * E));
+        Ext4Raw a = ext(r - 1);
+        void* args[] = {&d_p, &d_q, &d_p2, &d_q2, &a, &d_part, &len};
+        RCHK(cudaLaunchKernel(padded_hadamard_fix_and_sum(), dim3((unsigned)g), dim3((unsigned)BLOCK), args, hsmem, 0));
+        RCHK(sum_rows(2, g, out_rounds + 8 * (r - 3)));
+        if (r == log_stacking_height) RCHK(cudaMemcpy(out_stacked, d_p2, out_len * E, cudaMemcpyDeviceToHost));
+        mem.release(d_p);
+        mem.release(d_q);
+        d_p = d_p2;
+        d_q = d_q2;
+        len = out_len;
+    }
+    {
+        Ext4Raw a = ext(log_m - 1);
+        size_t width = 1;
+        const unsigned g = (unsigned)(((len + 1) / 2 + BLOCK - 1) / BLOCK);
+        for (int k = 0; k < 2; k++) {
+            void* in = k ? d_q : d_p;
+            void* args[] = {&in, &d_sum, &a, &len, &width};
+            RCHK(cudaLaunchKernel(mle_fix_last_variable_koala_bear_ext_ext_zero_padding(), dim3(g, 1), dim3((unsigned)BLOCK, 1), args, 0, 0));
+            RCHK(cudaMemcpy(out_pq + 4 * k, d_sum, E, cudaMemcpyDeviceToHost));
+        }
+    }
     return nullptr;
 }
 

@@ -304,3 +304,22 @@ def verify_shard(blob, heights, names, log_stack, max_log_rows, challenger, prep
     return int(f(ptr(blob), H, C.c_char_p(nm), C.c_uint32(log_stack), C.c_uint32(max_log_rows), C.c_uint32(log_blowup), C.c_uint32(num_queries),
                  C.c_uint32(pow_bits), C.c_uint32(batch_pow_bits), C.c_uint32(gkr_pow_bits), ptr(challenger.st), ptr(pc), ptr(words),
                  C.c_uint64(words.size)))
+
+
+def partial_lagrange(point):
+    """eq table of an ext point [n, 4] -> [2^n, 4]; the first coordinate is the most significant bit of the index"""
+    point = np.ascontiguousarray(point, dtype=np.uint32)
+    out = np.zeros((1 << point.shape[0], 4), np.uint32)
+    lib().orc_partial_lagrange(ptr(point), C.c_uint64(point.shape[0]), ptr(out))
+    return out
+
+
+def jagged_last_inputs():
+    """z_col [n, 4] and the Hadamard sumcheck claim [4] of this thread's last oracle jagged proof"""
+    claim = np.zeros(4, np.uint32)
+    f = lib().orc_jagged_last_inputs
+    f.restype = C.c_uint32
+    n = f(None, C.c_uint32(0), ptr(claim))
+    z_col = np.zeros((n, 4), np.uint32)
+    f(ptr(z_col), C.c_uint32(n), ptr(claim))
+    return z_col, claim

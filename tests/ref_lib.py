@@ -33,7 +33,8 @@ def lib():
         L = C.CDLL(SO)
         for n in ("ref_init", "ref_malloc", "ref_free", "ref_h2d", "ref_d2h", "ref_field_op", "ref_ext_op", "ref_permute", "ref_hash",
                   "ref_compress", "ref_merkle_tree", "ref_batch_coset_dft", "ref_batch", "ref_fold_mle_ext", "ref_fix_last_variable_ext",
-                  "ref_partial_lagrange_ext", "ref_grind", "ref_challenger_script", "ref_gkr_populate", "ref_zerocheck_node_sums"):
+                  "ref_partial_lagrange_ext", "ref_grind", "ref_challenger_script", "ref_gkr_populate", "ref_zerocheck_node_sums",
+                  "ref_jagged_sumcheck"):
             getattr(L, n).restype = C.c_char_p
         _chk(L.ref_init())
         _lib = L
@@ -349,3 +350,24 @@ def zerocheck_node_sums(chip, main, prep, pv, alpha_pows, E):
                                        C.c_uint32(main.shape[0]), _p(prepf), C.c_uint32(pw), C.c_uint32(h), _p(pv), C.c_uint32(pv.size), _p(ap.reshape(-1)),
                                        C.c_uint32(ap.shape[0]), _p(E.reshape(-1)), C.c_uint32(k), _p(out)))
     return out.reshape(3, 4)
+
+
+def jagged_sumcheck(dense, col_heights, eq_row, eq_col, challenges, log_stacking_height):
+    """the reference's jagged Hadamard sumcheck kernels (ref_jagged_sumcheck) on the base-field dense words, the element heights of its
+    columns, the eq tables of z_row and z_col and the round challenges in sampling order.  -> the raw sums, flat words: grid8 (8 ext) |
+    round 2 (2 ext) | rounds 3 .. log_m - 1 (2 ext each) | p_eval, q_eval | stacked evals (len(dense) >> log_stacking_height ext)"""
+    dense = np.ascontiguousarray(dense, np.uint32).reshape(-1)
+    eq_row = np.ascontiguousarray(eq_row, np.uint32).reshape(-1, 4)
+    eq_col = np.ascontiguousarray(eq_col, np.uint32).reshape(-1, 4)
+    ch = np.ascontiguousarray(challenges, np.uint32).reshape(-1, 4)
+    log_m = ch.shape[0]
+    h = np.ascontiguousarray(col_heights, np.uint64)
+    grid8, r2 = np.zeros(32, np.uint32), np.zeros(8, np.uint32)
+    rounds = np.zeros(max(1, 8 * (log_m - 3)), np.uint32)
+    pq = np.zeros(8, np.uint32)
+    stacked = np.zeros(4 * (dense.size >> log_stacking_height), np.uint32)
+    _chk(lib().ref_jagged_sumcheck(_p(dense), C.c_uint64(dense.size), h.ctypes.data_as(C.POINTER(C.c_uint64)), C.c_uint32(h.size),
+                                   _p(eq_row.reshape(-1)), C.c_uint64(eq_row.shape[0]), _p(eq_col.reshape(-1)), C.c_uint64(eq_col.shape[0]),
+                                   _p(ch.reshape(-1)), C.c_uint32(log_m), C.c_uint32(log_stacking_height), _p(grid8), _p(r2), _p(rounds), _p(pq),
+                                   _p(stacked)))
+    return np.concatenate([grid8, r2, rounds[:8 * (log_m - 3)], pq, stacked])
