@@ -501,6 +501,25 @@ int64_t orc_gkr_prove_verify(const uint32_t* machine_blob, const uint64_t* heigh
     return (int64_t)o.size();
 }
 
+// tests only: the inputs of this thread's last LogUp-GKR prove that the proof does not carry, as words: alpha | n_beta | beta_seed[n_beta] |
+// n_layers | per layer in proof order {lambda | claim = num_eval * lambda + den_eval | n_point | point[n_point]} (ext = 4 words).  The
+// words are written when they fit in cap; returns their number.
+uint64_t orc_gkr_last_inputs(uint32_t* out, uint64_t cap) {
+    const GkrProveInputs& in = gkr_last_inputs();
+    std::vector<uint32_t> o;
+    put(o, in.alpha);
+    o.push_back((uint32_t)in.beta_seed.size());
+    for (auto& e : in.beta_seed) put(o, e);
+    o.push_back((uint32_t)in.layers.size());
+    for (auto& l : in.layers) {
+        put(o, l.lambda); put(o, l.claim);
+        o.push_back((uint32_t)l.point.size());
+        for (auto& e : l.point) put(o, e);
+    }
+    if (out && o.size() <= cap) std::copy(o.begin(), o.end(), out);
+    return o.size();
+}
+
 
 // ---- whole shard: ShardProver::prove_shard_with_data (crates/hypercube/src/prover/shard.rs:650-792) + the restated
 // ShardVerifier::verify_shard (crates/hypercube/src/verifier/shard.rs:437-750; machine-shape / cluster checks that depend on the

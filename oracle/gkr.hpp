@@ -51,6 +51,12 @@ struct GkrProof {
     F witness;
 };
 
+// tests only: the inputs of this thread's last gkr_prove that are not in the proof (tests/test_ref_gkr.py replays them through the
+// reference's kernels): alpha, the beta seed and, per GKR layer in proof order, lambda, the evaluation point and the claim
+struct GkrLayerInputs { EF lambda, claim; std::vector<EF> point; };
+struct GkrProveInputs { EF alpha; std::vector<EF> beta_seed; std::vector<GkrLayerInputs> layers; };
+static inline GkrProveInputs& gkr_last_inputs() { static thread_local GkrProveInputs v; return v; }
+
 namespace gkr_detail {
 
 static inline Layer first_layer(const std::vector<GkrChip>& chips, const EF& alpha, const std::vector<EF>& betas, unsigned mlr) {
@@ -125,6 +131,7 @@ static inline GkrRoundProof prove_round(Layer L, const std::vector<EF>& eval_poi
     std::vector<EF> point = eval_point;
     EF eq_adj = EF::one(), pad_adj = EF::one();
     EF claim = num_eval * lambda + den_eval;
+    gkr_last_inputs().layers.push_back({lambda, claim, eval_point});
     PartialSumcheckProof& pf = rp.sc;
     pf.claimed_sum = claim;
     EF round_claim = claim;
@@ -254,6 +261,8 @@ static inline GkrProof gkr_prove(const std::vector<GkrChip>& chips, unsigned mlr
     std::vector<EF> beta_seed = ch.sample_point(bdim);
     (void)ch.sample_ext();  // _pv_challenge
     std::vector<EF> betas = partial_lagrange(beta_seed);
+    GkrProveInputs& rec = gkr_last_inputs();
+    rec = {alpha, beta_seed, {}};
     std::vector<Layer> layers;
     { OrcTrace t("gkr.first_layer"); layers.push_back(first_layer(chips, alpha, betas, mlr)); }
     { OrcTrace t("gkr.transitions"); while (layers.back().num_row_vars > 1) layers.push_back(transition(layers.back())); }

@@ -22,6 +22,10 @@
 #include "basefold/basefold.cuh"
 #include "mle/mle.cuh"
 #include "logup_gkr/tracegen.cuh"
+#include "logup_gkr/execution.cuh"
+#include "logup_gkr/first_layer.cuh"
+#include "logup_gkr/lookahead.cuh"
+#include "logup_gkr/round.cuh"
 #include "zerocheck/sequential.cuh"
 #include "jagged_sumcheck/jagged_sumcheck.cuh"
 #include "tracegen/jagged_tracegen/jagged.cuh"
@@ -411,64 +415,122 @@ const char* ref_challenger_script(uint32_t* st34, const uint32_t* ops, const uin
 
 
 // ---- LogUp-GKR first layer: the reference's interaction evaluation ------------------------------------------------------------------
-// populateLastCircuitLayer (sys/lib/logup_gkr/tracegen.cu:77-160) for ONE chip.  The interactions arrive in the flattened CSR form of
-// `Interactions<F>` (sys/include/logup_gkr/tracegen.cuh:20-36; host twin sp1-gpu/crates/logup_gkr/src/interactions.rs).  Output layout as
-// the kernel writes it: with q = ceil(ceil(height/2)/2), interaction j owns the row-pair slots [2 q j, 2 q j + ceil(height/2)); slot i
-// holds (numerator at row 2i, denominator at row 2i) and, 2 * output_height further, the same for row 2i+1; output_height = 2 q n.
-extern "C" void* logup_gkr_populate_last_circuit_layer();
+static cudaError_t dev_upload(DevScope& mem, const void* h, size_t bytes, void** d) {
+    cudaError_t e = mem.alloc(d, bytes);
+    if (e == cudaSuccess && bytes) e = cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice);
+    return e;
+}
+
+// The interactions of ONE chip in the flattened CSR form of `Interactions<F>` (sys/include/logup_gkr/tracegen.cuh:20-36; host twin
+// sp1-gpu/crates/logup_gkr/src/interactions.rs), every index local to the chip: values_ptr / mult_ptr have n_inter + 1 entries, vcw_ptr
+// n_values + 1, the column-weight lists n_vcw and n_mcw entries.
+struct InteractionsCsr {
+    const uint64_t *values_ptr, *mult_ptr, *vcw_ptr, *vcw_col, *mcw_col;
+    const uint8_t *vcw_is_prep, *mcw_is_prep, *is_send;
+    const uint32_t *vcw_weight, *values_constants, *mcw_weight, *mult_constants, *arg_indices;
+    uint32_t n_inter;
+    uint64_t n_values, n_vcw, n_mcw;
+};
+
+static cudaError_t upload_interactions(DevScope& mem, const InteractionsCsr& c, Interactions<felt_t>* I) {
+    std::vector<PairCol<felt_t>> vcw(c.n_vcw), mcw(c.n_mcw);
+    for (uint64_t i = 0; i < c.n_vcw; i++) { vcw[i].column_idx = c.vcw_col[i]; vcw[i].is_preprocessed = c.vcw_is_prep[i]; memcpy(&vcw[i].weight, &c.vcw_weight[i], 4); }
+    for (uint64_t i = 0; i < c.n_mcw; i++) { mcw[i].column_idx = c.mcw_col[i]; mcw[i].is_preprocessed = c.mcw_is_prep[i]; memcpy(&mcw[i].weight, &c.mcw_weight[i], 4); }
+    std::vector<uint8_t> send(c.is_send, c.is_send + c.n_inter);   // bool on the device side
+    cudaError_t e;
+    if ((e = dev_upload(mem, c.values_ptr, (c.n_inter + 1) * 8, (void**)&I->values_ptr)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, c.mult_ptr, (c.n_inter + 1) * 8, (void**)&I->multiplicities_ptr)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, c.vcw_ptr, (c.n_values + 1) * 8, (void**)&I->values_col_weights_ptr)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, vcw.data(), c.n_vcw * sizeof(PairCol<felt_t>), (void**)&I->values_col_weights)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, c.values_constants, c.n_values * 4, (void**)&I->values_constants)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, mcw.data(), c.n_mcw * sizeof(PairCol<felt_t>), (void**)&I->mult_col_weights)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, c.mult_constants, c.n_inter * 4, (void**)&I->mult_constants)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, c.arg_indices, c.n_inter * 4, (void**)&I->arg_indices)) != cudaSuccess) return e;
+    if ((e = dev_upload(mem, send.data(), c.n_inter, (void**)&I->is_send)) != cudaSuccess) return e;
+    I->num_interactions = c.n_inter;
+    return cudaSuccess;
+}
+
+// Chip by chip over CSR arrays that lie back to back: csr_enter reads the current chip's counts, csr_leave steps past its arrays.
+static void csr_enter(InteractionsCsr& c, uint32_t n_inter) {
+    c.n_inter = n_inter;
+    c.n_values = c.values_ptr[n_inter];
+    c.n_vcw = c.vcw_ptr[c.n_values];
+    c.n_mcw = c.mult_ptr[n_inter];
+}
+static void csr_leave(InteractionsCsr& c) {
+    c.values_ptr += c.n_inter + 1; c.mult_ptr += c.n_inter + 1; c.vcw_ptr += c.n_values + 1;
+    c.vcw_col += c.n_vcw; c.vcw_is_prep += c.n_vcw; c.vcw_weight += c.n_vcw; c.values_constants += c.n_values;
+    c.mcw_col += c.n_mcw; c.mcw_is_prep += c.n_mcw; c.mcw_weight += c.n_mcw;
+    c.mult_constants += c.n_inter; c.arg_indices += c.n_inter; c.is_send += c.n_inter;
+}
+
+// What interactionValue (sys/lib/logup_gkr/tracegen.cu:20-66) reads unchecked for one chip of `height` rows: column c of a source is
+// words [c * height, (c + 1) * height) of the chip's main (prep) table, of which main_avail (prep_avail) words exist; message k reads
+// betas[0 .. values + 1).  nullptr when every read is in bounds.
+static const char* check_interaction_reads(const InteractionsCsr& c, uint64_t height, uint64_t main_avail, uint64_t prep_avail, uint32_t n_betas) {
+    if (c.n_inter && n_betas < 1) return "ref_logup_gkr: no beta powers";
+    for (uint32_t j = 0; j < c.n_inter; j++)
+        if (c.values_ptr[j + 1] - c.values_ptr[j] + 1 > n_betas) return "ref_logup_gkr: a message longer than the beta table";
+    if (!height) return nullptr;   // an empty chip is padding: populateLastCircuitLayer reads no trace word
+    auto in_bounds = [&](uint64_t col, bool prep) { return (col + 1) * height <= (prep ? prep_avail : main_avail); };
+    for (uint64_t i = 0; i < c.n_vcw; i++)
+        if (!in_bounds(c.vcw_col[i], c.vcw_is_prep[i])) return "ref_logup_gkr: an interaction value reads past its chip's trace";
+    for (uint64_t i = 0; i < c.n_mcw; i++)
+        if (!in_bounds(c.mcw_col[i], c.mcw_is_prep[i])) return "ref_logup_gkr: a multiplicity reads past its chip's trace";
+    return nullptr;
+}
+
+// One populateLastCircuitLayer launch for one chip, as generate_first_layer issues it (sp1-gpu/crates/logup_gkr/src/tracegen.rs:94-139):
+// block 256, grid (ceil(max(h, 2).div_ceil(2) / (256 * 8)), ceil(n_inter / 4)), is_padding = (h == 0).  out_height is the layer's total
+// pair count: slot i of a chip's interaction holds row 2i at [i] and row 2i+1 at [i + 2 out_height].
+static cudaError_t launch_populate(Interactions<felt_t> I, const uint32_t* d_start, uint32_t* d_col, felt_t* d_num, ext_t* d_den,
+                                   felt_t* d_prep, felt_t* d_main, Ext4Raw alpha, ext_t* d_betas, size_t interaction_offset, size_t height,
+                                   size_t out_height) {
+    bool is_padding = height == 0;
+    const size_t half = (std::max<size_t>(height, 2) + 1) / 2;
+    void* args[] = {&I, &d_start, &d_col, &d_num, &d_den, &d_prep, &d_main, &alpha, &d_betas, &interaction_offset, &height, &out_height, &is_padding};
+    return cudaLaunchKernel(logup_gkr_populate_last_circuit_layer(), dim3((unsigned)((half + 2047) / 2048), (I.num_interactions + 3) / 4), dim3(256),
+                            args, 0, 0);
+}
+
+// populateLastCircuitLayer for ONE chip of height > 0 on its own.  Output layout as the kernel writes it: with q = ceil(ceil(height/2)/2), interaction j
+// owns the row-pair slots [2 q j, 2 q j + ceil(height/2)); slot i holds (numerator at row 2i, denominator at row 2i) and, 2 * output_height
+// further, the same for row 2i+1; output_height = 2 q n.
 const char* ref_gkr_populate(const uint32_t* h_prep, uint64_t prep_words, const uint32_t* h_main, uint64_t main_words, uint64_t height, uint32_t n_inter,
                              const uint64_t* values_ptr, const uint64_t* mult_ptr, const uint64_t* vcw_ptr, uint64_t n_values, const uint64_t* vcw_col,
                              const uint8_t* vcw_is_prep, const uint32_t* vcw_weight, uint64_t n_vcw, const uint32_t* values_constants,
                              const uint64_t* mcw_col, const uint8_t* mcw_is_prep, const uint32_t* mcw_weight, uint64_t n_mcw,
                              const uint32_t* mult_constants, const uint32_t* arg_indices, const uint8_t* is_send, const uint32_t* alpha4,
                              const uint32_t* betas, uint32_t n_betas, uint32_t* out_num, uint32_t* out_den, uint64_t* out_height) {
-    const uint64_t half = height ? (height + 1) / 2 : 1, q = (half + 1) / 2, outH = 2 * q * n_inter;
-    auto up = [](const void* h, size_t bytes, void** d) -> cudaError_t {
-        cudaError_t e = cudaMalloc(d, bytes ? bytes : 8);
-        if (e == cudaSuccess && bytes) e = cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice);
-        return e;
-    };
-    std::vector<PairCol<felt_t>> vcw(n_vcw), mcw(n_mcw);
-    for (uint64_t i = 0; i < n_vcw; i++) { vcw[i].column_idx = vcw_col[i]; vcw[i].is_preprocessed = vcw_is_prep[i]; memcpy(&vcw[i].weight, &vcw_weight[i], 4); }
-    for (uint64_t i = 0; i < n_mcw; i++) { mcw[i].column_idx = mcw_col[i]; mcw[i].is_preprocessed = mcw_is_prep[i]; memcpy(&mcw[i].weight, &mcw_weight[i], 4); }
-    std::vector<uint8_t> send(is_send, is_send + n_inter);   // bool on the device side
+    // an empty chip (is_padding) writes four slots per interaction, more than the 2 q = 2 this layout gives it: ref_logup_gkr covers that case
+    if (height == 0) return "ref_gkr_populate: height 0 is not supported (the padding path writes past an interaction's slots)";
+    const uint64_t half = (height + 1) / 2, q = (half + 1) / 2, outH = 2 * q * n_inter;
+    DevScope mem;   // every device buffer below is freed on every return
+    InteractionsCsr csr{values_ptr, mult_ptr, vcw_ptr, vcw_col, mcw_col, vcw_is_prep, mcw_is_prep, is_send, vcw_weight, values_constants,
+                        mcw_weight, mult_constants, arg_indices, n_inter, n_values, n_vcw, n_mcw};
+    Interactions<felt_t> I{};
+    RCHK(upload_interactions(mem, csr, &I));
     std::vector<uint32_t> start(n_inter + 1);
     for (uint32_t j = 0; j <= n_inter; j++) start[j] = (uint32_t)(q * j);
-    Interactions<felt_t> I{};
     void *d_prep, *d_main, *d_start, *d_col, *d_num, *d_den, *d_betas;
-    RCHK(up(values_ptr, (n_inter + 1) * 8, (void**)&I.values_ptr));
-    RCHK(up(mult_ptr, (n_inter + 1) * 8, (void**)&I.multiplicities_ptr));
-    RCHK(up(vcw_ptr, (n_values + 1) * 8, (void**)&I.values_col_weights_ptr));
-    RCHK(up(vcw.data(), n_vcw * sizeof(PairCol<felt_t>), (void**)&I.values_col_weights));
-    RCHK(up(values_constants, n_values * 4, (void**)&I.values_constants));
-    RCHK(up(mcw.data(), n_mcw * sizeof(PairCol<felt_t>), (void**)&I.mult_col_weights));
-    RCHK(up(mult_constants, n_inter * 4, (void**)&I.mult_constants));
-    RCHK(up(arg_indices, n_inter * 4, (void**)&I.arg_indices));
-    RCHK(up(send.data(), n_inter, (void**)&I.is_send));
-    I.num_interactions = n_inter;
-    RCHK(up(h_prep, prep_words * 4, &d_prep));
-    RCHK(up(h_main, main_words * 4, &d_main));
-    RCHK(up(start.data(), start.size() * 4, &d_start));
-    RCHK(up(betas, (size_t)n_betas * 16, &d_betas));
-    RCHK(cudaMalloc(&d_col, (2 * outH + 8) * 4));
-    RCHK(cudaMalloc(&d_num, 4 * outH * 4 + 16));
-    RCHK(cudaMalloc(&d_den, 4 * outH * 16 + 16));
+    RCHK(dev_upload(mem, h_prep, prep_words * 4, &d_prep));
+    RCHK(dev_upload(mem, h_main, main_words * 4, &d_main));
+    RCHK(dev_upload(mem, start.data(), start.size() * 4, &d_start));
+    RCHK(dev_upload(mem, betas, (size_t)n_betas * 16, &d_betas));
+    RCHK(mem.alloc(&d_col, (2 * outH + 8) * 4));
+    RCHK(mem.alloc(&d_num, 4 * outH * 4 + 16));
+    RCHK(mem.alloc(&d_den, 4 * outH * 16 + 16));
     RCHK(cudaMemset(d_num, 0, 4 * outH * 4 + 16));
     RCHK(cudaMemset(d_den, 0, 4 * outH * 16 + 16));
     Ext4Raw alpha;
     memcpy(&alpha, alpha4, 16);
-    size_t offset = 0, th = height, oh = outH;
-    bool is_padding = false;
-    void* args[] = {&I, &d_start, &d_col, &d_num, &d_den, &d_prep, &d_main, &alpha, &d_betas, &offset, &th, &oh, &is_padding};
-    dim3 block(64, 4), grid((unsigned)((half + 63) / 64), (n_inter + 3) / 4);
-    RCHK(cudaLaunchKernel(logup_gkr_populate_last_circuit_layer(), grid, block, args, 0, 0));
+    RCHK(launch_populate(I, (const uint32_t*)d_start, (uint32_t*)d_col, (felt_t*)d_num, (ext_t*)d_den, (felt_t*)d_prep, (felt_t*)d_main, alpha,
+                         (ext_t*)d_betas, 0, height, outH));
     RCHK(cudaDeviceSynchronize());
     RCHK(cudaMemcpy(out_num, d_num, 4 * outH * 4, cudaMemcpyDeviceToHost));
     RCHK(cudaMemcpy(out_den, d_den, 4 * outH * 16, cudaMemcpyDeviceToHost));
     *out_height = outH;
-    for (void* p : {(void*)I.values_ptr, (void*)I.multiplicities_ptr, (void*)I.values_col_weights_ptr, (void*)I.values_col_weights, (void*)I.values_constants,
-                    (void*)I.mult_col_weights, (void*)I.mult_constants, (void*)I.arg_indices, (void*)I.is_send, d_prep, d_main, d_start, d_col, d_num, d_den, d_betas})
-        cudaFree(p);
     return nullptr;
 }
 
@@ -658,6 +720,344 @@ const char* ref_jagged_sumcheck(const uint32_t* h_dense, uint64_t dense_len, con
     }
     return nullptr;
 }
+
+// ---- LogUp-GKR: the reference's circuit and round kernels -----------------------------------------------------------------------------
+extern "C" void* logup_gkr_first_sum_as_poly_circuit_layer();
+extern "C" void* logup_gkr_fix_and_sum_circuit_layer();
+extern "C" void* logup_gkr_fix_and_sum_last_circuit_layer();
+extern "C" void* logup_gkr_fix_and_sum_interactions_layer();
+extern "C" void* logup_gkr_fix_and_sum_first_layer();
+extern "C" void* jagged_fold_metadata_kernel();
+extern "C" uint32_t jagged_fold_metadata_block_dim();
+extern "C" uint32_t jagged_fold_metadata_section_size();
+extern "C" void* mle_fix_last_variable_koala_bear_ext_ext_constant_padding();
+
+#define CECHK(expr)                          \
+    do {                                     \
+        cudaError_t e_ = (expr);             \
+        if (e_ != cudaSuccess) return e_;    \
+    } while (0)
+
+// one circuit layer on the device: the JaggedMle kernel argument and its column heights (row-pair counts), from which the reference's
+// fold-metadata kernel derives the next layer's
+struct GkrCircuitDev {
+    JaggedMle<JaggedGkrLayer> mle;
+    uint32_t* heights;
+};
+
+// prove_logup_gkr's device work (sp1-gpu/crates/logup_gkr/src/lib.rs:177-253) with the challenges supplied instead of sampled, for chips
+// taken in the order given (the proof's chip order, which is the reference's chip-name order).
+//   chips      chip c: height chip_heights[c], chip_n_inter[c] interactions whose InteractionsCsr arrays lie back to back after chip c - 1's;
+//              its main (prep) columns start at h_main + main_off[c] (h_prep + prep_off[c]), column-major
+//   lambdas    per GKR layer in proof order (the top layer, one row variable, first; the leaf last): lambda
+//   points     per layer p: its evaluation point, v + p + 1 coordinates (interaction variables first), v = log2 of the padded interaction count
+//   challenges per layer p: its v + p + 1 sumcheck challenges in round order
+// Raw outputs, ext (4 words) each, in this order:
+//   the output numerators, then the output denominators: 2^(v+1) each (extractOutput, tracegen.rs:191-248 -> execution.rs:139-169)
+//   per layer p in proof order, n = v + p + 1 rounds:
+//     lookahead layer (p + 1 > 2 row variables, sumcheck.rs:941 / 1043): the 10-value grid of two_round_sum_* (sumcheck.rs:109-142),
+//       then (eval_0, eval_1/2 unscaled, eq_sum) of rounds 2 .. n - 1
+//     otherwise: (eval_0, eval_1/2 unscaled, eq_sum) of rounds 0 .. n - 1
+//     then n_0, n_1, d_0, d_1 of fixLastVariableInteractionsLayer (sumcheck.rs:467-517, 48-56)
+const char* ref_logup_gkr(uint32_t n_chips, const uint64_t* chip_heights, const uint32_t* chip_n_inter, const uint32_t* h_main, const uint64_t* main_off,
+                          uint64_t main_words, const uint32_t* h_prep, const uint64_t* prep_off, uint64_t prep_words, const uint64_t* values_ptr,
+                          const uint64_t* mult_ptr, const uint64_t* vcw_ptr, const uint64_t* vcw_col, const uint8_t* vcw_is_prep, const uint32_t* vcw_weight,
+                          const uint32_t* values_constants, const uint64_t* mcw_col, const uint8_t* mcw_is_prep, const uint32_t* mcw_weight,
+                          const uint32_t* mult_constants, const uint32_t* arg_indices, const uint8_t* is_send, const uint32_t* alpha4,
+                          const uint32_t* betas, uint32_t n_betas, uint32_t mlr, const uint32_t* lambdas, const uint32_t* points,
+                          const uint32_t* challenges, uint64_t point_words, uint32_t* out, uint64_t out_cap) {
+    // ---- host-side rejection of every input that would make an unchecked reference kernel fault or read unwritten memory
+    if (mlr < 3) return "ref_logup_gkr: max_log_row_count < 3 (tracegen.rs:229 underflows)";
+    uint64_t n_int = 0;
+    for (uint32_t c = 0; c < n_chips; c++) n_int += chip_n_inter[c];
+    if (n_int < 2) return "ref_logup_gkr: fewer than two interactions (v = 0: sumcheck.rs:534 launches the 4-parameter fixLastVariableLastCircuitLayer with 2 arguments)";
+    uint32_t v = 0;
+    while ((1ull << v) < n_int) v++;
+    const bool leaf_lookahead = mlr - 1 > 2;
+    std::vector<uint32_t> counts;   // interaction_row_counts (tracegen.rs:43-59): max(h, 8).div_ceil(4) row pairs per interaction
+    for (uint32_t c = 0; c < n_chips; c++) {
+        const uint64_t h = chip_heights[c];
+        if (h & 1) return "ref_logup_gkr: odd chip height (tracegen.rs:98 asserts)";
+        if (h > (1ull << mlr)) return "ref_logup_gkr: a chip taller than 2^max_log_row_count";
+        if (h && (h < 8 || h % 4)) return "ref_logup_gkr: a non-empty chip shorter than 8 rows or not a multiple of 4 (populateLastCircuitLayer leaves row pairs unwritten)";
+        const uint32_t cnt = (uint32_t)((std::max<uint64_t>(h, 8) + 3) / 4);
+        if (leaf_lookahead && (cnt & 1)) return "ref_logup_gkr: odd leaf pair height on a lookahead leaf (fixLastTwoVariablesTwoPadding traps, jagged.cuh:113-117)";
+        counts.insert(counts.end(), chip_n_inter[c], cnt);
+    }
+    const uint64_t n_out = 2ull << v;
+    uint64_t need = 8 * n_out;
+    for (uint32_t p = 0; p + 1 < mlr; p++) {
+        const uint64_t n = v + p + 1;
+        need += 4 * ((p + 1 > 2 ? 10 + 3 * (n - 2) : 3 * n) + 4);
+    }
+    if (out_cap < need) return "ref_logup_gkr: output buffer too small";
+    uint64_t layer_words = 0;
+    for (uint32_t p = 0; p + 1 < mlr; p++) layer_words += 4ull * (v + p + 1);
+    if (point_words != layer_words) return "ref_logup_gkr: the points / challenges do not have v + p + 1 coordinates per layer p";
+    {
+        InteractionsCsr c{values_ptr, mult_ptr, vcw_ptr, vcw_col, mcw_col, vcw_is_prep, mcw_is_prep, is_send, vcw_weight, values_constants,
+                          mcw_weight, mult_constants, arg_indices, 0, 0, 0, 0};
+        for (uint32_t k = 0; k < n_chips; k++) {
+            if (main_off[k] > main_words || prep_off[k] > prep_words) return "ref_logup_gkr: a chip's trace starts past the trace words";
+            csr_enter(c, chip_n_inter[k]);
+            if (const char* e = check_interaction_reads(c, chip_heights[k], main_words - main_off[k], prep_words - prep_off[k], n_betas)) return e;
+            csr_leave(c);
+        }
+    }
+
+    DevScope mem;   // every device buffer below is freed on every return
+    const size_t E = sizeof(kb31_extension_t), BLOCK = 256, smem = (BLOCK / 32) * E;
+    const uint32_t n_cols = (uint32_t)n_int;
+    auto ext = [](const uint32_t* w) { Ext4Raw a; memcpy(&a, w, 16); return a; };
+    void* d_sum;
+    RCHK(mem.alloc(&d_sum, 10 * E));
+    // DeviceTensor::sum_dim(1) of a [rows, n_blocks] tensor of per-block partials, appended to the raw outputs
+    uint32_t* o = out;
+    auto sum_rows = [&](void* part, uint32_t rows, size_t n_blocks) -> cudaError_t {
+        ref_sum_rows_kernel<<<1, 32>>>((const kb31_extension_t*)part, rows, (uint32_t)n_blocks, (kb31_extension_t*)d_sum);
+        CECHK(cudaGetLastError());
+        CECHK(cudaMemcpy(o, d_sum, rows * E, cudaMemcpyDeviceToHost));
+        o += 4 * rows;
+        return cudaSuccess;
+    };
+    // launch a summing kernel whose first argument is its [rows, grid] partials, then sum them
+    auto run_sum = [&](void* kernel, size_t grid, uint32_t rows, void** part, void** args) -> cudaError_t {
+        CECHK(mem.alloc(part, rows * grid * E));
+        CECHK(cudaLaunchKernel(kernel, dim3((unsigned)grid), dim3((unsigned)BLOCK), args, smem, 0));
+        return sum_rows(*part, rows, grid);
+    };
+    // fold_jagged_metadata_dev (sp1-gpu/crates/utils/src/jagged.rs:207-279): heights' = h.div_ceil(4) * 2 and their prefix sums
+    auto fold = [&](const uint32_t* d_h, uint32_t** new_h, uint32_t** new_start, uint32_t* total) -> cudaError_t {
+        const uint32_t sec = jagged_fold_metadata_section_size(), bd = jagged_fold_metadata_block_dim();
+        const uint32_t nb = std::max<uint32_t>((n_cols + sec - 1) / sec, 1);
+        void *bc, *fl, *sv;
+        CECHK(mem.alloc((void**)new_h, n_cols * 4));
+        CECHK(mem.alloc((void**)new_start, (n_cols + 1) * 4));
+        CECHK(mem.alloc(&bc, 4));
+        CECHK(mem.alloc(&fl, (nb + 1) * 4));
+        CECHK(mem.alloc(&sv, (nb + 1) * 4));
+        CECHK(cudaMemset(bc, 0, 4));
+        CECHK(cudaMemset(fl, 0, (nb + 1) * 4));
+        CECHK(cudaMemset(fl, 1, 4));   // flags[0] != 0: the first block does not wait
+        CECHK(cudaMemset(sv, 0, (nb + 1) * 4));
+        uint32_t n = n_cols;
+        void* args[] = {&d_h, &n, new_h, new_start, &bc, &fl, &sv};
+        CECHK(cudaLaunchKernel(jagged_fold_metadata_kernel(), dim3(nb), dim3(bd), args, 0, 0));
+        return cudaMemcpy(total, *new_start + n_cols, 4, cudaMemcpyDeviceToHost);
+    };
+    // the next circuit layer's buffers, its metadata advanced `folds` folds from the column heights d_h; Tensor [4, 1, 2 * height] and a
+    // colIndex of `height` entries, zeroed (the reference leaves them uninitialised; every entry read is written by the kernels)
+    auto new_circuit = [&](const uint32_t* d_h, int folds, GkrCircuitDev* next) -> cudaError_t {
+        uint32_t *h1, *s1, total;
+        CECHK(fold(d_h, &h1, &s1, &total));
+        if (folds == 2) CECHK(fold(h1, &h1, &s1, &total));
+        void *layer, *col;
+        CECHK(mem.alloc(&layer, 8 * (size_t)total * E));
+        CECHK(mem.alloc(&col, (size_t)total * 4));
+        CECHK(cudaMemset(layer, 0, 8 * (size_t)total * E));
+        CECHK(cudaMemset(col, 0, (size_t)total * 4));
+        next->mle.colIndex = (uint32_t*)col;
+        next->mle.startIndices = s1;
+        next->mle.denseData.layer = (ext_t*)layer;
+        next->mle.denseData.height = total;
+        next->heights = h1;
+        return cudaSuccess;
+    };
+    // DevicePoint::partial_lagrange (sp1-gpu/crates/cuda/src/mle/eval.rs:66-90): block 256, grid ceil(2^dim / 256)
+    auto eq_table = [&](const uint32_t* h_point, uint32_t dim, void** d_out) -> cudaError_t {
+        void* d_pt;
+        CECHK(dev_upload(mem, h_point, (size_t)dim * E, &d_pt));
+        CECHK(mem.alloc(d_out, (E << dim)));
+        size_t nv = dim;
+        void* args[] = {d_out, &d_pt, &nv};
+        return cudaLaunchKernel(partial_lagrange_koala_bear_extension(), dim3((unsigned)(((1ull << dim) + 255) / 256)), dim3(256), args, 0, 0);
+    };
+    // DeviceMle::fix_last_variable_constant_padding(alpha, zero) (sp1-gpu/crates/cuda/src/mle/restrict.rs:77-110): block 256,
+    // grid (ceil(out / (256 * 128)), 1)
+    auto eq_fix = [&](void** d_eq, size_t* len, Ext4Raw a) -> cudaError_t {
+        const size_t out_len = (*len + 1) / 2;
+        void* d_out;
+        CECHK(mem.alloc(&d_out, out_len * E));
+        Ext4Raw zero{};
+        size_t in_len = *len, width = 1;
+        void* args[] = {d_eq, &d_out, &zero, &a, &in_len, &width};
+        CECHK(cudaLaunchKernel(mle_fix_last_variable_koala_bear_ext_ext_constant_padding(), dim3((unsigned)((out_len + BLOCK * 128 - 1) / (BLOCK * 128)), 1),
+                               dim3((unsigned)BLOCK), args, 0, 0));
+        *d_eq = d_out;
+        *len = out_len;
+        return cudaSuccess;
+    };
+
+    // ---- first layer (generate_first_layer, tracegen.rs:36-166)
+    std::vector<uint32_t> start(n_cols + 1, 0);
+    for (uint32_t j = 0; j < n_cols; j++) start[j + 1] = start[j] + counts[j];
+    const size_t H0 = start[n_cols];
+    void *d_main, *d_prep, *d_betas, *d_start, *d_counts, *d_col, *d_num, *d_den;
+    RCHK(dev_upload(mem, h_main, main_words * 4, &d_main));
+    RCHK(dev_upload(mem, h_prep, prep_words * 4, &d_prep));
+    RCHK(dev_upload(mem, betas, (size_t)n_betas * E, &d_betas));
+    RCHK(dev_upload(mem, start.data(), start.size() * 4, &d_start));
+    RCHK(dev_upload(mem, counts.data(), counts.size() * 4, &d_counts));
+    RCHK(mem.alloc(&d_col, H0 * 4));
+    RCHK(mem.alloc(&d_num, 4 * H0 * 4));
+    RCHK(mem.alloc(&d_den, 4 * H0 * E));
+    RCHK(cudaMemset(d_col, 0, H0 * 4));
+    RCHK(cudaMemset(d_num, 0, 4 * H0 * 4));
+    RCHK(cudaMemset(d_den, 0, 4 * H0 * E));
+    {
+        const Ext4Raw alpha = ext(alpha4);
+        InteractionsCsr c{values_ptr, mult_ptr, vcw_ptr, vcw_col, mcw_col, vcw_is_prep, mcw_is_prep, is_send, vcw_weight, values_constants,
+                          mcw_weight, mult_constants, arg_indices, 0, 0, 0, 0};
+        size_t offset = 0;
+        for (uint32_t k = 0; k < n_chips; k++) {
+            csr_enter(c, chip_n_inter[k]);
+            if (c.n_inter) {   // a chip without interactions owns no column (a launch with grid.y = 0 would be an error)
+                Interactions<felt_t> I{};
+                RCHK(upload_interactions(mem, c, &I));
+                RCHK(launch_populate(I, (const uint32_t*)d_start, (uint32_t*)d_col, (felt_t*)d_num, (ext_t*)d_den, (felt_t*)d_prep + prep_off[k],
+                                     (felt_t*)d_main + main_off[k], alpha, (ext_t*)d_betas, offset, chip_heights[k], H0));
+            }
+            offset += c.n_inter;
+            csr_leave(c);
+        }
+    }
+    JaggedMle<JaggedFirstGkrLayer> leaf;
+    leaf.colIndex = (uint32_t*)d_col;
+    leaf.startIndices = (uint32_t*)d_start;
+    leaf.denseData.numeratorValues = (felt_t*)d_num;
+    leaf.denseData.denominatorValues = (ext_t*)d_den;
+    leaf.denseData.height = H0;
+
+    // ---- forward circuit (generate_gkr_circuit, tracegen.rs:211-244; execution.rs:26-115): block 256, grid ceil(height / (256 * 32))
+    std::vector<GkrCircuitDev> circ(mlr - 1);   // circ[k]: mlr - 1 - k row variables, k >= 1
+    RCHK(new_circuit((const uint32_t*)d_counts, 1, &circ[1]));
+    {
+        void* args[] = {&leaf, &circ[1].mle};
+        RCHK(cudaLaunchKernel(logup_gkr_first_layer_transition(), dim3((unsigned)((H0 + 8191) / 8192)), dim3(256), args, 0, 0));
+    }
+    for (uint32_t k = 2; k + 1 < mlr; k++) {
+        RCHK(new_circuit(circ[k - 1].heights, 1, &circ[k]));
+        void* args[] = {&circ[k - 1].mle, &circ[k].mle};
+        RCHK(cudaLaunchKernel(logup_gkr_circuit_transition(), dim3((unsigned)((circ[k - 1].mle.denseData.height + 8191) / 8192)), dim3(256), args, 0, 0));
+    }
+    {   // extract_outputs (execution.rs:139-169): block 256, grid ceil(2^v / (256 * 4))
+        void *d_on, *d_od;
+        RCHK(mem.alloc(&d_on, n_out * E));
+        RCHK(mem.alloc(&d_od, n_out * E));
+        size_t grid_height = n_out / 2;
+        void* args[] = {&circ[mlr - 2].mle, &d_on, &d_od, &grid_height};
+        RCHK(cudaLaunchKernel(logup_gkr_extract_output(), dim3((unsigned)((grid_height + 1023) / 1024)), dim3(256), args, 0, 0));
+        RCHK(cudaMemcpy(o, d_on, n_out * E, cudaMemcpyDeviceToHost));
+        RCHK(cudaMemcpy(o + 4 * n_out, d_od, n_out * E, cudaMemcpyDeviceToHost));
+        o += 8 * n_out;
+    }
+
+    // ---- per GKR layer, top down (prove_gkr_circuit, lib.rs:133-174 -> prove_round)
+    for (uint32_t p = 0; p + 1 < mlr; p++) {
+        const uint32_t k = mlr - 2 - p, R = p + 1, n = v + R;
+        Ext4Raw lambda = ext(lambdas + 4 * p);
+        auto ch = [&](uint32_t r) { return ext(challenges + 4 * r); };
+        void *eq_int, *eq_row, *part;
+        size_t eq_int_len = (size_t)1 << v, eq_row_len = (size_t)1 << R;
+        RCHK(eq_table(points, v, &eq_int));              // prove_first_round / prove_materialized_round (lib.rs:53-61, 89-97)
+        RCHK(eq_table(points + 4 * v, R, &eq_row));
+        GkrCircuitDev cur{}, next{};
+        uint32_t cur_r = R, r0;
+        void* guts = nullptr;   // the interactions layer, Tensor [4, ih]
+        size_t ih = 0;
+        if (R > 2) {   // two-round lookahead: sumcheck.rs:943-973 (leaf), 1050-1082 (circuit layer)
+            size_t H = k ? circ[k].mle.denseData.height : H0;
+            void* lm = k ? (void*)&circ[k].mle : (void*)&leaf;
+            {
+                void* args[] = {&part, lm, &eq_row, &eq_int, &lambda};
+                RCHK(run_sum(k ? logup_gkr_two_round_sum_circuit_layer() : logup_gkr_two_round_sum_first_layer(), (H + BLOCK * 64 - 1) / (BLOCK * 64), 10,
+                             &part, args));
+            }
+            RCHK(eq_fix(&eq_row, &eq_row_len, ch(0)));   // sumcheck.rs:312-313, 362-363
+            RCHK(eq_fix(&eq_row, &eq_row_len, ch(1)));
+            RCHK(new_circuit(k ? circ[k].heights : (const uint32_t*)d_counts, 2, &next));   // sumcheck.rs:221-282
+            Ext4Raw a1 = ch(0), a2 = ch(1);
+            void* args[] = {&part, lm, &next.mle, &a1, &a2, &eq_row, &eq_int, &lambda};
+            RCHK(run_sum(k ? logup_gkr_two_round_fix_and_sum_circuit_layer() : logup_gkr_two_round_fix_and_sum_first_layer(), (H + BLOCK * 32 - 1) / (BLOCK * 32),
+                         3, &part, args));
+            cur = next;
+            cur_r = R - 2;
+            r0 = 3;
+        } else if (k == 0) {   // leaf, one round at a time: sum_as_poly_first_layer (sumcheck.rs:396-465), fix_and_sum_first_layer (:563-650)
+            {
+                const size_t h = H0 >> 1;
+                void* args[] = {&part, &leaf, &eq_row, &eq_int, &lambda};
+                RCHK(run_sum(logup_gkr_sum_as_poly_first_layer(), ((h + BLOCK - 1) / BLOCK + 31) / 32, 3, &part, args));
+            }
+            Ext4Raw a = ch(0);
+            RCHK(new_circuit((const uint32_t*)d_counts, 1, &next));
+            RCHK(eq_fix(&eq_row, &eq_row_len, a));
+            const size_t h = H0 >> 1;
+            void* args[] = {&part, &leaf, &next.mle, &eq_row, &eq_int, &lambda, &a};
+            RCHK(run_sum(logup_gkr_fix_and_sum_first_layer(), (h + BLOCK * 32 - 1) / (BLOCK * 32), 3, &part, args));
+            cur = next;
+            cur_r = R - 1;
+            r0 = 2;
+        } else {   // circuit layer, first round: sum_as_poly_materialized_round (sumcheck.rs:652-691)
+            cur = circ[k];
+            const size_t H = cur.mle.denseData.height;
+            void* args[] = {&part, &cur.mle, &eq_row, &eq_int, &lambda};
+            RCHK(run_sum(eq_row_len == 2 ? logup_gkr_first_sum_as_poly_circuit_layer() : logup_gkr_sum_as_poly_circuit_layer(),
+                         ((H + BLOCK - 1) / BLOCK + 31) / 32, 3, &part, args));
+            r0 = 1;
+        }
+        // remaining rounds: fix_and_sum_materialized_round (sumcheck.rs:694-896) with the previous round's challenge
+        for (uint32_t r = r0; r < n; r++) {
+            Ext4Raw a = ch(r - 1);
+            if (guts) {   // interactions layer (:705-761): eq_interaction is folded first
+                RCHK(eq_fix(&eq_int, &eq_int_len, a));
+                size_t out_h = (ih + 1) / 2, in_h = ih;
+                void* d_out;
+                RCHK(mem.alloc(&d_out, 4 * out_h * E));
+                void* args[] = {&part, &guts, &d_out, &a, &in_h, &out_h, &eq_int, &lambda};
+                RCHK(run_sum(logup_gkr_fix_and_sum_interactions_layer(), ((ih + BLOCK - 1) / BLOCK + 31) / 32, 3, &part, args));
+                guts = d_out;
+                ih = out_h;
+            } else if (cur_r == 1) {   // last row variable (:767-814): the layer becomes the interactions layer
+                const size_t h = cur.mle.denseData.height >> 1;
+                void* d_out;
+                RCHK(mem.alloc(&d_out, 4 * h * E));
+                RCHK(eq_fix(&eq_row, &eq_row_len, a));
+                JaggedGkrLayer dense = cur.mle.denseData;
+                void* args[] = {&part, &dense, &a, &d_out, &eq_int, &lambda};
+                RCHK(run_sum(logup_gkr_fix_and_sum_last_circuit_layer(), ((h + BLOCK - 1) / BLOCK + 31) / 32, 3, &part, args));
+                guts = d_out;
+                ih = h;
+            } else {   // circuit layer (:815-893)
+                RCHK(eq_fix(&eq_row, &eq_row_len, a));
+                RCHK(new_circuit(cur.heights, 1, &next));
+                const size_t H = cur.mle.denseData.height;
+                void* args[] = {&part, &cur.mle, &next.mle, &a, &eq_row, &eq_int, &lambda};
+                RCHK(run_sum(logup_gkr_fix_and_sum_circuit_layer(), ((H + BLOCK - 1) / BLOCK + 31) / 32, 3, &part, args));
+                cur = next;
+                cur_r--;
+            }
+        }
+        if (!guts) return "ref_logup_gkr: the rounds did not reach the interaction variables";
+        {   // fix_last_variable_materialized_round on the interactions layer (:476-517): block 256, grid ceil(height / (256 * 32))
+            Ext4Raw a = ch(n - 1);
+            size_t out_h = (ih + 1) / 2, in_h = ih;
+            if (out_h != 1) return "ref_logup_gkr: the interactions layer did not fold to one entry";
+            void* d_out;
+            RCHK(mem.alloc(&d_out, 4 * E));
+            void* args[] = {&guts, &d_out, &a, &in_h, &out_h};
+            RCHK(cudaLaunchKernel(logup_gkr_fix_last_variable_interactions_layer(), dim3((unsigned)((ih + BLOCK * 32 - 1) / (BLOCK * 32))), dim3((unsigned)BLOCK),
+                                  args, 0, 0));
+            RCHK(cudaMemcpy(o, d_out, 4 * E, cudaMemcpyDeviceToHost));
+            o += 16;
+        }
+        points += 4 * n;
+        challenges += 4 * n;
+    }
+    RCHK(cudaDeviceSynchronize());
+    return nullptr;
+}
+
 
 }  // extern "C"
 

@@ -323,3 +323,22 @@ def jagged_last_inputs():
     z_col = np.zeros((n, 4), np.uint32)
     f(ptr(z_col), C.c_uint32(n), ptr(claim))
     return z_col, claim
+
+
+def gkr_last_inputs():
+    """the inputs of this thread's last oracle LogUp-GKR prove that the proof does not carry:
+    -> (alpha [4], beta_seed [n, 4], per GKR layer in proof order (lambda [4], claim [4], evaluation point [m, 4]))"""
+    f = lib().orc_gkr_last_inputs
+    f.restype = C.c_uint64
+    n = f(None, C.c_uint64(0))
+    w = np.zeros(n, np.uint32)
+    f(ptr(w), C.c_uint64(n))
+    alpha = w[0:4]; nb = int(w[4]); o = 5
+    beta = w[o:o + 4 * nb].reshape(nb, 4); o += 4 * nb
+    layers = []
+    nl = int(w[o]); o += 1
+    for _ in range(nl):
+        lam, claim = w[o:o + 4], w[o + 4:o + 8]; m = int(w[o + 8]); o += 9
+        layers.append((lam, claim, w[o:o + 4 * m].reshape(m, 4))); o += 4 * m
+    assert o == n
+    return alpha, beta, layers

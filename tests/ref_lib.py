@@ -34,7 +34,7 @@ def lib():
         for n in ("ref_init", "ref_malloc", "ref_free", "ref_h2d", "ref_d2h", "ref_field_op", "ref_ext_op", "ref_permute", "ref_hash",
                   "ref_compress", "ref_merkle_tree", "ref_batch_coset_dft", "ref_batch", "ref_fold_mle_ext", "ref_fix_last_variable_ext",
                   "ref_partial_lagrange_ext", "ref_grind", "ref_challenger_script", "ref_gkr_populate", "ref_zerocheck_node_sums",
-                  "ref_jagged_sumcheck"):
+                  "ref_jagged_sumcheck", "ref_logup_gkr"):
             getattr(L, n).restype = C.c_char_p
         _chk(L.ref_init())
         _lib = L
@@ -281,12 +281,12 @@ def parse_interactions(blob, offset, n_chips):
     return out
 
 
-def gkr_populate(inter, main, prep, alpha, betas):
-    """the reference's populateLastCircuitLayer for one chip.  inter: one chip of parse_interactions; main / prep: [w, h] column-major.
-    -> (num [n_inter, h] uint32, den [n_inter, h, 4])"""
-    LEAF_PREP = 2
-    h = main.shape[1]
-    n = len(inter)
+LEAF_PREP = 2
+
+
+def _interaction_csr(inter):
+    """one chip of parse_interactions in the flattened CSR form of the reference's `Interactions<F>` (sys/include/logup_gkr/tracegen.cuh),
+    indices local to the chip: dict of the arrays ref_gkr_populate / ref_logup_gkr take"""
     values_ptr, mult_ptr, vcw_ptr = [0], [0], [0]
     vcw, mcw, vconst, mconst, args, send = [], [], [], [], [], []
     for is_send, arg, (mc, mterms), vals in inter:
@@ -300,9 +300,32 @@ def gkr_populate(inter, main, prep, alpha, betas):
         mult_ptr.append(len(mcw))
         args.append(int(((arg << 32) % 0x7F000001)))
         send.append(1 if is_send else 0)
-    u64 = lambda x: np.ascontiguousarray(np.array(x if len(x) else [0], dtype=np.uint64))
-    u32 = lambda x: np.ascontiguousarray(np.array(x if len(x) else [0], dtype=np.uint32))
-    u8 = lambda x: np.ascontiguousarray(np.array(x if len(x) else [0], dtype=np.uint8))
+    return dict(values_ptr=(values_ptr, np.uint64), mult_ptr=(mult_ptr, np.uint64), vcw_ptr=(vcw_ptr, np.uint64),
+                vcw_col=([c for c, _, _ in vcw], np.uint64), vcw_is_prep=([p for _, p, _ in vcw], np.uint8), vcw_weight=([w for _, _, w in vcw], np.uint32),
+                values_constants=(vconst, np.uint32), mcw_col=([c for c, _, _ in mcw], np.uint64), mcw_is_prep=([p for _, p, _ in mcw], np.uint8),
+                mcw_weight=([w for _, _, w in mcw], np.uint32), mult_constants=(mconst, np.uint32), arg_indices=(args, np.uint32),
+                is_send=(send, np.uint8))
+
+
+def _arr(x, dt):
+    """a contiguous array of dtype dt, one zero entry when empty (never a null pointer)"""
+    return np.ascontiguousarray(np.array(x if len(x) else [0], dtype=dt))
+
+
+_CTYPES = {np.uint64: C.c_uint64, np.uint32: C.c_uint32, np.uint8: C.c_uint8}
+
+
+def _ptr(a):
+    return a.ctypes.data_as(C.POINTER(_CTYPES[a.dtype.type]))
+
+
+def gkr_populate(inter, main, prep, alpha, betas):
+    """the reference's populateLastCircuitLayer for one chip.  inter: one chip of parse_interactions; main / prep: [w, h] column-major.
+    -> (num [n_inter, h] uint32, den [n_inter, h, 4])"""
+    h = main.shape[1]
+    n = len(inter)
+    a = {k: _arr(x, dt) for k, (x, dt) in _interaction_csr(inter).items()}
+    n_values, n_vcw, n_mcw = int(a["values_ptr"][-1]), int(a["vcw_ptr"][-1]), int(a["mult_ptr"][-1])
     half = (h + 1) // 2 if h else 1
     q = (half + 1) // 2
     outH = 2 * q * n
@@ -311,17 +334,12 @@ def gkr_populate(inter, main, prep, alpha, betas):
     oh = C.c_uint64()
     mainf = np.ascontiguousarray(main, np.uint32).reshape(-1)
     prepf = np.ascontiguousarray(prep, np.uint32).reshape(-1) if prep is not None and prep.size else np.zeros(1, np.uint32)
-    a_vp, a_mp, a_vcp = u64(values_ptr), u64(mult_ptr), u64(vcw_ptr)
-    a_vc, a_vip, a_vw = u64([c for c, _, _ in vcw]), u8([p for _, p, _ in vcw]), u32([w for _, _, w in vcw])
-    a_mc, a_mip, a_mw = u64([c for c, _, _ in mcw]), u8([p for _, p, _ in mcw]), u32([w for _, _, w in mcw])
-    a_vconst, a_mconst, a_args, a_send = u32(vconst), u32(mconst), u32(args), u8(send)
     alpha = np.ascontiguousarray(alpha, np.uint32); betas = np.ascontiguousarray(betas, np.uint32)
-    p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint64))
-    p8 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint8))
     _chk(lib().ref_gkr_populate(_p(prepf), C.c_uint64(prepf.size if prep is not None and prep.size else 0), _p(mainf), C.c_uint64(mainf.size), C.c_uint64(h),
-                                C.c_uint32(n), p64(a_vp), p64(a_mp), p64(a_vcp), C.c_uint64(len(vconst)), p64(a_vc), p8(a_vip), _p(a_vw), C.c_uint64(len(vcw)),
-                                _p(a_vconst), p64(a_mc), p8(a_mip), _p(a_mw), C.c_uint64(len(mcw)), _p(a_mconst), _p(a_args), p8(a_send), _p(alpha),
-                                _p(betas.reshape(-1)), C.c_uint32(betas.shape[0]), _p(num), _p(den.reshape(-1)), C.byref(oh)))
+                                C.c_uint32(n), _ptr(a["values_ptr"]), _ptr(a["mult_ptr"]), _ptr(a["vcw_ptr"]), C.c_uint64(n_values), _ptr(a["vcw_col"]),
+                                _ptr(a["vcw_is_prep"]), _ptr(a["vcw_weight"]), C.c_uint64(n_vcw), _ptr(a["values_constants"]), _ptr(a["mcw_col"]),
+                                _ptr(a["mcw_is_prep"]), _ptr(a["mcw_weight"]), C.c_uint64(n_mcw), _ptr(a["mult_constants"]), _ptr(a["arg_indices"]),
+                                _ptr(a["is_send"]), _p(alpha), _p(betas.reshape(-1)), C.c_uint32(betas.shape[0]), _p(num), _p(den.reshape(-1)), C.byref(oh)))
     assert oh.value == outH
     out_num = np.zeros((n, h), np.uint32); out_den = np.zeros((n, h, 4), np.uint32)
     for j in range(n):
@@ -331,6 +349,50 @@ def gkr_populate(inter, main, prep, alpha, betas):
         out_den[j, 0::2] = den[base:base + half][: (h + 1) // 2]
         out_den[j, 1::2] = den[base + 2 * outH:base + 2 * outH + half][: h // 2]
     return out_num, out_den
+
+
+def gkr_layer_words(v, p):
+    """the words ref_logup_gkr returns for GKR layer p (in proof order: p + 1 row variables, n = v + p + 1 rounds): the 10-value grid and
+    3 sums per round from round 2 on for a lookahead layer (more than 2 row variables), 3 sums per round otherwise, then n0, n1, d0, d1"""
+    n = v + p + 1
+    return 4 * ((10 + 3 * (n - 2) if p + 1 > 2 else 3 * n) + 4)
+
+
+def gkr_raw_words(v, mlr):
+    """the number of words ref_logup_gkr returns for 2^v padded interactions and max_log_row_count mlr: the output numerators and
+    denominators (2^(v+1) ext each), then every layer"""
+    return 8 * (2 << v) + sum(gkr_layer_words(v, p) for p in range(mlr - 1))
+
+
+def logup_gkr(chip_inters, heights, mains, preps, alpha, betas, mlr, lambdas, points, challenges):
+    """the reference's LogUp-GKR kernels (ref_logup_gkr): first layer, forward circuit and every layer's sumcheck rounds with the challenges
+    supplied.  chip_inters: parse_interactions of the machine; mains / preps: [w, h] column-major (preps[k] None without preprocessed
+    columns); lambdas [L, 4], points / challenges: per GKR layer in proof order, [v + p + 1, 4] each.  -> the raw words (see ref_launcher.cu)"""
+    csr = [_interaction_csr(i) for i in chip_inters]
+    a = {k: _arr([x for c in csr for x in c[k][0]], csr[0][k][1]) for k in csr[0]}
+    main_parts = [np.ascontiguousarray(m, np.uint32).reshape(-1) for m in mains]
+    prep_parts = [np.ascontiguousarray(p, np.uint32).reshape(-1) if p is not None else np.zeros(0, np.uint32) for p in preps]
+    main_off = np.ascontiguousarray(np.cumsum([0] + [m.size for m in main_parts])[:-1], np.uint64)
+    prep_off = np.ascontiguousarray(np.cumsum([0] + [p.size for p in prep_parts])[:-1], np.uint64)
+    mainf = _arr(np.concatenate(main_parts), np.uint32)
+    prepf = _arr(np.concatenate(prep_parts), np.uint32)
+    hs = np.ascontiguousarray(heights, np.uint64)
+    ni = np.ascontiguousarray([len(i) for i in chip_inters], np.uint32)
+    total = int(ni.sum())
+    v = max(total - 1, 0).bit_length()
+    out = np.zeros(gkr_raw_words(v, mlr), np.uint32)
+    pts = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint32).reshape(-1) for p in points]), np.uint32)
+    chs = np.ascontiguousarray(np.concatenate([np.asarray(c, np.uint32).reshape(-1) for c in challenges]), np.uint32)
+    assert pts.size == chs.size
+    lam = np.ascontiguousarray(lambdas, np.uint32).reshape(-1)
+    alpha = np.ascontiguousarray(alpha, np.uint32); betas = np.ascontiguousarray(betas, np.uint32).reshape(-1)
+    _chk(lib().ref_logup_gkr(C.c_uint32(len(heights)), _ptr(hs), _ptr(ni), _p(mainf), _ptr(main_off), C.c_uint64(mainf.size), _p(prepf), _ptr(prep_off),
+                             C.c_uint64(prepf.size), *[_ptr(a[k]) for k in ("values_ptr", "mult_ptr", "vcw_ptr", "vcw_col", "vcw_is_prep", "vcw_weight",
+                                                                            "values_constants", "mcw_col", "mcw_is_prep", "mcw_weight", "mult_constants",
+                                                                            "arg_indices", "is_send")],
+                             _p(alpha), _p(betas), C.c_uint32(betas.size // 4), C.c_uint32(mlr), _p(lam), _p(pts), _p(chs), C.c_uint64(pts.size),
+                             _p(out), C.c_uint64(out.size)))
+    return out
 
 
 def zerocheck_node_sums(chip, main, prep, pv, alpha_pows, E):
