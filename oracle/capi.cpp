@@ -391,13 +391,25 @@ int64_t orc_zerocheck_prove_verify(const uint32_t* machine_blob, const uint64_t*
     }
     ZerocheckResult r = zerocheck_prove(chips, alpha, gamma, gp, claims, pv, max_log_rows, ch);
     chal_store(ch, challenger_state);
-    const char* err = zerocheck_verify(chips, r.opened, gp, om, op, r.proof, pv, max_log_rows, vch);
+    const char* err = g_skip_verify ? nullptr : zerocheck_verify(chips, r.opened, gp, om, op, r.proof, pv, max_log_rows, vch);
     if (err) { std::fprintf(stderr, "oracle zerocheck verifier rejected oracle proof: %s\n", err); return -1; }
     std::vector<uint32_t> o;
     put(o, r.proof);
     for (auto& c : r.opened) { for (auto& e : c.prep) put(o, e); for (auto& e : c.main) put(o, e); }
     if (out) { if (o.size() > cap) return -2; std::copy(o.begin(), o.end(), out); }
     return (int64_t)o.size();
+}
+
+// tests only: the inputs of this thread's last zerocheck prove as words: alpha | gamma | lambda | claimed sum | n | challenges[n] in round
+// order (ext = 4 words).  The words are written when they fit in cap; returns their number.
+uint64_t orc_zerocheck_last_inputs(uint32_t* out, uint64_t cap) {
+    const ZerocheckProveInputs& in = zerocheck_last_inputs();
+    std::vector<uint32_t> o;
+    put(o, in.alpha); put(o, in.gamma); put(o, in.lambda); put(o, in.claimed_sum);
+    o.push_back((uint32_t)in.challenges.size());
+    for (auto& e : in.challenges) put(o, e);
+    if (out && o.size() <= cap) std::copy(o.begin(), o.end(), out);
+    return o.size();
 }
 
 

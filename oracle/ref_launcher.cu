@@ -27,6 +27,12 @@
 #include "logup_gkr/lookahead.cuh"
 #include "logup_gkr/round.cuh"
 #include "zerocheck/sequential.cuh"
+#include "zerocheck/aggregate.cuh"
+#include "zerocheck/geq_corrections.cuh"
+#include "zerocheck/gkr_sweep.cuh"
+#include "zerocheck/jagged_mle.cuh"
+#include "zerocheck/pad_adj.cuh"
+#include "jagged_assist/chip_layouts.cuh"
 #include "jagged_sumcheck/jagged_sumcheck.cuh"
 #include "tracegen/jagged_tracegen/jagged.cuh"
 #include "runtime/exception.cuh"
@@ -738,6 +744,27 @@ extern "C" void* mle_fix_last_variable_koala_bear_ext_ext_constant_padding();
         if (e_ != cudaSuccess) return e_;    \
     } while (0)
 
+// fold_jagged_metadata_dev (sp1-gpu/crates/utils/src/jagged.rs:207-279, zerocheck/src/primitives.rs:53-112): from the n_cols column
+// heights d_h (row pairs), the folded heights h.div_ceil(4) * 2 and their exclusive prefix sums (n_cols + 1 entries, the last = *total)
+static cudaError_t fold_metadata(DevScope& mem, const uint32_t* d_h, uint32_t n_cols, uint32_t** new_h, uint32_t** new_start, uint32_t* total) {
+    const uint32_t sec = jagged_fold_metadata_section_size(), bd = jagged_fold_metadata_block_dim();
+    const uint32_t nb = std::max<uint32_t>((n_cols + sec - 1) / sec, 1);
+    void *bc, *fl, *sv;
+    CECHK(mem.alloc((void**)new_h, n_cols * 4));
+    CECHK(mem.alloc((void**)new_start, (n_cols + 1) * 4));
+    CECHK(mem.alloc(&bc, 4));
+    CECHK(mem.alloc(&fl, (nb + 1) * 4));
+    CECHK(mem.alloc(&sv, (nb + 1) * 4));
+    CECHK(cudaMemset(bc, 0, 4));
+    CECHK(cudaMemset(fl, 0, (nb + 1) * 4));
+    CECHK(cudaMemset(fl, 1, 4));   // flags[0] != 0: the first block does not wait
+    CECHK(cudaMemset(sv, 0, (nb + 1) * 4));
+    uint32_t n = n_cols;
+    void* args[] = {&d_h, &n, new_h, new_start, &bc, &fl, &sv};
+    CECHK(cudaLaunchKernel(jagged_fold_metadata_kernel(), dim3(nb), dim3(bd), args, 0, 0));
+    return cudaMemcpy(total, *new_start + n_cols, 4, cudaMemcpyDeviceToHost);
+}
+
 // one circuit layer on the device: the JaggedMle kernel argument and its column heights (row-pair counts), from which the reference's
 // fold-metadata kernel derives the next layer's
 struct GkrCircuitDev {
@@ -826,24 +853,8 @@ const char* ref_logup_gkr(uint32_t n_chips, const uint64_t* chip_heights, const 
         CECHK(cudaLaunchKernel(kernel, dim3((unsigned)grid), dim3((unsigned)BLOCK), args, smem, 0));
         return sum_rows(*part, rows, grid);
     };
-    // fold_jagged_metadata_dev (sp1-gpu/crates/utils/src/jagged.rs:207-279): heights' = h.div_ceil(4) * 2 and their prefix sums
-    auto fold = [&](const uint32_t* d_h, uint32_t** new_h, uint32_t** new_start, uint32_t* total) -> cudaError_t {
-        const uint32_t sec = jagged_fold_metadata_section_size(), bd = jagged_fold_metadata_block_dim();
-        const uint32_t nb = std::max<uint32_t>((n_cols + sec - 1) / sec, 1);
-        void *bc, *fl, *sv;
-        CECHK(mem.alloc((void**)new_h, n_cols * 4));
-        CECHK(mem.alloc((void**)new_start, (n_cols + 1) * 4));
-        CECHK(mem.alloc(&bc, 4));
-        CECHK(mem.alloc(&fl, (nb + 1) * 4));
-        CECHK(mem.alloc(&sv, (nb + 1) * 4));
-        CECHK(cudaMemset(bc, 0, 4));
-        CECHK(cudaMemset(fl, 0, (nb + 1) * 4));
-        CECHK(cudaMemset(fl, 1, 4));   // flags[0] != 0: the first block does not wait
-        CECHK(cudaMemset(sv, 0, (nb + 1) * 4));
-        uint32_t n = n_cols;
-        void* args[] = {&d_h, &n, new_h, new_start, &bc, &fl, &sv};
-        CECHK(cudaLaunchKernel(jagged_fold_metadata_kernel(), dim3(nb), dim3(bd), args, 0, 0));
-        return cudaMemcpy(total, *new_start + n_cols, 4, cudaMemcpyDeviceToHost);
+    auto fold = [&](const uint32_t* d_h, uint32_t** new_h, uint32_t** new_start, uint32_t* total) {
+        return fold_metadata(mem, d_h, n_cols, new_h, new_start, total);
     };
     // the next circuit layer's buffers, its metadata advanced `folds` folds from the column heights d_h; Tensor [4, 1, 2 * height] and a
     // colIndex of `height` entries, zeroed (the reference leaves them uninitialised; every entry read is written by the kernels)
@@ -1058,6 +1069,443 @@ const char* ref_logup_gkr(uint32_t n_chips, const uint64_t* chip_heights, const 
     return nullptr;
 }
 
+}  // extern "C"
+
+// ---- zerocheck: the reference's zerocheck prover kernels ------------------------------------------------------------------------------
+// One chip's constraint program as the machine blob stores it (include/sp1b200.h): the chunk the reference's lowering would emit for it.
+struct ZcBlobChip {
+    uint32_t main_w, prep_w, n_constraints, ni, nl, nc, npub, na, max_reg;
+    const uint32_t *instrs, *leaves, *consts, *publics, *assert_regs, *assert_alphas;
+};
+
+// Every read the interpreter (sequential.cu:50-108, pad_adj.cu) makes without a check: an opcode it knows (others __trap), a leaf, constant
+// and public-value index inside its table, a leaf column inside the chip's trace, a register written before it is read (an unwritten one
+// holds the previous row's value) and an alpha index below the chip's constraint count.  max_reg = the highest register used + 1, as
+// sp1-gpu/crates/air/src/ir/bytecode.rs:208-209 computes it.
+static const char* zc_check_program(ZcBlobChip& c, uint32_t n_pv) {
+    std::vector<uint8_t> written(1024, 0);
+    uint32_t top = 0;
+    auto ok = [&](uint32_t r) { return r < 1024 && written[r]; };
+    for (uint32_t i = 0; i < c.ni; i++) {
+        const uint32_t op = c.instrs[2 * i] & 0xff, o = c.instrs[2 * i] >> 16, a = c.instrs[2 * i + 1] & 0xffff, b = c.instrs[2 * i + 1] >> 16;
+        switch (op) {
+        case BC_LOAD_LEAF: {
+            if (a >= c.nl) return "ref_zerocheck: a leaf index past the chip's leaf table";
+            const uint32_t src = c.leaves[2 * a] & 0xff, col = c.leaves[2 * a + 1];
+            if (src == LEAF_SOURCE_MAIN_LOCAL ? col >= c.main_w : (src != LEAF_SOURCE_PREPROCESSED_LOCAL || col >= c.prep_w))
+                return "ref_zerocheck: a leaf outside the chip's columns";
+            break;
+        }
+        case BC_LOAD_CONST: if (a >= c.nc) return "ref_zerocheck: a constant index past the chip's constants"; break;
+        case BC_LOAD_PUBLIC: if (a >= c.npub || c.publics[a] >= n_pv) return "ref_zerocheck: a public-value index out of range"; break;
+        case BC_ADD_F: case BC_SUB_F: case BC_MUL_F: if (!ok(a) || !ok(b)) return "ref_zerocheck: a register read before it is written"; break;
+        case BC_NEG_F: if (!ok(a)) return "ref_zerocheck: a register read before it is written"; break;
+        default: return "ref_zerocheck: an unknown opcode (the interpreter traps)";
+        }
+        if (o >= 1024) return "ref_zerocheck: a program above 1024 registers (the largest MAX_REGS template)";
+        written[o] = 1;
+        top = std::max(top, o + 1);
+    }
+    for (uint32_t i = 0; i < c.na; i++) {
+        if (!ok(c.assert_regs[i])) return "ref_zerocheck: an assert on a register that is never written";
+        if (c.assert_alphas[i] >= c.n_constraints) return "ref_zerocheck: an assert's alpha index past the chip's constraint count";
+    }
+    c.max_reg = top;
+    return nullptr;
+}
+
+// the MAX_REGS template that covers max_reg (prover.rs:828-852, 1180-1196, 1877-1893)
+static void* zc_tier_kernel(uint32_t max_reg, void* (*const k[6])()) {
+    return k[max_reg <= 32 ? 0 : max_reg <= 64 ? 1 : max_reg <= 128 ? 2 : max_reg <= 256 ? 3 : max_reg <= 512 ? 4 : 5]();
+}
+
+extern "C" {
+
+// zerocheck() (sp1-gpu/crates/zerocheck/src/prover.rs:2412-2741) on the fused first-two-rounds path, with lambda and the round challenges
+// supplied instead of sampled and the host-side tables computed by the caller.  One chunk per chip: the blob's program (no ColumnTile).
+//   blob         the machine blob; chip k has heights[k] rows, main (prep) columns at h_main + main_off[k] (h_prep + prep_off[k]), column-major
+//   prep_pad_rows  the rows of the one preprocessed padding column between the preprocessed and the main columns (zero data)
+//   alpha_pows   powers_of_alpha: alpha^0 .. alpha^(max_constraints - 1) reversed;  gkr_pows: gamma^1 .. gamma^n_gkr;
+//   lambda_pows  lambda^0 .. lambda^(n_chips - 1) reversed;  zeta: the mlr coordinates of the GKR point;  challenges: mlr, in round order
+// The jagged trace is built as the reference's own zerocheck harness builds it (zerocheck/src/lib.rs:1240-1330): every chip's preprocessed
+// columns, the padding column, every chip's main columns.  Raw outputs, ext (4 words) each:
+//   the padded-row adjustment of every chip (zerocheck_pad_adj, prover.rs:1207-1259)
+//   the 16 totals of evaluate_zerocheck_bivariate (prover.rs:1908-2160): 12 node totals, then the corners c = 2x + y
+//   per later round r = 2 .. mlr - 1: the 3 totals of evaluate_zerocheck (prover.rs:1434-1772) at the nodes {0, 2, 4}
+//   per column, in column order (padding column included): the folded value zerocheck() demultiplexes (prover.rs:2692-2702), 0 for an
+//   empty column
+// Chips of height 0 are supported: the dispatch builders skip them, the chip-layouts kernel gives them height 0 and the geq kernel sums
+// over no rows.  Rejected before any launch: max_log_row_count < 2 (no fused path), a height that is not a multiple of 4 (odd heights break
+// the row-pair loads; heights = 2 mod 4 trap in fixLastTwoVariablesTwoPadding, jagged.cuh:113-117), a height above 2^mlr, a chip with rows
+// but no columns, and every program fault zc_check_program lists.
+const char* ref_zerocheck(const uint32_t* blob, const uint64_t* heights, const uint32_t* h_main, const uint64_t* main_off, uint64_t main_words,
+                          const uint32_t* h_prep, const uint64_t* prep_off, uint64_t prep_words, uint32_t prep_pad_rows, const uint32_t* pv,
+                          uint32_t n_pv, const uint32_t* alpha_pows, uint32_t n_alpha, const uint32_t* gkr_pows, uint32_t n_gkr,
+                          const uint32_t* lambda_pows, uint32_t mlr, const uint32_t* zeta, const uint32_t* challenges, uint32_t* out,
+                          uint64_t out_cap) {
+    // ---- host-side rejection of every input that would make an unchecked reference kernel fault or read unwritten memory
+    if (mlr < 2 || mlr > 24) return "ref_zerocheck: need 2 <= max_log_row_count <= 24 (the fused first two rounds need two variables)";
+    const uint32_t n = blob[0];
+    if (n == 0) return "ref_zerocheck: no chips";
+    std::vector<ZcBlobChip> chips(n);
+    {
+        const uint32_t* b = blob + 1;
+        for (auto& c : chips) {
+            c.main_w = b[0]; c.prep_w = b[1]; c.n_constraints = b[2];
+            c.ni = b[4]; c.nl = b[5]; c.nc = b[6]; c.npub = b[7]; c.na = b[8];
+            b += 9;
+            c.instrs = b; b += 2 * c.ni;
+            c.leaves = b; b += 2 * c.nl;
+            c.consts = b; b += c.nc;
+            c.publics = b; b += c.npub;
+            c.assert_regs = b; b += c.na;
+            c.assert_alphas = b; b += c.na;
+        }
+    }
+    uint32_t max_nc = 0, max_cols = 0, total_prep_w = 0, total_main_w = 0;
+    for (uint32_t k = 0; k < n; k++) {
+        ZcBlobChip& c = chips[k];
+        const uint64_t h = heights[k];
+        if (h % 4) return "ref_zerocheck: a height that is not a multiple of 4 (fixLastTwoVariablesTwoPadding traps on odd pair heights)";
+        if (h > (1ull << mlr)) return "ref_zerocheck: a chip taller than 2^max_log_row_count";
+        if (h && c.main_w + c.prep_w == 0) return "ref_zerocheck: a chip with rows but no columns (the chip-layouts kernel gives it height 0)";
+        if (main_off[k] + c.main_w * h > main_words || prep_off[k] + c.prep_w * h > prep_words) return "ref_zerocheck: a chip's trace runs past the trace words";
+        if (const char* e = zc_check_program(c, n_pv)) return e;
+        max_nc = std::max(max_nc, c.n_constraints);
+        max_cols = std::max(max_cols, c.main_w + c.prep_w);
+        total_prep_w += c.prep_w;
+        total_main_w += c.main_w;
+    }
+    if (n_alpha < max_nc) return "ref_zerocheck: fewer alpha powers than the largest constraint count";
+    if (n_gkr < max_cols) return "ref_zerocheck: fewer gkr powers than the widest chip's columns";
+    if (prep_pad_rows == 0 || prep_pad_rows % 4 || prep_pad_rows > (1u << mlr))
+        return "ref_zerocheck: the padding column needs a non-zero multiple of 4 rows, at most 2^max_log_row_count";
+    const uint32_t n_cols = total_prep_w + 1 + total_main_w;
+    if (out_cap < 4ull * (n + 16 + 3 * (mlr - 2) + n_cols)) return "ref_zerocheck: output buffer too small";
+
+    // ---- the jagged trace (build_chip_column_layouts, prover.rs:1271-1294; the layout of zerocheck/src/lib.rs:1240-1330)
+    std::vector<uint32_t> colh;                 // column heights in row pairs
+    std::vector<ChipColumnLayoutEntry> entries(n);
+    std::vector<uint32_t> dense;
+    uint64_t total_pairs = 0;
+    for (uint32_t k = 0; k < n; k++) total_pairs += (uint64_t)(chips[k].prep_w + chips[k].main_w) * heights[k] / 2;
+    total_pairs += prep_pad_rows / 2;
+    if (total_pairs >= (1ull << 31)) return "ref_zerocheck: the trace is too long for the kernels' 32-bit lengths";
+    dense.reserve(2 * total_pairs);
+    for (uint32_t k = 0, cp = 0; k < n; k++) {
+        entries[k].prep_col_idx = cp;
+        entries[k].prep_width = chips[k].prep_w;
+        const uint64_t h = heights[k];
+        for (uint32_t j = 0; j < chips[k].prep_w; j++) {
+            colh.push_back((uint32_t)(h / 2));
+            dense.insert(dense.end(), h_prep + prep_off[k] + j * h, h_prep + prep_off[k] + (j + 1) * h);
+        }
+        cp += chips[k].prep_w;
+    }
+    colh.push_back(prep_pad_rows / 2);
+    dense.insert(dense.end(), prep_pad_rows, 0u);
+    for (uint32_t k = 0, cm = total_prep_w + 1; k < n; k++) {
+        entries[k].main_col_idx = cm;
+        entries[k].main_width = chips[k].main_w;
+        const uint64_t h = heights[k];
+        for (uint32_t j = 0; j < chips[k].main_w; j++) {
+            colh.push_back((uint32_t)(h / 2));
+            dense.insert(dense.end(), h_main + main_off[k] + j * h, h_main + main_off[k] + (j + 1) * h);
+        }
+        cm += chips[k].main_w;
+    }
+    std::vector<uint32_t> start(n_cols + 1, 0), col_index(total_pairs);
+    for (uint32_t c = 0; c < n_cols; c++) {
+        std::fill(col_index.begin() + start[c], col_index.begin() + start[c] + colh[c], c);
+        start[c + 1] = start[c] + colh[c];
+    }
+    const std::vector<uint32_t> input_colh = colh;
+    // the layout tracker's chip height in elements (ShardLayoutTracker::chip_height_elements): the chip's main height, else its prep height
+    auto chip_height = [&](uint32_t k) {
+        return chips[k].main_w ? 2 * colh[entries[k].main_col_idx] : chips[k].prep_w ? 2 * colh[entries[k].prep_col_idx] : 0u;
+    };
+    auto fold_host = [&]() { for (auto& h : colh) h = (h + 3) / 4 * 2; };
+
+    DevScope mem;   // every device buffer below is freed on every return
+    const size_t E = sizeof(kb31_extension_t);
+    auto ext = [](const uint32_t* w) { Ext4Raw a; memcpy(&a, w, 16); return a; };
+    void *d_dense, *d_col, *d_start, *d_colh, *d_entries, *d_layouts, *d_pv, *d_alpha, *d_gkr, *d_lambda, *d_geq, *d_pad_adj, *d_gkr_info;
+    RCHK(dev_upload(mem, dense.data(), dense.size() * 4, &d_dense));
+    RCHK(dev_upload(mem, col_index.data(), col_index.size() * 4, &d_col));
+    RCHK(dev_upload(mem, start.data(), start.size() * 4, &d_start));
+    RCHK(dev_upload(mem, colh.data(), colh.size() * 4, &d_colh));
+    RCHK(dev_upload(mem, entries.data(), entries.size() * sizeof(ChipColumnLayoutEntry), &d_entries));
+    RCHK(mem.alloc(&d_layouts, n * sizeof(ChipLayout)));
+    RCHK(dev_upload(mem, pv, (size_t)n_pv * 4, &d_pv));
+    RCHK(dev_upload(mem, alpha_pows, (size_t)n_alpha * E, &d_alpha));
+    RCHK(dev_upload(mem, gkr_pows, (size_t)n_gkr * E, &d_gkr));
+    RCHK(dev_upload(mem, lambda_pows, (size_t)n * E, &d_lambda));
+    // launch_chip_layouts_kernel (prover.rs:1299-1331): block 128
+    auto chip_layouts = [&]() {
+        void* args[] = {&d_start, &d_colh, &d_entries, (void*)&n, &d_layouts};
+        return cudaLaunchKernel(jagged_chip_layouts_kernel(), dim3((n + 127) / 128), dim3(128), args, 0, 0);
+    };
+    RCHK(chip_layouts());
+
+    // ---- the chunk statics and the sequential tiers (build_seq_tiers, prover.rs:1086-1152; WIDE_GKR_THRESHOLD = 256, :1077)
+    std::vector<ChunkStatic> statics(n);
+    for (uint32_t k = 0; k < n; k++) {
+        const ZcBlobChip& c = chips[k];
+        std::vector<uint16_t> regs16(c.assert_regs, c.assert_regs + c.na);
+        ChunkStatic& s = statics[k];
+        RCHK(dev_upload(mem, c.instrs, (size_t)c.ni * 8, (void**)&s.instrs));
+        RCHK(dev_upload(mem, c.leaves, (size_t)c.nl * 8, (void**)&s.leaves));
+        RCHK(dev_upload(mem, c.consts, (size_t)c.nc * 4, (void**)&s.consts));
+        RCHK(dev_upload(mem, c.publics, (size_t)c.npub * 4, (void**)&s.publics));
+        RCHK(dev_upload(mem, regs16.data(), (size_t)c.na * 2, (void**)&s.assert_regs));
+        RCHK(dev_upload(mem, c.assert_alphas, (size_t)c.na * 4, (void**)&s.assert_alphas));
+        s.n_instrs = c.ni;
+        s.n_asserts = c.na;
+        s.chip_idx = k;
+        const bool decoupled = c.main_w + c.prep_w > 256;
+        s.gkr_main_width = decoupled ? 0 : c.main_w;    // the carrier chunk's inline GKR widths
+        s.gkr_prep_width = decoupled ? 0 : c.prep_w;
+        s.chip_alpha_offset = std::max(max_nc, 1u) - c.n_constraints;
+    }
+    uint32_t n_high = 0;
+    for (auto& c : chips) n_high += c.max_reg > 256;
+    const bool split = n_high > 0 && n_high * 10 <= n;
+    struct Tier { std::vector<ChunkStatic> st; std::vector<uint32_t> chip; uint32_t max_reg = 0; void* d_st = nullptr; };
+    Tier tiers[2];
+    for (uint32_t k = 0; k < n; k++) {
+        Tier& t = tiers[split && chips[k].max_reg > 256 ? 1 : 0];
+        t.st.push_back(statics[k]);
+        t.chip.push_back(k);
+        t.max_reg = std::max(t.max_reg, chips[k].max_reg);
+    }
+    for (auto& t : tiers)
+        if (!t.st.empty()) RCHK(dev_upload(mem, t.st.data(), t.st.size() * sizeof(ChunkStatic), &t.d_st));
+    auto block_size = [](const Tier& t) { return t.max_reg > 128 ? 64u : 256u; };   // prover.rs:1451-1472
+
+    // ---- padded-row adjustment (compute_padded_row_adjustment, prover.rs:1207-1259): block 64, one chunk per thread
+    std::vector<uint32_t> pad_adj(4 * n, 0);
+    {
+        static void* (*const K[6])() = {zerocheck_pad_adj_32_kernel, zerocheck_pad_adj_64_kernel, zerocheck_pad_adj_128_kernel,
+                                        zerocheck_pad_adj_256_kernel, zerocheck_pad_adj_512_kernel, zerocheck_pad_adj_1024_kernel};
+        for (auto& t : tiers) {
+            if (t.st.empty()) continue;
+            uint32_t nch = (uint32_t)t.st.size();
+            void* d_o;
+            RCHK(mem.alloc(&d_o, nch * E));
+            void* args[] = {&t.d_st, &nch, &d_pv, &d_alpha, &d_o};
+            RCHK(cudaLaunchKernel(zc_tier_kernel(t.max_reg, K), dim3((nch + 63) / 64), dim3(64), args, 0, 0));
+            std::vector<uint32_t> o(4 * nch);
+            RCHK(cudaMemcpy(o.data(), d_o, nch * E, cudaMemcpyDeviceToHost));
+            for (uint32_t i = 0; i < nch; i++) memcpy(&pad_adj[4 * t.chip[i]], &o[4 * i], 16);
+        }
+    }
+    memcpy(out, pad_adj.data(), pad_adj.size() * 4);
+    uint32_t* o = out + 4 * n;
+    RCHK(dev_upload(mem, pad_adj.data(), pad_adj.size() * 4, &d_pad_adj));
+    // the geq chips: a Sequential carrier and a non-zero padded-row adjustment (prover.rs:989-1005)
+    std::vector<uint32_t> geq_chips;
+    for (uint32_t k = 0; k < n; k++)
+        if (pad_adj[4 * k] | pad_adj[4 * k + 1] | pad_adj[4 * k + 2] | pad_adj[4 * k + 3]) geq_chips.push_back(k);
+    uint32_t n_geq = (uint32_t)geq_chips.size();
+    void* d_geq_chips;
+    RCHK(dev_upload(mem, geq_chips.data(), geq_chips.size() * 4, &d_geq_chips));
+    {   // VirtualGeq::new(height, 1, 0, num_vars) per chip (prover.rs:958-969)
+        std::vector<VirtualGeqState> g(n);
+        const uint32_t one[4] = {0x01fffffeu, 0, 0, 0};   // 1 in Montgomery form
+        for (uint32_t k = 0; k < n; k++) {
+            g[k].threshold = (uint32_t)heights[k];
+            g[k].num_vars = mlr;
+            memcpy(&g[k].geq_coefficient, one, 16);
+            memset(&g[k].eq_coefficient, 0, 16);
+        }
+        RCHK(dev_upload(mem, g.data(), g.size() * sizeof(VirtualGeqState), &d_geq));
+    }
+    std::vector<ChipGkrInfo> gkr_info(n);
+    std::vector<uint32_t> gkr_active;   // the decoupled-GKR chips (prover.rs:942-951): wider than 256 columns
+    for (uint32_t k = 0; k < n; k++) {
+        gkr_info[k] = {chips[k].main_w, chips[k].prep_w};
+        if (chips[k].main_w + chips[k].prep_w > 256) gkr_active.push_back(k);
+    }
+    RCHK(dev_upload(mem, gkr_info.data(), gkr_info.size() * sizeof(ChipGkrInfo), &d_gkr_info));
+    // zerocheck_fix_geq_state (prover.rs:2229-2246, 2334-2353): block 128, one thread per chip
+    auto fix_geq = [&](const uint32_t* a4) {
+        Ext4Raw a = ext(a4);
+        void* args[] = {&d_geq, (void*)&n, &a};
+        return cudaLaunchKernel(zerocheck_fix_geq_state_kernel(), dim3((n + 127) / 128), dim3(128), args, 0, 0);
+    };
+    // DevicePoint::partial_lagrange of zeta's first dim coordinates: block 256
+    auto eq_table = [&](uint32_t dim, void** d_out) -> cudaError_t {
+        void* d_pt;
+        CECHK(dev_upload(mem, zeta, (size_t)dim * E, &d_pt));
+        CECHK(mem.alloc(d_out, E << dim));
+        size_t nv = dim;
+        void* args[] = {d_out, &d_pt, &nv};
+        return cudaLaunchKernel(partial_lagrange_koala_bear_extension(), dim3((unsigned)(((1ull << dim) + 255) / 256)), dim3(256), args, 0, 0);
+    };
+    // row tiles of `rows` rows (pairs or quadruples): one BlockDispatch per tile (prover.rs:1518-1537, 1942-1962)
+    auto tiles = [](std::vector<BlockDispatch>& d, uint32_t id, uint32_t rows, uint32_t tile) {
+        for (uint32_t r = 0; r < rows; r += tile) d.push_back(BlockDispatch{id, r, std::min(rows - r, tile)});
+    };
+    const unsigned SMEM = 8 * E;   // (256 / 32) ext_t for every 256-thread reduction
+
+    // ---- rounds 0 and 1: evaluate_zerocheck_bivariate (prover.rs:1908-2160)
+    {
+        const uint32_t dim = mlr - 2;
+        void *d_eq, *d_nodes, *d_corners, *d_tot;
+        RCHK(eq_table(dim, &d_eq));
+        std::vector<BlockDispatch> disp[2], corner;
+        for (int t = 0; t < 2; t++)
+            for (uint32_t i = 0; i < tiers[t].chip.size(); i++) tiles(disp[t], i, (chip_height(tiers[t].chip[i]) + 3) / 4, block_size(tiers[t]));
+        for (uint32_t k = 0; k < n; k++)
+            if (chips[k].main_w + chips[k].prep_w) tiles(corner, k, (chip_height(k) + 3) / 4, 256);
+        const size_t node_slots = (disp[0].size() + disp[1].size() + n_geq) * 12, corner_slots = corner.size() * 4;
+        RCHK(mem.alloc(&d_nodes, std::max<size_t>(node_slots, 1) * E));
+        RCHK(mem.alloc(&d_corners, std::max<size_t>(corner_slots, 1) * E));
+        RCHK(mem.alloc(&d_tot, 16 * E));
+        static void* (*const K[6])() = {zerocheck_fused_sequential_bivariate_kb_32_kernel, zerocheck_fused_sequential_bivariate_kb_64_kernel,
+                                        zerocheck_fused_sequential_bivariate_kb_128_kernel, zerocheck_fused_sequential_bivariate_kb_256_kernel,
+                                        zerocheck_fused_sequential_bivariate_kb_512_kernel, zerocheck_fused_sequential_bivariate_kb_1024_kernel};
+        size_t slot = 0;
+        for (int t = 0; t < 2; t++) {
+            if (disp[t].empty()) continue;
+            void *d_disp, *part = (char*)d_nodes + slot * E;
+            RCHK(dev_upload(mem, disp[t].data(), disp[t].size() * sizeof(BlockDispatch), &d_disp));
+            const unsigned bs = block_size(tiers[t]);
+            void* args[] = {&d_disp, &tiers[t].d_st, &d_layouts, &d_dense, &d_pv, &d_alpha, &d_eq, &d_lambda, (void*)&dim, &part};
+            RCHK(cudaLaunchKernel(zc_tier_kernel(tiers[t].max_reg, K), dim3((unsigned)disp[t].size()), dim3(bs), args, (bs / 32) * E, 0));
+            slot += disp[t].size() * 12;
+        }
+        if (n_geq) {
+            void* part = (char*)d_nodes + slot * E;
+            void* args[] = {&d_geq_chips, &n_geq, &d_geq, &d_pad_adj, &d_lambda, &d_layouts, &d_eq, (void*)&dim, &part};
+            RCHK(cudaLaunchKernel(zerocheck_geq_corrections_bivariate_kernel(), dim3(n_geq), dim3(256), args, SMEM, 0));
+        }
+        if (!corner.empty()) {
+            void* d_disp;
+            RCHK(dev_upload(mem, corner.data(), corner.size() * sizeof(BlockDispatch), &d_disp));
+            void* args[] = {&d_disp, &d_layouts, &d_gkr_info, &d_dense, &d_gkr, &d_eq, &d_lambda, (void*)&dim, &d_corners};
+            RCHK(cudaLaunchKernel(zerocheck_gkr_corner_sweep_kb_kernel(), dim3((unsigned)corner.size()), dim3(256), args, SMEM, 0));
+        }
+        {   // zerocheck_aggregate_partials_strided: grid = stride, block 256
+            uint32_t ns = (uint32_t)node_slots, cs = (uint32_t)corner_slots, s12 = 12, s4 = 4;
+            void* t4 = (char*)d_tot + 12 * E;
+            void* a1[] = {&d_nodes, &ns, &s12, &d_tot};
+            void* a2[] = {&d_corners, &cs, &s4, &t4};
+            RCHK(cudaLaunchKernel(zerocheck_aggregate_partials_strided_kernel(), dim3(12), dim3(256), a1, SMEM, 0));
+            RCHK(cudaLaunchKernel(zerocheck_aggregate_partials_strided_kernel(), dim3(4), dim3(256), a2, SMEM, 0));
+        }
+        RCHK(cudaMemcpy(o, d_tot, 16 * E, cudaMemcpyDeviceToHost));
+        o += 64;
+    }
+
+    // ---- zerocheck_fix_last_two_variables (prover.rs:2295-2387 -> primitives.rs:238-335)
+    uint32_t length = (uint32_t)total_pairs;   // the input's pair count
+    {
+        fold_host(); fold_host();
+        uint64_t want = 0;
+        for (auto h : colh) want += h;
+        uint32_t *h1, *s1, *h2, *s2, total;
+        RCHK(fold_metadata(mem, (const uint32_t*)d_colh, n_cols, &h1, &s1, &total));
+        RCHK(fold_metadata(mem, h1, n_cols, &h2, &s2, &total));
+        if (total != want) return "ref_zerocheck: the fold metadata disagrees with the h.div_ceil(4) * 2 recurrence";
+        void *d_out, *d_ocol;
+        RCHK(mem.alloc(&d_out, 2ull * total * E));
+        RCHK(mem.alloc(&d_ocol, (size_t)total * 4));
+        JaggedMle<DenseBuffer<felt_t>> in;
+        in.colIndex = (uint32_t*)d_col; in.startIndices = (uint32_t*)d_start; in.denseData.data = (felt_t*)d_dense;
+        JaggedMle<DenseBuffer<ext_t>> nx;
+        nx.colIndex = (uint32_t*)d_ocol; nx.startIndices = s2; nx.denseData.data = (ext_t*)d_out;
+        uint32_t n_quads = length / 2;
+        Ext4Raw a1 = ext(challenges), a2 = ext(challenges + 4);
+        void* args[] = {&in, &nx, &n_quads, &a1, &a2};
+        RCHK(cudaLaunchKernel(fix_last_two_variables_jagged_felt(), dim3(std::max<uint32_t>((n_quads + 65535) / 65536, 256)), dim3(256), args, 0, 0));
+        RCHK(fix_geq(challenges));
+        RCHK(fix_geq(challenges + 4));
+        d_dense = d_out; d_col = d_ocol; d_start = s2; d_colh = h2;
+        length = total;
+        RCHK(chip_layouts());
+    }
+
+    // ---- rounds 2 .. mlr - 1: evaluate_zerocheck (prover.rs:1434-1796) then zerocheck_fix_last_variable (prover.rs:2189-2285)
+    for (uint32_t r = 2; r < mlr; r++) {
+        const uint32_t dim = mlr - r - 1;
+        void *d_eq, *d_part, *d_tot;
+        RCHK(eq_table(dim, &d_eq));
+        std::vector<BlockDispatch> disp[2], gkr;
+        for (int t = 0; t < 2; t++)
+            for (uint32_t i = 0; i < tiers[t].chip.size(); i++) tiles(disp[t], i, chip_height(tiers[t].chip[i]) / 2, block_size(tiers[t]) * 4);
+        for (uint32_t k : gkr_active) tiles(gkr, k, chip_height(k) / 2, 256 * 4);
+        const size_t slots = (disp[0].size() + disp[1].size() + n_geq + gkr.size()) * 3;
+        RCHK(mem.alloc(&d_part, std::max<size_t>(slots, 1) * E));
+        RCHK(mem.alloc(&d_tot, 3 * E));
+        static void* (*const K[6])() = {zerocheck_fused_sequential_ext_32_kernel, zerocheck_fused_sequential_ext_64_kernel,
+                                        zerocheck_fused_sequential_ext_128_kernel, zerocheck_fused_sequential_ext_256_kernel,
+                                        zerocheck_fused_sequential_ext_512_kernel, zerocheck_fused_sequential_ext_1024_kernel};
+        size_t slot = 0;
+        for (int t = 0; t < 2; t++) {
+            if (disp[t].empty()) continue;
+            void *d_disp, *part = (char*)d_part + slot * E;
+            RCHK(dev_upload(mem, disp[t].data(), disp[t].size() * sizeof(BlockDispatch), &d_disp));
+            const unsigned bs = block_size(tiers[t]);
+            void* args[] = {&d_disp, &tiers[t].d_st, &d_layouts, &d_dense, &d_pv, &d_alpha, &d_eq, &d_lambda, &d_gkr, (void*)&dim, &part};
+            RCHK(cudaLaunchKernel(zc_tier_kernel(tiers[t].max_reg, K), dim3((unsigned)disp[t].size(), 1, 3), dim3(bs), args, (bs / 32) * E, 0));
+            slot += disp[t].size() * 3;
+        }
+        if (n_geq) {
+            void* part = (char*)d_part + slot * E;
+            void* args[] = {&d_geq_chips, &n_geq, &d_geq, &d_pad_adj, &d_lambda, &d_layouts, &d_eq, (void*)&dim, &part};
+            RCHK(cudaLaunchKernel(zerocheck_geq_corrections_kernel(), dim3(n_geq), dim3(256), args, SMEM, 0));
+            slot += n_geq * 3;
+        }
+        if (!gkr.empty()) {
+            void *d_disp, *part = (char*)d_part + slot * E;
+            RCHK(dev_upload(mem, gkr.data(), gkr.size() * sizeof(BlockDispatch), &d_disp));
+            void* args[] = {&d_disp, &d_layouts, &d_gkr_info, &d_dense, &d_gkr, &d_eq, &d_lambda, (void*)&dim, &part};
+            RCHK(cudaLaunchKernel(zerocheck_gkr_sweep_ext_kernel(), dim3((unsigned)gkr.size(), 1, 3), dim3(256), args, SMEM, 0));
+        }
+        {   // zerocheck_aggregate_partials: one block of 256
+            uint32_t ns = (uint32_t)slots;
+            void* args[] = {&d_part, &ns, &d_tot};
+            RCHK(cudaLaunchKernel(zerocheck_aggregate_partials_kernel(), dim3(1), dim3(256), args, SMEM, 0));
+        }
+        RCHK(cudaMemcpy(o, d_tot, 3 * E, cudaMemcpyDeviceToHost));
+        o += 12;
+        // evaluate_jagged_fix_last_variable (primitives.rs:127-225): block 256, grid max(ceil(length / 2^16), 256)
+        fold_host();
+        uint32_t *h1, *s1, total;
+        RCHK(fold_metadata(mem, (const uint32_t*)d_colh, n_cols, &h1, &s1, &total));
+        void *d_out, *d_ocol;
+        RCHK(mem.alloc(&d_out, 2ull * total * E));
+        RCHK(mem.alloc(&d_ocol, (size_t)total * 4));
+        JaggedMle<DenseBuffer<ext_t>> in, nx;
+        in.colIndex = (uint32_t*)d_col; in.startIndices = (uint32_t*)d_start; in.denseData.data = (ext_t*)d_dense;
+        nx.colIndex = (uint32_t*)d_ocol; nx.startIndices = s1; nx.denseData.data = (ext_t*)d_out;
+        Ext4Raw a = ext(challenges + 4 * r);
+        void* args[] = {&in, &nx, &length, &a};
+        RCHK(cudaLaunchKernel(fix_last_variable_jagged_ext(), dim3(std::max<uint32_t>((length + 65535) / 65536, 256)), dim3(256), args, 0, 0));
+        RCHK(fix_geq(challenges + 4 * r));
+        mem.release(d_dense);
+        d_dense = d_out; d_col = d_ocol; d_start = s1; d_colh = h1;
+        length = total;
+        RCHK(chip_layouts());
+    }
+
+    // ---- the folded values zerocheck() demultiplexes (prover.rs:2692-2702): 4 entries per non-empty column after the last fold
+    size_t nonempty = 0;
+    for (uint32_t h : input_colh) nonempty += h != 0;
+    if (2ull * length != 4 * nonempty) return "ref_zerocheck: the folded trace does not hold 4 entries per non-empty column";
+    std::vector<uint32_t> fin(8ull * length);   // 2 * length ext elements
+    RCHK(cudaMemcpy(fin.data(), d_dense, fin.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t c = 0, idx = 0; c < n_cols; c++) {
+        if (input_colh[c]) {
+            memcpy(o + 4 * c, &fin[4 * idx], 16);
+            idx += 4;
+        } else {
+            memset(o + 4 * c, 0, 16);
+        }
+    }
+    return nullptr;
+}
 
 }  // extern "C"
 

@@ -95,6 +95,12 @@ struct ZerocheckResult {
     std::vector<ChipOpened> opened;  // in chip order
 };
 
+// tests only: the inputs of this thread's last zerocheck_prove (tests/test_ref_zerocheck.py replays them through the reference's
+// kernels): the constraint batching challenge alpha, the opening batching challenge gamma, lambda, the claimed sum and the round
+// challenges in round order
+struct ZerocheckProveInputs { EF alpha, gamma, lambda, claimed_sum; std::vector<EF> challenges; };
+static inline ZerocheckProveInputs& zerocheck_last_inputs() { static thread_local ZerocheckProveInputs v; return v; }
+
 namespace zc_detail {
 struct State {
     size_t h, mw, pw;
@@ -211,6 +217,8 @@ static inline ZerocheckResult zerocheck_prove(const std::vector<ZcChip>& chips, 
     ZerocheckResult res;
     PartialSumcheckProof& pf = res.proof;
     for (const EF& c : claims) pf.claimed_sum = pf.claimed_sum * lambda + c;
+    ZerocheckProveInputs& rec = zerocheck_last_inputs();
+    rec = {batching_challenge, gkr_challenge, lambda, pf.claimed_sum, {}};
     std::vector<EF> round_claims = claims;
     std::vector<Uni> unis(chips.size());
     for (unsigned rd = 0; rd < max_log_rows; rd++) {
@@ -228,6 +236,7 @@ static inline ZerocheckResult zerocheck_prove(const std::vector<ZcChip>& chips, 
         ch.observe_ext_slice(rlc.c.data(), rlc.c.size());
         pf.polys.push_back(rlc);
         EF alpha = ch.sample_ext();
+        rec.challenges.push_back(alpha);
         pf.point.insert(pf.point.begin(), alpha);
         for (size_t k = 0; k < chips.size(); k++) {
             State& s = st[k];

@@ -72,6 +72,48 @@ def n_interactions(blob):
     return total
 
 
+def oracle_zerocheck(rng, blob, heights, mains, preps, pv, mlr):
+    """the oracle's zerocheck proof of a machine at a random GKR point from a random transcript state, both drawn from rng.
+    -> (GKR point, challenger state before the proof, the column openings at the GKR point, proof words, challenger state after it)"""
+    gp = O.rand_field(rng, (mlr, 4))
+    ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
+    st0 = ch.st.copy()
+    openings, owords = O.zerocheck_prove_verify(blob, heights, mains, preps, pv, mlr, gp, ch)
+    return gp, st0, openings, owords, ch.st.copy()
+
+
+def _ext_mul(a, b):
+    out = np.zeros(4, np.uint32)
+    O.lib().orc_ext_mul(O.ptr(np.ascontiguousarray(a, dtype=np.uint32)), O.ptr(np.ascontiguousarray(b, dtype=np.uint32)), O.ptr(out))
+    return out
+
+
+def _ext_add(a, b):
+    return ((a.astype(np.uint64) + b) % O.P).astype(np.uint32)
+
+
+def product_zerocheck(lib, mach, heights, mains, preps, pv, gp, st0, openings):
+    """the product's zerocheck (Lib.zerocheck) on the inputs of oracle_zerocheck: alpha and gamma sampled from st0 as the oracle samples
+    them, the per-chip claims sum_j gamma^(j+1) * opening_j (main then prep).  -> (proof words, challenger state after the proof)"""
+    import torch
+    from sp1_b200.lib import HostChallenger
+    hc = HostChallenger(st0.copy())
+    alpha = hc.sample(4); gamma = hc.sample(4)
+    claims, k = [], 0
+    for m, p in zip(mains, preps):
+        w = m.shape[0] + (p.shape[0] if p is not None else 0)
+        acc, g = np.zeros(4, np.uint32), gamma.copy()
+        for j in range(w):
+            acc = _ext_add(acc, _ext_mul(openings[k + j], g))
+            g = _ext_mul(g, gamma)
+        claims.append(acc); k += w
+    d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
+    d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
+    torch.cuda.synchronize()
+    words = lib.zerocheck(mach, heights, d_mains, d_preps, pv, gp, alpha, gamma, np.stack(claims), hc.st)
+    return words, hc.st
+
+
 def dense_main(mains):
     """the main traces back to back (the prove_shard input)"""
     parts = [np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]

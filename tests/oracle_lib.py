@@ -342,3 +342,16 @@ def gkr_last_inputs():
         layers.append((lam, claim, w[o:o + 4 * m].reshape(m, 4))); o += 4 * m
     assert o == n
     return alpha, beta, layers
+
+
+def zerocheck_last_inputs():
+    """the inputs of this thread's last oracle zerocheck prove: -> (alpha [4], gamma [4], lambda [4], claimed sum [4], the round
+    challenges in round order [n, 4])"""
+    f = lib().orc_zerocheck_last_inputs
+    f.restype = C.c_uint64
+    n = f(None, C.c_uint64(0))
+    w = np.zeros(n, np.uint32)
+    f(ptr(w), C.c_uint64(n))
+    m = int(w[16])
+    assert n == 17 + 4 * m
+    return w[0:4], w[4:8], w[8:12], w[12:16], w[17:].reshape(m, 4)

@@ -34,7 +34,7 @@ def lib():
         for n in ("ref_init", "ref_malloc", "ref_free", "ref_h2d", "ref_d2h", "ref_field_op", "ref_ext_op", "ref_permute", "ref_hash",
                   "ref_compress", "ref_merkle_tree", "ref_batch_coset_dft", "ref_batch", "ref_fold_mle_ext", "ref_fix_last_variable_ext",
                   "ref_partial_lagrange_ext", "ref_grind", "ref_challenger_script", "ref_gkr_populate", "ref_zerocheck_node_sums",
-                  "ref_jagged_sumcheck", "ref_logup_gkr"):
+                  "ref_jagged_sumcheck", "ref_logup_gkr", "ref_zerocheck"):
             getattr(L, n).restype = C.c_char_p
         _chk(L.ref_init())
         _lib = L
@@ -392,6 +392,35 @@ def logup_gkr(chip_inters, heights, mains, preps, alpha, betas, mlr, lambdas, po
                                                                             "arg_indices", "is_send")],
                              _p(alpha), _p(betas), C.c_uint32(betas.size // 4), C.c_uint32(mlr), _p(lam), _p(pts), _p(chs), C.c_uint64(pts.size),
                              _p(out), C.c_uint64(out.size)))
+    return out
+
+
+def zerocheck_raw_words(n_chips, n_cols, mlr):
+    """the number of words ref_zerocheck returns: the padded-row adjustment of every chip, the 16 totals of the fused first two rounds,
+    3 totals per later round and one value per column of the jagged trace (ext each)"""
+    return 4 * (n_chips + 16 + 3 * (mlr - 2) + n_cols)
+
+
+def zerocheck(blob, heights, mains, preps, prep_pad_rows, pv, alpha_pows, gkr_pows, lambda_pows, mlr, zeta, challenges):
+    """the reference's zerocheck kernels (ref_zerocheck) with the host tables and challenges supplied: mains / preps [w, h] column-major
+    (preps[k] None without preprocessed columns); alpha_pows, gkr_pows, lambda_pows, zeta, challenges [*, 4].  -> the raw words (see
+    ref_launcher.cu)"""
+    main_parts = [np.ascontiguousarray(m, np.uint32).reshape(-1) for m in mains]
+    prep_parts = [np.ascontiguousarray(p, np.uint32).reshape(-1) if p is not None else np.zeros(0, np.uint32) for p in preps]
+    main_off = np.ascontiguousarray(np.cumsum([0] + [m.size for m in main_parts])[:-1], np.uint64)
+    prep_off = np.ascontiguousarray(np.cumsum([0] + [p.size for p in prep_parts])[:-1], np.uint64)
+    mainf = _arr(np.concatenate(main_parts), np.uint32)
+    prepf = _arr(np.concatenate(prep_parts), np.uint32)
+    n_cols = sum(m.shape[0] for m in mains) + sum(p.shape[0] for p in preps if p is not None) + 1
+    out = np.zeros(zerocheck_raw_words(len(heights), n_cols, mlr), np.uint32)
+    t = {k: np.ascontiguousarray(np.asarray(v, np.uint32).reshape(-1, 4)) for k, v in
+         dict(a=alpha_pows, g=gkr_pows, l=lambda_pows, z=zeta, c=challenges).items()}
+    pv = _arr(pv, np.uint32)
+    _chk(lib().ref_zerocheck(_p(np.ascontiguousarray(blob, np.uint32)), _ptr(np.ascontiguousarray(heights, np.uint64)), _p(mainf), _ptr(main_off),
+                             C.c_uint64(sum(m.size for m in main_parts)), _p(prepf), _ptr(prep_off), C.c_uint64(sum(p.size for p in prep_parts)),
+                             C.c_uint32(prep_pad_rows), _p(pv), C.c_uint32(len(pv)), _p(_arr(t["a"].reshape(-1), np.uint32)), C.c_uint32(t["a"].shape[0]),
+                             _p(_arr(t["g"].reshape(-1), np.uint32)), C.c_uint32(t["g"].shape[0]), _p(t["l"].reshape(-1)), C.c_uint32(mlr),
+                             _p(t["z"].reshape(-1)), _p(t["c"].reshape(-1)), _p(out), C.c_uint64(out.size)))
     return out
 
 

@@ -3,21 +3,10 @@
 import numpy as np
 import pytest
 
-from tests import oracle_lib as O
-from tests.machines import Chip, spec_machine, workload_machine
+from tests.machines import Chip, oracle_zerocheck, product_zerocheck, spec_machine, workload_machine
 from tests.test_oracle import _synth_machine
 
 pytestmark = pytest.mark.gpu
-
-
-def _ext_mul(a, b):
-    out = np.zeros(4, np.uint32)
-    O.lib().orc_ext_mul(O.ptr(np.ascontiguousarray(a, dtype=np.uint32)), O.ptr(np.ascontiguousarray(b, dtype=np.uint32)), O.ptr(out))
-    return out
-
-
-def _ext_add(a, b):
-    return ((a.astype(np.uint64) + b) % O.P).astype(np.uint32)
 
 
 @pytest.mark.parametrize("spec,mlr", [
@@ -49,31 +38,12 @@ def test_zerocheck_matches_oracle(spec, mlr):
 
 
 def _check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr):
-    import torch
-    from sp1_b200.lib import HostChallenger
-    gp = O.rand_field(rng, (mlr, 4))
-    ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
-    och = ch.clone()
-    openings, owords = O.zerocheck_prove_verify(blob, heights, mains, preps, pv, mlr, gp, och)
-    hc = HostChallenger(ch.st.copy())
-    alpha = hc.sample(4); gamma = hc.sample(4)
-    # claims = sum_j gamma^(j+1) * opening_j, chip by chip (main then prep), from the openings at the gkr point
-    claims, k = [], 0
-    for m, p in zip(mains, preps):
-        w = m.shape[0] + (p.shape[0] if p is not None else 0)
-        acc, g = np.zeros(4, np.uint32), gamma.copy()
-        for j in range(w):
-            acc = _ext_add(acc, _ext_mul(openings[k + j], g))
-            g = _ext_mul(g, gamma)
-        claims.append(acc); k += w
-    d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
-    d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
-    torch.cuda.synchronize()
-    words = lib.zerocheck(mach, heights, d_mains, d_preps, pv, gp, alpha, gamma, np.stack(claims), hc.st)
+    gp, st0, openings, owords, ost = oracle_zerocheck(rng, blob, heights, mains, preps, pv, mlr)
+    words, st = product_zerocheck(lib, mach, heights, mains, preps, pv, gp, st0, openings)
     assert words.size == owords.size, (words.size, owords.size)
     bad = np.nonzero(words != owords)[0]
     assert bad.size == 0, f"first differing words {bad[:8]} of {words.size}"
-    assert (hc.st == och.st).all()
+    assert (st == ost).all()
 
 
 # calibrated chips: constraint counts from the workloads' chip_stats.json range (up to 9 per group), filler main columns, several
