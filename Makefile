@@ -18,4 +18,4 @@ golden:
 clean:
 	$(MAKE) -C sp1_b200/csrc clean
 	$(MAKE) -C examples clean
-	rm -f oracle/liboracle.so
+	rm -f oracle/liboracle.so oracle/libdebugoracle.so

@@ -259,6 +259,33 @@ sp1b200_err sp1b200_setup_and_prove_shard(sp1b200_ctx* ctx, const sp1b200_machin
                                           sp1b200_jagged_round** prep_round_out, uint32_t* h_proof, uint64_t proof_cap_words,
                                           uint64_t* h_proof_words);
 
+/* ---- shard checks (the reference's cfg(sp1_debug_constraints) build; nothing of the transcript is touched) -------------------------
+ * Both take the shard inputs of sp1b200_prove_shard (same validation: prep_round = the round committed at setup or NULL, its heights
+ * equal to the main heights, every height <= 2^max_log_row_count; main_dense_any = host pointer, device pointer or upload slot), so a
+ * shim can call them right before proving.  A failing check is not an error: the call returns NULL and writes the report.  Errors
+ * are malformed input and out_cap_words too small (*h_out_words then holds the size needed; the context stays usable).  Every
+ * device allocation comes from the context's pool and is returned before the call ends.  Field words are Montgomery words. */
+
+/* debug_constraints_all_chips (crates/hypercube/src/debug.rs:27-130): every real row 0 .. h-1 of every chip (height 0 = skipped)
+ * through the chip's constraints in the base field, over main columns, preprocessed columns and public values.  A constraint is
+ * named by its assert's alpha index (alpha index i <-> alpha^(n_constraints-1-i): the constraint's position in the chip's eval order).
+ * Report words: n_failing_chips | per failing chip, ascending: chip | n_failing_rows | n_listed = min(n_failing_rows,
+ * max_rows_per_chip) | per listed row (the lowest failing rows, ascending): row | n_failed | failed constraint indices, ascending. */
+sp1b200_err sp1b200_debug_constraints(sp1b200_ctx* ctx, const sp1b200_machine* machine, sp1b200_jagged_round* prep_round,
+                                      const uint32_t* main_dense_any, const uint64_t* h_heights, const uint32_t* h_public_values,
+                                      uint32_t n_public_values, uint32_t max_rows_per_chip, uint32_t* h_out, uint64_t out_cap_words,
+                                      uint64_t* h_out_words);
+
+/* debug_interactions_with_all_chips (crates/hypercube/src/lookup/debug.rs:48-200): over rows 0 .. h-1 and the (row, interaction)
+ * pairs with a non-zero multiplicity, the net multiplicity (sends - receives, in F) of every distinct key (kind = arg_index,
+ * n_values, values); a key is unbalanced when its net is not zero.  Keys are listed in order of first occurrence, records ranked by
+ * (chip, row, interaction index in the blob: sends, then receives); the chip list holds every chip with a record of the key.
+ * Report words: n_unbalanced (u64: lo, hi) | n_listed = min(n_unbalanced, max_keys) | per listed key: kind | n_values |
+ * values[n_values] | net | first chip | first interaction index | first row | n_chips | per chip, ascending: chip | net. */
+sp1b200_err sp1b200_debug_interactions(sp1b200_ctx* ctx, const sp1b200_machine* machine, sp1b200_jagged_round* prep_round,
+                                       const uint32_t* main_dense_any, const uint64_t* h_heights, uint32_t max_keys, uint32_t* h_out,
+                                       uint64_t out_cap_words, uint64_t* h_out_words);
+
 /* ---- ShardProof wire format (SURVEY 8f.4) ----------------------------------------------------------------------------------------
  * The reference moves shard proofs between prover workers, the recursion tree and the verifier as bincode(ShardProof)
  * (crates/hypercube/src/verifier/proof.rs:47-61 and the nested types listed in csrc/wire.cu; bincode 1.3 default configuration:

@@ -189,9 +189,67 @@ class AirProver {
         return out;
     }
 
+    // The reference's cfg(sp1_debug_constraints) checks on the inputs of prove_shard_with_pk (nothing of the transcript is touched).
+    // debug_constraints: chips whose real rows violate a constraint, each with its number of failing rows and the failed constraint
+    // indices of its lowest max_rows failing rows (crates/hypercube/src/debug.rs:27-130; the reference prints three rows per chip).
+    struct FailingRow { uint32_t row; std::vector<uint32_t> constraints; };
+    struct FailingChip { uint32_t chip; uint32_t n_failing_rows; std::vector<FailingRow> rows; };
+    std::vector<FailingChip> debug_constraints(const ProvingKey& pk, const uint32_t* main_dense_any, const std::vector<uint64_t>& heights,
+                                               const std::vector<uint32_t>& public_values, uint32_t max_rows = 3) {
+        if (heights.size() != chips_.size()) throw Error("debug_constraints: one height per chip expected");
+        std::vector<uint32_t> w = report([&](uint32_t* out, uint64_t cap, uint64_t* n) {
+            return sp1b200_debug_constraints(ctx_, machine_, pk.round_, main_dense_any, heights.data(), public_values.data(),
+                                             (uint32_t)public_values.size(), max_rows, out, cap, n);
+        });
+        std::vector<FailingChip> out(w[0]);
+        size_t p = 1;
+        for (FailingChip& c : out) {
+            c.chip = w[p]; c.n_failing_rows = w[p + 1]; c.rows.resize(w[p + 2]); p += 3;
+            for (FailingRow& r : c.rows) { r.row = w[p]; r.constraints.assign(w.begin() + p + 2, w.begin() + p + 2 + w[p + 1]); p += 2 + w[p + 1]; }
+        }
+        return out;
+    }
+    // debug_interactions: the keys (kind, values) whose sends and receives do not balance, in order of first occurrence, with every
+    // chip that has a record of the key (crates/hypercube/src/lookup/debug.rs:48-200)
+    struct UnbalancedKey {
+        uint32_t kind; std::vector<uint32_t> values; uint32_t net;
+        uint32_t first_chip, first_interaction, first_row;
+        std::vector<std::pair<uint32_t, uint32_t>> chips;   // (chip, net)
+    };
+    struct InteractionReport { uint64_t n_unbalanced = 0; std::vector<UnbalancedKey> keys; };
+    InteractionReport debug_interactions(const ProvingKey& pk, const uint32_t* main_dense_any, const std::vector<uint64_t>& heights,
+                                         uint32_t max_keys = 16) {
+        if (heights.size() != chips_.size()) throw Error("debug_interactions: one height per chip expected");
+        std::vector<uint32_t> w = report([&](uint32_t* out, uint64_t cap, uint64_t* n) {
+            return sp1b200_debug_interactions(ctx_, machine_, pk.round_, main_dense_any, heights.data(), max_keys, out, cap, n);
+        });
+        InteractionReport r;
+        r.n_unbalanced = w[0] | ((uint64_t)w[1] << 32);
+        r.keys.resize(w[2]);
+        size_t p = 3;
+        for (UnbalancedKey& k : r.keys) {
+            k.kind = w[p]; k.values.assign(w.begin() + p + 2, w.begin() + p + 2 + w[p + 1]); p += 2 + w[p + 1];
+            k.net = w[p]; k.first_chip = w[p + 1]; k.first_interaction = w[p + 2]; k.first_row = w[p + 3];
+            k.chips.resize(w[p + 4]); p += 5;
+            for (auto& c : k.chips) { c = {w[p], w[p + 1]}; p += 2; }
+        }
+        return r;
+    }
+
     sp1b200_ctx* context() const { return ctx_; }
 
   private:
+    // a report call, retried once with the capacity the library asks for
+    template <class Call>
+    static std::vector<uint32_t> report(Call call) {
+        std::vector<uint32_t> w(1 << 16);
+        uint64_t n = 0;
+        sp1b200_err e = call(w.data(), w.size(), &n);
+        if (e && n > w.size()) { w.resize(n); e = call(w.data(), w.size(), &n); }
+        check(e);
+        w.resize(n);
+        return w;
+    }
     static constexpr uint64_t kCapWords = 1ull << 24;
     sp1b200_params params_;
     sp1b200_ctx* ctx_ = nullptr;

@@ -14,12 +14,20 @@
 //    thousand values, which the host transcript driver folds directly.
 #include "ctx.cuh"
 #include "challenger.cuh"
+#include "debug_fp.cuh"
 #include "hostfield.hpp"
 #include "kb31.cuh"
 #include "sumcheck.cuh"
 #include <algorithm>
+#include <map>
 #include <memory>
 #include <vector>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/discard_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 
 #include "machine.cuh"
 
@@ -494,6 +502,163 @@ const uint32_t* parse_vcol(const uint32_t* b, const uint32_t* end, HostInteracti
     return b;
 }
 
+// ---- interaction check (debug_interactions_with_all_chips, crates/hypercube/src/lookup/debug.rs:48-200) ------------------------
+// A record is one (chip, row, interaction) with its signed multiplicity (sends +, receives -); its rank (chip, row, interaction
+// index) is its position in the reference's iteration order.  Records are sorted by the fingerprint of their key (debug_fp.cuh),
+// each run of equal fingerprints is summed, and every record of a run is compared with its predecessor by FULL key: a run that
+// mixes keys is flagged and resolved on the host.
+struct DbgChip { const uint32_t* main; const uint32_t* prep; uint64_t h; uint32_t rank0, I, inter0, chip; };  // chips with records
+
+__device__ __forceinline__ uint32_t dbg_vcol(const VColDev& v, const TermDev* __restrict__ terms, const DbgChip& c, uint64_t row) {
+    uint32_t a = v.constant;
+    for (uint32_t q = 0; q < v.n_terms; q++) {
+        const TermDev tm = terms[v.term_start + q];
+        a = kb::add(a, kb::mul(__ldg((tm.source == LEAF_MAIN ? c.main : c.prep) + (uint64_t)tm.col * c.h + row), tm.weight));
+    }
+    return a;
+}
+struct DbgRec { DbgChip c; InterDev in; uint32_t row, t; };  // t = index into the chip table
+__device__ __forceinline__ DbgRec dbg_decode(const DbgChip* __restrict__ chips, int n, const InterDev* __restrict__ inter, uint32_t rank) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (chips[mid].rank0 <= rank) lo = mid; else hi = mid - 1; }
+    DbgRec r;
+    r.t = (uint32_t)lo; r.c = chips[lo];
+    const uint32_t local = rank - r.c.rank0;
+    r.row = local / r.c.I;
+    r.in = inter[r.c.inter0 + (local - r.row * r.c.I)];
+    return r;
+}
+__device__ __forceinline__ uint32_t dbg_signed_mult(const DbgRec& r, const VColDev* __restrict__ vcols, const TermDev* __restrict__ terms) {
+    const uint32_t x = dbg_vcol(vcols[r.in.vcol_start], terms, r.c, r.row);
+    return r.in.is_send ? x : kb::neg(x);
+}
+
+// per rank: sort key = fingerprint of the record's key (dbgfp::NONE when its multiplicity is zero), value = the rank; counts[0] += live
+__global__ void __launch_bounds__(256) gkr_dbg_records_kernel(const DbgChip* __restrict__ chips, int n_chips, const InterDev* __restrict__ inter,
+                                                              const VColDev* __restrict__ vcols, const TermDev* __restrict__ terms, uint32_t n,
+                                                              uint64_t* __restrict__ keys, uint32_t* __restrict__ ranks, uint32_t* __restrict__ counts) {
+    const uint32_t rank = blockIdx.x * blockDim.x + threadIdx.x;
+    bool live = false;
+    if (rank < n) {
+        const DbgRec r = dbg_decode(chips, n_chips, inter, rank);
+        uint64_t key = dbgfp::NONE;
+        if (dbg_signed_mult(r, vcols, terms)) {
+            live = true;
+            dbgfp::Acc f;
+            f.head(r.in.arg_index, r.in.n_values);
+            for (uint32_t q = 0; q < r.in.n_values; q++) f.value(q, dbg_vcol(vcols[r.in.vcol_start + 1 + q], terms, r.c, r.row));
+            key = f.get();
+        }
+        keys[rank] = key; ranks[rank] = rank;
+    }
+    const uint32_t bits = __ballot_sync(0xffffffffu, live);
+    if ((threadIdx.x & 31) == 0 && bits) atomicAdd(counts, (uint32_t)__popc(bits));
+}
+
+// per sorted position i < n_live: the signed multiplicity, bit 31 set when the record's key differs from its predecessor's although
+// their fingerprints are equal
+__global__ void __launch_bounds__(256) gkr_dbg_eval_kernel(const DbgChip* __restrict__ chips, int n_chips, const InterDev* __restrict__ inter,
+                                                           const VColDev* __restrict__ vcols, const TermDev* __restrict__ terms,
+                                                           const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ranks, uint32_t n_live,
+                                                           uint32_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_live) return;
+    const DbgRec r = dbg_decode(chips, n_chips, inter, ranks[i]);
+    uint32_t bad = 0;
+    if (i > 0 && keys[i] == keys[i - 1]) {
+        const DbgRec p = dbg_decode(chips, n_chips, inter, ranks[i - 1]);
+        if (p.in.arg_index != r.in.arg_index || p.in.n_values != r.in.n_values) bad = 1;
+        for (uint32_t q = 0; !bad && q < r.in.n_values; q++)
+            bad = dbg_vcol(vcols[r.in.vcol_start + 1 + q], terms, r.c, r.row) != dbg_vcol(vcols[p.in.vcol_start + 1 + q], terms, p.c, p.row);
+    }
+    out[i] = dbg_signed_mult(r, vcols, terms) | bad << 31;
+}
+
+// run aggregate = (first position << 32) | (mixed-key bit << 31) | net multiplicity
+struct DbgRunOp {
+    __device__ __forceinline__ uint64_t operator()(uint64_t x, uint64_t y) const {
+        const uint32_t a = (uint32_t)x, b = (uint32_t)y;
+        const uint32_t lo = kb::add(a & 0x7fffffffu, b & 0x7fffffffu) | ((a | b) & 0x80000000u);
+        return ((uint64_t)min((uint32_t)(x >> 32), (uint32_t)(y >> 32)) << 32) | lo;
+    }
+};
+struct DbgPosValue {
+    const uint32_t* v;
+    __device__ __forceinline__ uint64_t operator()(uint32_t i) const { return ((uint64_t)i << 32) | v[i]; }
+};
+struct DbgNonZero {
+    __device__ __forceinline__ bool operator()(uint32_t x) const { return x != 0; }
+};
+
+// per run: a mixed run goes to `mixed` (counts[1]); an unbalanced one is flagged at its first record's rank with run index + 1 (counts[0])
+__global__ void __launch_bounds__(256) gkr_dbg_flag_kernel(const uint64_t* __restrict__ agg, uint32_t n_runs, const uint32_t* __restrict__ ranks,
+                                                           uint32_t* __restrict__ flags, uint32_t* __restrict__ counts, uint32_t* __restrict__ mixed,
+                                                           uint32_t mixed_cap) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_runs) return;
+    const uint64_t a = agg[r];
+    const uint32_t lo = (uint32_t)a;
+    if (lo >> 31) {
+        const uint32_t j = atomicAdd(counts + 1, 1u);
+        if (j < mixed_cap) mixed[j] = r;
+    } else if (lo) {
+        flags[ranks[a >> 32]] = r + 1;
+        atomicAdd(counts, 1u);
+    }
+}
+
+__device__ __forceinline__ void dbg_run_extent(const uint64_t* agg, uint32_t n_runs, uint32_t n_live, uint32_t r, uint32_t& s, uint32_t& e) {
+    s = (uint32_t)(agg[r] >> 32);
+    e = r + 1 < n_runs ? (uint32_t)(agg[r + 1] >> 32) : n_live;
+}
+
+// one block per listed run (runs1[b] = run index + 1): out[b * stride ..] = kind, n_values, values[255], first rank, then per chip-table
+// entry (net, number of records)
+__global__ void __launch_bounds__(256) gkr_dbg_key_kernel(const DbgChip* __restrict__ chips, int n_chips, const InterDev* __restrict__ inter,
+                                                          const VColDev* __restrict__ vcols, const TermDev* __restrict__ terms,
+                                                          const uint64_t* __restrict__ agg, uint32_t n_runs, uint32_t n_live,
+                                                          const uint32_t* __restrict__ ranks, const uint32_t* __restrict__ runs1,
+                                                          uint32_t* __restrict__ out, uint32_t stride) {
+    extern __shared__ __align__(16) unsigned char dbg_smem[];
+    unsigned long long* sums = reinterpret_cast<unsigned long long*>(dbg_smem);
+    uint32_t* cnt = reinterpret_cast<uint32_t*>(sums + n_chips);
+    for (int c = threadIdx.x; c < n_chips; c += blockDim.x) { sums[c] = 0; cnt[c] = 0; }
+    __syncthreads();
+    uint32_t s, e;
+    dbg_run_extent(agg, n_runs, n_live, runs1[blockIdx.x] - 1, s, e);
+    for (uint32_t pos = s + threadIdx.x; pos < e; pos += blockDim.x) {
+        const DbgRec r = dbg_decode(chips, n_chips, inter, ranks[pos]);
+        atomicAdd(&sums[r.t], (unsigned long long)dbg_signed_mult(r, vcols, terms));
+        atomicAdd(&cnt[r.t], 1u);
+    }
+    __syncthreads();
+    uint32_t* o = out + (uint64_t)blockIdx.x * stride;
+    if (threadIdx.x == 0) {
+        const DbgRec r = dbg_decode(chips, n_chips, inter, ranks[s]);
+        o[0] = r.in.arg_index; o[1] = r.in.n_values;
+        for (uint32_t q = 0; q < r.in.n_values; q++) o[2 + q] = dbg_vcol(vcols[r.in.vcol_start + 1 + q], terms, r.c, r.row);
+        o[257] = ranks[s];
+    }
+    for (int c = threadIdx.x; c < n_chips; c += blockDim.x) { o[258 + 2 * c] = (uint32_t)(sums[c] % kb::P); o[259 + 2 * c] = cnt[c]; }
+}
+
+// every record of the mixed runs (one block per run) as words {rank, signed multiplicity, kind, n_values, values}; used[0] = words needed
+__global__ void __launch_bounds__(256) gkr_dbg_collect_kernel(const DbgChip* __restrict__ chips, int n_chips, const InterDev* __restrict__ inter,
+                                                              const VColDev* __restrict__ vcols, const TermDev* __restrict__ terms,
+                                                              const uint64_t* __restrict__ agg, uint32_t n_runs, uint32_t n_live,
+                                                              const uint32_t* __restrict__ ranks, const uint32_t* __restrict__ mixed,
+                                                              uint32_t* __restrict__ out, uint32_t* __restrict__ used, uint32_t cap) {
+    uint32_t s, e;
+    dbg_run_extent(agg, n_runs, n_live, mixed[blockIdx.x], s, e);
+    for (uint32_t pos = s + threadIdx.x; pos < e; pos += blockDim.x) {
+        const DbgRec r = dbg_decode(chips, n_chips, inter, ranks[pos]);
+        const uint32_t nw = 4 + r.in.n_values, at = atomicAdd(used, nw);
+        if ((uint64_t)at + nw > cap) continue;
+        out[at] = ranks[pos]; out[at + 1] = dbg_signed_mult(r, vcols, terms); out[at + 2] = r.in.arg_index; out[at + 3] = r.in.n_values;
+        for (uint32_t q = 0; q < r.in.n_values; q++) out[at + 4 + q] = dbg_vcol(vcols[r.in.vcol_start + 1 + q], terms, r.c, r.row);
+    }
+}
+
 }  // namespace
 
 // parses the interaction section that follows the AIR records in the machine blob (called by sp1b200_machine_create);
@@ -538,3 +703,172 @@ sp1b200_err sp1b200_logup_gkr(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
 }
 
 #include "gkr_driver.inc"
+
+// debug_interactions_with_all_chips (crates/hypercube/src/lookup/debug.rs:48-200) on the device; report words as
+// sp1b200_debug_interactions (include/sp1b200.h).  Device memory: 24 B per (row, interaction) of the shard (two 8-byte sort-key and
+// two 4-byte rank buffers, reused for the run sums and flags) plus the sort's temporary storage.
+sp1b200_err sp1b200_debug_interactions_device(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint64_t* h_heights, const uint32_t* const* d_main,
+                                              const uint32_t* const* d_prep, uint32_t max_keys, std::vector<uint32_t>& words) {
+    const HostInteractions& H = *static_cast<const HostInteractions*>(m->interactions);
+    const size_t nch = m->chips.size();
+    cudaStream_t st = ctx->stream;
+    std::vector<DbgChip> tab;
+    std::vector<InterDev> flat;
+    uint64_t n_total = 0;
+    for (size_t c = 0; c < nch; c++) {
+        const uint32_t I = (uint32_t)H.per_chip[c].size();
+        if (h_heights[c] && I)
+            tab.push_back(DbgChip{d_main[c], m->chips[c].prep_w ? d_prep[c] : nullptr, h_heights[c], (uint32_t)n_total, I, (uint32_t)flat.size(), (uint32_t)c});
+        flat.insert(flat.end(), H.per_chip[c].begin(), H.per_chip[c].end());
+        n_total += h_heights[c] * I;
+        if (n_total > 0x7fffffffu) return sp1b200_set_error("debug_interactions: more than 2^31 - 1 (row, interaction) pairs in the shard");
+    }
+    struct Key { uint32_t first_rank; std::vector<uint32_t> w; };   // w: kind .. the per-chip list, without the first-occurrence words
+    std::vector<Key> keys;
+    uint64_t n_unbalanced = 0;
+    auto emit = [&]() {
+        // merge the two sources in first-occurrence order; first occurrence = (chip, interaction, row) words from the rank
+        std::sort(keys.begin(), keys.end(), [](const Key& a, const Key& b) { return a.first_rank < b.first_rank; });
+        const size_t n_listed = std::min<uint64_t>(keys.size(), max_keys);
+        words = {(uint32_t)n_unbalanced, (uint32_t)(n_unbalanced >> 32), (uint32_t)n_listed};
+        for (size_t j = 0; j < n_listed; j++) {
+            const Key& k = keys[j];
+            size_t t = 0;
+            while (t + 1 < tab.size() && tab[t + 1].rank0 <= k.first_rank) t++;
+            const uint32_t local = k.first_rank - tab[t].rank0, row = local / tab[t].I;
+            const uint32_t nv = k.w[1];
+            words.insert(words.end(), k.w.begin(), k.w.begin() + 3 + nv);            // kind, n_values, values, net
+            words.push_back(tab[t].chip); words.push_back(local - row * tab[t].I); words.push_back(row);
+            words.insert(words.end(), k.w.begin() + 3 + nv, k.w.end());              // n_chips, per chip (chip, net)
+        }
+    };
+    if (!n_total) { emit(); return nullptr; }
+    DevFree mem(ctx);
+    PhaseTimer t_all(ctx, "debug_interactions.total");
+    const uint32_t n = (uint32_t)n_total;
+    DbgChip* d_tab; InterDev* d_inter; VColDev* d_vcols; TermDev* d_terms; uint32_t* d_counts;
+    SP1_TRY(mem.alloc((void**)&d_tab, tab.size() * sizeof(DbgChip)));
+    SP1_TRY(mem.alloc((void**)&d_inter, flat.size() * sizeof(InterDev)));
+    SP1_TRY(mem.alloc((void**)&d_vcols, H.vcols.size() * sizeof(VColDev)));
+    SP1_TRY(mem.alloc((void**)&d_terms, (H.terms.size() + 1) * sizeof(TermDev)));
+    SP1_TRY(mem.alloc((void**)&d_counts, 8 * 4));
+    SP1_CUDA(cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(DbgChip), cudaMemcpyHostToDevice, st));
+    SP1_CUDA(cudaMemcpyAsync(d_inter, flat.data(), flat.size() * sizeof(InterDev), cudaMemcpyHostToDevice, st));
+    SP1_CUDA(cudaMemcpyAsync(d_vcols, H.vcols.data(), H.vcols.size() * sizeof(VColDev), cudaMemcpyHostToDevice, st));
+    if (!H.terms.empty()) SP1_CUDA(cudaMemcpyAsync(d_terms, H.terms.data(), H.terms.size() * sizeof(TermDev), cudaMemcpyHostToDevice, st));
+    SP1_CUDA(cudaMemsetAsync(d_counts, 0, 8 * 4, st));
+    const int nt = (int)tab.size();
+    // counts: [0] unbalanced runs, [1] mixed runs, [2] live records, [3] runs, [4] words of the mixed-run records
+    uint64_t *d_k0, *d_k1; uint32_t *d_v0, *d_v1;
+    SP1_TRY(mem.alloc((void**)&d_k0, (size_t)n * 8)); SP1_TRY(mem.alloc((void**)&d_k1, (size_t)n * 8));
+    SP1_TRY(mem.alloc((void**)&d_v0, (size_t)n * 4)); SP1_TRY(mem.alloc((void**)&d_v1, (size_t)n * 4));
+    SP1_LAUNCH(ctx, gkr_dbg_records_kernel, blocks_for(n), 256, 0, d_tab, nt, d_inter, d_vcols, d_terms, n, d_k0, d_v0, d_counts + 2);
+    cub::DoubleBuffer<uint64_t> kb_(d_k0, d_k1);
+    cub::DoubleBuffer<uint32_t> vb_(d_v0, d_v1);
+    {
+        size_t tb = 0; void* d_tmp = nullptr;
+        SP1_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, kb_, vb_, (int)n, 0, 63, st));
+        SP1_TRY(mem.alloc(&d_tmp, tb));
+        SP1_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, kb_, vb_, (int)n, 0, 63, st));
+        ctx->launches++;
+    }
+    uint32_t cnt[8];
+    SP1_CUDA(cudaMemcpyAsync(cnt, d_counts, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+    SP1_CUDA(cudaStreamSynchronize(st));
+    const uint32_t n_live = cnt[2];
+    if (!n_live) { t_all.stop(); emit(); return nullptr; }
+    const uint64_t* d_keys = kb_.Current();
+    uint64_t* d_agg = kb_.Alternate();
+    const uint32_t* d_ranks = vb_.Current();
+    uint32_t* d_scratch = vb_.Alternate();   // signed multiplicities by position, then unbalanced-run flags by rank
+    SP1_LAUNCH(ctx, gkr_dbg_eval_kernel, blocks_for(n_live), 256, 0, d_tab, nt, d_inter, d_vcols, d_terms, d_keys, d_ranks, n_live, d_scratch);
+    {
+        auto vals = thrust::make_transform_iterator(thrust::counting_iterator<uint32_t>(0), DbgPosValue{d_scratch});
+        size_t tb = 0; void* d_tmp = nullptr;
+        SP1_CUDA(cub::DeviceReduce::ReduceByKey(nullptr, tb, d_keys, thrust::make_discard_iterator(), vals, d_agg, d_counts + 3, DbgRunOp{}, (int)n_live, st));
+        SP1_TRY(mem.alloc(&d_tmp, tb));
+        SP1_CUDA(cub::DeviceReduce::ReduceByKey(d_tmp, tb, d_keys, thrust::make_discard_iterator(), vals, d_agg, d_counts + 3, DbgRunOp{}, (int)n_live, st));
+        ctx->launches++;
+    }
+    SP1_CUDA(cudaMemcpyAsync(cnt, d_counts, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+    SP1_CUDA(cudaStreamSynchronize(st));
+    const uint32_t n_runs = cnt[3];
+    constexpr uint32_t MIXED_CAP = 4096, MIXED_WORDS = 1u << 24;
+    uint32_t* d_mixed;
+    SP1_TRY(mem.alloc((void**)&d_mixed, MIXED_CAP * 4));
+    SP1_CUDA(cudaMemsetAsync(d_scratch, 0, (size_t)n * 4, st));
+    SP1_LAUNCH(ctx, gkr_dbg_flag_kernel, blocks_for(n_runs), 256, 0, d_agg, n_runs, d_ranks, d_scratch, d_counts, d_mixed, MIXED_CAP);
+    SP1_CUDA(cudaMemcpyAsync(cnt, d_counts, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+    SP1_CUDA(cudaStreamSynchronize(st));
+    const uint32_t n_unb = cnt[0], n_mixed = cnt[1];
+    if (n_mixed > MIXED_CAP) return sp1b200_set_error("debug_interactions: %u runs of equal fingerprints mix different keys (at most %u are resolved)", n_mixed, MIXED_CAP);
+    n_unbalanced = n_unb;
+    // the first max_keys unbalanced runs in rank order: compaction of the flags (run index + 1) into the sort-key buffer, no longer needed
+    const uint32_t n_dev = std::min(n_unb, max_keys);
+    if (n_dev) {
+        uint32_t* d_sel = reinterpret_cast<uint32_t*>(kb_.Current());
+        size_t tb = 0; void* d_tmp = nullptr;
+        SP1_CUDA(cub::DeviceSelect::If(nullptr, tb, d_scratch, d_sel, d_counts + 5, (int)n, DbgNonZero{}, st));
+        SP1_TRY(mem.alloc(&d_tmp, tb));
+        SP1_CUDA(cub::DeviceSelect::If(d_tmp, tb, d_scratch, d_sel, d_counts + 5, (int)n, DbgNonZero{}, st));
+        ctx->launches++;
+        const uint32_t stride = 258 + 2 * (uint32_t)nt, batch = 1024;
+        const size_t smem = (size_t)nt * 12;
+        if (smem > 48 * 1024) return sp1b200_set_error("debug_interactions: %d chips with interactions exceed the per-key table", nt);
+        uint32_t* d_out;
+        SP1_TRY(mem.alloc((void**)&d_out, (size_t)std::min(n_dev, batch) * stride * 4));
+        std::vector<uint32_t> h((size_t)std::min(n_dev, batch) * stride);
+        for (uint32_t b0 = 0; b0 < n_dev; b0 += batch) {
+            const uint32_t nb = std::min(batch, n_dev - b0);
+            SP1_LAUNCH(ctx, gkr_dbg_key_kernel, nb, 256, smem, d_tab, nt, d_inter, d_vcols, d_terms, d_agg, n_runs, n_live, d_ranks, d_sel + b0, d_out, stride);
+            SP1_CUDA(cudaMemcpyAsync(h.data(), d_out, (size_t)nb * stride * 4, cudaMemcpyDeviceToHost, st));
+            SP1_CUDA(cudaStreamSynchronize(st));
+            for (uint32_t j = 0; j < nb; j++) {
+                const uint32_t* o = &h[(size_t)j * stride];
+                Key k; k.first_rank = o[257];
+                k.w.assign(o, o + 2 + o[1]);
+                uint64_t net = 0; uint32_t n_chips = 0;
+                for (int t = 0; t < nt; t++) if (o[259 + 2 * t]) { net += o[258 + 2 * t]; n_chips++; }
+                k.w.push_back((uint32_t)(net % kb::P)); k.w.push_back(n_chips);
+                for (int t = 0; t < nt; t++) if (o[259 + 2 * t]) { k.w.push_back(tab[t].chip); k.w.push_back(o[258 + 2 * t]); }
+                keys.push_back(std::move(k));
+            }
+        }
+    }
+    // runs whose records do not all share one key: every record back to the host, grouped by full key
+    if (n_mixed) {
+        uint32_t* d_rec;
+        SP1_TRY(mem.alloc((void**)&d_rec, (size_t)MIXED_WORDS * 4));
+        SP1_LAUNCH(ctx, gkr_dbg_collect_kernel, n_mixed, 256, 0, d_tab, nt, d_inter, d_vcols, d_terms, d_agg, n_runs, n_live, d_ranks, d_mixed, d_rec,
+                   d_counts + 4, MIXED_WORDS);
+        SP1_CUDA(cudaMemcpyAsync(cnt, d_counts, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+        SP1_CUDA(cudaStreamSynchronize(st));
+        if (cnt[4] > MIXED_WORDS) return sp1b200_set_error("debug_interactions: the runs of colliding fingerprints hold %u words of records (at most %u)", cnt[4], MIXED_WORDS);
+        std::vector<uint32_t> rec(cnt[4]);
+        SP1_CUDA(cudaMemcpyAsync(rec.data(), d_rec, (size_t)cnt[4] * 4, cudaMemcpyDeviceToHost, st));
+        SP1_CUDA(cudaStreamSynchronize(st));
+        std::vector<const uint32_t*> recs;
+        for (size_t o = 0; o < rec.size(); o += 4 + rec[o + 3]) recs.push_back(&rec[o]);
+        std::sort(recs.begin(), recs.end(), [](const uint32_t* a, const uint32_t* b) { return a[0] < b[0]; });
+        struct Group { uint32_t first_rank; uint64_t net = 0; std::map<uint32_t, uint64_t> chips; };
+        std::map<std::vector<uint32_t>, Group> groups;
+        for (const uint32_t* r : recs) {
+            size_t t = 0;
+            while (t + 1 < tab.size() && tab[t + 1].rank0 <= r[0]) t++;
+            auto it = groups.emplace(std::vector<uint32_t>(r + 2, r + 4 + r[3]), Group{r[0]}).first;
+            it->second.net += r[1];
+            it->second.chips[tab[t].chip] += r[1];
+        }
+        for (auto& [key, g] : groups) {
+            if (g.net % kb::P == 0) continue;
+            n_unbalanced++;
+            Key k; k.first_rank = g.first_rank; k.w = key;
+            k.w.push_back((uint32_t)(g.net % kb::P)); k.w.push_back((uint32_t)g.chips.size());
+            for (auto& [c, x] : g.chips) { k.w.push_back(c); k.w.push_back((uint32_t)(x % kb::P)); }
+            keys.push_back(std::move(k));
+        }
+    }
+    t_all.stop();
+    emit();
+    return nullptr;
+}

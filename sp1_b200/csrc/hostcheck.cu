@@ -2,6 +2,7 @@
 // test-suite check the exact code the kernels run (lazy-reduction bounds, half-product Montgomery forms) against the
 // oracle before any GPU time is spent.  Test support only; not part of include/sp1b200.h.
 #include "poseidon2.cuh"
+#include "debug_fp.cuh"
 #include "hostfield.hpp"
 #include "zc_lower.hpp"
 #include <cstring>
@@ -124,6 +125,11 @@ int sp1b200_hostcheck_zc_lower(const uint32_t* chip, const uint32_t* main_row, c
     }
     acc.store(out + 4);
     return (int)L.n_regs;
+}
+
+// The interaction check's key fingerprint (debug_fp.cuh): 62 bits, two linear forms over F of (kind, n_values, values)
+uint64_t sp1b200_hostcheck_fingerprint(uint32_t kind, uint32_t n_values, const uint32_t* values) {
+    return dbgfp::fingerprint(kind, n_values, values);
 }
 
 // Host transcript arithmetic (hostfield.hpp): product, inverse, and the batched-inversion Lagrange interpolation through 4 / 5 nodes

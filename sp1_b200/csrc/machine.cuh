@@ -40,3 +40,13 @@ struct sp1b200_machine {
 };
 
 void* sp1b200_parse_interactions(const uint32_t* b, const uint32_t* end, size_t n_chips, const uint32_t* widths);
+
+// the two shard checks behind sp1b200_debug_constraints / sp1b200_debug_interactions (report words as include/sp1b200.h documents):
+// zerocheck.cu and gkr.cu.  d_main[k] / d_prep[k]: device pointers to chip k's columns, column-major with stride h_heights[k].
+typedef const char* sp1b200_err;
+struct sp1b200_ctx;
+sp1b200_err sp1b200_debug_constraints_device(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint64_t* h_heights, const uint32_t* const* d_main,
+                                             const uint32_t* const* d_prep, const uint32_t* h_pv, uint32_t n_pv, uint32_t max_rows,
+                                             std::vector<uint32_t>& words);
+sp1b200_err sp1b200_debug_interactions_device(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint64_t* h_heights, const uint32_t* const* d_main,
+                                              const uint32_t* const* d_prep, uint32_t max_keys, std::vector<uint32_t>& words);

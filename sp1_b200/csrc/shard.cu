@@ -12,7 +12,87 @@
 #include <string>
 #include <vector>
 
+// Chip column pointers inside the dense main buffer (tables back to back) and the preprocessed round, with the checks that the round
+// matches the machine and the main heights.  `who` prefixes the error messages.
+static sp1b200_err chip_pointers(const char* who, const sp1b200_machine* m, const sp1b200_jagged_round* prep_round, const uint32_t* d_main_dense,
+                                 const uint64_t* h_heights, std::vector<const uint32_t*>& d_main, std::vector<const uint32_t*>& d_prep) {
+    const size_t nch = m->chips.size();
+    d_main.assign(nch, nullptr); d_prep.assign(nch, nullptr);
+    uint64_t off = 0, poff = 0; size_t pt = 0;
+    for (size_t k = 0; k < nch; k++) {
+        d_main[k] = d_main_dense + off;
+        off += h_heights[k] * m->chips[k].main_w;
+        if (m->chips[k].prep_w) {
+            if (!prep_round || pt + 2 >= prep_round->row_counts.size() + 0 || prep_round->col_counts[pt] != m->chips[k].prep_w)
+                return sp1b200_set_error("%s: preprocessed round does not match the machine at chip %zu", who, k);
+            if (prep_round->row_counts[pt] != h_heights[k])
+                return sp1b200_set_error("%s: chip %zu: preprocessed height %llu != main height %llu", who, k,
+                                         (unsigned long long)prep_round->row_counts[pt], (unsigned long long)h_heights[k]);
+            d_prep[k] = prep_round->d_dense + poff;
+            poff += prep_round->row_counts[pt] * prep_round->col_counts[pt];
+            pt++;
+        }
+    }
+    return nullptr;
+}
+
+// The inputs of sp1b200_prove_shard for the two shard checks: heights within 2^max_log_row_count, the main tables on the device
+// (a host buffer is staged through the pool; an upload slot is waited for in stream order and released after `run`), chip pointers.
+template <class Run>
+static sp1b200_err with_shard_inputs(const char* who, sp1b200_ctx* ctx, const sp1b200_machine* m, const sp1b200_jagged_round* prep_round,
+                                     const uint32_t* main_dense_any, const uint64_t* h_heights, Run run) {
+    const size_t nch = m->chips.size();
+    const uint32_t mlr = ctx->params.max_log_row_count;
+    uint64_t area = 0;
+    for (size_t k = 0; k < nch; k++) {
+        if (h_heights[k] > ((uint64_t)1 << mlr))
+            return sp1b200_set_error("%s: chip %zu has %llu rows > 2^%u", who, k, (unsigned long long)h_heights[k], mlr);
+        area += h_heights[k] * m->chips[k].main_w;
+    }
+    if (area && !main_dense_any) return sp1b200_set_error("%s: main_dense_any is NULL", who);
+    const int up_slot = sp1b200_upload_acquire(ctx, main_dense_any);
+    DevBuf main;
+    sp1b200_err e = main.in(ctx, main_dense_any, area * 4);
+    std::vector<const uint32_t*> d_main, d_prep;
+    if (!e) e = chip_pointers(who, m, prep_round, static_cast<const uint32_t*>(main.d), h_heights, d_main, d_prep);
+    if (!e) e = run(d_main, d_prep);
+    sp1b200_upload_release(ctx, up_slot);
+    return e;
+}
+
+static sp1b200_err deliver(const char* who, const std::vector<uint32_t>& words, uint32_t* h_out, uint64_t cap, uint64_t* h_words) {
+    if (h_words) *h_words = words.size();
+    if (words.size() > cap) return sp1b200_set_error("%s: report needs %zu words, capacity %llu", who, words.size(), (unsigned long long)cap);
+    if (h_out) memcpy(h_out, words.data(), words.size() * 4);
+    return nullptr;
+}
+
 extern "C" {
+
+// debug_constraints_all_chips (crates/hypercube/src/debug.rs:27-130) on the device: report words in include/sp1b200.h
+sp1b200_err sp1b200_debug_constraints(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b200_jagged_round* prep_round, const uint32_t* main_dense_any,
+                                      const uint64_t* h_heights, const uint32_t* h_pv, uint32_t n_pv, uint32_t max_rows_per_chip, uint32_t* h_out,
+                                      uint64_t out_cap_words, uint64_t* h_out_words) { SP1_DEVICE_GUARD(ctx);
+    std::vector<uint32_t> words;
+    SP1_TRY(with_shard_inputs("debug_constraints", ctx, m, prep_round, main_dense_any, h_heights,
+                              [&](const std::vector<const uint32_t*>& d_main, const std::vector<const uint32_t*>& d_prep) {
+                                  return sp1b200_debug_constraints_device(ctx, m, h_heights, d_main.data(), d_prep.data(), h_pv, n_pv,
+                                                                          max_rows_per_chip, words);
+                              }));
+    return deliver("debug_constraints", words, h_out, out_cap_words, h_out_words);
+}
+
+// debug_interactions_with_all_chips (crates/hypercube/src/lookup/debug.rs:48-200) on the device: report words in include/sp1b200.h
+sp1b200_err sp1b200_debug_interactions(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b200_jagged_round* prep_round, const uint32_t* main_dense_any,
+                                       const uint64_t* h_heights, uint32_t max_keys, uint32_t* h_out, uint64_t out_cap_words,
+                                       uint64_t* h_out_words) { SP1_DEVICE_GUARD(ctx);
+    std::vector<uint32_t> words;
+    SP1_TRY(with_shard_inputs("debug_interactions", ctx, m, prep_round, main_dense_any, h_heights,
+                              [&](const std::vector<const uint32_t*>& d_main, const std::vector<const uint32_t*>& d_prep) {
+                                  return sp1b200_debug_interactions_device(ctx, m, h_heights, d_main.data(), d_prep.data(), max_keys, words);
+                              }));
+    return deliver("debug_interactions", words, h_out, out_cap_words, h_out_words);
+}
 
 // Proof words: [5][len_0..len_4] then the sections
 //   0 main commitment (8) | 1 LogUp-GKR proof (sp1b200_logup_gkr words) | 2 zerocheck proof + opened values (sp1b200_zerocheck words) |
@@ -49,24 +129,8 @@ sp1b200_err sp1b200_prove_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b
         for (size_t i = 0; i < len; i++) ch.observe(hf::to_monty((uint8_t)chip_names[k][i]));
     }
     // chip column pointers inside the dense buffers
-    std::vector<const uint32_t*> d_main(nch, nullptr), d_prep(nch, nullptr);
-    {
-        uint64_t off = 0, poff = 0; size_t pt = 0;
-        for (size_t k = 0; k < nch; k++) {
-            d_main[k] = main_round->d_dense + off;
-            off += h_heights[k] * m->chips[k].main_w;
-            if (m->chips[k].prep_w) {
-                if (!prep_round || pt + 2 >= prep_round->row_counts.size() + 0 || prep_round->col_counts[pt] != m->chips[k].prep_w)
-                    return sp1b200_set_error("prove_shard: preprocessed round does not match the machine at chip %zu", k);
-                if (prep_round->row_counts[pt] != h_heights[k])
-                    return sp1b200_set_error("prove_shard: chip %zu: preprocessed height %llu != main height %llu", k,
-                                             (unsigned long long)prep_round->row_counts[pt], (unsigned long long)h_heights[k]);
-                d_prep[k] = prep_round->d_dense + poff;
-                poff += prep_round->row_counts[pt] * prep_round->col_counts[pt];
-                pt++;
-            }
-        }
-    }
+    std::vector<const uint32_t*> d_main, d_prep;
+    SP1_TRY(chip_pointers("prove_shard", m, prep_round, main_round->d_dense, h_heights, d_main, d_prep));
     uint32_t st[34];
     ch.store(st);
     // per-context scratch for the phase outputs, allocated once and reused by every shard proven on this context (uninitialised:

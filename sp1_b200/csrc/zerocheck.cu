@@ -81,27 +81,28 @@ __device__ __forceinline__ int find_job(const J* __restrict__ jobs, int n, uint3
 // the three evaluations run in lockstep: one instruction fetch, three independent products in flight, one pass over the
 // columns).  RF_SMEM: shared memory [reg][node][thread]; RF_LOCAL: a local array (<= 128 registers); RF_GLOBAL: the same
 // [reg][node][thread] layout in a per-block slice of a global workspace (coalesced, sized by the program's real pressure, L1/L2
-// resident for the hot registers) for programs of up to 1024 live registers.
+// resident for the hot registers) for programs of up to 1024 live registers.  NODES: values per register (3 for the sumcheck,
+// 1 for the constraint check, which evaluates each row once).
 enum { RF_SMEM = 0, RF_LOCAL = 1, RF_GLOBAL = 2 };
-template <class K, int RF> struct RegFile;
-template <class K> struct RegFile<K, RF_SMEM> {
+template <class K, int RF, int NODES = 3> struct RegFile;
+template <class K, int NODES> struct RegFile<K, RF_SMEM, NODES> {
     K* base;
     __device__ __forceinline__ RegFile(unsigned char* smem, void*, uint32_t) : base(reinterpret_cast<K*>(smem) + threadIdx.x) {}
-    __device__ __forceinline__ K get(uint32_t r, int n) const { return base[(r * 3 + n) * ZC_BLOCK]; }
-    __device__ __forceinline__ void set(uint32_t r, int n, const K& v) { base[(r * 3 + n) * ZC_BLOCK] = v; }
+    __device__ __forceinline__ K get(uint32_t r, int n) const { return base[(r * NODES + n) * ZC_BLOCK]; }
+    __device__ __forceinline__ void set(uint32_t r, int n, const K& v) { base[(r * NODES + n) * ZC_BLOCK] = v; }
 };
-template <class K> struct RegFile<K, RF_LOCAL> {
-    K regs[ZC_LOCAL_REGS * 3];
+template <class K, int NODES> struct RegFile<K, RF_LOCAL, NODES> {
+    K regs[ZC_LOCAL_REGS * NODES];
     __device__ __forceinline__ RegFile(unsigned char*, void*, uint32_t) {}
-    __device__ __forceinline__ K get(uint32_t r, int n) const { return regs[r * 3 + n]; }
-    __device__ __forceinline__ void set(uint32_t r, int n, const K& v) { regs[r * 3 + n] = v; }
+    __device__ __forceinline__ K get(uint32_t r, int n) const { return regs[r * NODES + n]; }
+    __device__ __forceinline__ void set(uint32_t r, int n, const K& v) { regs[r * NODES + n] = v; }
 };
-template <class K> struct RegFile<K, RF_GLOBAL> {
+template <class K, int NODES> struct RegFile<K, RF_GLOBAL, NODES> {
     K* base;
     __device__ __forceinline__ RegFile(unsigned char*, void* ws, uint32_t ws_regs)
-        : base(static_cast<K*>(ws) + (size_t)blockIdx.x * ws_regs * 3 * ZC_BLOCK + threadIdx.x) {}
-    __device__ __forceinline__ K get(uint32_t r, int n) const { return base[(size_t)(r * 3 + n) * ZC_BLOCK]; }
-    __device__ __forceinline__ void set(uint32_t r, int n, const K& v) { base[(size_t)(r * 3 + n) * ZC_BLOCK] = v; }
+        : base(static_cast<K*>(ws) + (size_t)blockIdx.x * ws_regs * NODES * ZC_BLOCK + threadIdx.x) {}
+    __device__ __forceinline__ K get(uint32_t r, int n) const { return base[(size_t)(r * NODES + n) * ZC_BLOCK]; }
+    __device__ __forceinline__ void set(uint32_t r, int n, const K& v) { base[(size_t)(r * NODES + n) * ZC_BLOCK] = v; }
 };
 
 // column values at the nodes t = 0, 2, 4 of row pair i:  z, z + 2d, z + 4d  with d = o - z (o = 0 past the last real row)
@@ -314,6 +315,83 @@ __global__ void __launch_bounds__(256) zc_batch0_kernel(const ZcFixJob* __restri
         sd = kb::ext_add(sd, kb::ext_mul_base(g, kb::sub(b, a)));
     }
     kb::ext_store(job.out + 4 * i, kb::ext_add(sa, kb::ext_mul(alpha, sd)));
+}
+
+// ---- constraint check (debug_constraints_all_chips, crates/hypercube/src/debug.rs:27-79) -----------------------------------
+// The lowered stream of every chip interpreted at ONE node, row by row in the base field: an assert fails when its register is not
+// zero.  Pass 1 (LISTED = false): rows 0 .. n-1, one bit per row in the chip's failing-row bitmap (one ballot per warp of 32
+// consecutive rows) and the chip's failing-row count.  Pass 2 (LISTED = true): only the rows in job.rows, each writing a bitmap of
+// the alpha indices of its failed asserts.
+struct ZcDbgJob {
+    const uint32_t* main; const uint32_t* prep; uint64_t h;   // the chip's columns, column-major with stride h
+    const uint32_t* rows;  // pass 2: the rows to re-evaluate
+    uint32_t* out;         // pass 1: failing-row bitmap; pass 2: per listed row, a bitmap of cwords words over the chip's constraints
+    uint32_t* count;       // pass 1: failing-row counter
+    uint32_t n, blk_start, nblk, chip, cwords, pad;
+};
+static_assert(sizeof(ZcDbgJob) == 72, "ZcDbgJob layout");
+
+template <int RF, bool LISTED>
+__global__ void __launch_bounds__(ZC_BLOCK) zc_debug_kernel(const ZcDbgJob* __restrict__ jobs, int n_jobs, const ChipProg* __restrict__ chips,
+                                                            const uint32_t* __restrict__ pv, void* __restrict__ ws, uint32_t ws_regs) {
+    extern __shared__ __align__(16) unsigned char zc_smem[];
+    const ZcDbgJob job = jobs[find_job(jobs, n_jobs, blockIdx.x)];
+    const ChipProg& prog = chips[job.chip];
+    RegFile<uint32_t, RF, 1> rf(zc_smem, ws, ws_regs);
+    const ZcInstr* __restrict__ zc = prog.zc;
+    const uint32_t n_zc = prog.n_zc, lane = threadIdx.x & 31;
+    // warp-uniform loop over groups of 32 consecutive work items, so that every lane reaches the ballot
+    for (uint64_t t0 = (uint64_t)(blockIdx.x - job.blk_start) * ZC_BLOCK + (threadIdx.x - lane); t0 < job.n; t0 += (uint64_t)job.nblk * ZC_BLOCK) {
+        const uint64_t t = t0 + lane;
+        bool fail = false;
+        if (t < job.n) {
+            const uint64_t row = LISTED ? job.rows[t] : t;
+            for (uint32_t pc = 0; pc < n_zc; pc++) {
+                const ZcInstr in = zc[pc];
+                switch (in.op) {
+                    case ZC_LOAD_MAIN: rf.set(in.out, 0, __ldg(job.main + (uint64_t)((uint32_t)in.a | ((uint32_t)in.b << 16)) * job.h + row)); break;
+                    case ZC_LOAD_PREP: rf.set(in.out, 0, __ldg(job.prep + (uint64_t)((uint32_t)in.a | ((uint32_t)in.b << 16)) * job.h + row)); break;
+                    case ZC_CONST: rf.set(in.out, 0, prog.consts[in.a]); break;
+                    case ZC_PUBLIC: rf.set(in.out, 0, pv[prog.publics[in.a]]); break;
+                    case ZC_ADD: rf.set(in.out, 0, kb::add(rf.get(in.a, 0), rf.get(in.b, 0))); break;
+                    case ZC_SUB: rf.set(in.out, 0, kb::sub(rf.get(in.a, 0), rf.get(in.b, 0))); break;
+                    case ZC_MUL: rf.set(in.out, 0, kb::mul(rf.get(in.a, 0), rf.get(in.b, 0))); break;
+                    case ZC_NEG: rf.set(in.out, 0, kb::neg(rf.get(in.a, 0))); break;
+                    case ZC_ASSERT:
+                        if (rf.get(in.a, 0)) {
+                            fail = true;
+                            if (LISTED) job.out[t * job.cwords + (in.b >> 5)] |= 1u << (in.b & 31);
+                        }
+                        break;
+                    default: __trap();
+                }
+            }
+        }
+        if (!LISTED) {
+            const uint32_t bits = __ballot_sync(0xffffffffu, fail);
+            if (lane == 0 && bits) { job.out[t0 >> 5] = bits; atomicAdd(job.count, (uint32_t)__popc(bits)); }
+        }
+    }
+}
+
+// the lowest `take` set bits of a chip's failing-row bitmap, ascending: one warp per chip, 32 bitmap words per step
+struct ZcDbgSelect { const uint32_t* bits; uint32_t* rows; uint32_t n_words, take; };
+__global__ void __launch_bounds__(32) zc_debug_select_kernel(const ZcDbgSelect* __restrict__ jobs) {
+    const ZcDbgSelect s = jobs[blockIdx.x];
+    const uint32_t lane = threadIdx.x;
+    uint32_t taken = 0;
+    for (uint32_t w0 = 0; w0 < s.n_words && taken < s.take; w0 += 32) {
+        uint32_t word = w0 + lane < s.n_words ? s.bits[w0 + lane] : 0u;
+        const uint32_t c = __popc(word);
+        uint32_t incl = c;
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t x = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= (uint32_t)d) incl += x;
+        }
+        for (uint32_t rank = taken + incl - c; word && rank < s.take; rank++, word &= word - 1)
+            s.rows[rank] = (w0 + lane) * 32 + (uint32_t)(__ffs(word) - 1);
+        taken += __shfl_sync(0xffffffffu, incl, 31);
+    }
 }
 
 // host interpreter on the all-zero row (padded_row_adjustment, shard.rs:520-537): Σ powers[alpha_idx] * reg
@@ -787,3 +865,136 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
 }
 
 }  // extern "C"
+
+// debug_constraints_all_chips (crates/hypercube/src/debug.rs:27-79) on the device; report words as sp1b200_debug_constraints
+// (include/sp1b200.h).  d_main[k] / d_prep[k]: the chips' columns (column-major, stride h_heights[k]).
+sp1b200_err sp1b200_debug_constraints_device(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint64_t* h_heights, const uint32_t* const* d_main,
+                                             const uint32_t* const* d_prep, const uint32_t* h_pv, uint32_t n_pv, uint32_t max_rows,
+                                             std::vector<uint32_t>& words) {
+    const size_t nchips = m->chips.size();
+    for (size_t k = 0; k < nchips; k++) {
+        for (uint32_t pi : m->host[k].publics)
+            if (pi >= n_pv) return sp1b200_set_error("debug_constraints: chip %zu reads public value %u but only %u were passed", k, pi, n_pv);
+        if (m->chips[k].zc_regs > ZC_GLOBAL_REGS)
+            return sp1b200_set_error("debug_constraints: chip %zu needs %u live registers (> %d)", k, m->chips[k].zc_regs, ZC_GLOBAL_REGS);
+    }
+    cudaStream_t st = ctx->stream;
+    DevFree mem(ctx);
+    PhaseTimer t_all(ctx, "debug_constraints.total");
+    uint32_t* d_pv;
+    SP1_TRY(mem.alloc((void**)&d_pv, (n_pv ? n_pv : 1) * 4));
+    if (n_pv) SP1_CUDA(cudaMemcpyAsync(d_pv, h_pv, n_pv * 4, cudaMemcpyHostToDevice, st));
+    static const uint32_t TIER_REGS[3] = {8, 16, 32};   // the zerocheck kernels' tiers (one node: 4 / 8 / 16 KiB per block)
+    auto tier_of = [&](uint32_t regs) { for (int t = 0; t < 3; t++) if (regs <= TIER_REGS[t]) return t; return regs <= (uint32_t)ZC_LOCAL_REGS ? 3 : 4; };
+    struct Launch { size_t job0; uint32_t n_jobs, blocks, regs; int tier; };
+    // one launch per register-file tier over every chip of that tier; n_of(k) = work items of chip k (0: no job)
+    auto plan = [&](std::vector<ZcDbgJob>& jobs, std::vector<Launch>& launches, size_t& ws_bytes, auto n_of, auto fill) {
+        for (int tier = 0; tier < 5; tier++) {
+            Launch Lc{jobs.size(), 0, 0, 0, tier};
+            for (size_t k = 0; k < nchips; k++) {
+                const uint64_t n = n_of(k);
+                if (!n || tier_of(m->chips[k].zc_regs) != tier) continue;
+                unsigned nb = std::min<unsigned>(blocks_for(n, ZC_BLOCK), 132 * 4);
+                if (tier == 4) nb = std::min(nb, ZC_GLOBAL_MAXB);
+                ZcDbgJob j{};
+                j.main = d_main[k]; j.prep = m->chips[k].prep_w ? d_prep[k] : nullptr; j.h = h_heights[k];
+                j.n = (uint32_t)n; j.blk_start = Lc.blocks; j.nblk = nb; j.chip = (uint32_t)k;
+                fill(k, j);
+                jobs.push_back(j);
+                Lc.n_jobs++; Lc.blocks += nb; Lc.regs = std::max(Lc.regs, m->chips[k].zc_regs);
+            }
+            if (Lc.n_jobs) {
+                launches.push_back(Lc);
+                if (tier == 4) ws_bytes = std::max(ws_bytes, (size_t)Lc.blocks * Lc.regs * ZC_BLOCK * 4);
+            }
+        }
+    };
+    auto run = [&](const std::vector<ZcDbgJob>& jobs, const std::vector<Launch>& launches, size_t ws_bytes, bool listed) -> sp1b200_err {
+        ZcDbgJob* d_jobs;
+        void* d_ws = nullptr;
+        SP1_TRY(mem.alloc((void**)&d_jobs, (jobs.size() + 1) * sizeof(ZcDbgJob)));
+        if (!jobs.empty()) SP1_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(ZcDbgJob), cudaMemcpyHostToDevice, st));
+        if (ws_bytes) SP1_TRY(mem.alloc(&d_ws, ws_bytes));
+        for (const Launch& Lc : launches) {
+            auto go = [&](auto kern, size_t smem) -> sp1b200_err {
+                SP1_LAUNCH(ctx, kern, Lc.blocks, ZC_BLOCK, smem, d_jobs + Lc.job0, (int)Lc.n_jobs, m->d_chips, d_pv, d_ws, Lc.regs);
+                return nullptr;
+            };
+            sp1b200_err e;
+            if (Lc.tier == 4) e = listed ? go(zc_debug_kernel<RF_GLOBAL, true>, 0) : go(zc_debug_kernel<RF_GLOBAL, false>, 0);
+            else if (Lc.tier == 3) e = listed ? go(zc_debug_kernel<RF_LOCAL, true>, 0) : go(zc_debug_kernel<RF_LOCAL, false>, 0);
+            else e = listed ? go(zc_debug_kernel<RF_SMEM, true>, (size_t)Lc.regs * ZC_BLOCK * 4)
+                            : go(zc_debug_kernel<RF_SMEM, false>, (size_t)Lc.regs * ZC_BLOCK * 4);
+            SP1_TRY(e);
+        }
+        return nullptr;
+    };
+
+    // pass 1: every real row of every chip -> failing-row bitmaps and counts
+    std::vector<uint64_t> bm_off(nchips);
+    uint64_t bm_words = 0;
+    for (size_t k = 0; k < nchips; k++) { bm_off[k] = bm_words; bm_words += (h_heights[k] + 31) / 32; }
+    uint32_t *d_bm, *d_cnt;
+    SP1_TRY(mem.alloc((void**)&d_bm, (bm_words ? bm_words : 1) * 4));
+    SP1_TRY(mem.alloc((void**)&d_cnt, (nchips ? nchips : 1) * 4));
+    SP1_CUDA(cudaMemsetAsync(d_bm, 0, (bm_words ? bm_words : 1) * 4, st));
+    SP1_CUDA(cudaMemsetAsync(d_cnt, 0, (nchips ? nchips : 1) * 4, st));
+    {
+        std::vector<ZcDbgJob> jobs; std::vector<Launch> launches; size_t ws = 0;
+        plan(jobs, launches, ws, [&](size_t k) { return h_heights[k]; },
+             [&](size_t k, ZcDbgJob& j) { j.out = d_bm + bm_off[k]; j.count = d_cnt + k; });
+        SP1_TRY(run(jobs, launches, ws, false));
+    }
+    std::vector<uint32_t> cnt(nchips);
+    if (nchips) SP1_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, nchips * 4, cudaMemcpyDeviceToHost, st));
+    SP1_CUDA(cudaStreamSynchronize(st));
+
+    // the lowest max_rows failing rows of each failing chip, then pass 2 over those rows only
+    std::vector<uint64_t> row_off(nchips), cbm_off(nchips);
+    std::vector<uint32_t> take(nchips), cwords(nchips);
+    uint64_t n_rows = 0, n_cbm = 0;
+    std::vector<ZcDbgSelect> sel;
+    uint32_t* d_rows;
+    for (size_t k = 0; k < nchips; k++) {
+        take[k] = std::min(cnt[k], max_rows);
+        cwords[k] = (m->chips[k].n_constraints + 31) / 32;
+        row_off[k] = n_rows; n_rows += take[k];
+        cbm_off[k] = n_cbm; n_cbm += (uint64_t)take[k] * cwords[k];
+    }
+    SP1_TRY(mem.alloc((void**)&d_rows, (n_rows ? n_rows : 1) * 4));
+    std::vector<uint32_t> rows(n_rows), cbm(n_cbm);
+    if (n_rows) {
+        for (size_t k = 0; k < nchips; k++)
+            if (take[k]) sel.push_back(ZcDbgSelect{d_bm + bm_off[k], d_rows + row_off[k], (uint32_t)((h_heights[k] + 31) / 32), take[k]});
+        ZcDbgSelect* d_sel;
+        uint32_t* d_cbm;
+        SP1_TRY(mem.alloc((void**)&d_sel, sel.size() * sizeof(ZcDbgSelect)));
+        SP1_TRY(mem.alloc((void**)&d_cbm, (n_cbm ? n_cbm : 1) * 4));
+        SP1_CUDA(cudaMemcpyAsync(d_sel, sel.data(), sel.size() * sizeof(ZcDbgSelect), cudaMemcpyHostToDevice, st));
+        SP1_CUDA(cudaMemsetAsync(d_cbm, 0, (n_cbm ? n_cbm : 1) * 4, st));
+        SP1_LAUNCH(ctx, zc_debug_select_kernel, (unsigned)sel.size(), 32, 0, d_sel);
+        std::vector<ZcDbgJob> jobs; std::vector<Launch> launches; size_t ws = 0;
+        plan(jobs, launches, ws, [&](size_t k) { return (uint64_t)take[k]; },
+             [&](size_t k, ZcDbgJob& j) { j.rows = d_rows + row_off[k]; j.out = d_cbm + cbm_off[k]; j.cwords = cwords[k]; });
+        SP1_TRY(run(jobs, launches, ws, true));
+        SP1_CUDA(cudaMemcpyAsync(rows.data(), d_rows, n_rows * 4, cudaMemcpyDeviceToHost, st));
+        if (n_cbm) SP1_CUDA(cudaMemcpyAsync(cbm.data(), d_cbm, n_cbm * 4, cudaMemcpyDeviceToHost, st));
+        SP1_CUDA(cudaStreamSynchronize(st));
+    }
+    t_all.stop();
+    words.assign(1, 0);
+    for (size_t k = 0; k < nchips; k++) {
+        if (!cnt[k]) continue;
+        words[0]++;
+        words.push_back((uint32_t)k); words.push_back(cnt[k]); words.push_back(take[k]);
+        for (uint32_t i = 0; i < take[k]; i++) {
+            words.push_back(rows[row_off[k] + i]);
+            const size_t n_at = words.size();
+            words.push_back(0);
+            const uint32_t* b = &cbm[cbm_off[k] + (uint64_t)i * cwords[k]];
+            for (uint32_t c = 0; c < m->chips[k].n_constraints; c++)
+                if ((b[c >> 5] >> (c & 31)) & 1) { words.push_back(c); words[n_at]++; }
+        }
+    }
+    return nullptr;
+}

@@ -59,6 +59,7 @@ ERR_FUNCS = [
     "sp1b200_stacked_commit", "sp1b200_stacked_prove", "sp1b200_jagged_commit", "sp1b200_jagged_column_claims",
     "sp1b200_jagged_prove", "sp1b200_machine_create", "sp1b200_zerocheck", "sp1b200_logup_gkr", "sp1b200_prove_shard",
     "sp1b200_setup_and_prove_shard", "sp1b200_shard_proof_to_bincode", "sp1b200_shard_proof_from_bincode",
+    "sp1b200_debug_constraints", "sp1b200_debug_interactions",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
@@ -260,6 +261,32 @@ class Lib:
                                              _ptr(rw), _ptr(challenger_state), _ptr(out), C.c_uint64(cap_words), C.byref(nw)))
         return out[:nw.value].copy()
 
+    def _debug_call(self, fn, args, cap_words):
+        out = np.empty(max(1, cap_words), np.uint32)
+        nw = C.c_uint64()
+        self._chk(fn(self.ctx, *args, _ptr(out), C.c_uint64(cap_words), C.byref(nw)))
+        return out[:nw.value].copy()
+
+    def debug_constraints_words(self, machine, prep_round, main_dense, heights, pv, max_rows=3, cap_words=1 << 22):
+        """sp1b200_debug_constraints: the report words (include/sp1b200.h)"""
+        H = (C.c_uint64 * len(heights))(*heights)
+        pv = np.ascontiguousarray(pv, dtype=np.uint32)
+        return self._debug_call(self.L.sp1b200_debug_constraints, (machine, prep_round, _ptr(main_dense), H, _ptr(pv), C.c_uint32(pv.size),
+                                                                  C.c_uint32(max_rows)), cap_words)
+
+    def debug_interactions_words(self, machine, prep_round, main_dense, heights, max_keys=16, cap_words=1 << 22):
+        """sp1b200_debug_interactions: the report words (include/sp1b200.h)"""
+        H = (C.c_uint64 * len(heights))(*heights)
+        return self._debug_call(self.L.sp1b200_debug_interactions, (machine, prep_round, _ptr(main_dense), H, C.c_uint32(max_keys)), cap_words)
+
+    def debug_constraints(self, machine, prep_round, main_dense, heights, pv, max_rows=3, cap_words=1 << 22):
+        """-> {chip: {"n_failing_rows": n, "rows": {row: [failed constraint indices]}}} (empty when every constraint holds)"""
+        return parse_constraint_report(self.debug_constraints_words(machine, prep_round, main_dense, heights, pv, max_rows, cap_words))
+
+    def debug_interactions(self, machine, prep_round, main_dense, heights, max_keys=16, cap_words=1 << 22):
+        """-> {"n_unbalanced": n, "keys": [{"kind", "values", "net", "first": (chip, interaction, row), "chips": {chip: net}}]}"""
+        return parse_interaction_report(self.debug_interactions_words(machine, prep_round, main_dense, heights, max_keys, cap_words))
+
     def setup_and_prove_shard(self, machine, prep_dense, prep_rows, prep_cols, vk_tail, main_dense, heights, names, pv, challenger_state,
                               replay=None, cap_words=1 << 24):
         """AirProver::setup_and_prove_shard: -> (prep_commit[8], prep_round handle, proof words); challenger_state = the state BEFORE
@@ -301,6 +328,35 @@ class Lib:
         w = C.c_uint32()
         self._chk(self.L.sp1b200_grind(self.ctx, _ptr(st), C.c_uint32(bits), C.byref(w)))
         return int(w.value), st
+
+
+def parse_constraint_report(w):
+    """report words of sp1b200_debug_constraints -> {chip: {"n_failing_rows": n, "rows": {row: [constraint indices]}}}"""
+    w = [int(x) for x in w]
+    out, p = {}, 1
+    for _ in range(w[0]):
+        chip, n_fail, n_listed = w[p:p + 3]; p += 3
+        rows = {}
+        for _ in range(n_listed):
+            row, n = w[p:p + 2]; p += 2
+            rows[row] = w[p:p + n]; p += n
+        out[chip] = {"n_failing_rows": n_fail, "rows": rows}
+    assert p == len(w), "malformed constraint report"
+    return out
+
+
+def parse_interaction_report(w):
+    """report words of sp1b200_debug_interactions -> {"n_unbalanced": n, "keys": [...]} (keys in order of first occurrence)"""
+    w = [int(x) for x in w]
+    keys, p = [], 3
+    for _ in range(w[2]):
+        kind, nv = w[p:p + 2]; p += 2
+        vals = w[p:p + nv]; p += nv
+        net, chip, inter, row, n_chips = w[p:p + 5]; p += 5
+        chips = {w[p + 2 * i]: w[p + 2 * i + 1] for i in range(n_chips)}; p += 2 * n_chips
+        keys.append({"kind": kind, "values": vals, "net": net, "first": (chip, inter, row), "chips": chips})
+    assert p == len(w), "malformed interaction report"
+    return {"n_unbalanced": w[0] | (w[1] << 32), "keys": keys}
 
 
 class HostChallenger:

@@ -1,0 +1,317 @@
+"""GPU tests of the shard checks (sp1b200_debug_constraints / sp1b200_debug_interactions) against the restated reference checks
+(oracle/debug.hpp), word for word: register-file tiers, calibrated and workload machines, odd heights and height 0, clean traces and
+corruptions, crafted fingerprint collisions, the three kinds of main-trace pointer, errors, memory, and a full-size S2c shard."""
+import numpy as np
+import pytest
+
+from sp1_b200 import synth_air as SA
+from sp1_b200.lib import parse_constraint_report, parse_interaction_report
+from tests import machines as M
+from tests import debug_oracle_lib as DO
+from tests import oracle_lib as O
+from tests.test_debug_checks import colliding_keys, constant_key_machine, cross_chip_machine
+from tests.test_oracle import _synth_machine
+
+pytestmark = pytest.mark.gpu
+P = O.P
+
+TIER_SPECS = [
+    ([(5, 1, False), (0, 2, False), (6, 1, True)], 3),
+    ([(512, 6, False, True), (300, 14, True, True), (1024, 28, False, True), (96, 40, False, True), (2047, 3, True)], 12),
+    ([(192, 250, False, True), (64, 500, True, True), (8191, 3, True), (96, 1000, False, True), (600, 300, False, True)], 13),
+]
+
+
+def _lib(mlr):
+    from sp1_b200 import Lib
+    return Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21))
+
+
+def _prep_round(lib, preps):
+    ps = [p for p in preps if p is not None]
+    return lib.jagged_commit(ps)[1] if ps else None
+
+
+def _check(lib, mach, prep_round, blob, heights, mains, preps, pv, max_rows=3, max_keys=16, inter=True):
+    dense = M.dense_main(mains)
+    got = lib.debug_constraints_words(mach, prep_round, dense, heights, pv, max_rows)
+    want_c = want = DO.debug_constraints(blob, heights, mains, preps, pv, max_rows)
+    assert got.tolist() == want.tolist(), (parse_constraint_report(got), parse_constraint_report(want))
+    if inter:
+        got = lib.debug_interactions_words(mach, prep_round, dense, heights, max_keys)
+        want = DO.debug_interactions(blob, heights, mains, preps, max_keys)
+        assert got.tolist() == want.tolist(), (parse_interaction_report(got), parse_interaction_report(want))
+    return parse_constraint_report(want_c)
+
+
+def _corrupt_cells(rng, mains, n_chips=3):
+    live = [k for k, m in enumerate(mains) if m.size]
+    for k in rng.choice(live, size=min(n_chips, len(live)), replace=False):
+        m = mains[k]
+        for _ in range(2):
+            c, r = int(rng.integers(0, m.shape[0])), int(rng.integers(0, m.shape[1]))
+            m[c, r] = (int(m[c, r]) + 1 + int(rng.integers(0, 1000))) % P
+
+
+@pytest.mark.parametrize("spec,mlr", TIER_SPECS)
+def test_constraint_report_register_tiers(spec, mlr):
+    rng = np.random.default_rng(1700 + mlr)
+    blob, heights, mains, preps, pv = _synth_machine(rng, spec)
+    lib = _lib(mlr)
+    mach = lib.machine_create(blob)
+    pr = _prep_round(lib, preps)
+    assert _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False) == {}
+    _corrupt_cells(rng, mains)
+    assert _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False)
+    # more failing rows than max_rows: a broken column of the widest chip; a changed public value fails every row that loads it
+    k = int(np.argmax(heights))
+    mains[k][2, :] = (mains[k][2, :].astype(np.uint64) + 1).astype(np.uint32) % P
+    rep = _check(lib, mach, pr, blob, heights, mains, preps, pv, max_rows=2, inter=False)
+    assert rep[k]["n_failing_rows"] > 2 and len(rep[k]["rows"]) == 2
+    pv2 = pv.copy(); pv2[0] = (int(pv2[0]) + 1) % P
+    rep = _check(lib, mach, pr, blob, heights, mains, preps, pv2, max_rows=5, inter=False)
+    assert all(rep[c]["n_failing_rows"] == heights[c] for c in range(len(heights)) if heights[c])
+    if pr is not None:
+        lib.jagged_round_free(pr)
+    lib.machine_free(mach)
+    lib.close()
+
+
+CALIBRATED = [M.Chip(700, 4, True, 36, 5, 3), M.Chip(96, 14, False, 120, 0, 0, [12, 4, 9, 5]), M.Chip(0, 2, True, 18, 1, 2),
+              M.Chip(33, 1, True, 9, 7, 35), M.Chip(2048, 40, False, 360, 2, 0, [9] * 6)]
+
+
+@pytest.mark.parametrize("case", ["calibrated", "tinyc", "tinyr"])
+def test_reports_on_calibrated_and_workload_machines(case):
+    rng = np.random.default_rng(1800)
+    if case == "calibrated":
+        blob, heights, mains, preps, pv, _ = M.spec_machine(rng, CALIBRATED)
+        mlr = 11
+    else:
+        blob, heights, mains, preps, pv, _ = M.workload_machine(case, seed=1801, max_log_rows=12, scale=0.25)
+        mlr = 12
+    lib = _lib(mlr)
+    mach = lib.machine_create(blob)
+    pr = _prep_round(lib, preps)
+    _check(lib, mach, pr, blob, heights, mains, preps, pv)
+    words = lib.debug_interactions_words(mach, pr, M.dense_main(mains), heights)
+    assert words.tolist() == [0, 0, 0]
+    _corrupt_cells(rng, mains)
+    _check(lib, mach, pr, blob, heights, mains, preps, pv)
+    if pr is not None:
+        lib.jagged_round_free(pr)
+    lib.machine_free(mach)
+    lib.close()
+
+
+def _inter_case(blob, heights, mains, preps, max_keys=16, mlr=8):
+    lib = _lib(mlr)
+    mach = lib.machine_create(blob)
+    pr = _prep_round(lib, preps)
+    got = lib.debug_interactions_words(mach, pr, M.dense_main(mains), heights, max_keys)
+    want = DO.debug_interactions(blob, heights, mains, preps, max_keys)
+    if pr is not None:
+        lib.jagged_round_free(pr)
+    lib.machine_free(mach)
+    lib.close()
+    assert got.tolist() == want.tolist(), (parse_interaction_report(got), parse_interaction_report(want))
+    return parse_interaction_report(want)
+
+
+def test_interaction_report_cross_chip():
+    rng = np.random.default_rng(1900)
+    blob, heights, mains, preps = cross_chip_machine(rng, h=200, mult_col_kind4=True)
+    assert _inter_case(blob, heights, mains, preps)["n_unbalanced"] == 0
+    mains[1][0, 17] = (int(mains[1][0, 17]) + 1) % P                       # one changed value
+    _inter_case(blob, heights, mains, preps)
+    blob, heights, mains, preps = cross_chip_machine(rng, h=200, mult_col_kind4=True)
+    one = int(O.to_monty(np.array([1]))[0])
+    r = int(np.nonzero(mains[1][3] == one)[0][0])
+    mains[1][3, r] = 0                                                     # one changed multiplicity
+    assert _inter_case(blob, heights, mains, preps)["n_unbalanced"] == 2
+    mains[0][3, :] = 0                                                     # the sender's multiplicity column zeroed: > max_keys keys
+    rep = _inter_case(blob, heights, mains, preps, max_keys=5)
+    assert rep["n_unbalanced"] > 5 and len(rep["keys"]) == 5
+
+
+def _blob_segments(blob):
+    """-> (per chip program words, per chip interaction words) of a machine blob"""
+    b = [int(x) for x in blob]
+    progs, inters, p = [], [], 1
+    for _ in range(b[0]):
+        ni, nl, nc, npub, na = b[p + 4:p + 9]
+        ln = 9 + 2 * ni + 2 * nl + nc + npub + 2 * na
+        progs.append(b[p:p + ln]); p += ln
+    for _ in range(b[0]):
+        q = p + 1
+        for _ in range(b[p]):
+            nv = b[q + 2]; q += 3
+            for _ in range(nv + 1):
+                q += 2 + 3 * b[q]
+        inters.append(b[p:q]); p = q
+    assert p == len(b)
+    return progs, inters
+
+
+def _bump_first_receive(iw):
+    """interaction words of one chip with the constant of the first receive's first value column + 1"""
+    iw = list(iw)
+    q = 1
+    for _ in range(iw[0]):
+        is_send, nv = iw[q], iw[q + 2]
+        q += 3
+        q += 2 + 3 * iw[q]                                  # multiplicity vcol
+        if not is_send and nv:
+            iw[q + 1] = (iw[q + 1] + int(O.to_monty(np.array([1]))[0])) % P
+            return iw
+        for _ in range(nv):
+            q += 2 + 3 * iw[q]
+    raise ValueError("no receive with a value")
+
+
+def test_interaction_report_edited_receive():
+    """an existing calibrated blob with one receive's virtual-column constant changed"""
+    rng = np.random.default_rng(1901)
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, [M.Chip(300, 2, False, None, 0, 0, [4, 5]), M.Chip(129, 1, True, 9, 0, 1, [9])])
+    progs, inters = _blob_segments(blob)
+    inters[1] = _bump_first_receive(inters[1])
+    blob2 = SA.machine_blob_with_interactions(progs, inters)
+    assert blob2.size == blob.size and (blob2 != blob).sum() == 1
+    rep = _inter_case(blob2, heights, mains, preps, mlr=9)
+    assert rep["n_unbalanced"] > 0 and all(set(k["chips"]) == {1} for k in rep["keys"])
+
+
+def test_interaction_report_fingerprint_collisions():
+    rng = np.random.default_rng(1902)
+    A, B = colliding_keys(rng)
+    # A sent, B received: two keys (grouping by fingerprint alone would find them balanced)
+    blob, heights, mains, preps = constant_key_machine(rng, [[(1, 5, A)], [(0, 5, B)]], [7, 7])
+    rep = _inter_case(blob, heights, mains, preps)
+    assert rep["n_unbalanced"] == 2
+    # A and B each sent and received: nothing
+    blob, heights, mains, preps = constant_key_machine(rng, [[(1, 5, A), (1, 5, B)], [(0, 5, B), (0, 5, A)]], [9, 9])
+    assert _inter_case(blob, heights, mains, preps)["n_unbalanced"] == 0
+
+
+def test_pointer_kinds_errors_memory_and_proof_unchanged():
+    import torch
+    rng = np.random.default_rng(2000)
+    spec = [(1024, 2, True), (256 + 32, 3, False), (0, 1, False), (2048, 1, True)]
+    from tests.test_oracle import _synth_machine_gkr
+    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
+    mains[1][2, 7] = (int(mains[1][2, 7]) + 3) % P
+    lib = _lib(11)
+    mach = lib.machine_create(blob)
+    pr = _prep_round(lib, preps)
+    dense = M.dense_main(mains)
+    ref_c = lib.debug_constraints_words(mach, pr, dense, heights, pv)
+    ref_i = lib.debug_interactions_words(mach, pr, dense, heights)
+    assert ref_c.tolist() == DO.debug_constraints(blob, heights, mains, preps, pv).tolist()
+    assert ref_i.tolist() == DO.debug_interactions(blob, heights, mains, preps).tolist()
+    d = torch.from_numpy(dense.view(np.int32)).cuda()
+    pinned = torch.from_numpy(dense.view(np.int32)).pin_memory()
+    for src in (d, lib.upload_begin(pinned, 0)):
+        assert lib.debug_constraints_words(mach, pr, src, heights, pv).tolist() == ref_c.tolist()
+        assert lib.debug_interactions_words(mach, pr, src, heights).tolist() == ref_i.tolist()
+    # errors: capacity, mismatched preprocessed round; the context stays usable
+    from sp1_b200.lib import Sp1B200Error
+    with pytest.raises(Sp1B200Error, match="capacity"):
+        lib.debug_constraints_words(mach, pr, dense, heights, pv, cap_words=2)
+    with pytest.raises(Sp1B200Error, match="capacity"):
+        lib.debug_interactions_words(mach, pr, dense, heights, cap_words=2)
+    with pytest.raises(Sp1B200Error, match="preprocessed"):
+        lib.debug_constraints_words(mach, None, dense, heights, pv)
+    with pytest.raises(Sp1B200Error, match="preprocessed"):
+        lib.debug_interactions_words(mach, None, dense, heights)
+    assert lib.debug_constraints_words(mach, pr, dense, heights, pv).tolist() == ref_c.tolist()
+    # repeated calls: device memory in use stays flat after the first
+    used = []
+    for _ in range(4):
+        lib.debug_constraints_words(mach, pr, dense, heights, pv); lib.debug_interactions_words(mach, pr, dense, heights)
+        torch.cuda.synchronize()
+        free, total = torch.cuda.mem_get_info(0)
+        used.append(total - free)
+    assert max(used[1:]) - min(used[1:]) < (8 << 20), used
+    # a proof after either check equals the proof without it (clean trace)
+    mains[1][2, 7] = (int(mains[1][2, 7]) - 3) % P
+    dense = M.dense_main(mains)
+    names = [f"Chip{i:02d}" for i in range(len(heights))]
+    proofs = []
+    for pre in (None, "c", "i"):
+        if pre == "c":
+            assert lib.debug_constraints_words(mach, pr, dense, heights, pv).tolist() == [0]
+        if pre == "i":
+            assert lib.debug_interactions_words(mach, pr, dense, heights).tolist() == [0, 0, 0]
+        st = O.Challenger().st.copy()
+        proofs.append(lib.prove_shard(mach, pr, dense, heights, names, pv, st))
+    assert all((p_.size == proofs[0].size and (p_ == proofs[0]).all()) for p_ in proofs)
+    lib.jagged_round_free(pr)
+    lib.machine_free(mach)
+    lib.close()
+
+
+def test_full_size_s2c_shard():
+    """one full-size S2c shard built on the device: clean -> both reports empty; one corrupted cell -> that (chip, row) with the
+    constraints the oracle finds for that row alone; one chip's receive made unbalanced in the blob -> the oracle's report for that chip"""
+    import torch
+    from sp1_b200 import Lib
+    from sp1_b200 import workload as W
+    mach_d = W.synthetic_machine("S2c", seed=42)
+    specs, blob = mach_d["specs"], mach_d["blob"]
+    heights = [sp.h for sp in specs]
+    parts, preps = [], []
+    for i, sp in enumerate(specs):
+        m, p = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, 12345, 500 + i, 0, extra_cols=sp.extra, extra_prep=sp.extra_prep)
+        parts.append(m); preps.append(p)
+    dense = torch.cat(parts).contiguous()
+    pv = O.to_monty(np.array([12345, 5, 6, 7]))
+    lib = Lib(0)
+    mach = lib.machine_create(blob)
+    pts = [(p.view(-1, sp.h).cpu().numpy().view(np.uint32)) for p, sp in zip(preps, specs) if p is not None]
+    pr = lib.jagged_commit(pts)[1] if pts else None
+    assert lib.debug_constraints_words(mach, pr, dense, heights, pv).tolist() == [0]
+    assert lib.debug_interactions_words(mach, pr, dense, heights).tolist() == [0, 0, 0]
+    k = int(np.argmax(heights)); row = heights[k] - 5
+    off = sum(h * (6 * sp.g + (1 if sp.wp else 0) + sp.extra) for h, sp in zip(heights[:k], specs[:k]))
+    cell = off + 2 * heights[k] + row
+    dense[cell] = int((int(dense[cell].item()) + 1) % P)
+    rep = parse_constraint_report(lib.debug_constraints_words(mach, pr, dense, heights, pv))
+    main_k = dense[off:off + heights[k] * (6 * specs[k].g + (1 if specs[k].wp else 0) + specs[k].extra)].view(-1, heights[k])
+    one_row = np.ascontiguousarray(main_k[:, row:row + 1].cpu().numpy().view(np.uint32))
+    prep_row = None if preps[k] is None else np.ascontiguousarray(preps[k].view(-1, heights[k])[:, row:row + 1].cpu().numpy().view(np.uint32))
+    # the oracle on chip k's row alone (a one-chip machine with that chip's program)
+    alone = DO.debug_constraints(_one_chip_blob(blob, k), [1], [one_row], [prep_row], pv)
+    want = parse_constraint_report(alone)
+    assert list(rep) == [k] and rep[k]["n_failing_rows"] == 1 and rep[k]["rows"] == {row: want[0]["rows"][0]}
+    dense[cell] = int((int(dense[cell].item()) - 1) % P)
+    # one chip's receive made unbalanced in the blob (the smallest chip with interactions, so that the oracle runs on it alone)
+    progs, inters = _blob_segments(blob)
+    c = min((i for i in range(len(specs)) if heights[i] and inters[i][0]), key=lambda i: heights[i])
+    inters2 = list(inters); inters2[c] = _bump_first_receive(inters[c])
+    mach2 = lib.machine_create(SA.machine_blob_with_interactions(progs, inters2))
+    got = parse_interaction_report(lib.debug_interactions_words(mach2, pr, dense, heights, max_keys=1 << 17))
+    lib.machine_free(mach2)
+    offc = sum(h * (6 * sp.g + (1 if sp.wp else 0) + sp.extra) for h, sp in zip(heights[:c], specs[:c]))
+    main_c = dense[offc:offc + heights[c] * (6 * specs[c].g + (1 if specs[c].wp else 0) + specs[c].extra)].view(-1, heights[c])
+    prep_c = None if preps[c] is None else preps[c].view(-1, heights[c]).cpu().numpy().view(np.uint32)
+    want = parse_interaction_report(DO.debug_interactions(SA.machine_blob_with_interactions([progs[c]], [inters2[c]]), [heights[c]],
+                                                         [main_c.cpu().numpy().view(np.uint32)], [prep_c], max_keys=1 << 17))
+    # the same unbalanced keys and nets; chip c carries the whole net.  A key can also occur (balanced) in other chips - the synthetic
+    # traces share small values such as 0 between chips - and those chips are listed with net 0, possibly as the first occurrence.
+    assert 0 < want["n_unbalanced"] == got["n_unbalanced"] == len(want["keys"]) == len(got["keys"])
+    by_key = lambda rep: {(k["kind"], tuple(k["values"])): k for k in rep["keys"]}
+    g_, w_ = by_key(got), by_key(want)
+    assert set(g_) == set(w_)
+    for key, w in w_.items():
+        g = g_[key]
+        assert g["net"] == w["net"] and g["chips"][c] == w["net"] and all(x == 0 for ch, x in g["chips"].items() if ch != c)
+        if set(g["chips"]) == {c}:
+            assert g["first"] == (c,) + w["first"][1:]
+    lib.jagged_round_free(pr) if pr is not None else None
+    lib.machine_free(mach)
+    lib.close()
+
+
+def _one_chip_blob(blob, k):
+    """chip k's constraint program as a one-chip machine without interactions"""
+    return SA.machine_blob([_blob_segments(blob)[0][k]])
