@@ -43,95 +43,18 @@ void host_compress(const uint32_t* l, const uint32_t* r, uint32_t* out8) {
     for (int j = 0; j < 8; j++) out8[j] = st[j];
 }
 
-// per-column claims: out[c] = sum_{r < rows} row_eq[r] * col[r]   (one block per column)
-__global__ void __launch_bounds__(256) column_claims_kernel(const uint32_t* __restrict__ dense, const uint64_t* __restrict__ col_start,
-                                                            const uint64_t* __restrict__ col_rows, const uint32_t* __restrict__ row_eq,
-                                                            uint32_t* __restrict__ out) {
-    const uint64_t c = blockIdx.x;
-    const uint32_t* col = dense + col_start[c];
-    const uint64_t rows = col_rows[c];
-    uint32_t a0 = 0, a1 = 0, a2 = 0, a3 = 0;
-    for (uint64_t i = threadIdx.x; i < rows; i += blockDim.x) {
-        uint32_t x = __ldg(col + i);
-        uint4 v = __ldg(reinterpret_cast<const uint4*>(row_eq + 4 * i));
-        a0 = kb::add(a0, kb::mul(x, v.x)); a1 = kb::add(a1, kb::mul(x, v.y));
-        a2 = kb::add(a2, kb::mul(x, v.z)); a3 = kb::add(a3, kb::mul(x, v.w));
-    }
-    const Ext v[1] = {Ext{{a0, a1, a2, a3}}};
-    block_reduce<1>(v, out, Mail{});  // -> out[c * 4 ..]
-}
-
-// jagged little polynomial: ext[i] = col_eq[c(i)] * row_eq[i - prefix[c(i)]] for i < prefix[ncols], else 0.
-// c(i) = the last column with prefix[c] <= i (zero-height columns share a prefix value: the last one has the non-empty range).
-// start[i >> JP_SHIFT] (built on the host from the same prefix sums) is a column at or before c(i), so the search is a short
-// forward walk instead of a binary search per element.
-constexpr int JP_SHIFT = 12;
-__global__ void __launch_bounds__(256) jagged_poly_kernel(const uint64_t* __restrict__ prefix, uint32_t ncols, const uint32_t* __restrict__ start,
-                                                          const uint32_t* __restrict__ col_eq, const uint32_t* __restrict__ row_eq, uint64_t N,
-                                                          uint32_t* __restrict__ ext) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N) return;
-    Ext v = kb::ext_zero();
-    if (i < prefix[ncols]) {
-        uint32_t lo = start[i >> JP_SHIFT];
-        while (lo + 1 < ncols && prefix[lo + 1] <= i) lo++;
-        v = kb::ext_mul(kb::ext_load(col_eq + 4 * lo), kb::ext_load(row_eq + 4 * (i - prefix[lo])));
-    }
-    kb::ext_store(ext + 4 * i, v);
-}
-
 struct SegTable {  // the virtual long base vector = concatenation of the rounds' dense buffers, then zeros
     const uint32_t* ptr[8];
     uint64_t end[8];
     int n;
 };
-__device__ __forceinline__ uint32_t seg_load(const SegTable& t, uint64_t i) {
-    uint64_t start = 0;
-#pragma unroll 1
-    for (int s = 0; s < t.n; s++) { if (i < t.end[s]) return __ldg(t.ptr[s] + (i - start)); start = t.end[s]; }
-    return 0;
-}
 
-// round 0: sum_j ext[2j]*base[2j]  and  sum_j (ext[2j]+ext[2j+1]) * (base[2j]+base[2j+1])   (base in F)
-__global__ void __launch_bounds__(256) hadamard_sum0_kernel(SegTable base, const uint32_t* __restrict__ ext, uint64_t npairs,
-                                                            uint32_t* __restrict__ partial, Mail mail) {
-    Ext s0 = kb::ext_zero(), sh = kb::ext_zero();
-    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < npairs; j += (uint64_t)gridDim.x * blockDim.x) {
-        uint32_t b0 = seg_load(base, 2 * j), b1 = seg_load(base, 2 * j + 1);
-        Ext e0 = kb::ext_load(ext + 8 * j), e1 = kb::ext_load(ext + 8 * j + 4);
-        s0 = kb::ext_add(s0, kb::ext_mul_base(e0, b0));
-        sh = kb::ext_add(sh, kb::ext_mul_base(kb::ext_add(e0, e1), kb::add(b0, b1)));
-    }
-    block_reduce<2>({s0, sh}, partial, mail);
-}
-
-// fix the last variable of round 0 (base F -> EF) and accumulate round-1 sums
-__global__ void __launch_bounds__(256) hadamard_fold0_kernel(SegTable base, const uint32_t* __restrict__ ext, uint64_t nout_pairs, Ext alpha,
-                                                             uint32_t* __restrict__ base_out, uint32_t* __restrict__ ext_out,
-                                                             uint32_t* __restrict__ partial, uint64_t nout, Mail mail) {
-    Ext s0 = kb::ext_zero(), sh = kb::ext_zero();
-    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nout_pairs; j += (uint64_t)gridDim.x * blockDim.x) {
-        Ext nb[2], ne[2];
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            uint64_t o = 2 * j + h;  // output index; inputs 2o, 2o+1
-            if (o < nout) {
-                uint32_t b0 = seg_load(base, 2 * o), b1 = seg_load(base, 2 * o + 1);
-                Ext e0 = kb::ext_load(ext + 8 * o), e1 = kb::ext_load(ext + 8 * o + 4);
-                nb[h] = kb::ext_add(kb::ext_from_base(b0), kb::ext_mul_base(alpha, kb::sub(b1, b0)));
-                ne[h] = kb::ext_add(e0, kb::ext_mul(alpha, kb::ext_sub(e1, e0)));
-                kb::ext_store(base_out + 4 * o, nb[h]);
-                kb::ext_store(ext_out + 4 * o, ne[h]);
-            } else { nb[h] = kb::ext_zero(); ne[h] = kb::ext_zero(); }
-        }
-        s0 = kb::ext_add(s0, kb::ext_mul(ne[0], nb[0]));
-        sh = kb::ext_add(sh, kb::ext_mul(kb::ext_add(ne[0], ne[1]), kb::ext_add(nb[0], nb[1])));
-    }
-    block_reduce<2>({s0, sh}, partial, mail);
-}
-
-// ---- rounds 0 .. K-1 summed straight from the base-field trace ("aligned" path) -----------------------------------------------
-// ext[i] = col_eq[c(i)] * row_eq[i - prefix[c]].  When 2^K divides every column prefix sum (the reference pads trace heights to
+// ---- rounds 0 .. K-1 summed straight from the base-field trace, then one fold pass to level K ----------------------------------
+// The jagged little polynomial is ext[i] = col_eq[c(i)] * row_eq[i - prefix[c(i)]] for i < prefix[ncols], else 0.
+// c(i) = the last column with prefix[c] <= i (zero-height columns share a prefix value: the last one has the non-empty range).
+// start[i >> JP_SHIFT] (built on the host from the same prefix sums) is a column at or before c(i), so the search is a short
+// forward walk instead of a binary search per element.
+// When 2^K divides every column prefix sum (the reference pads trace heights to
 // multiples of 32, crates/hypercube/src/util.rs:57), every aligned block of 2^(r+1) <= 2^K entries lies in one column, and after
 // r folds by alpha_0 .. alpha_{r-1} both sides of the sumcheck stay in closed form over the base-field trace b:
 //   dense_r[o] = sum_{t < 2^r} w_r[t] b[o 2^r + t],            w_r[t] = prod_{s < r} (bit s of t ? alpha_s : 1 - alpha_s)
@@ -141,7 +64,9 @@ __global__ void __launch_bounds__(256) hadamard_fold0_kernel(SegTable base, cons
 // trace: per block of 2^(r+1) words, two EF x F weighted sums (lazy 64-bit accumulation) and two products with the L_r table; the
 // factor col_eq[c] * eq_hi[h] is applied once per (column, high row bits) run of a lane.  After round K-1 one pass writes the
 // level-K dense and eq arrays (2^(log_m - K) EF entries each) and sums round K; hadamard_fold_kernel takes it from there.
-// K = 0 (some column starts at an odd index) keeps the materialised path above.
+// K = 0 (some column starts at an odd index) has no trace rounds: the fold pass to level 0 (w_0 = {1}, L_0 = eq_lo) lifts the trace
+// to EF, writes the eq array and sums round 0.
+constexpr int JP_SHIFT = 12;
 constexpr int JK_MAX = 5;   // rounds summed from the trace at most (K = 4 measured slower on S2c, DESIGN.md §3.5)
 constexpr int JK_LOW = 10;  // low row bits of the eq_lo factor (the shared tables: 2 x 2^9 EF for round 0)
 struct JWeights { Ext w[1 << JK_MAX]; };  // w_r[t], t < 2^r
@@ -255,7 +180,7 @@ __global__ void __launch_bounds__(256) jagged_fold_to_kernel(SegTable base, cons
                                                              JWeights W, uint64_t area, uint64_t nout_pairs, uint32_t* __restrict__ base_out,
                                                              uint32_t* __restrict__ ext_out, uint32_t* __restrict__ partial, uint64_t nout, Mail mail) {
     constexpr int NW = 1 << K;  // words per level-K entry
-    __shared__ Ext tL[1 << (JK_LOW - 1)];  // L_K[u], u < 2^(lb - K)
+    __shared__ Ext tL[1 << (JK_LOW - (K > 0))];  // L_K[u], u < 2^(lb - K)
     for (uint32_t u = threadIdx.x; u < (1u << (lb - K)); u += blockDim.x) tL[u] = folded_eq_lo<K>(W, eq_lo, u);
     __syncthreads();
     const uint64_t lomask = (1ull << lb) - 1;
@@ -526,24 +451,21 @@ sp1b200_err sp1b200_jagged_column_claims(sp1b200_ctx* ctx, const sp1b200_jagged_
     const uint32_t mlr = ctx->params.max_log_row_count;
     DevFree mem(ctx);
     uint32_t *d_z, *d_eq, *d_out;
-    uint64_t *d_start, *d_rows;
-    std::vector<uint64_t> start, nrows;
+    std::vector<EvalTable> tabs;  // the round's tables without the two padding tables
     uint64_t off = 0;
-    for (size_t t = 0; t + 2 < r->row_counts.size(); t++)
-        for (uint64_t c = 0; c < r->col_counts[t]; c++) { start.push_back(off); nrows.push_back(r->row_counts[t]); off += r->row_counts[t]; }
-    const size_t nc = start.size();
+    uint32_t nc = 0;
+    for (size_t t = 0; t + 2 < r->row_counts.size(); t++) {
+        tabs.push_back(EvalTable{r->d_dense + off, r->row_counts[t], (uint32_t)r->col_counts[t], nc});
+        off += r->row_counts[t] * r->col_counts[t]; nc += (uint32_t)r->col_counts[t];
+    }
     if (!nc) return nullptr;
     SP1_TRY(mem.alloc((void**)&d_z, mlr * 16));
     SP1_TRY(mem.alloc((void**)&d_eq, ((size_t)16) << mlr));
-    SP1_TRY(mem.alloc((void**)&d_out, nc * 16));
-    SP1_TRY(mem.alloc((void**)&d_start, nc * 8));
-    SP1_TRY(mem.alloc((void**)&d_rows, nc * 8));
+    SP1_TRY(mem.alloc((void**)&d_out, (size_t)nc * 16));
     SP1_CUDA(cudaMemcpyAsync(d_z, h_z_row, mlr * 16, cudaMemcpyHostToDevice, ctx->stream));
-    SP1_CUDA(cudaMemcpyAsync(d_start, start.data(), nc * 8, cudaMemcpyHostToDevice, ctx->stream));
-    SP1_CUDA(cudaMemcpyAsync(d_rows, nrows.data(), nc * 8, cudaMemcpyHostToDevice, ctx->stream));
     SP1_TRY(launch_eq_table(ctx, d_z, (int)mlr, d_eq));
-    SP1_LAUNCH(ctx, column_claims_kernel, (unsigned)nc, 256, 0, r->d_dense, d_start, d_rows, d_eq, d_out);
-    SP1_CUDA(cudaMemcpyAsync(h_out, d_out, nc * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    SP1_TRY(launch_table_evals(ctx, tabs, d_eq, d_out, nc));
+    SP1_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)nc * 16, cudaMemcpyDeviceToHost, ctx->stream));
     SP1_CUDA(cudaStreamSynchronize(ctx->stream));
     return nullptr;
 }
@@ -574,6 +496,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     { uint64_t s = 0; for (uint64_t hgt : heights) { prefix.push_back(s); s += hgt; } prefix.push_back(prefix.back() + heights.back()); }
     const uint32_t lm = hf::log2_ceil(prefix.back());
     if (lm < ls) return sp1b200_set_error("jagged_prove: internal: log_m < log_stacking_height");
+    if (lm < 2) return sp1b200_set_error("jagged_prove: fewer than two sumcheck variables (log_m = %u)", lm);
     const uint64_t N = (uint64_t)1 << lm;
     const uint32_t ncv = hf::log2_ceil(total_cols);
     std::vector<E4> z_col(ncv), z_row(mlr);
@@ -597,29 +520,25 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
 
     // K = the rounds summed straight from the base-field trace (see jagged_round_kernel): every aligned 2^K block must lie in one
     // column (2^K divides every prefix sum), in one segment (K <= log_stacking_height) and in one run of 2^lb rows (K <= lb); round
-    // K must still exist (K <= log_m - 1).  K = 0 materialises the little polynomial (odd column starts).
+    // K must still exist (K <= log_m - 1).  K = 0 (odd column starts): no trace rounds, round 0 comes from the fold pass.
     const int lb = (int)std::min<uint32_t>(JK_LOW, mlr);
-    uint32_t K = std::min<uint32_t>({(uint32_t)JK_MAX, ls, lm ? lm - 1 : 0, (uint32_t)lb});
+    uint32_t K = std::min<uint32_t>({(uint32_t)JK_MAX, ls, lm - 1, (uint32_t)lb});
     for (uint64_t p : prefix)
         if (p) K = std::min<uint32_t>(K, (uint32_t)__builtin_ctzll(p));
     const uint64_t area = prefix.back();
 
-    // device tables: col_eq (over last log2_ceil(ncols) coords of z_col == all of z_col), the row eq table(s), prefix sums
-    uint32_t *d_coleq, *d_zrow, *d_roweq = nullptr, *d_eqhi = nullptr, *d_eqlo = nullptr, *d_ext, *d_ext2, *d_b, *d_b2, *d_partial;
+    // device tables: col_eq (over last log2_ceil(ncols) coords of z_col == all of z_col), the row eq factors, prefix sums
+    uint32_t *d_coleq, *d_zrow, *d_eqhi, *d_eqlo, *d_ext, *d_ext2, *d_b, *d_b2, *d_partial;
     uint64_t* d_prefix;
     SP1_TRY(mem.alloc((void**)&d_coleq, col_eq_full.size() * 16));
     SP1_CUDA(cudaMemcpyAsync(d_coleq, col_eq_full.data(), col_eq_full.size() * 16, cudaMemcpyHostToDevice, st));
     SP1_TRY(mem.alloc((void**)&d_zrow, mlr * 16));
     SP1_CUDA(cudaMemcpyAsync(d_zrow, h_z_row, mlr * 16, cudaMemcpyHostToDevice, st));
-    if (K) {  // row_eq = eq_hi (x) eq_lo: z_row[0 .. mlr-lb) is the high (most significant) part
-        SP1_TRY(mem.alloc((void**)&d_eqhi, ((size_t)16) << (mlr - lb)));
-        SP1_TRY(mem.alloc((void**)&d_eqlo, ((size_t)16) << lb));
-        SP1_TRY(launch_eq_table(ctx, d_zrow, (int)(mlr - lb), d_eqhi));
-        SP1_TRY(launch_eq_table(ctx, d_zrow + 4 * (mlr - lb), lb, d_eqlo));
-    } else {
-        SP1_TRY(mem.alloc((void**)&d_roweq, ((size_t)16) << mlr));
-        SP1_TRY(launch_eq_table(ctx, d_zrow, (int)mlr, d_roweq));
-    }
+    // row_eq = eq_hi (x) eq_lo: z_row[0 .. mlr-lb) is the high (most significant) part
+    SP1_TRY(mem.alloc((void**)&d_eqhi, ((size_t)16) << (mlr - lb)));
+    SP1_TRY(mem.alloc((void**)&d_eqlo, ((size_t)16) << lb));
+    SP1_TRY(launch_eq_table(ctx, d_zrow, (int)(mlr - lb), d_eqhi));
+    SP1_TRY(launch_eq_table(ctx, d_zrow + 4 * (mlr - lb), lb, d_eqlo));
     SP1_TRY(mem.alloc((void**)&d_prefix, prefix.size() * 8));
     SP1_CUDA(cudaMemcpyAsync(d_prefix, prefix.data(), prefix.size() * 8, cudaMemcpyHostToDevice, st));
     // start[b] = last column with prefix <= b << JP_SHIFT (two-pointer walk over the blocks of the real area)
@@ -635,26 +554,14 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     uint32_t* d_jp_start;
     SP1_TRY(mem.alloc((void**)&d_jp_start, jp_start.size() * 4));
     SP1_CUDA(cudaMemcpyAsync(d_jp_start, jp_start.data(), jp_start.size() * 4, cudaMemcpyHostToDevice, st));
-    // working arrays: level K (written by the fold pass after round K-1) and level K+1; later levels reuse them in turn
-    if (K) {
-        SP1_TRY(mem.alloc((void**)&d_b, (N >> K) * 16));
-        SP1_TRY(mem.alloc((void**)&d_ext, (N >> K) * 16));
-        SP1_TRY(mem.alloc((void**)&d_b2, ((N >> (K + 1)) + 1) * 16));
-        SP1_TRY(mem.alloc((void**)&d_ext2, ((N >> (K + 1)) + 1) * 16));
-    } else {
-        SP1_TRY(mem.alloc((void**)&d_ext, N * 16));
-        SP1_TRY(mem.alloc((void**)&d_ext2, (N / 2) * 16));
-        SP1_TRY(mem.alloc((void**)&d_b, (N / 2) * 16));
-        SP1_TRY(mem.alloc((void**)&d_b2, (N / 4 + 1) * 16));
-    }
+    // working arrays: level K (written by the fold pass to level K) and level K+1; later levels reuse them in turn
+    SP1_TRY(mem.alloc((void**)&d_b, (N >> K) * 16));
+    SP1_TRY(mem.alloc((void**)&d_ext, (N >> K) * 16));
+    SP1_TRY(mem.alloc((void**)&d_b2, ((N >> (K + 1)) + 1) * 16));
+    SP1_TRY(mem.alloc((void**)&d_ext2, ((N >> (K + 1)) + 1) * 16));
     const unsigned MAXB = 132 * 8;  // eight blocks per SM of an H100
     static_assert(132 * 8 * 8 + 16 <= SP1_MAIL_WORDS, "round partials must fit the mailbox payload");
     d_partial = sp1b200_mail_dev(ctx);  // the round kernels post their block partials straight into the mailbox
-    {
-        PhaseTimer t(ctx, "jagged.little_poly");
-        if (!K) SP1_LAUNCH(ctx, jagged_poly_kernel, blocks_for(N), 256, 0, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, d_roweq, N, d_ext);
-        t.stop();
-    }
     SegTable seg{};
     seg.n = (int)n_rounds;
     { uint64_t e = 0; for (uint32_t r = 0; r < n_rounds; r++) { seg.ptr[r] = rounds[r]->d_dense; e += rounds[r]->padded_area; seg.end[r] = e; } }
@@ -668,50 +575,45 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     std::vector<E4> w{E4::one()};  // w_r (see jagged_round_kernel): the weights of the 2^r trace words behind one level-r entry
     JWeights dw{};
     auto load_weights = [&]() { for (size_t t = 0; t < w.size(); t++) for (int l = 0; l < 4; l++) dw.w[t].c[l] = w[t].c[l]; };
-    // round R < K from the trace; contiguous span of blocks per warp (multiple of 32), over the real area only
-    auto launch_round = [&](uint32_t R, const Mail& mail, unsigned& g) -> sp1b200_err {
-        const uint64_t nblk = area >> (R + 1);
-        g = grid_for(nblk);
-        const uint64_t warps = (uint64_t)g * 8, span = std::max<uint64_t>((((nblk + warps - 1) / warps) + 31) / 32 * 32, 32);
-#define SP1_JROUND(r) case r: SP1_LAUNCH(ctx, jagged_round_kernel<r>, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, \
+    // the sums of round r come from jagged_round_kernel<r> when r < K, from jagged_fold_to_kernel<K> (which writes level K) when
+    // r == K, and from hadamard_fold_kernel fixing alpha_{r-1} when r > K (r = log_m: the last fold, for the dense evaluation)
+    uint32_t *cur_b = d_b, *cur_e = d_ext, *nxt_b = d_b2, *nxt_e = d_ext2;
+    auto launch_sums = [&](uint32_t r, const Ext& alpha, const Mail& mail, unsigned& g) -> sp1b200_err {
+        if (r < K) {  // contiguous span of blocks per warp (multiple of 32), over the real area only
+            const uint64_t nblk = area >> (r + 1);
+            g = grid_for(nblk);
+            const uint64_t warps = (uint64_t)g * 8, span = std::max<uint64_t>((((nblk + warps - 1) / warps) + 31) / 32 * 32, 32);
+#define SP1_JROUND(k) case k: SP1_LAUNCH(ctx, jagged_round_kernel<k>, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, \
                                          d_eqhi, d_eqlo, lb, dw, nblk, span, d_partial, mail); break;
-        switch (R) { SP1_JROUND(0) SP1_JROUND(1) SP1_JROUND(2) SP1_JROUND(3) SP1_JROUND(4)
-                     default: return sp1b200_set_error("jagged_prove: internal: trace round %u", R); }
+            switch (r) { SP1_JROUND(0) SP1_JROUND(1) SP1_JROUND(2) SP1_JROUND(3) SP1_JROUND(4)
+                         default: return sp1b200_set_error("jagged_prove: internal: trace round %u", r); }
 #undef SP1_JROUND
-        static_assert(JK_MAX == 5, "one jagged_round_kernel instance per round below JK_MAX");
-        return nullptr;
-    };
-    auto launch_fold_to = [&](const Mail& mail, uint32_t* out_b, uint32_t* out_e, unsigned& g) -> sp1b200_err {
-        const uint64_t nout = N >> K, nout_pairs = nout / 2;
-        g = grid_for(nout_pairs);
+            static_assert(JK_MAX == 5, "one jagged_round_kernel instance per round below JK_MAX");
+        } else if (r == K) {
+            const uint64_t nout = N >> K, nout_pairs = nout / 2;
+            g = grid_for(nout_pairs);
 #define SP1_JFOLD(k) case k: SP1_LAUNCH(ctx, jagged_fold_to_kernel<k>, g, 256, 0, seg, d_prefix, (uint32_t)total_cols, d_jp_start, d_coleq, \
-                                        d_eqhi, d_eqlo, lb, dw, area, nout_pairs, out_b, out_e, d_partial, nout, mail); break;
-        switch (K) { SP1_JFOLD(1) SP1_JFOLD(2) SP1_JFOLD(3) SP1_JFOLD(4) SP1_JFOLD(5)
-                     default: return sp1b200_set_error("jagged_prove: internal: fold to level %u", K); }
+                                        d_eqhi, d_eqlo, lb, dw, area, nout_pairs, cur_b, cur_e, d_partial, nout, mail); break;
+            switch (K) { SP1_JFOLD(0) SP1_JFOLD(1) SP1_JFOLD(2) SP1_JFOLD(3) SP1_JFOLD(4) SP1_JFOLD(5)
+                         default: return sp1b200_set_error("jagged_prove: internal: fold to level %u", K); }
 #undef SP1_JFOLD
+        } else {
+            const uint64_t nout = N >> r;
+            g = grid_for((nout + 1) / 2);
+            SP1_LAUNCH(ctx, hadamard_fold_kernel, g, 256, 0, cur_b, cur_e, (nout + 1) / 2, alpha, nxt_b, nxt_e, d_partial, nout, mail);
+            std::swap(cur_b, nxt_b); std::swap(cur_e, nxt_e);
+        }
         return nullptr;
     };
-    uint32_t *cur_b = nullptr, *cur_e = d_ext, *nxt_b = d_b, *nxt_e = K ? d_ext : d_ext2;
-    unsigned prev_g = 0;
-    uint32_t prev_seq = 0;
+    unsigned prev_g;
+    const Mail first = sp1b200_mail_next(ctx);
+    uint32_t prev_seq = first.seq;
+    load_weights();
+    SP1_TRY(launch_sums(0, Ext{}, first, prev_g));
     for (uint32_t rd = 0; rd < lm; rd++) {
-        const uint64_t n = N >> rd;  // current length
-        E4 s2[2];  // eval_0, eval_half
+        E4 s2[2];  // eval_0, eval_half, accumulated by the previous launch
         E4 &e0 = s2[0], &eh = s2[1];
-        unsigned g;
-        if (rd == 0) {
-            const Mail mail = sp1b200_mail_next(ctx);
-            if (K) {
-                load_weights();
-                SP1_TRY(launch_round(0, mail, g));
-            } else {
-                g = grid_for(n / 2);
-                SP1_LAUNCH(ctx, hadamard_sum0_kernel, g, 256, 0, seg, cur_e, n / 2, d_partial, mail);
-            }
-            SP1_TRY(sum_mail_partials(ctx, mail.seq, g, s2));
-        } else {
-            SP1_TRY(sum_mail_partials(ctx, prev_seq, prev_g, s2));  // accumulated by the previous launch
-        }
+        SP1_TRY(sum_mail_partials(ctx, prev_seq, prev_g, s2));
         E4 e1 = round_claim - e0;
         E4 c[3];
         interp_0_1_half(e0, e1, eh * hf::inv(hf::to_monty(4)), c);
@@ -723,8 +625,6 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         point.insert(point.begin(), alpha);
         round_claim = eval3(c, alpha);
         // fix the variable; the same launch accumulates the next round's sums (unless this was the last round)
-        const uint64_t nout = n / 2;
-        const Ext da = to_ext(alpha);
         const Mail mail = sp1b200_mail_next(ctx); prev_seq = mail.seq;
         if (rd < K) {  // w_{rd+1}[t] = w_rd[t mod 2^rd] * (bit rd of t ? alpha : 1 - alpha)
             const size_t m = w.size();
@@ -732,25 +632,10 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             for (size_t t = 0; t < m; t++) { w[m + t] = w[t] * alpha; w[t] = w[t] * (E4::one() - alpha); }
             load_weights();
         }
-        if (rd + 1 < K) {
-            SP1_TRY(launch_round(rd + 1, mail, g));
-        } else if (K && rd + 1 == K) {
-            SP1_TRY(launch_fold_to(mail, nxt_b, nxt_e, g));
-            cur_b = nxt_b; cur_e = nxt_e; nxt_b = d_b2; nxt_e = d_ext2;
-        } else if (rd == 0) {
-            g = grid_for((nout + 1) / 2);
-            SP1_LAUNCH(ctx, hadamard_fold0_kernel, g, 256, 0, seg, cur_e, (nout + 1) / 2, da, nxt_b, nxt_e, d_partial, nout, mail);
-            cur_b = nxt_b; cur_e = nxt_e; nxt_b = d_b2; nxt_e = d_ext;  // d_ext (the materialised polynomial) is free again
-        } else {
-            g = grid_for((nout + 1) / 2);
-            SP1_LAUNCH(ctx, hadamard_fold_kernel, g, 256, 0, cur_b, cur_e, (nout + 1) / 2, da, nxt_b, nxt_e, d_partial, nout, mail);
-            std::swap(cur_b, nxt_b); std::swap(cur_e, nxt_e);
-        }
-        prev_g = g;
+        SP1_TRY(launch_sums(rd + 1, to_ext(alpha), mail, prev_g));
     }
     // component evaluations: base[0] (the dense trace at the sumcheck point), ext[0]
     // (posted by the last fold launch next to its, unused, partial sums: payload EF slot 2)
-    if (lm < 2) return sp1b200_set_error("jagged_prove: fewer than two sumcheck variables (log_m = %u)", lm);
     SP1_TRY(sp1b200_mail_wait(ctx, prev_seq));
     const E4 base_eval = E4::load(sp1b200_mail_host(ctx) + 8);
     t_sc.stop();

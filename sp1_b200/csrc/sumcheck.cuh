@@ -1,7 +1,7 @@
 // Plumbing shared by the sumcheck and PCS drivers (gkr.cu, zerocheck.cu, jagged.cu, pcs.cu; ntt.cu for root_pow): pool scope,
 // launch geometry, the eq table, the block reduction that posts to the mailbox and the host sums of its per-block partials.
 // Everything here is inline or a template (an unused internal-linkage function would be compiled and warned about in every
-// including translation unit); the two table kernels live once, in sumcheck.cu.
+// including translation unit); the table kernels live once, in sumcheck.cu.
 #pragma once
 #include "ctx.cuh"
 #include "hostfield.hpp"
@@ -35,6 +35,12 @@ __device__ __forceinline__ uint32_t root_pow(const uint32_t* __restrict__ TH, co
 sp1b200_err launch_eq_table(sp1b200_ctx* ctx, const uint32_t* d_point, int k, uint32_t* d_out);
 // E'[j] = E[2j] + E[2j+1], j < n_out: drops the last coordinate of the eq point (sumcheck.cu)
 sp1b200_err launch_halve_eq(sp1b200_ctx* ctx, const uint32_t* d_E, uint64_t n_out, uint32_t* d_out);
+
+// `width` base-field columns of `height` rows each, column-major at `cols`; their evaluations go to out[first_out ..]
+struct EvalTable { const uint32_t* cols; uint64_t height; uint32_t width, first_out; };
+// out[t.first_out + c] = sum_{r < t.height} eq[r] * t.cols[c * t.height + r] for every table t, in two launches (sumcheck.cu).
+// d_out holds n_out EF values; the ones no table writes are zero.  Tables with no rows or no columns are skipped.
+sp1b200_err launch_table_evals(sp1b200_ctx* ctx, const std::vector<EvalTable>& tables, const uint32_t* d_eq, uint32_t* d_out, size_t n_out);
 
 // NE extension sums per block -> partial[block][4 NE] (the mailbox payload: the host transcript polls the flag, ctx.cuh); a null
 // mail flag makes it a plain reduction.  Warp shuffles + one barrier (the late sumcheck rounds are latency-bound: a shared-memory

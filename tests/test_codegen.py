@@ -63,6 +63,15 @@ def test_rs_encode_tiles_keep_their_occupancy():
     assert regs <= 32 and spill == 0 and smem == 8192
 
 
+def test_jagged_fold_to_kernels_keep_their_shared_memory():
+    """the level-0 fold pass (odd column starts) needs an eq_lo table of 2^10 EF; the instances the aligned traces run keep 2^9,
+    so their occupancy does not change with it"""
+    t = _ptxas("jagged")
+    for k in range(6):
+        regs, spill, smem = _find(t, f"jagged_fold_to_kernelILi{k}E")
+        assert spill == 0 and smem == (16640 if k == 0 else 8448), (k, regs, spill, smem)
+
+
 def test_permutation_instruction_mix():
     """dynamic opcode histogram of one permutation (tools/sass_dyn.py, loop trip counts 4 / 5 / 4): the subtractive s-box reduction keeps it
     at ~4.9 k instructions (round-1 code: 5 456) with no IMAD.MOV negations and (almost) no IMAD.X carries, 296 wide products"""

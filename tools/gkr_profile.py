@@ -77,16 +77,10 @@ def jagged_bytes_model(area, lm, k):
     that reads it again and writes the level-k dense and eq arrays, then one fix-and-sum pass per round on EF arrays"""
     m = defaultdict(float)
     N = 1 << lm
-    if k == 0:
-        m["jagged_poly_kernel"] = 16 * N
-        m["hadamard_sum0_kernel"] = 4 * area + 16 * N
-        m["hadamard_fold0_kernel"] = 4 * area + 16 * N + 32 * (N >> 1)
-        first = 1
-    else:
+    if k:
         m["jagged_round_kernel"] = k * 4 * area
-        m["jagged_fold_to_kernel"] = 4 * area + 32 * (N >> k)
-        first = k
-    m["hadamard_fold_kernel"] = sum(32 * (N >> r) + 32 * (N >> (r + 1)) for r in range(first, lm))
+    m["jagged_fold_to_kernel"] = 4 * area + 32 * (N >> k)
+    m["hadamard_fold_kernel"] = sum(32 * (N >> r) + 32 * (N >> (r + 1)) for r in range(k, lm))
     return m
 
 
@@ -177,7 +171,7 @@ def main():
         lines.append(f"{n:40s} {cnt[n]:8d} {tot[n]:9.3f} {100 * tot[n] / allms:5.1f}% {1e3 * tot[n] / cnt[n]:9.1f}")
     by_base = defaultdict(float)   # template instances summed: the byte model is per kernel family
     for n, v in tot.items():
-        if n.startswith("gkr_"):
+        if n.startswith(("gkr_", "table_evals_")):   # table_evals_*: the chip openings (sumcheck.cu)
             by_base[re.sub(r"<.*", "", n)] += v
     lines.append(f"{'GKR kernel family':40s} {'ms':>9s} {'model GB':>9s} {'GB/s':>7s}")
     for n in sorted(by_base, key=lambda k: -by_base[k]):
@@ -185,7 +179,7 @@ def main():
         lines.append(f"{n:40s} {by_base[n]:9.3f}" + (f" {gb:9.3f} {gb / (by_base[n] / 1e3):7.0f}" if gb else ""))
     gkr_ms = sum(by_base.values())
     gkr_gb = sum(model.get(n, 0.0) for n in by_base) / 1e9
-    lines.append(f"GKR kernels (gkr_*): {gkr_ms:.3f} ms ({100 * gkr_ms / allms:.1f}% of device time), modelled {gkr_gb:.2f} GB")
+    lines.append(f"GKR kernels (gkr_*, table_evals_*): {gkr_ms:.3f} ms ({100 * gkr_ms / allms:.1f}% of device time), modelled {gkr_gb:.2f} GB")
     area, lm, k = jagged_layout([prep_heights, main_heights], lib.params["log_stacking_height"], mlr)
     jmodel = jagged_bytes_model(area, lm, k)
     jfam = defaultdict(float)   # the jagged sumcheck and the PCS passes over the same trace
