@@ -125,6 +125,7 @@ void sp1b200_ctx_destroy(sp1b200_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->d_TH) cudaFree(c->d_TH);
     if (c->d_TL) cudaFree(c->d_TL);
+    if (c->d_T8) cudaFree(c->d_T8);
     if (c->d_mail_counter) cudaFree(c->d_mail_counter);
     if (c->h_mail) cudaFreeHost(c->h_mail);
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }

@@ -22,6 +22,7 @@ struct sp1b200_ctx {
     // TH[i] = w^(i * 2^12), TL[j] = w^j  with w = two-adic generator of order 2^24 (Montgomery words)
     uint32_t* d_TH = nullptr;
     uint32_t* d_TL = nullptr;
+    uint32_t* d_T8 = nullptr;  // per-pass radix-8 twiddles of the RS-encode kernels (rs_twiddles.cuh), 16 KiB
     uint64_t launches = 0;
     bool force_generic_ntt = false;  // SP1B200_GENERIC_NTT=1: reference (slow) kernels, used to cross-check the fast path
     std::map<std::string, float> phase_ms;

@@ -2,6 +2,7 @@
 // test-suite check the exact code the kernels run (lazy-reduction bounds, half-product Montgomery forms) against the
 // oracle before any GPU time is spent.  Test support only; not part of include/sp1b200.h.
 #include "poseidon2.cuh"
+#include "rs_twiddles.cuh"
 #include "debug_fp.cuh"
 #include "hostfield.hpp"
 #include "zc_lower.hpp"
@@ -48,6 +49,11 @@ void sp1b200_hostcheck_ext_inv(const uint32_t* a, uint32_t* out, uint64_t n) {
         kb::Ext r = kb::ext_inv(x);
         for (int k = 0; k < 4; k++) out[4 * i + k] = r.c[k];
     }
+}
+// the RS-encode kernels' per-pass twiddle table (rs_twiddles.cuh), rs_tw::WORDS words, built by the same code as on the device
+uint32_t sp1b200_hostcheck_rs_tw8(uint32_t* out) {
+    for (uint32_t i = 0; i < rs_tw::WORDS; i++) out[i] = rs_tw::word(i / 8, (int)(i % 8));
+    return rs_tw::WORDS;
 }
 void sp1b200_hostcheck_field(const uint32_t* a, const uint32_t* b, uint32_t* add, uint32_t* sub, uint32_t* mul, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) { add[i] = kb::add(a[i], b[i]); sub[i] = kb::sub(a[i], b[i]); mul[i] = kb::mul(a[i], b[i]); }

@@ -16,6 +16,7 @@
 #include "ctx.cuh"
 #include <cstdlib>
 #include "kb31.cuh"
+#include "rs_twiddles.cuh"
 #include "sumcheck.cuh"
 
 namespace {
@@ -27,6 +28,11 @@ __global__ void init_tables_kernel(uint32_t* TH, uint32_t* TL) {
     uint32_t w = kb::pow(kb::to_monty_c(3), 127);
     TL[i] = kb::pow(w, i);
     TH[i] = kb::pow(w, (uint64_t)i << 12);
+}
+
+__global__ void init_tw8_kernel(uint32_t* T8) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < rs_tw::WORDS) T8[i] = rs_tw::word(i / 8, (int)(i % 8));
 }
 
 // ---- generic step A: coset expansion + size-2^L1 DIF over the strided (hi) axis ---------------------------
@@ -123,23 +129,19 @@ __device__ __forceinline__ void dif8(uint32_t (&v)[8], const uint32_t (&wA)[4], 
     for (int h = 0; h < 8; h += 2) { uint32_t a = v[h], c = v[h + 1]; v[h] = kb::add(a, c); v[h + 1] = submul(a, c, wC); }
 }
 
-// twiddles for a radix-8 pass whose top stage has 2^s points and whose elements are spaced `stride` apart:
-// local element j sits at offset j*stride + low inside its 2^s block  (stride = 2^(s-3))
-__device__ __forceinline__ void load_tw8(const uint32_t* __restrict__ TH, int s, uint32_t low, uint32_t (&wA)[4], uint32_t (&wB)[2],
-                                         uint32_t& wC) {
-    const uint32_t stride = 1u << (s - 3);
-#pragma unroll
-    for (int j = 0; j < 4; j++) wA[j] = __ldg(TH + ((j * stride + low) << (12 - s)));
-#pragma unroll
-    for (int j = 0; j < 2; j++) wB[j] = __ldg(TH + ((j * stride + low) << (13 - s)));
-    wC = __ldg(TH + (low << (14 - s)));
+// twiddles of a radix-8 pass from the per-pass table (rs_twiddles.cuh): entry 2^(s-3) + low for a pass whose top stage has 2^s points,
+// element j of the thread at offset j*2^(s-3) + low of its block; two 16-byte loads that stay L1/L2-hot (16 KiB, shared by every row)
+__device__ __forceinline__ void load_tw8(const uint4* __restrict__ T8, uint32_t entry, uint32_t (&wA)[4], uint32_t (&wB)[2], uint32_t& wC) {
+    const uint4 a = __ldg(T8 + 2 * entry), c = __ldg(T8 + 2 * entry + 1);
+    wA[0] = a.x; wA[1] = a.y; wA[2] = a.z; wA[3] = a.w;
+    wB[0] = c.x; wB[1] = c.y; wC = c.z;
 }
 
 // ---- fast step B: one 2048-point row per block of 256 threads, in place --------------------------------
 __device__ __forceinline__ int swzB(int e) { return e ^ (((e >> 5) & 7) << 2); }
 
 __global__ void __launch_bounds__(256) rs_step_b_2048(uint32_t* __restrict__ buf, int L1, int b, const uint32_t* __restrict__ TH,
-                                                      const uint32_t* __restrict__ TL) {
+                                                      const uint32_t* __restrict__ TL, const uint4* __restrict__ T8) {
     __shared__ uint32_t sm[2048];
     constexpr int L2 = 11;
     const int L = L1 + L2;
@@ -159,39 +161,44 @@ __global__ void __launch_bounds__(256) rs_step_b_2048(uint32_t* __restrict__ buf
 #pragma unroll
         for (int j = 0; j < 8; j++) { v[j] = kb::mul(v[j], tw); if (j < 7) tw = kb::mul(tw, step); }
     }
-    load_tw8(TH, 11, t, wA, wB, wC);
+    load_tw8(T8, 256 + t, wA, wB, wC);
     dif8(v, wA, wB, wC);
+    // swzB only mixes bits 5..7 into bits 2..4, so a multiple of 256 (pass 1, pass 4) or of 32 (pass 2) passes through it
+    const int s1 = swzB(t);
 #pragma unroll
-    for (int j = 0; j < 8; j++) sm[swzB(j * 256 + t)] = v[j];
+    for (int j = 0; j < 8; j++) sm[j * 256 + s1] = v[j];
     __syncthreads();
     // pass 2: bits 7..5
     {
         const int low = t & 31, hib = t >> 5;
+        const int b2 = hib * 256 + low;    // swzB(b2 + 32 j) = (b2 ^ 4 j) + 32 j
 #pragma unroll
-        for (int j = 0; j < 8; j++) v[j] = sm[swzB(hib * 256 + j * 32 + low)];
-        load_tw8(TH, 8, low, wA, wB, wC);
+        for (int j = 0; j < 8; j++) v[j] = sm[(b2 ^ (j << 2)) + j * 32];
+        load_tw8(T8, 32 + low, wA, wB, wC);
         dif8(v, wA, wB, wC);
 #pragma unroll
-        for (int j = 0; j < 8; j++) sm[swzB(hib * 256 + j * 32 + low)] = v[j];
+        for (int j = 0; j < 8; j++) sm[(b2 ^ (j << 2)) + j * 32] = v[j];
     }
     __syncthreads();
     // pass 3: bits 4..2
     {
         const int low = t & 3, hib = t >> 2;
+        const int b3 = swzB(hib * 32 + low);   // swzB(hib 32 + 4 j + low) = b3 ^ 4 j
 #pragma unroll
-        for (int j = 0; j < 8; j++) v[j] = sm[swzB(hib * 32 + j * 4 + low)];
-        load_tw8(TH, 5, low, wA, wB, wC);
+        for (int j = 0; j < 8; j++) v[j] = sm[b3 ^ (j << 2)];
+        load_tw8(T8, 4 + low, wA, wB, wC);
         dif8(v, wA, wB, wC);
 #pragma unroll
-        for (int j = 0; j < 8; j++) sm[swzB(hib * 32 + j * 4 + low)] = v[j];
+        for (int j = 0; j < 8; j++) sm[b3 ^ (j << 2)] = v[j];
     }
     __syncthreads();
     // pass 4: bits 1..0 (radix 4, only non-trivial twiddle is the 4th root), two groups per thread, 16-byte I/O
     const uint32_t w4 = __ldg(TH + 1024);
+    const int s4 = swzB(4 * t);
 #pragma unroll
     for (int k = 0; k < 2; k++) {
         const int g = t + k * 256;
-        uint4 x = *reinterpret_cast<const uint4*>(&sm[swzB(4 * g)]);
+        uint4 x = *reinterpret_cast<const uint4*>(&sm[k * 1024 + s4]);
         uint32_t a0 = kb::add(x.x, x.z), a1 = kb::add(x.y, x.w);
         uint32_t a2 = kb::sub(x.x, x.z), a3 = submul(x.y, x.w, w4);
         uint4 y = make_uint4(kb::add(a0, a1), kb::sub(a0, a1), kb::add(a2, a3), kb::sub(a2, a3));
@@ -201,11 +208,19 @@ __global__ void __launch_bounds__(256) rs_step_b_2048(uint32_t* __restrict__ buf
 
 // ---- fast step A: tile of 8 consecutive lo x all 2^L1 hi, L1 = 3*NP + 1, 2^L1 threads ----------------------
 __device__ __forceinline__ int swzA(int e) { return e ^ (((e >> 7) & 1) << 4); }
+// swzA(base + j * stride) with the swizzle of `base` formed once: a multiple of 256 leaves bit 7 alone, 128 flips it with j
+__device__ __forceinline__ int swzA_at(int base, int sbase, int j, int stride) {
+    if (stride % 256 == 0) return sbase + j * stride;
+    if (stride == 128) return (sbase ^ ((j & 1) << 4)) + j * 128;
+    return swzA(base + j * stride);
+}
 
-// MINB = 2 caps the kernel at 32 registers (9 words spill to local memory) so that two 1024-thread blocks share an SM
+// MINB = 2 caps the kernel at 32 registers (no spill with the table twiddles and the hoisted swizzles) so that two 1024-thread blocks
+// share an SM
 template <int L1, int MINB = 1>
 __global__ void __launch_bounds__(1 << L1, MINB) rs_step_a_fast(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int L2, int b,
-                                                          const uint32_t* __restrict__ TH, const uint32_t* __restrict__ TL) {
+                                                          const uint32_t* __restrict__ TH, const uint32_t* __restrict__ TL,
+                                                          const uint4* __restrict__ T8) {
     static_assert(L1 % 3 == 1 && L1 >= 7, "L1 = 3k+1, at least two radix-8 passes");
     constexpr int NP = L1 / 3;           // radix-8 passes; the last stage (hi bit 0) is a warp shuffle
     constexpr int TILE = 8 << L1;
@@ -226,6 +241,10 @@ __global__ void __launch_bounds__(1 << L1, MINB) rs_step_a_fast(const uint32_t* 
         if (r == 0) {
 #pragma unroll
             for (int j = 0; j < 8; j++) v[j] = src[j];
+        } else if (sh >= 12) {
+            // zeta^(hi r) = TH[(hi r) << (sh - 12)]: one table load per element (4 distinct addresses per warp) instead of a product chain
+#pragma unroll
+            for (int j = 0; j < 8; j++) v[j] = kb::mul(src[j], __ldg(TH + (((uint32_t)(j * (1 << (L1 - 3)) + x) * r) << (sh - 12))));
         } else {
             uint32_t tw = root_pow(TH, TL, ((uint32_t)x * r) << sh);
             const uint32_t step = root_pow(TH, TL, ((uint32_t)r << (L1 - 3)) << sh);
@@ -233,10 +252,11 @@ __global__ void __launch_bounds__(1 << L1, MINB) rs_step_a_fast(const uint32_t* 
             for (int j = 0; j < 8; j++) { v[j] = kb::mul(src[j], tw); if (j < 7) tw = kb::mul(tw, step); }
         }
         // pass 0: hi bits L1-1 .. L1-3
-        load_tw8(TH, L1, x, wA, wB, wC);
+        load_tw8(T8, (1u << (L1 - 3)) + x, wA, wB, wC);
         dif8(v, wA, wB, wC);
+        const int su = swzA(u);
 #pragma unroll
-        for (int j = 0; j < 8; j++) sm[swzA(j * (TILE / 8) + u)] = v[j];
+        for (int j = 0; j < 8; j++) sm[swzA_at(u, su, j, TILE / 8)] = v[j];
         __syncthreads();
 #pragma unroll
         for (int k = 1; k < NP; k++) {
@@ -245,13 +265,14 @@ __global__ void __launch_bounds__(1 << L1, MINB) rs_step_a_fast(const uint32_t* 
             const int low = x & ((1 << nlow) - 1), high = x >> nlow;
             const int base = ((high << (hb + 1)) + low) * 8 + lo;
             const int stride = 8 << nlow;
+            const int sbase = swzA(base);
 #pragma unroll
-            for (int j = 0; j < 8; j++) v[j] = sm[swzA(base + j * stride)];
-            load_tw8(TH, hb + 1, low, wA, wB, wC);
+            for (int j = 0; j < 8; j++) v[j] = sm[swzA_at(base, sbase, j, stride)];
+            load_tw8(T8, (1u << (hb - 2)) + low, wA, wB, wC);
             dif8(v, wA, wB, wC);
             if (k < NP - 1) {
 #pragma unroll
-                for (int j = 0; j < 8; j++) sm[swzA(base + j * stride)] = v[j];
+                for (int j = 0; j < 8; j++) sm[swzA_at(base, sbase, j, stride)] = v[j];
                 __syncthreads();
             } else {
                 // last stage: hi bit 0 lives in bit 3 of the thread index -> partner lane = lane ^ 8, twiddle 1
@@ -276,7 +297,7 @@ static sp1b200_err launch_step_a_fast(sp1b200_ctx* ctx, const uint32_t* in, uint
     const size_t smem = 2 * (size_t)(8 << L1) * sizeof(uint32_t);
     SP1_CUDA(cudaFuncSetAttribute(rs_step_a_fast<L1, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 g((1u << L2) / 8, nc);
-    SP1_LAUNCH(ctx, (rs_step_a_fast<L1, MINB>), g, 1 << L1, smem, in, out, L2, b, ctx->d_TH, ctx->d_TL);
+    SP1_LAUNCH(ctx, (rs_step_a_fast<L1, MINB>), g, 1 << L1, smem, in, out, L2, b, ctx->d_TH, ctx->d_TL, reinterpret_cast<const uint4*>(ctx->d_T8));
     return nullptr;
 }
 
@@ -284,6 +305,8 @@ sp1b200_err sp1b200_init_tables(sp1b200_ctx* ctx) {
     SP1_CUDA(cudaMalloc(&ctx->d_TH, 4096 * sizeof(uint32_t)));
     SP1_CUDA(cudaMalloc(&ctx->d_TL, 4096 * sizeof(uint32_t)));
     SP1_LAUNCH(ctx, init_tables_kernel, 16, 256, 0, ctx->d_TH, ctx->d_TL);
+    SP1_CUDA(cudaMalloc(&ctx->d_T8, rs_tw::WORDS * sizeof(uint32_t)));
+    SP1_LAUNCH(ctx, init_tw8_kernel, rs_tw::WORDS / 256, 256, 0, ctx->d_T8);
     return nullptr;
 }
 
@@ -319,14 +342,14 @@ sp1b200_err sp1b200_rs_encode_device(sp1b200_ctx* ctx, const uint32_t* d_msg, ui
     for (uint64_t c0 = 0; c0 < ncols; c0 += group) {
         unsigned nc = (unsigned)((ncols - c0 < group) ? (ncols - c0) : group);
         dim3 gA((1u << L2) / T, nc), gB(1u << (L1 + b), nc);
-        // two 1024-thread blocks per SM (32 registers, a few words of spill) instead of one 52-register block; SP1B200_RS_A_OCC2=0
+        // two 1024-thread blocks per SM (32 registers) instead of one 52-register block; SP1B200_RS_A_OCC2=0
         // selects the one-block build
         static const bool occ2 = [] { const char* e = getenv("SP1B200_RS_A_OCC2"); return !(e && e[0] == '0'); }();
         if (fast && L1 == 10 && occ2) SP1_TRY((launch_step_a_fast<10, 2>(ctx, d_msg + c0 * n, d_out + c0 * M, L2, b, nc)));
         else if (fast && L1 == 10) SP1_TRY(launch_step_a_fast<10>(ctx, d_msg + c0 * n, d_out + c0 * M, L2, b, nc));
         else if (fast && L1 == 7) SP1_TRY(launch_step_a_fast<7>(ctx, d_msg + c0 * n, d_out + c0 * M, L2, b, nc));
         else SP1_LAUNCH(ctx, rs_step_a_generic, gA, threadsA, smemA, d_msg + c0 * n, d_out + c0 * M, L1, L2, b, T, ctx->d_TH, ctx->d_TL);
-        if (fast) SP1_LAUNCH(ctx, rs_step_b_2048, gB, 256, 0, d_out + c0 * M, L1, b, ctx->d_TH, ctx->d_TL);
+        if (fast) SP1_LAUNCH(ctx, rs_step_b_2048, gB, 256, 0, d_out + c0 * M, L1, b, ctx->d_TH, ctx->d_TL, reinterpret_cast<const uint4*>(ctx->d_T8));
         else SP1_LAUNCH(ctx, rs_step_b_generic, gB, threadsB, smemB, d_out + c0 * M, L1, L2, b, ctx->d_TH, ctx->d_TL);
     }
     return nullptr;
