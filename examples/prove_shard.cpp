@@ -57,7 +57,14 @@ int main(int argc, char** argv) {
 
         sp1b200::AirProver prover(0, params, chips, blob);
         sp1b200::ProvingKey pk = prover.setup_from_vk(prep.data(), heights);
+        sp1b200::Challenger vch = ch;   // the verifier starts from the same post-vk transcript
         const std::vector<uint32_t> proof = prover.prove_shard_with_pk(pk, main_dense.data(), heights, pv, ch);
+        // check the proof just made before it leaves this process
+        bool has_prep = false;
+        for (const auto& c : chips) has_prep |= c.preprocessed_width != 0;
+        const sp1b200::AirProver::Verdict verdict = prover.verify_shard(has_prep ? &pk.commit : nullptr, proof, heights, vch);
+        std::printf("verify_shard: %s\n", verdict.reason.c_str());
+        if (!verdict.accepted() || vch != ch) { std::fprintf(stderr, "prove_shard: the proof does not verify (%s)\n", verdict.reason.c_str()); return 1; }
 
         std::ofstream out(argv[2], std::ios::binary);
         out.write(reinterpret_cast<const char*>(pk.commit.data()), 32);

@@ -306,6 +306,74 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
                                              const uint32_t* h_main_w, const uint32_t* h_prep_w, const uint8_t* h_bytes, uint64_t n_bytes,
                                              uint64_t* h_heights_out, uint32_t* h_proof, uint64_t cap_words, uint64_t* h_words);
 
+/* ---- shard verifier (ShardVerifier::verify_shard, crates/hypercube/src/verifier/shard.rs:437-750) ---------------------------------
+ * Checks the flat words of sp1b200_prove_shard against the machine, the chip heights and names and the context's parameters
+ * (log_stacking_height, max_log_row_count, log_blowup, num_queries and the three PoW bit counts) the prover used.
+ * h_prep_commit8: the verifying key's preprocessed commitment (NULL when no chip has preprocessed columns).  h_challenger34: the
+ * transcript after the caller observed the verifying key (the state sp1b200_prove_shard starts from).  Heights come from the caller:
+ * the flat words do not carry the proof's `degree` points (sp1b200_shard_proof_from_bincode recovers them from bincode(ShardProof)).
+ * Every Merkle opening, the BaseFold query fold chains and the jagged evaluation's column sum run on the device (context stream and
+ * pool); the transcript, the PoW checks, the sumcheck rounds and the constraints at the zerocheck point run on the host.
+ *
+ * *h_verdict = SP1B200_VERDICT_ACCEPT: the proof is valid and h_challenger34 holds the verifier's final state (equal to the prover's).
+ * Any other verdict rejects the proof and names the first failing check, in verify_shard's order; h_challenger34 is then left
+ * unchanged.  A rejection is not an error.  Errors: the words do not parse as a proof of this machine's shape (section lengths,
+ * counts beyond the layout's limits, opening heights other than the context's, trailing words, a field word >= p), malformed
+ * arguments (a height >= 2^(max_log_row_count+1), a public value index beyond the proof's public values, NULL pointers), device
+ * failures.  The context stays usable after a rejection or an error.
+ * Not checked, as they need the Rust machine definition: the public-values length against PROOF_MAX_NUM_PVS, chip clusters, and the
+ * machine-specific public-values interactions (the expected LogUp cumulative sum is 0). */
+#define SP1B200_VERDICT_ACCEPT 0u
+#define SP1B200_VERDICT_POW 1u                          /* "Pow": the LogUp-GKR or the BaseFold query grinding witness */
+#define SP1B200_VERDICT_INVALID_SHAPE 2u                /* "InvalidShape": GKR output length, zerocheck rounds */
+#define SP1B200_VERDICT_ZERO_DENOMINATOR 3u             /* "ZeroDenominator" */
+#define SP1B200_VERDICT_CUMULATIVE_SUM_MISMATCH 4u      /* "CumulativeSumMismatch" */
+#define SP1B200_VERDICT_INVALID_SHAPE_ROUNDS 5u         /* "InvalidShape(rounds)": GKR layer count */
+#define SP1B200_VERDICT_INCONSISTENT_SUMCHECK_CLAIM 6u  /* "InconsistentSumcheckClaim": GKR layer claim */
+#define SP1B200_VERDICT_SUMCHECK_PROOF_SHAPE 7u         /* "InvalidProofShape": a sumcheck's round count or degree */
+#define SP1B200_VERDICT_SUMCHECK_CLAIMED_SUM 8u         /* "InconsistencyWithClaimedSum": a sumcheck's first round */
+#define SP1B200_VERDICT_SUMCHECK_ROUND 9u               /* "SumcheckRoundInconsistency" */
+#define SP1B200_VERDICT_SUMCHECK_POINT 10u              /* "InvalidProofShape(point)" */
+#define SP1B200_VERDICT_SUMCHECK_EVAL 11u               /* "InconsistencyWithEval": a sumcheck's final evaluation */
+#define SP1B200_VERDICT_INCONSISTENT_EVALUATION 12u     /* "InconsistentEvaluation": GKR layer evaluation */
+#define SP1B200_VERDICT_LAST_LAYER_DIMENSION 13u        /* "InvalidLastLayerDimension" */
+#define SP1B200_VERDICT_TRACE_POINT_MISMATCH 14u        /* "TracePointMismatch" */
+#define SP1B200_VERDICT_INVALID_SHAPE_OPENINGS 15u      /* "InvalidShape(openings)" */
+#define SP1B200_VERDICT_NUMERATOR_EVALUATION 16u        /* "NumeratorEvaluationMismatch" */
+#define SP1B200_VERDICT_DENOMINATOR_EVALUATION 17u      /* "DenominatorEvaluationMismatch" */
+#define SP1B200_VERDICT_OPENING_SHAPE 18u               /* "OpeningShape" */
+#define SP1B200_VERDICT_HEIGHT_BITS 19u                 /* "InvalidHeightBitDecomposition" */
+#define SP1B200_VERDICT_HEIGHT_TOO_LARGE 20u            /* "HeightTooLarge": a height above 2^max_log_row_count */
+#define SP1B200_VERDICT_CONSTRAINTS_EVAL 21u            /* "ConstraintsCheckFailed(InconsistencyWithEval)" */
+#define SP1B200_VERDICT_CONSTRAINTS_CLAIMED_SUM 22u     /* "ConstraintsCheckFailed(InconsistencyWithClaimedSum)" */
+#define SP1B200_VERDICT_INCORRECT_SHAPE 23u             /* "IncorrectShape": jagged / stacked shapes */
+#define SP1B200_VERDICT_INCORRECT_TABLE_SIZES 24u       /* "IncorrectTableSizes": row/column counts or commitments */
+#define SP1B200_VERDICT_AREA_OUT_OF_BOUNDS 25u          /* "AreaOutOfBounds" */
+#define SP1B200_VERDICT_DUMMY_TABLES 26u                /* "IncorrectShape(dummy tables)" */
+#define SP1B200_VERDICT_SUMCHECK_CLAIM_MISMATCH 27u     /* "SumcheckClaimMismatch": jagged claim */
+#define SP1B200_VERDICT_MONOTONICITY 28u                /* "MonotonicityCheckFailed" */
+#define SP1B200_VERDICT_JAGGED_EVALUATION 29u           /* "JaggedEvaluationFailed" */
+#define SP1B200_VERDICT_JAGGED_EVAL_PROOF 30u           /* "JaggedEvalProofVerificationFailed" */
+#define SP1B200_VERDICT_STACKING 31u                    /* "StackingError" */
+#define SP1B200_VERDICT_BATCH_POW 32u                   /* "BatchPow" */
+#define SP1B200_VERDICT_FRI_LENGTH 33u                  /* "SumcheckFriLengthMismatch" */
+#define SP1B200_VERDICT_BASEFOLD_SUMCHECK 34u           /* "Sumcheck": a BaseFold univariate message */
+#define SP1B200_VERDICT_TWO_ADICITY 35u                 /* "TwoAdicityOverflow" */
+#define SP1B200_VERDICT_TCS_COMPONENT 36u               /* "TcsError(component)": a commitment round's opening */
+#define SP1B200_VERDICT_QUERY_VALUE 37u                 /* "QueryValueMismatch" */
+#define SP1B200_VERDICT_TCS_QUERY 38u                   /* "TcsError(query)": a fold round's opening */
+#define SP1B200_VERDICT_QUERY_FINAL_POLY 39u            /* "QueryFinalPolyMismatch" */
+#define SP1B200_VERDICT_SUMCHECK_FINAL_POLY 40u         /* "SumcheckFinalPolyMismatch" */
+#define SP1B200_VERDICT_PREPROCESSED_WIDTHS 41u         /* "InvalidShape(preprocessed widths)": the preprocessed round's leading
+                                                           column counts differ from the chips' preprocessed widths (shard.rs:506-523) */
+#define SP1B200_VERDICT_CHIP_TABLES 42u                 /* "InvalidShape(chip tables)": a round's table row counts differ from the
+                                                           chip heights or its column counts from the chip widths (shard.rs:662-742) */
+sp1b200_err sp1b200_verify_shard(sp1b200_ctx* ctx, const sp1b200_machine* machine, const uint32_t* h_prep_commit8,
+                                 const uint64_t* h_heights, const char* const* chip_names, const uint32_t* h_proof, uint64_t n_words,
+                                 uint32_t* h_challenger34, uint32_t* h_verdict);
+/* the name of a verdict code (the reason string above; "Accepted" for 0, "Unknown" beyond the list) */
+const char* sp1b200_verdict_name(uint32_t verdict);
+
 #ifdef __cplusplus
 }
 #endif

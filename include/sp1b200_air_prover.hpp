@@ -174,6 +174,28 @@ class AirProver {
         return {std::move(pk), std::vector<uint32_t>(proof_buf_.begin(), proof_buf_.begin() + n)};
     }
 
+    // ShardVerifier::verify_shard (crates/hypercube/src/verifier/shard.rs:437-750) on proof words of prove_shard_with_pk /
+    // setup_and_prove_shard (sp1b200_verify_shard).  prep_commit: the verifying key's preprocessed commitment (nullptr when no chip has
+    // preprocessed columns); `challenger` is the transcript after the verifying key was observed, the state the prover started from.
+    // On acceptance `challenger` becomes the verifier's final state (equal to the prover's); on rejection it is left unchanged and the
+    // verdict names the first failing check.  Words that do not parse as a proof of this machine throw.
+    struct Verdict {
+        uint32_t code = SP1B200_VERDICT_ACCEPT;
+        std::string reason;
+        bool accepted() const { return code == SP1B200_VERDICT_ACCEPT; }
+    };
+    Verdict verify_shard(const Digest* prep_commit, const std::vector<uint32_t>& proof_words, const std::vector<uint64_t>& heights,
+                         Challenger& challenger) {
+        if (heights.size() != chips_.size()) throw Error("verify_shard: one height per chip expected");
+        std::vector<const char*> names;
+        for (const Chip& c : chips_) names.push_back(c.name.c_str());
+        Verdict v;
+        check(sp1b200_verify_shard(ctx_, machine_, prep_commit ? prep_commit->data() : nullptr, heights.data(), names.data(), proof_words.data(),
+                                   proof_words.size(), challenger.data(), &v.code));
+        v.reason = sp1b200_verdict_name(v.code);
+        return v;
+    }
+
     // bincode(ShardProof) of a proof returned by prove_shard_with_pk / setup_and_prove_shard: the bytes the reference's workers, recursion
     // tree and verifier exchange (crates/hypercube/src/verifier/proof.rs:47-61; sp1b200_shard_proof_to_bincode)
     std::vector<uint8_t> to_bincode(const std::vector<uint32_t>& proof_words, const std::vector<uint64_t>& heights) const {

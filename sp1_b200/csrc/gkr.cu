@@ -36,16 +36,6 @@ namespace {
 using kb::Ext;
 using hf::E4;
 
-struct TermDev { uint32_t source, col, weight; };
-struct VColDev { uint32_t term_start, n_terms, constant; };
-struct InterDev { uint32_t is_send, arg_index, n_values, vcol_start; };
-
-struct HostInteractions {  // parsed from the machine blob's interaction section
-    std::vector<std::vector<InterDev>> per_chip;
-    std::vector<VColDev> vcols;
-    std::vector<TermDev> terms;
-};
-
 struct ChipJob {           // one chip inside a batched launch
     uint64_t work_start;   // prefix of work items
     uint64_t in_off, out_off;  // element offsets of the chip's arrays in the in / out arenas

@@ -24,6 +24,17 @@ struct HostProg {  // host copy for the padded-row adjustment (one evaluation on
     std::vector<std::pair<uint32_t, uint32_t>> zc_pieces;
 };
 
+// LogUp interactions (crates/hypercube/src/lookup/interaction.rs:11-22), parsed from the machine blob's interaction section (gkr.cu).
+// A virtual column is constant + sum weight * column; an interaction's multiplicity is vcols[vcol_start], its values follow.
+struct TermDev { uint32_t source, col, weight; };
+struct VColDev { uint32_t term_start, n_terms, constant; };
+struct InterDev { uint32_t is_send, arg_index, n_values, vcol_start; };
+struct HostInteractions {
+    std::vector<std::vector<InterDev>> per_chip;   // sends first, then receives
+    std::vector<VColDev> vcols;
+    std::vector<TermDev> terms;
+};
+
 void sp1b200_free_interactions(void* p);
 
 struct sp1b200_machine {

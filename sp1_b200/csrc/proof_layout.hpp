@@ -1,0 +1,197 @@
+// The flat proof words of sp1b200_prove_shard, read in one place: the wire format (wire.cu) and the shard verifier (verify.cu) both
+// walk a proof through parse_shard_proof, so the two cannot disagree about the layout.  Host code only.
+//
+// Words: [5][len_0..len_4] then the sections
+//   0 main commitment (8)
+//   1 LogUp-GKR: n_out | numerator ext[n_out] | denominator ext[n_out] | n_rounds | per round {n0 n1 d0 d1 ext, sumcheck} |
+//     point ext[max_log_row_count] | per chip {main openings ext[main_w], preprocessed openings ext[prep_w]} | witness
+//   2 zerocheck: sumcheck | per chip {preprocessed evaluations ext[prep_w], main evaluations ext[main_w]}
+//   3 evaluation proof: univariate_messages ext[2 log_stacking_height] | fri_commitments digest[log_stacking_height] |
+//     per commitment round an opening of width ncols[round] | per fold round an opening of width 8 | final_poly ext |
+//     pow_witness | batch_grinding_witness | batch_evaluations ext[ncols[round]] per round | Hadamard sumcheck | jagged-eval sumcheck |
+//     per round {n_tables, (rows, cols) per table} | original commitments digest[n_rounds] | expected_eval ext | max_log_row_count | log_m
+//   4 public values
+// sumcheck = n_polys | per poly {n_coeffs, coeffs ext} | claimed_sum ext | point ext[n_polys] | eval ext
+// opening  = values[num_queries][width] | root digest | log_height | width | paths digest[num_queries][log_height]
+// Every length read from the words is checked against the words that remain before it is used.
+#pragma once
+#include <algorithm>
+#include <cstddef>
+#include <cstdint>
+#include <utility>
+#include <vector>
+
+namespace layout {
+
+// limits on the counts a proof carries (anything larger cannot come from a prover of this library)
+constexpr uint32_t MAX_GKR_OUTPUTS = 1u << 24;
+constexpr uint32_t MAX_ROUNDS = 64;         // GKR layers
+constexpr uint32_t MAX_SUMCHECK_VARS = 4096;
+constexpr uint32_t MAX_COEFFS = 64;
+constexpr uint32_t MAX_LOG_HEIGHT = 64;
+constexpr uint32_t MAX_TABLES = 1u << 20;
+
+struct FlatReader {
+    const uint32_t* p; const uint32_t* end; bool ok = true;
+    uint32_t u() { if (p >= end) { ok = false; return 0; } return *p++; }
+    const uint32_t* take(size_t n) { if ((size_t)(end - p) < n) { ok = false; p = end; return nullptr; } const uint32_t* r = p; p += n; return r; }
+};
+
+struct Sumcheck {
+    std::vector<const uint32_t*> polys;   // coefficients, ext each
+    std::vector<uint32_t> n_coeffs;
+    const uint32_t* claimed_sum = nullptr;
+    const uint32_t* point = nullptr;      // ext[polys.size()]
+    const uint32_t* eval = nullptr;
+};
+struct Opening {
+    const uint32_t* values = nullptr;     // [num_queries][width]
+    const uint32_t* root = nullptr;
+    uint32_t log_height = 0, width = 0;
+    const uint32_t* paths = nullptr;      // [num_queries][log_height] digests
+};
+struct GkrRound { const uint32_t* nd = nullptr; Sumcheck sc; };   // nd: n0 n1 d0 d1, ext each
+
+// The machine's side of the layout: chip widths, the protocol parameters and the stacked column count of every commitment round.
+struct Shape {
+    size_t n_chips = 0;
+    const uint32_t* main_w = nullptr; const uint32_t* prep_w = nullptr;
+    uint32_t max_log_row_count = 0, log_stacking_height = 0, num_queries = 0;
+    std::vector<size_t> ncols;            // per commitment round: {preprocessed,} main
+};
+
+// ncols of a shard: ceil(area / 2^log_stacking_height), at least 1, per round (a preprocessed round only if a chip has such columns)
+inline std::vector<size_t> round_columns(size_t n_chips, const uint64_t* heights, const uint32_t* main_w, const uint32_t* prep_w, uint32_t log_stack) {
+    uint64_t prep_area = 0, main_area = 0; bool has_prep = false;
+    for (size_t k = 0; k < n_chips; k++) {
+        main_area += heights[k] * main_w[k];
+        if (prep_w[k]) { has_prep = true; prep_area += heights[k] * prep_w[k]; }
+    }
+    const uint64_t S = (uint64_t)1 << log_stack;
+    std::vector<size_t> n;
+    if (has_prep) n.push_back((size_t)std::max<uint64_t>((prep_area + S - 1) / S, 1));
+    n.push_back((size_t)std::max<uint64_t>((main_area + S - 1) / S, 1));
+    return n;
+}
+
+struct ShardProof {
+    const uint32_t* commit = nullptr;
+    const uint32_t* pv = nullptr; uint32_t n_pv = 0;
+    // LogUp-GKR
+    uint32_t n_out = 0; const uint32_t* out_num = nullptr; const uint32_t* out_den = nullptr;
+    std::vector<GkrRound> rounds;
+    const uint32_t* gkr_point = nullptr;
+    std::vector<const uint32_t*> gkr_main, gkr_prep;
+    const uint32_t* gkr_witness = nullptr;
+    // zerocheck
+    Sumcheck zc;
+    std::vector<const uint32_t*> zc_prep, zc_main;
+    // evaluation proof
+    const uint32_t* univariate = nullptr;   // ext[2 * log_stacking_height]
+    const uint32_t* fri_commits = nullptr;  // digest[log_stacking_height]
+    std::vector<Opening> component, query;
+    const uint32_t* final_poly = nullptr;
+    const uint32_t* pow_witness = nullptr; const uint32_t* batch_witness = nullptr;
+    std::vector<const uint32_t*> batch_evals;
+    Sumcheck jagged_sc, jagged_eval;
+    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> rc_cc;
+    const uint32_t* merkle_commits = nullptr;
+    const uint32_t* expected_eval = nullptr;
+    uint32_t max_log_rows = 0, log_m = 0;
+};
+
+inline bool read_sumcheck(FlatReader& r, Sumcheck& s) {
+    const uint32_t n = r.u();
+    if (!r.ok || n > MAX_SUMCHECK_VARS) return false;
+    s.polys.resize(n); s.n_coeffs.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t m = r.u();
+        if (!r.ok || m > MAX_COEFFS) return false;
+        s.n_coeffs[i] = m;
+        s.polys[i] = r.take(4 * (size_t)m);
+    }
+    s.claimed_sum = r.take(4);
+    s.point = r.take(4 * (size_t)n);
+    s.eval = r.take(4);
+    return r.ok;
+}
+
+// nullptr, or what is wrong with the opening
+inline const char* read_opening(FlatReader& r, Opening& o, size_t nq, size_t width) {
+    o.values = r.take(nq * width);
+    o.root = r.take(8);
+    o.log_height = r.u(); o.width = r.u();
+    if (r.ok && (o.width != width || o.log_height > MAX_LOG_HEIGHT)) return "evaluation proof section: opening width / height words do not match the layout";
+    if (r.ok) o.paths = r.take(nq * (size_t)o.log_height * 8);
+    return r.ok ? nullptr : "evaluation proof section: section is shorter than its layout";
+}
+
+// Splits and walks the words.  Returns nullptr on success, else what is wrong (prefixed by the section).
+inline const char* parse_shard_proof(const uint32_t* w, uint64_t n_words, const Shape& s, ShardProof& v) {
+    if (!w || n_words < 6 || w[0] != 5) return "not a shard proof (header)";
+    const uint64_t l0 = w[1], l1 = w[2], l2 = w[3], l3 = w[4], l4 = w[5];
+    if (6 + l0 + l1 + l2 + l3 + l4 != n_words || l0 != 8) return "section lengths do not add up";
+    const uint32_t* s0 = w + 6; const uint32_t* s1 = s0 + l0; const uint32_t* s2 = s1 + l1; const uint32_t* s3 = s2 + l2; const uint32_t* s4 = s3 + l3;
+    v.commit = s0; v.pv = s4; v.n_pv = (uint32_t)l4;
+    const size_t nch = s.n_chips, nq = s.num_queries;
+    const uint32_t mlr = s.max_log_row_count, ls = s.log_stacking_height;
+    {   // LogUp-GKR
+        FlatReader r{s1, s2};
+        v.n_out = r.u();
+        if (!r.ok || v.n_out > MAX_GKR_OUTPUTS) return "LogUp-GKR section: output count out of range";
+        v.out_num = r.take(4 * (size_t)v.n_out); v.out_den = r.take(4 * (size_t)v.n_out);
+        const uint32_t nr = r.u();
+        if (!r.ok || nr > MAX_ROUNDS) return "LogUp-GKR section: round count out of range";
+        v.rounds.resize(nr);
+        for (auto& q : v.rounds) {
+            q.nd = r.take(16);
+            if (!read_sumcheck(r, q.sc)) return "LogUp-GKR section: malformed round sumcheck";
+        }
+        v.gkr_point = r.take(4 * (size_t)mlr);
+        v.gkr_main.resize(nch); v.gkr_prep.resize(nch);
+        for (size_t k = 0; k < nch; k++) { v.gkr_main[k] = r.take(4 * (size_t)s.main_w[k]); v.gkr_prep[k] = r.take(4 * (size_t)s.prep_w[k]); }
+        v.gkr_witness = r.take(1);
+        if (!r.ok) return "LogUp-GKR section: section is shorter than its layout";
+        if (r.p != s2) return "LogUp-GKR section: trailing words";
+    }
+    {   // zerocheck and opened values
+        FlatReader r{s2, s3};
+        if (!read_sumcheck(r, v.zc)) return "zerocheck section: malformed sumcheck";
+        v.zc_prep.resize(nch); v.zc_main.resize(nch);
+        for (size_t k = 0; k < nch; k++) { v.zc_prep[k] = r.take(4 * (size_t)s.prep_w[k]); v.zc_main[k] = r.take(4 * (size_t)s.main_w[k]); }
+        if (!r.ok) return "zerocheck section: section is shorter than its layout";
+        if (r.p != s3) return "zerocheck section: trailing words";
+    }
+    {   // evaluation proof
+        FlatReader r{s3, s4};
+        const size_t n_rounds = s.ncols.size();
+        v.univariate = r.take(8 * (size_t)ls);
+        v.fri_commits = r.take(8 * (size_t)ls);
+        if (!r.ok) return "evaluation proof section: section is shorter than its layout";
+        v.component.resize(n_rounds); v.query.resize(ls);
+        for (size_t q = 0; q < n_rounds; q++)
+            if (const char* e = read_opening(r, v.component[q], nq, s.ncols[q])) return e;
+        for (uint32_t q = 0; q < ls; q++)
+            if (const char* e = read_opening(r, v.query[q], nq, 8)) return e;
+        v.final_poly = r.take(4); v.pow_witness = r.take(1); v.batch_witness = r.take(1);
+        v.batch_evals.resize(n_rounds);
+        for (size_t q = 0; q < n_rounds; q++) v.batch_evals[q] = r.take(4 * s.ncols[q]);
+        if (!r.ok) return "evaluation proof section: section is shorter than its layout";
+        if (!read_sumcheck(r, v.jagged_sc) || !read_sumcheck(r, v.jagged_eval)) return "evaluation proof section: malformed sumcheck";
+        v.rc_cc.resize(n_rounds);
+        for (auto& t : v.rc_cc) {
+            const uint32_t cnt = r.u();
+            if (!r.ok || cnt > MAX_TABLES || (uint64_t)cnt * 2 > (uint64_t)(r.end - r.p)) return "evaluation proof section: table count out of range";
+            t.resize(cnt);
+            for (auto& rc : t) { rc.first = r.u(); rc.second = r.u(); }
+        }
+        v.merkle_commits = r.take(8 * n_rounds);
+        v.expected_eval = r.take(4);
+        v.max_log_rows = r.u(); v.log_m = r.u();
+        if (!r.ok) return "evaluation proof section: section is shorter than its layout";
+        if (r.p != s4) return "evaluation proof section: trailing words";
+    }
+    return nullptr;
+}
+
+}  // namespace layout

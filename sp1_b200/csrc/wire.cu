@@ -29,17 +29,12 @@
 // back to back (p3 BinomialExtensionField serialises `value: [F; 4]` as a tuple); [F; 8] = 8 words; String = u64 length + bytes.
 #include "ctx.cuh"
 #include "hostfield.hpp"
+#include "proof_layout.hpp"
 #include <cstring>
 #include <string>
 #include <vector>
 
 namespace {
-
-struct FlatReader {
-    const uint32_t* p; const uint32_t* end; bool ok = true;
-    uint32_t u() { if (p >= end) { ok = false; return 0; } return *p++; }
-    const uint32_t* take(size_t n) { if ((size_t)(end - p) < n) { ok = false; p = end; return nullptr; } const uint32_t* r = p; p += n; return r; }
-};
 
 struct BinWriter {
     std::vector<uint8_t> b;
@@ -47,51 +42,39 @@ struct BinWriter {
     void u32(uint32_t v) { for (int i = 0; i < 4; i++) b.push_back((uint8_t)(v >> (8 * i))); }
     void u64(uint64_t v) { for (int i = 0; i < 8; i++) b.push_back((uint8_t)(v >> (8 * i))); }
     void f(uint32_t monty) { u32(hf::from_monty(monty)); }
-    bool fs(const uint32_t* w, size_t n) { if (!w) return false; for (size_t i = 0; i < n; i++) f(w[i]); return true; }
+    void fs(const uint32_t* w, size_t n) { for (size_t i = 0; i < n; i++) f(w[i]); }
     void str(const char* s) { const size_t n = strlen(s); u64(n); b.insert(b.end(), s, s + n); }
     void dims(std::initializer_list<uint64_t> d) { u64(d.size()); for (uint64_t x : d) u64(x); }
 };
 
-// PartialSumcheckProof, flat: n_polys, per poly {n_coeffs, coeffs ext}, claimed_sum, point ext[n_polys], eval
-bool put_sumcheck(FlatReader& r, BinWriter& w) {
-    const uint32_t n = r.u();
-    if (!r.ok || n > 4096) return false;
+// PartialSumcheckProof
+void put_sumcheck(const layout::Sumcheck& s, BinWriter& w) {
+    const size_t n = s.polys.size();
     w.u64(n);
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t m = r.u();
-        if (!r.ok || m > 64) return false;
-        w.u64(m);
-        if (!w.fs(r.take(4 * (size_t)m), 4 * (size_t)m)) return false;
-    }
-    if (!w.fs(r.take(4), 4)) return false;       // claimed_sum
+    for (size_t i = 0; i < n; i++) { w.u64(s.n_coeffs[i]); w.fs(s.polys[i], 4 * (size_t)s.n_coeffs[i]); }
+    w.fs(s.claimed_sum, 4);
     w.u64(n);
-    if (!w.fs(r.take(4 * (size_t)n), 4 * (size_t)n)) return false;   // point
-    return w.fs(r.take(4), 4);                   // eval
+    w.fs(s.point, 4 * n);
+    w.fs(s.eval, 4);
 }
 
 // MleEval<EF> of n evaluations = Tensor { storage, dimensions [n] }
-bool put_mle_eval(FlatReader& r, BinWriter& w, size_t n) {
+void put_mle_eval(const uint32_t* e, BinWriter& w, size_t n) {
     w.u64(n);
-    if (n && !w.fs(r.take(4 * n), 4 * n)) return false;
+    w.fs(e, 4 * n);
     w.dims({(uint64_t)n});
-    return true;
 }
 
-// MerkleTreeOpeningAndProof, flat: values[q][width], root, log_height, width, paths[q][log_height] digest
-bool put_opening(FlatReader& r, BinWriter& w, size_t nq, size_t width, const char** why) {
-    w.u64(nq * width);
-    if (!w.fs(r.take(nq * width), nq * width)) return false;
-    w.dims({(uint64_t)nq, (uint64_t)width});
-    const uint32_t* root = r.take(8);
-    const uint32_t lh = r.u(), wd = r.u();
-    if (!r.ok) return false;
-    if (wd != width || lh > 64) { *why = "opening width / height words do not match the layout"; return false; }
-    w.fs(root, 8);
-    w.u64(lh); w.u64(wd);
-    w.u64(nq * (uint64_t)lh);
-    if (!w.fs(r.take(nq * (size_t)lh * 8), nq * (size_t)lh * 8)) return false;
-    w.dims({(uint64_t)nq, (uint64_t)lh});
-    return true;
+// MerkleTreeOpeningAndProof
+void put_opening(const layout::Opening& o, BinWriter& w, size_t nq) {
+    w.u64(nq * o.width);
+    w.fs(o.values, nq * o.width);
+    w.dims({(uint64_t)nq, (uint64_t)o.width});
+    w.fs(o.root, 8);
+    w.u64(o.log_height); w.u64(o.width);
+    w.u64(nq * (uint64_t)o.log_height);
+    w.fs(o.paths, nq * (size_t)o.log_height * 8);
+    w.dims({(uint64_t)nq, (uint64_t)o.log_height});
 }
 
 struct BinReader {
@@ -173,98 +156,63 @@ sp1b200_err sp1b200_shard_proof_to_bincode(const sp1b200_params* params, uint32_
     const uint32_t mlr = params->max_log_row_count, ls = params->log_stacking_height, nq = params->num_queries;
     if (mlr > 62 || ls > 62) return sp1b200_set_error("shard_proof_to_bincode: parameters out of range");
     if (!names_sorted(chip_names, nch)) return sp1b200_set_error("shard_proof_to_bincode: chip names must be strictly ascending (BTreeMap order)");
-    if (n_words < 6 || h_proof[0] != 5) return sp1b200_set_error("shard_proof_to_bincode: not a shard proof (header)");
-    const uint64_t l0 = h_proof[1], l1 = h_proof[2], l2 = h_proof[3], l3 = h_proof[4], l4 = h_proof[5];
-    if (6 + l0 + l1 + l2 + l3 + l4 != n_words || l0 != 8) return sp1b200_set_error("shard_proof_to_bincode: section lengths do not add up to %llu words", (unsigned long long)n_words);
-    const uint32_t* s0 = h_proof + 6; const uint32_t* s1 = s0 + l0; const uint32_t* s2 = s1 + l1; const uint32_t* s3 = s2 + l2; const uint32_t* s4 = s3 + l3;
-    uint64_t prep_area = 0, main_area = 0; bool has_prep = false;
-    for (size_t k = 0; k < nch; k++) {
+    for (size_t k = 0; k < nch; k++)
         if (h_heights[k] >> (mlr + 1)) return sp1b200_set_error("shard_proof_to_bincode: chip %zu: height does not fit %u bits", k, mlr + 1);
-        main_area += h_heights[k] * h_main_w[k];
-        if (h_prep_w[k]) { has_prep = true; prep_area += h_heights[k] * h_prep_w[k]; }
-    }
+    layout::Shape shape;
+    shape.n_chips = nch; shape.main_w = h_main_w; shape.prep_w = h_prep_w;
+    shape.max_log_row_count = mlr; shape.log_stacking_height = ls; shape.num_queries = nq;
+    shape.ncols = layout::round_columns(nch, h_heights, h_main_w, h_prep_w, ls);
+    layout::ShardProof v;
+    if (const char* why = layout::parse_shard_proof(h_proof, n_words, shape, v))
+        return sp1b200_set_error("shard_proof_to_bincode: %s (%llu words)", why, (unsigned long long)n_words);
     BinWriter w;
     w.b.reserve(n_words * 4 + 4096);
-    const char* why = "section is shorter than its layout";
-#define WIRE_FAIL(sec) return sp1b200_set_error("shard_proof_to_bincode: %s section: %s", sec, why)
     // public_values, main_commitment
-    w.u64(l4); w.fs(s4, l4);
-    w.fs(s0, 8);
-    {   // logup_gkr_proof
-        FlatReader r{s1, s2};
-        const uint32_t n_out = r.u();
-        if (!r.ok || n_out > (1u << 24)) WIRE_FAIL("LogUp-GKR");
-        for (int side = 0; side < 2; side++) {   // circuit_output.numerator, .denominator: Mle { Tensor [n_out, 1] }
-            w.u64(n_out);
-            if (!w.fs(r.take(4 * (size_t)n_out), 4 * (size_t)n_out)) WIRE_FAIL("LogUp-GKR");
-            w.dims({n_out, 1});
-        }
-        const uint32_t nr = r.u();
-        if (!r.ok || nr > 64) WIRE_FAIL("LogUp-GKR");
-        w.u64(nr);
-        for (uint32_t i = 0; i < nr; i++) {
-            if (!w.fs(r.take(16), 16)) WIRE_FAIL("LogUp-GKR");
-            if (!put_sumcheck(r, w)) WIRE_FAIL("LogUp-GKR");
-        }
-        w.u64(mlr);
-        if (!w.fs(r.take(4 * (size_t)mlr), 4 * (size_t)mlr)) WIRE_FAIL("LogUp-GKR");
-        w.u64(nch);
-        for (size_t k = 0; k < nch; k++) {
-            w.str(chip_names[k]);
-            if (!put_mle_eval(r, w, h_main_w[k])) WIRE_FAIL("LogUp-GKR");
-            if (h_prep_w[k]) { w.u8(1); if (!put_mle_eval(r, w, h_prep_w[k])) WIRE_FAIL("LogUp-GKR"); }
-            else w.u8(0);
-        }
-        if (!w.fs(r.take(1), 1) || r.p != s2) WIRE_FAIL("LogUp-GKR");
+    w.u64(v.n_pv); w.fs(v.pv, v.n_pv);
+    w.fs(v.commit, 8);
+    // logup_gkr_proof: circuit_output.numerator, .denominator = Mle { Tensor [n_out, 1] }
+    for (const uint32_t* side : {v.out_num, v.out_den}) { w.u64(v.n_out); w.fs(side, 4 * (size_t)v.n_out); w.dims({v.n_out, 1}); }
+    w.u64(v.rounds.size());
+    for (auto& q : v.rounds) { w.fs(q.nd, 16); put_sumcheck(q.sc, w); }
+    w.u64(mlr);
+    w.fs(v.gkr_point, 4 * (size_t)mlr);
+    w.u64(nch);
+    for (size_t k = 0; k < nch; k++) {
+        w.str(chip_names[k]);
+        put_mle_eval(v.gkr_main[k], w, h_main_w[k]);
+        if (h_prep_w[k]) { w.u8(1); put_mle_eval(v.gkr_prep[k], w, h_prep_w[k]); }
+        else w.u8(0);
     }
-    {   // zerocheck_proof, opened_values
-        FlatReader r{s2, s3};
-        if (!put_sumcheck(r, w)) WIRE_FAIL("zerocheck");
-        w.u64(nch);
-        for (size_t k = 0; k < nch; k++) {
-            w.str(chip_names[k]);
-            const size_t pw = h_prep_w[k], mw = h_main_w[k];
-            w.u64(pw); if (pw && !w.fs(r.take(4 * pw), 4 * pw)) WIRE_FAIL("zerocheck");
-            w.u64(mw); if (mw && !w.fs(r.take(4 * mw), 4 * mw)) WIRE_FAIL("zerocheck");
-            w.u64(mlr + 1);   // degree: Point::from_usize(height, max_log_row_count + 1), most significant bit first
-            for (int i = (int)mlr; i >= 0; i--) w.u32((uint32_t)((h_heights[k] >> i) & 1));
-        }
-        if (!r.ok || r.p != s3) WIRE_FAIL("zerocheck");
+    w.fs(v.gkr_witness, 1);
+    // zerocheck_proof, opened_values
+    put_sumcheck(v.zc, w);
+    w.u64(nch);
+    for (size_t k = 0; k < nch; k++) {
+        w.str(chip_names[k]);
+        w.u64(h_prep_w[k]); w.fs(v.zc_prep[k], 4 * (size_t)h_prep_w[k]);
+        w.u64(h_main_w[k]); w.fs(v.zc_main[k], 4 * (size_t)h_main_w[k]);
+        w.u64(mlr + 1);   // degree: Point::from_usize(height, max_log_row_count + 1), most significant bit first
+        for (int i = (int)mlr; i >= 0; i--) w.u32((uint32_t)((h_heights[k] >> i) & 1));
     }
     {   // evaluation_proof
-        FlatReader r{s3, s4};
-        const uint64_t S = (uint64_t)1 << ls;
-        std::vector<size_t> ncols;
-        if (has_prep) ncols.push_back((size_t)std::max<uint64_t>((prep_area + S - 1) / S, 1));
-        ncols.push_back((size_t)std::max<uint64_t>((main_area + S - 1) / S, 1));
-        const size_t n_rounds = ncols.size();
+        const size_t n_rounds = shape.ncols.size();
+        w.u64(ls); w.fs(v.univariate, 8 * (size_t)ls);   // univariate_messages: Vec<[EF; 2]>
+        w.u64(ls); w.fs(v.fri_commits, 8 * (size_t)ls);  // fri_commitments
+        w.u64(n_rounds);
+        for (auto& o : v.component) put_opening(o, w, nq);
         w.u64(ls);
-        if (!w.fs(r.take(8 * (size_t)ls), 8 * (size_t)ls)) WIRE_FAIL("evaluation proof");   // univariate_messages: Vec<[EF; 2]>
-        w.u64(ls);
-        if (!w.fs(r.take(8 * (size_t)ls), 8 * (size_t)ls)) WIRE_FAIL("evaluation proof");   // fri_commitments
+        for (auto& o : v.query) put_opening(o, w, nq);
+        w.fs(v.final_poly, 4); w.fs(v.pow_witness, 1); w.fs(v.batch_witness, 1);
         w.u64(n_rounds);
-        for (size_t q = 0; q < n_rounds; q++) if (!put_opening(r, w, nq, ncols[q], &why)) WIRE_FAIL("evaluation proof");
-        w.u64(ls);
-        for (uint32_t q = 0; q < ls; q++) if (!put_opening(r, w, nq, 8, &why)) WIRE_FAIL("evaluation proof");
-        if (!w.fs(r.take(6), 6)) WIRE_FAIL("evaluation proof");   // final_poly, pow_witness, batch_grinding_witness
+        for (size_t q = 0; q < n_rounds; q++) put_mle_eval(v.batch_evals[q], w, shape.ncols[q]);
+        put_sumcheck(v.jagged_sc, w); put_sumcheck(v.jagged_eval, w);
         w.u64(n_rounds);
-        for (size_t q = 0; q < n_rounds; q++) if (!put_mle_eval(r, w, ncols[q])) WIRE_FAIL("evaluation proof");
-        if (!put_sumcheck(r, w) || !put_sumcheck(r, w)) WIRE_FAIL("evaluation proof");
+        for (auto& t : v.rc_cc) { w.u64(t.size()); for (auto& rc : t) { w.u64(rc.first); w.u64(rc.second); } }
         w.u64(n_rounds);
-        for (size_t q = 0; q < n_rounds; q++) {
-            const uint32_t cnt = r.u();
-            if (!r.ok || cnt > (1u << 20)) WIRE_FAIL("evaluation proof");
-            w.u64(cnt);
-            for (uint32_t i = 0; i < cnt; i++) { const uint32_t a = r.u(), b = r.u(); w.u64(a); w.u64(b); }
-        }
-        w.u64(n_rounds);
-        if (!w.fs(r.take(8 * n_rounds), 8 * n_rounds)) WIRE_FAIL("evaluation proof");
-        if (!w.fs(r.take(4), 4)) WIRE_FAIL("evaluation proof");
-        const uint32_t a = r.u(), b = r.u();
-        w.u64(a); w.u64(b);
-        if (!r.ok || r.p != s4) WIRE_FAIL("evaluation proof");
+        w.fs(v.merkle_commits, 8 * n_rounds);
+        w.fs(v.expected_eval, 4);
+        w.u64(v.max_log_rows); w.u64(v.log_m);
     }
-#undef WIRE_FAIL
     if (h_out_bytes) *h_out_bytes = w.b.size();
     if (h_out) {
         if (w.b.size() > cap_bytes) return sp1b200_set_error("shard_proof_to_bincode: needs %zu bytes, capacity %llu", w.b.size(), (unsigned long long)cap_bytes);

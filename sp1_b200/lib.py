@@ -46,6 +46,7 @@ def load():
         L.sp1b200_challenger_check_witness.restype = C.c_int
         L.sp1b200_machine_num_chips.restype = C.c_uint32
         L.sp1b200_machine_chip_regs.restype = C.c_uint32
+        L.sp1b200_verdict_name.restype = C.c_char_p
         for name in ERR_FUNCS:
             getattr(L, name).restype = C.c_char_p
         _cdll = L
@@ -59,12 +60,13 @@ ERR_FUNCS = [
     "sp1b200_stacked_commit", "sp1b200_stacked_prove", "sp1b200_jagged_commit", "sp1b200_jagged_column_claims",
     "sp1b200_jagged_prove", "sp1b200_machine_create", "sp1b200_zerocheck", "sp1b200_logup_gkr", "sp1b200_prove_shard",
     "sp1b200_setup_and_prove_shard", "sp1b200_shard_proof_to_bincode", "sp1b200_shard_proof_from_bincode",
-    "sp1b200_debug_constraints", "sp1b200_debug_interactions",
+    "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
                "sp1b200_launch_count", "sp1b200_last_phase_ms", "sp1b200_commit_free", "sp1b200_jagged_round_free",
-               "sp1b200_machine_free", "sp1b200_machine_num_chips", "sp1b200_machine_chip_regs"]
+               "sp1b200_machine_free", "sp1b200_machine_num_chips", "sp1b200_machine_chip_regs",
+               "sp1b200_verdict_name"]
 
 
 def _ptr(a):
@@ -261,6 +263,20 @@ class Lib:
                                              _ptr(rw), _ptr(challenger_state), _ptr(out), C.c_uint64(cap_words), C.byref(nw)))
         return out[:nw.value].copy()
 
+    def verify_shard(self, machine, prep_commit, heights, names, words, challenger_state):
+        """ShardVerifier::verify_shard on the flat proof words.  challenger_state: the transcript after the verifying key was observed
+        (not modified).  -> (verdict, challenger): verdict 0 accepts, and challenger is then the verifier's final state; otherwise
+        verdict names the first failing check (verdict_name) and challenger is the state passed in."""
+        n = len(heights)
+        H = (C.c_uint64 * max(1, n))(*heights)
+        NM = (C.c_char_p * max(1, n))(*[s.encode() for s in names])
+        w = np.ascontiguousarray(words, dtype=np.uint32)
+        st = np.ascontiguousarray(challenger_state, dtype=np.uint32).copy()
+        pc = None if prep_commit is None else np.ascontiguousarray(prep_commit, dtype=np.uint32)
+        verdict = C.c_uint32()
+        self._chk(self.L.sp1b200_verify_shard(self.ctx, machine, _ptr(pc), H, NM, _ptr(w), C.c_uint64(w.size), _ptr(st), C.byref(verdict)))
+        return int(verdict.value), st
+
     def _debug_call(self, fn, args, cap_words):
         out = np.empty(max(1, cap_words), np.uint32)
         nw = C.c_uint64()
@@ -357,6 +373,11 @@ def parse_interaction_report(w):
         keys.append({"kind": kind, "values": vals, "net": net, "first": (chip, inter, row), "chips": chips})
     assert p == len(w), "malformed interaction report"
     return {"n_unbalanced": w[0] | (w[1] << 32), "keys": keys}
+
+
+def verdict_name(verdict):
+    """the reason a verdict of verify_shard names ("Accepted" for 0)"""
+    return load().sp1b200_verdict_name(C.c_uint32(verdict)).decode()
 
 
 class HostChallenger:
