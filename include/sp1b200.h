@@ -321,8 +321,9 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
  * counts beyond the layout's limits, opening heights other than the context's, trailing words, a field word >= p), malformed
  * arguments (a height >= 2^(max_log_row_count+1), a public value index beyond the proof's public values, NULL pointers), device
  * failures.  The context stays usable after a rejection or an error.
- * Not checked, as they need the Rust machine definition: the public-values length against PROOF_MAX_NUM_PVS, chip clusters, and the
- * machine-specific public-values interactions (the expected LogUp cumulative sum is 0). */
+ * Not checked, as they need the Rust machine definition: chip clusters and the machine-specific public-values interactions (the expected
+ * LogUp cumulative sum is 0).  The public-values length against PROOF_MAX_NUM_PVS and the checks across shards are made by
+ * sp1b200_verify_core_proof. */
 #define SP1B200_VERDICT_ACCEPT 0u
 #define SP1B200_VERDICT_POW 1u                          /* "Pow": the LogUp-GKR or the BaseFold query grinding witness */
 #define SP1B200_VERDICT_INVALID_SHAPE 2u                /* "InvalidShape": GKR output length, zerocheck rounds */
@@ -371,8 +372,72 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
 sp1b200_err sp1b200_verify_shard(sp1b200_ctx* ctx, const sp1b200_machine* machine, const uint32_t* h_prep_commit8,
                                  const uint64_t* h_heights, const char* const* chip_names, const uint32_t* h_proof, uint64_t n_words,
                                  uint32_t* h_challenger34, uint32_t* h_verdict);
-/* the name of a verdict code (the reason string above; "Accepted" for 0, "Unknown" beyond the list) */
+/* the name of a verdict code of sp1b200_verify_shard or sp1b200_verify_core_proof (the reason strings; "Accepted" for 0, "Unknown"
+ * beyond the lists) */
 const char* sp1b200_verdict_name(uint32_t verdict);
+
+/* ---- core-proof verifier (SP1Prover::verify, crates/prover/src/verify.rs:109-524) --------------------------------------------------
+ * Verifies a core proof: the n_shards flat proofs (sp1b200_prove_shard words) of one execution, all of the same machine, chip names
+ * and context parameters; h_heights[s * n_chips + k] = chip k's height in shard s.  The verifying key is h_prep_commit8 (always
+ * observed; passed on to the shard checks only when a chip has preprocessed columns) followed by h_vk_tail, the words
+ * sp1b200_setup_and_prove_shard takes: pc_start[3] | initial_global_cumulative_sum x[7] y[7] | enable_untrusted_programs | 6 zeros,
+ * so n_vk_tail must be 24 (the build without mprotect).  Field words are Montgomery words.
+ * Order of checks, as the reference's: every shard parses (else an error, as sp1b200_verify_shard); EmptyProof; the public values
+ * across shards (PublicValues<[F;4],[F;3],[F;4],F> without mprotect: length PROOF_MAX_NUM_PVS = 187; one first execution shard;
+ * timestamps from [0,0,0,1]; program counters from vk.pc_start to HALT_PC = [1,0,0]; exit codes; one proof nonce; memory
+ * init/finalize addresses and page indices; committed-value and deferred-proof digests and commit-syscall flags); TooManyShards;
+ * the global cumulative sum (vk.initial_global_cumulative_sum plus every shard's digest, one septic-curve SepticDigest addition per
+ * shard, must be the zero digest); then every shard's verify_shard from a fresh transcript that observed the verifying key.
+ * The one deviation from the reference: where an incomplete curve addition meets a zero denominator the reference panics; this
+ * returns SP1B200_VERDICT_PV_EXCEPTIONAL_ADDITION.
+ * *h_verdict: 0 accepts; otherwise the first failing check (names: sp1b200_verdict_name, "InvalidPublicValues(<reason>)" with the
+ * reference's reason strings).  *h_shard: the shard at which the failing check's loop stopped; n_shards for the end-of-chain checks
+ * (first execution shard not set, not halted, zero address never initialised / finalised, COMMIT syscalls never called,
+ * TooManyShards, cumulative sum not zero); for InvalidShardProof the lowest failing shard, and *h_shard_verdict that shard's own
+ * verify_shard code (0 for every other verdict; the two code spaces stay apart).  On accept h_final_challengers (optional,
+ * [n_shards][34]) receives every shard verifier's final transcript state.
+ * The shards' host phases run on host_threads threads (0 = the hardware concurrency); their device work runs in one launch per kernel
+ * for each batch of consecutive shards with at most 2^26 proof words (the environment variable SP1B200_VERIFY_BATCH_WORDS can lower
+ * the cap; batching never changes a verdict).  A rejection is not an error; the context stays usable after either. */
+#define SP1B200_VERDICT_EMPTY_PROOF 43u                 /* EmptyProof: a core proof without shards */
+#define SP1B200_VERDICT_TOO_MANY_SHARDS 44u             /* TooManyShards: 2^24 shards or more */
+#define SP1B200_VERDICT_INVALID_SHARD_PROOF 45u         /* InvalidShardProof: *h_shard_verdict holds the shard's verify_shard code */
+#define SP1B200_VERDICT_PV_LENGTH 46u                   /* invalid public values length */
+#define SP1B200_VERDICT_PV_FIRST_SHARD_MULTIPLE 47u     /* is_first_execution_shard is set to one for multiple shards */
+#define SP1B200_VERDICT_PV_FIRST_SHARD_NOT_BOOLEAN 48u  /* is_first_execution_shard is not boolean */
+#define SP1B200_VERDICT_PV_FIRST_SHARD_NOT_SET 49u      /* first execution shard is not set */
+#define SP1B200_VERDICT_PV_INITIAL_TIMESTAMP 50u        /* invalid initial timestamp */
+#define SP1B200_VERDICT_PV_TIMESTAMP_UNCHANGED 51u      /* timestamp should change on execution shard */
+#define SP1B200_VERDICT_PV_TIMESTAMP_CHANGED 52u        /* timestamp should not change on non-execution shard */
+#define SP1B200_VERDICT_PV_PC_START_VK 53u              /* pc_start != vk.pc_start: ... */
+#define SP1B200_VERDICT_PV_PC_START_PREV 54u            /* pc_start != prev_next_pc: ... */
+#define SP1B200_VERDICT_PV_PC_NON_EXECUTION 55u         /* pc_start != next_pc: ... non-execution shards */
+#define SP1B200_VERDICT_PV_NOT_HALTED 56u               /* next_pc != HALT_PC: execution should have halted */
+#define SP1B200_VERDICT_PV_PREV_EXIT_CODE 57u           /* public_values.prev_exit_code != prev_exit_code: ... */
+#define SP1B200_VERDICT_PV_EXIT_CODE_NON_EXECUTION 58u  /* prev_exit_code != exit_code: exit code should be same in non-execution shards */
+#define SP1B200_VERDICT_PV_EXIT_CODE_CHANGED 59u        /* prev_exit_code != exit_code: exit code should change at most once */
+#define SP1B200_VERDICT_PV_PROOF_NONCE 60u              /* proof_nonce != proof_nonce_first_shard */
+#define SP1B200_VERDICT_PV_INIT_ADDR 61u                /* previous_init_addr != last_init_addr_prev */
+#define SP1B200_VERDICT_PV_FINALIZE_ADDR 62u            /* previous_finalize_addr != last_finalize_addr_prev */
+#define SP1B200_VERDICT_PV_INIT_PAGE_IDX 63u            /* previous_init_page_idx != last_init_page_idx_prev */
+#define SP1B200_VERDICT_PV_FINALIZE_PAGE_IDX 64u        /* previous_finalize_page_idx != last_finalize_page_idx_prev */
+#define SP1B200_VERDICT_PV_UNTRUSTED_PROGRAMS 65u       /* public_values.is_untrusted_programs_enabled != vk...enable_untrusted_programs */
+#define SP1B200_VERDICT_PV_NEVER_INITIALIZED 66u        /* the zero address was never initialized */
+#define SP1B200_VERDICT_PV_NEVER_FINALIZED 67u          /* the zero address was never finalized */
+#define SP1B200_VERDICT_PV_COMMITTED_VALUE_DIGEST 68u   /* prev_committed_value_digest doesn't equal the previous shard's ... */
+#define SP1B200_VERDICT_PV_DEFERRED_PROOFS_DIGEST 69u   /* prev_deferred_proofs_digest doesn't equal the previous shard's ... */
+#define SP1B200_VERDICT_PV_COMMIT_SYSCALL 70u           /* prev_commit_syscall doesn't equal the previous shard's commit_syscall */
+#define SP1B200_VERDICT_PV_COMMIT_DEFERRED_SYSCALL 71u  /* prev_commit_deferred_syscall doesn't equal the previous shard's ... */
+#define SP1B200_VERDICT_PV_COMMIT_NEVER_CALLED 72u      /* COMMIT syscall was never called */
+#define SP1B200_VERDICT_PV_COMMIT_DEFERRED_NEVER_CALLED 73u/* COMMIT_DEFERRED_PROOFS syscall was never called */
+#define SP1B200_VERDICT_PV_GLOBAL_CUMULATIVE_SUM 74u    /* global cumulative sum is not zero */
+#define SP1B200_VERDICT_PV_EXCEPTIONAL_ADDITION 75u     /* global cumulative sum: exceptional point addition (this library only, see above) */
+#define SP1B200_VERDICT_CORE_COUNT 76u                  /* one past the last code */
+sp1b200_err sp1b200_verify_core_proof(sp1b200_ctx* ctx, const sp1b200_machine* machine, const uint32_t* h_prep_commit8,
+                                      const uint32_t* h_vk_tail, uint32_t n_vk_tail, uint32_t n_shards, const uint64_t* h_heights,
+                                      const char* const* chip_names, const uint32_t* const* h_proofs, const uint64_t* h_n_words,
+                                      uint32_t host_threads, uint32_t* h_final_challengers, uint32_t* h_verdict, uint32_t* h_shard,
+                                      uint32_t* h_shard_verdict);
 
 #ifdef __cplusplus
 }

@@ -13,6 +13,7 @@
 // pool, mailbox and pair of upload slots) and proves one shard at a time; hold several per GPU for throughput (DESIGN.md 3.4).
 // Header-only over include/sp1b200.h; link with -lsp1b200.
 #pragma once
+#include <algorithm>
 #include <array>
 #include <cstdint>
 #include <map>
@@ -193,6 +194,46 @@ class AirProver {
         check(sp1b200_verify_shard(ctx_, machine_, prep_commit ? prep_commit->data() : nullptr, heights.data(), names.data(), proof_words.data(),
                                    proof_words.size(), challenger.data(), &v.code));
         v.reason = sp1b200_verdict_name(v.code);
+        return v;
+    }
+
+    // SP1Prover::verify (crates/prover/src/verify.rs:109-524) on a core proof: the proof words of every shard of one execution, with
+    // each shard's chip heights, against the verifying key prep_commit + vk_tail (24 words, as setup_and_prove_shard takes them;
+    // sp1b200_verify_core_proof).  Shards that do not parse throw.  On acceptance final_challengers holds each shard verifier's final
+    // state; for InvalidShardProof, `shard` is the lowest failing shard and shard_code / shard_reason its verify_shard verdict.
+    struct CoreVerdict {
+        uint32_t code = SP1B200_VERDICT_ACCEPT, shard = 0, shard_code = SP1B200_VERDICT_ACCEPT;
+        std::string reason, shard_reason;
+        std::vector<Challenger> final_challengers;
+        bool accepted() const { return code == SP1B200_VERDICT_ACCEPT; }
+    };
+    CoreVerdict verify_core_proof(const Digest& prep_commit, const std::vector<uint32_t>& vk_tail,
+                                  const std::vector<std::vector<uint32_t>>& shard_words, const std::vector<std::vector<uint64_t>>& heights,
+                                  uint32_t host_threads = 0) {
+        if (heights.size() != shard_words.size()) throw Error("verify_core_proof: one height list per shard expected");
+        std::vector<const char*> names;
+        for (const Chip& c : chips_) names.push_back(c.name.c_str());
+        std::vector<uint64_t> h, nw;
+        std::vector<const uint32_t*> words;
+        for (size_t s = 0; s < shard_words.size(); s++) {
+            if (heights[s].size() != chips_.size()) throw Error("verify_core_proof: one height per chip expected");
+            h.insert(h.end(), heights[s].begin(), heights[s].end());
+            words.push_back(shard_words[s].data());
+            nw.push_back(shard_words[s].size());
+        }
+        std::vector<uint32_t> fin(34 * shard_words.size());
+        CoreVerdict v;
+        check(sp1b200_verify_core_proof(ctx_, machine_, prep_commit.data(), vk_tail.data(), (uint32_t)vk_tail.size(), (uint32_t)shard_words.size(),
+                                        h.data(), names.data(), words.data(), nw.data(), host_threads, fin.data(), &v.code, &v.shard,
+                                        &v.shard_code));
+        v.reason = sp1b200_verdict_name(v.code);
+        v.shard_reason = sp1b200_verdict_name(v.shard_code);
+        if (v.accepted())
+            for (size_t s = 0; s < shard_words.size(); s++) {
+                Challenger c;
+                std::copy(fin.begin() + 34 * s, fin.begin() + 34 * (s + 1), c.data());
+                v.final_challengers.push_back(c);
+            }
         return v;
     }
 

@@ -5,6 +5,7 @@
 #include "rs_twiddles.cuh"
 #include "debug_fp.cuh"
 #include "hostfield.hpp"
+#include "septic.hpp"
 #include "zc_lower.hpp"
 #include <cstring>
 #include <type_traits>
@@ -162,5 +163,35 @@ int sp1b200_hostcheck_interpolate(const uint32_t* xs, const uint32_t* ys, uint32
     else if (n == 5) go(std::integral_constant<int, 5>{});
     else return -1;
     return 0;
+}
+
+// The core-proof verifier's septic arithmetic (septic.hpp), Montgomery words: n products and inverses of septic elements (7 words
+// each); n curve additions add_incomplete(p, q) of points (14 words: x then y), ok[i] = 0 on the exceptional case; SepticDigest
+// addition; and the three constant points zero, starting digest, dummy (42 words).
+void sp1b200_hostcheck_septic(const uint32_t* a, const uint32_t* b, uint32_t* mul_out, uint32_t* inv_out, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        const sep::E7 x = sep::E7::load(a + 7 * i), y = sep::E7::load(b + 7 * i);
+        (x * y).store(mul_out + 7 * i);
+        sep::inv(x).store(inv_out + 7 * i);
+    }
+}
+void sp1b200_hostcheck_septic_curve_add(const uint32_t* p, const uint32_t* q, uint32_t* out, uint32_t* ok, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        const sep::Point a{sep::E7::load(p + 14 * i), sep::E7::load(p + 14 * i + 7)}, b{sep::E7::load(q + 14 * i), sep::E7::load(q + 14 * i + 7)};
+        sep::Point r{};
+        ok[i] = sep::add_incomplete(a, b, r);
+        r.x.store(out + 14 * i); r.y.store(out + 14 * i + 7);
+    }
+}
+int sp1b200_hostcheck_septic_digest_add(const uint32_t* a, const uint32_t* b, uint32_t* out) {
+    const sep::Point x{sep::E7::load(a), sep::E7::load(a + 7)}, y{sep::E7::load(b), sep::E7::load(b + 7)};
+    sep::Point r{};
+    if (!sep::digest_add(x, y, r)) return 0;
+    r.x.store(out); r.y.store(out + 7);
+    return 1;
+}
+void sp1b200_hostcheck_septic_constants(uint32_t* out42) {
+    const sep::Point pts[3] = {sep::digest_zero(), sep::digest_start(), sep::dummy_point()};
+    for (int i = 0; i < 3; i++) { pts[i].x.store(out42 + 14 * i); pts[i].y.store(out42 + 14 * i + 7); }
 }
 }

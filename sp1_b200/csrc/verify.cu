@@ -1,14 +1,17 @@
-// ShardVerifier::verify_shard (crates/hypercube/src/verifier/shard.rs:437-750) on the flat proof words of sp1b200_prove_shard.
-// The transcript, the PoW checks, the GKR / zerocheck / jagged sumcheck rounds, the branching program and every chip's constraints at
-// the zerocheck point run on the host (a few thousand extension-field operations).  The work that grows with the number of queries runs
-// on the device, in three kernels on the context's stream with memory from its pool:
-//   verify_merkle_kernel   every Merkle opening of the proof (all commitment rounds and all FRI fold rounds, every query): leaf hash,
+// ShardVerifier::verify_shard (crates/hypercube/src/verifier/shard.rs:437-750) on the flat proof words of sp1b200_prove_shard, for one
+// shard (sp1b200_verify_shard) or for every shard of a core proof (sp1b200_verify_core_proof, verify_core.cu).
+// A shard is verified in two phases.  The host phase - the transcript, the PoW checks, the GKR / zerocheck / jagged sumcheck rounds, the
+// branching program and every chip's constraints at the zerocheck point (a few thousand extension-field operations) - touches no CUDA
+// API: it records the device work the queries need (ShardWork), so the host phases of many shards can run on as many threads.  The
+// device phase then runs the recorded work of a batch of shards in three kernels on the context's stream with memory from its pool:
+//   verify_merkle_kernel   every Merkle opening of every shard (all commitment rounds and all FRI fold rounds, every query): leaf hash,
 //                          path walk, root comparison; and each opening's tensor commitment compress(root, hash([log_h, width]))
-//   verify_fold_kernel     per query: the batched codeword value, the fold chain through the log_stacking_height rounds, final_poly
-//   verify_jagged_kernel   sum_c col_eq[c] * eq(prefix_c || prefix_{c+1}, point) over every jagged column
-// Their flags and partial sums are copied back once, at the end of the call.  Checks are reported in verify_shard's order: a check
-// whose inputs come from the device is recorded when the transcript reaches it and resolved after the copy, so the verdict names
-// the first failing check, as the reference's verifier (and the oracle's restatement of it) would.
+//   verify_fold_kernel     per (shard, query): the batched codeword value, the fold chain through the log_stacking_height rounds,
+//                          final_poly
+//   verify_jagged_kernel   per shard, sum_c col_eq[c] * eq(prefix_c || prefix_{c+1}, point) over every jagged column
+// Their flags and partial sums are copied back once per batch.  Checks are reported in verify_shard's order: a check whose inputs come
+// from the device is recorded when the transcript reaches it and resolved after the copy, so the verdict names the first failing check,
+// as the reference's verifier (and the oracle's restatement of it) would.
 #include "ctx.cuh"
 #include "challenger.cuh"
 #include "hostfield.hpp"
@@ -16,8 +19,12 @@
 #include "poseidon2.cuh"
 #include "proof_layout.hpp"
 #include "sumcheck.cuh"
+#include "verify.cuh"
+#include <atomic>
 #include <chrono>
 #include <cstring>
+#include <memory>
+#include <thread>
 #include <vector>
 
 // Poseidon2 sponge / 2-to-1 compression on the host (the transcript's permutation), for the verifier's few table-size hashes
@@ -43,8 +50,8 @@ using kb::Ext;
 // ---- device part ----------------------------------------------------------------------------------------------------------------
 
 // one opening: `width` values per query at values_off, log_h sibling digests per query at paths_off (word offsets into the evaluation
-// section on the device); the leaf index of query q is idx[q] >> shift
-struct OpenJob { uint32_t values_off, width, paths_off, root_off, commit_off, log_h, shift, pad; };
+// sections on the device); the leaf index of query q is idx[idx_off + q] >> shift (idx_off: the shard's first query index)
+struct OpenJob { uint32_t values_off, width, paths_off, root_off, commit_off, log_h, shift, idx_off; };
 
 __device__ __forceinline__ void hash_row(const uint32_t* __restrict__ v, uint32_t n, uint32_t (&d)[8]) {
     uint32_t s[16];
@@ -83,7 +90,7 @@ __global__ void __launch_bounds__(128) verify_merkle_kernel(const OpenJob* __res
         const OpenJob j = jobs[t / nq];
         const uint32_t q = t % nq;
         hash_row(ev + j.values_off + (uint64_t)q * j.width, j.width, d);
-        uint32_t index = __ldg(idx + q) >> j.shift;
+        uint32_t index = __ldg(idx + j.idx_off + q) >> j.shift;
         const uint32_t* sib = ev + j.paths_off + (uint64_t)q * j.log_h * 8;
         for (uint32_t k = 0; k < j.log_h; k++, sib += 8) {
             uint32_t s[8], o[8];
@@ -110,8 +117,10 @@ __global__ void __launch_bounds__(128) verify_merkle_kernel(const OpenJob* __res
     }
 }
 
-// per query q: Σ_c coeff_c · v_c over the component columns of every round, then the fold chain.  out[q] = first round whose opened
-// pair does not hold the running value (len if none), out[nq + q] = 1 when the chain ends away from final_poly.
+// per shard (blockIdx.y) and query q: Σ_c coeff_c · v_c over the component columns of every round, then the fold chain.
+// out[q] = first round whose opened pair does not hold the running value (len if none), out[nq + q] = 1 when the chain ends away from
+// final_poly.  The *_off / *_at words place the shard's inputs and outputs: ev offsets into the evaluation sections, aux offsets into
+// the auxiliary words, out_at into the output words.
 struct FoldArgs {
     uint32_t nq, len, n_comp;
     uint32_t comp_off[2], comp_w[2];
@@ -119,12 +128,15 @@ struct FoldArgs {
     uint32_t log_n;    // len + log_blowup
     uint32_t minus1;
     uint32_t final_off;
+    uint32_t idx_at, coeff_at, beta_at, fold_off_at, out_at;
 };
-__global__ void __launch_bounds__(128) verify_fold_kernel(FoldArgs a, const uint32_t* __restrict__ ev, const uint32_t* __restrict__ fold_off,
-                                                          const uint32_t* __restrict__ idx, const uint32_t* __restrict__ coeffs,
-                                                          const uint32_t* __restrict__ betas, uint32_t* __restrict__ out) {
+__global__ void __launch_bounds__(128) verify_fold_kernel(const FoldArgs* __restrict__ args, const uint32_t* __restrict__ ev,
+                                                          const uint32_t* __restrict__ aux, uint32_t* __restrict__ out_all) {
+    const FoldArgs a = args[blockIdx.y];
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= a.nq) return;
+    const uint32_t *idx = aux + a.idx_at, *coeffs = aux + a.coeff_at, *betas = aux + a.beta_at, *fold_off = aux + a.fold_off_at;
+    uint32_t* out = out_all + a.out_at;
     Ext folded = kb::ext_zero();
     uint32_t k = 0;
     for (uint32_t r = 0; r < a.n_comp; r++) {
@@ -149,10 +161,16 @@ __global__ void __launch_bounds__(128) verify_fold_kernel(FoldArgs a, const uint
     out[a.nq + q] = first_bad == a.len && !kb::ext_eq(folded, ld4(ev + a.final_off));
 }
 
-// sum_c col_eq[c] * prod_i eq(bit_i, point_i) over the 2 (log_m + 1) bits of prefix[c] || prefix[c+1] (most significant first), one
-// column per thread; per-block sums to partial[block]
-__global__ void __launch_bounds__(256) verify_jagged_kernel(const uint64_t* __restrict__ prefix, uint32_t n_cols, const uint32_t* __restrict__ col_eq,
-                                                            const uint32_t* __restrict__ point, uint32_t nb, uint32_t* __restrict__ partial) {
+// per shard (blockIdx.y): sum_c col_eq[c] * prod_i eq(bit_i, point_i) over the 2 (log_m + 1) bits of prefix[c] || prefix[c+1] (most
+// significant first), one column per thread; per-block sums to partial[block] of the shard's own partial range
+struct JagArgs { uint32_t prefix_at, n_cols, col_eq_at, point_at, nb, partial_at; };   // aux offsets (prefix_at in 64-bit words)
+__global__ void __launch_bounds__(256) verify_jagged_kernel(const JagArgs* __restrict__ args, const uint32_t* __restrict__ aux,
+                                                            uint32_t* __restrict__ out_all) {
+    const JagArgs ja = args[blockIdx.y];
+    const uint64_t* prefix = reinterpret_cast<const uint64_t*>(aux) + ja.prefix_at;
+    const uint32_t *col_eq = aux + ja.col_eq_at, *point = aux + ja.point_at;
+    const uint32_t n_cols = ja.n_cols, nb = ja.nb;
+    uint32_t* partial = out_all + ja.partial_at;
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     Ext acc[1] = {kb::ext_zero()};
     if (c < n_cols) {
@@ -224,6 +242,7 @@ static_assert(V_QUERY_FINAL_POLY == SP1B200_VERDICT_QUERY_FINAL_POLY, "verdict c
 static_assert(V_SUMCHECK_FINAL_POLY == SP1B200_VERDICT_SUMCHECK_FINAL_POLY, "verdict code differs from include/sp1b200.h");
 static_assert(V_PREP_WIDTHS == SP1B200_VERDICT_PREPROCESSED_WIDTHS, "verdict code differs from include/sp1b200.h");
 static_assert(V_CHIP_TABLES == SP1B200_VERDICT_CHIP_TABLES, "verdict code differs from include/sp1b200.h");
+static_assert(V_COUNT == SP1B200_VERDICT_EMPTY_PROOF, "the core-proof verdicts follow the shard verdicts");
 const char* const VERDICT_NAMES[V_COUNT] = {
     "Accepted", "Pow", "InvalidShape", "ZeroDenominator", "CumulativeSumMismatch", "InvalidShape(rounds)", "InconsistentSumcheckClaim",
     "InvalidProofShape", "InconsistencyWithClaimedSum", "SumcheckRoundInconsistency", "InvalidProofShape(point)", "InconsistencyWithEval",
@@ -291,38 +310,49 @@ struct BranchingProgram {
     }
 };
 
-// a check whose inputs the device computes, resolved after the final copy
-struct Deferred { uint32_t code; std::vector<uint32_t> flag_ranges; };   // flag_ranges: [begin, end) pairs into the flag words
+// a check whose inputs the device computes, resolved after the final copy; job: the opening job (local index) of a TcsError check
+struct Deferred { uint32_t code; uint32_t job; };
+constexpr uint32_t NO_JOB = ~0u;
 
+// one shard's verifier: the host phase (run) records the device work, resolve() reads the device results back in verify_shard's order
 struct Verifier {
-    sp1b200_ctx* ctx;
+    const sp1b200_params& prm;
     const sp1b200_machine* m;
     const HostInteractions& H;
     const layout::ShardProof& p;
     const uint64_t* heights;
+    const char* const* names;
     const std::vector<size_t>& ncols;
+    const uint32_t* prep_commit8;
     const uint32_t* ev_base;   // host start of the evaluation section (device offsets are relative to it)
     uint64_t ev_words;
     HostChallenger ch;
-    DevFree mem;
     uint32_t mlr, ls, lb, nq;
-    // device outputs: merkle flags | fold words (2 nq) | jagged partials; copied back once
-    uint32_t* d_out = nullptr;
-    size_t n_merkle_flags = 0, fold_at = 0, jag_at = 0, out_words = 0;
-    unsigned jag_blocks = 0;
-    bool launched = false, fold_launched = false;
-    cudaEvent_t ev[5] = {};   // merkle start / end = fold start, fold end, jagged start, jagged end
-    // jagged eval: acc * bp == eval is checked after the copy
-    E4 jag_bp, jag_expect;
-    bool jag_pending = false;
 
-    Verifier(sp1b200_ctx* c, const sp1b200_machine* mm, const layout::ShardProof& pp, const uint64_t* h, const std::vector<size_t>& nc,
-             const uint32_t* evb, uint64_t evw)
-        : ctx(c), m(mm), H(*static_cast<const HostInteractions*>(mm->interactions)), p(pp), heights(h), ncols(nc), ev_base(evb), ev_words(evw),
-          mem(c) {
-        mlr = c->params.max_log_row_count; ls = c->params.log_stacking_height; lb = c->params.log_blowup; nq = c->params.num_queries;
+    // outcome of the host phase: `verdict` is a failure found before any device check; otherwise the deferred checks, then host_fail,
+    // then tail_fail (the chip-table check) decide
+    uint32_t verdict = V_ACCEPT, host_fail = V_ACCEPT, tail_fail = V_ACCEPT;
+    std::vector<Deferred> deferred;
+    // recorded device work.  Jagged column sum: the column prefix sums, eq(z_col, c) and the jagged-eval point; acc * jag_bp ==
+    // jag_expect is checked after the copy
+    bool jag = false;
+    std::vector<uint64_t> prefix;
+    std::vector<uint32_t> col_eq, jag_point;
+    uint32_t jag_nb = 0, jag_cols = 0;
+    E4 jag_bp, jag_expect;
+    // BaseFold queries: openings (offsets into the evaluation section), query indices, batching coefficients, fold betas, the fold
+    // rounds' value offsets, and the fold arguments (offsets relative to this shard)
+    bool fold = false;
+    std::vector<OpenJob> jobs;
+    std::vector<uint32_t> idx, coeff_words, beta_words, fold_offs;
+    FoldArgs fa{};
+
+    Verifier(const sp1b200_params& pr, const sp1b200_machine* mm, const layout::ShardProof& pp, const uint64_t* h, const char* const* nm,
+             const std::vector<size_t>& nc, const uint32_t* pc8)
+        : prm(pr), m(mm), H(*static_cast<const HostInteractions*>(mm->interactions)), p(pp), heights(h), names(nm), ncols(nc),
+          prep_commit8(pc8), ev_base(pp.univariate), ev_words((uint64_t)(pp.pv - pp.univariate)) {
+        mlr = pr.max_log_row_count; ls = pr.log_stacking_height; lb = pr.log_blowup; nq = pr.num_queries;
     }
-    ~Verifier() { for (auto e : ev) if (e) cudaEventDestroy(e); }
 
     uint32_t off(const uint32_t* ptr) const { return (uint32_t)(ptr - ev_base); }
     void observe_ext(const E4& e) { ch.observe_n(e.c, 4); }
@@ -370,7 +400,7 @@ struct Verifier {
         size_t arity = 1, ni = 0;
         for (auto& c : H.per_chip) { ni += c.size(); for (auto& in : c) arity = std::max<size_t>(arity, in.n_values + 1); }
         const unsigned bdim = hf::log2_ceil(arity);
-        if (!ch.check_witness(ctx->params.gkr_pow_bits, p.gkr_witness[0])) return V_POW;
+        if (!ch.check_witness(prm.gkr_pow_bits, p.gkr_witness[0])) return V_POW;
         const E4 alpha = sample_ext();
         const std::vector<E4> beta_seed = sample_point(bdim);
         (void)sample_ext();
@@ -498,33 +528,20 @@ struct Verifier {
         return V_ACCEPT;
     }
 
-    sp1b200_err ensure_out() {
-        if (d_out) return nullptr;
-        n_merkle_flags = (size_t)(ncols.size() + ls) * (nq + 1);
-        fold_at = n_merkle_flags;
-        jag_at = fold_at + 2 * (size_t)nq;
-        out_words = jag_at + 4 * (size_t)jag_blocks;
-        SP1_TRY(mem.alloc((void**)&d_out, out_words * 4));
-        SP1_CUDA(cudaMemsetAsync(d_out, 0, out_words * 4, ctx->stream));
-        for (auto& e : ev) SP1_CUDA(cudaEventCreate(&e));
-        return nullptr;
-    }
-
     // JaggedPcsVerifier::verify_trusted_evaluations (slop/crates/jagged/src/verifier.rs:113-384) with the stacked and BaseFold verifiers
     // behind it; commitments = {preprocessed,} main
-    sp1b200_err jagged(const std::vector<const uint32_t*>& commitments, uint32_t* verdict) {
-        *verdict = V_ACCEPT;
+    void jagged(const std::vector<const uint32_t*>& commitments) {
         const size_t nr = commitments.size();
-        for (auto& v : p.rc_cc) if (v.empty()) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+        for (auto& v : p.rc_cc) if (v.empty()) { verdict = V_INCORRECT_SHAPE; return; }
         // column heights as (rows, cols) runs; totals in 128 bits so that no count in the words can wrap them
         unsigned __int128 total_cols = 0, total_area = 0;
         for (auto& v : p.rc_cc) for (auto& rc : v) { total_cols += rc.second; total_area += (unsigned __int128)rc.first * rc.second; }
-        if (total_cols == 0) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+        if (total_cols == 0) { verdict = V_INCORRECT_SHAPE; return; }
         const uint64_t area64 = total_area >> 63 ? ~(uint64_t)0 : (uint64_t)total_area;
-        if (p.max_log_rows != mlr || p.log_m != hf::log2_ceil(area64) || total_area >> 63) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+        if (p.max_log_rows != mlr || p.log_m != hf::log2_ceil(area64) || total_area >> 63) { verdict = V_INCORRECT_SHAPE; return; }
         // log_m matches the area, so the columns with rows are few; a column count that is absurd only through empty tables cannot be
         // laid out
-        if (total_cols > ((uint64_t)1 << 24)) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+        if (total_cols > ((uint64_t)1 << 24)) { verdict = V_INCORRECT_SHAPE; return; }
         const size_t n_cols = (size_t)total_cols;
         std::vector<uint64_t> prefix;
         prefix.reserve(n_cols + 1);
@@ -539,13 +556,13 @@ struct Verifier {
         std::vector<std::vector<E4>> claims(nr);
         for (size_t r = 0; r < nr; r++) {
             const auto& v = p.rc_cc[r];
-            if (v.size() < 2) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+            if (v.size() < 2) { verdict = V_INCORRECT_SHAPE; return; }
             uint64_t expect = 0, area = 0;
             for (size_t t = 0; t + 2 < v.size(); t++) { expect += v[t].second; area += (uint64_t)v[t].first * v[t].second; }
             // the claims of round r are the zerocheck's opened values of that round's columns, in chip order
             size_t have = 0;
             for (size_t k = 0; k < m->chips.size(); k++) have += (nr == 2 && r == 0) ? m->chips[k].prep_w : m->chips[k].main_w;
-            if (have != expect) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+            if (have != expect) { verdict = V_INCORRECT_SHAPE; return; }
             for (size_t k = 0; k < m->chips.size(); k++) {
                 const bool prep = nr == 2 && r == 0;
                 const uint32_t w = prep ? m->chips[k].prep_w : m->chips[k].main_w;
@@ -558,87 +575,77 @@ struct Verifier {
             uint32_t h[8], cm[8];
             host_hash(meta.data(), meta.size(), h);
             host_compress(p.merkle_commits + 8 * r, h, cm);
-            if (memcmp(cm, commitments[r], 32)) { *verdict = V_INCORRECT_TABLE_SIZES; return nullptr; }
-            if (area == 0 || area >= ((uint64_t)1 << 30)) { *verdict = V_AREA_OUT_OF_BOUNDS; return nullptr; }
+            if (memcmp(cm, commitments[r], 32)) { verdict = V_INCORRECT_TABLE_SIZES; return; }
+            if (area == 0 || area >= ((uint64_t)1 << 30)) { verdict = V_AREA_OUT_OF_BOUNDS; return; }
             const uint64_t next = ((area + S - 1) / S) * S, av = next - area, ac = std::max<uint64_t>((av + R - 1) / R, 1);
             if (v[v.size() - 2].second + 1 != ac || v.back().second != 1 || v[v.size() - 2].first != R || v.back().first != av - (ac - 1) * R) {
-                *verdict = V_DUMMY_TABLES; return nullptr;
+                verdict = V_DUMMY_TABLES; return;
             }
-            for (auto& rc : v) if (rc.first > R) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
+            for (auto& rc : v) if (rc.first > R) { verdict = V_INCORRECT_SHAPE; return; }
             round_area[r] = area; added_vals[r] = av; added_cols[r] = ac;
         }
-        if (p.log_m >= 30) { *verdict = V_AREA_OUT_OF_BOUNDS; return nullptr; }
+        if (p.log_m >= 30) { verdict = V_AREA_OUT_OF_BOUNDS; return; }
         std::vector<E4> column_claims;
         for (size_t r = 0; r < nr; r++) { column_claims.insert(column_claims.end(), claims[r].begin(), claims[r].end()); column_claims.resize(column_claims.size() + added_cols[r]); }
-        if (prefix.size() != column_claims.size() + 1) { *verdict = V_INCORRECT_SHAPE; return nullptr; }
-        if (neq(mle_eval(column_claims, z_col), ld(p.jagged_sc.claimed_sum))) { *verdict = V_SUMCHECK_CLAIM_MISMATCH; return nullptr; }
-        if ((*verdict = sumcheck(p.jagged_sc, p.log_m, 2))) return nullptr;
-        for (size_t c = 0; c + 1 < prefix.size(); c++) if (prefix[c] > prefix[c + 1]) { *verdict = V_MONOTONICITY; return nullptr; }
+        if (prefix.size() != column_claims.size() + 1) { verdict = V_INCORRECT_SHAPE; return; }
+        if (neq(mle_eval(column_claims, z_col), ld(p.jagged_sc.claimed_sum))) { verdict = V_SUMCHECK_CLAIM_MISMATCH; return; }
+        if ((verdict = sumcheck(p.jagged_sc, p.log_m, 2))) return;
+        for (size_t c = 0; c + 1 < prefix.size(); c++) if (prefix[c] > prefix[c + 1]) { verdict = V_MONOTONICITY; return; }
         // JaggedEvalSumcheckConfig::jagged_evaluation (slop/crates/jagged/src/jagged_eval/sumcheck_eval.rs:45-155)
         const uint32_t lm = p.log_m;
         observe_ext(ld(p.jagged_eval.claimed_sum));
-        if ((*verdict = sumcheck(p.jagged_eval, 2 * (lm + 1), 2))) return nullptr;
+        if ((verdict = sumcheck(p.jagged_eval, 2 * (lm + 1), 2))) return;
         {
             const std::vector<E4> jp = ext_vec(p.jagged_eval.point, 2 * (lm + 1));
             const std::vector<E4> first(jp.begin(), jp.begin() + lm + 1), second(jp.begin() + lm + 1, jp.end());
             const std::vector<E4> z_row = ext_vec(p.zc.point, mlr), z_trace = ext_vec(p.jagged_sc.point, p.jagged_sc.polys.size());
             jag_bp = BranchingProgram{z_row, z_trace, std::max(z_row.size(), z_trace.size())}.eval(first, second);
             jag_expect = ld(p.jagged_eval.eval);
-            // the column sum on the device: col_eq from the shared eq-table launcher, one thread per column
-            jag_blocks = blocks_for(n_cols);
-            SP1_TRY(ensure_out());
-            const int kz = (int)z_col.size();
-            std::vector<uint32_t> hz(4 * (size_t)kz + 8 * (size_t)(lm + 1));
-            for (int i = 0; i < kz; i++) z_col[i].store(&hz[4 * i]);
-            memcpy(&hz[4 * (size_t)kz], p.jagged_eval.point, 32 * (size_t)(lm + 1));
-            uint32_t *d_pts, *d_col_eq; uint64_t* d_prefix;
-            SP1_TRY(mem.alloc((void**)&d_pts, hz.size() * 4));
-            SP1_TRY(mem.alloc((void**)&d_col_eq, ((size_t)4 << kz) * 4));
-            SP1_TRY(mem.alloc((void**)&d_prefix, prefix.size() * 8));
-            SP1_CUDA(cudaMemcpyAsync(d_pts, hz.data(), hz.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-            SP1_CUDA(cudaMemcpyAsync(d_prefix, prefix.data(), prefix.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-            SP1_CUDA(cudaEventRecord(ev[3], ctx->stream));
-            SP1_TRY(launch_eq_table(ctx, d_pts, kz, d_col_eq));
-            SP1_LAUNCH(ctx, verify_jagged_kernel, jag_blocks, 256, 0, d_prefix, (uint32_t)n_cols, d_col_eq, d_pts + 4 * kz, lm + 1, d_out + jag_at);
-            SP1_CUDA(cudaEventRecord(ev[4], ctx->stream));
-            jag_pending = true;
-            launched = true;
+            // the column sum on the device, one thread per column; eq(z_col, c) is tabled here
+            const std::vector<E4> eq = hf::partial_lagrange(z_col);
+            col_eq.resize(4 * eq.size());
+            for (size_t c = 0; c < eq.size(); c++) eq[c].store(&col_eq[4 * c]);
+            jag_point.assign(p.jagged_eval.point, p.jagged_eval.point + 8 * (size_t)(lm + 1));
+            jag_nb = lm + 1;
+            jag_cols = (uint32_t)n_cols;
+            this->prefix = std::move(prefix);
+            jag = true;
         }
         const E4 jagged_eval = ld(p.jagged_eval.claimed_sum);
         // (the check acc == eval of the jagged-eval sumcheck is resolved with the device flags; nothing below reads acc)
-        deferred.push_back(Deferred{V_JAGGED_EVALUATION, {}});
-        if (neq(ld(p.expected_eval) * jagged_eval, ld(p.jagged_sc.eval))) { host_fail = V_JAGGED_EVAL_PROOF; return nullptr; }
+        deferred.push_back(Deferred{V_JAGGED_EVALUATION, NO_JOB});
+        if (neq(ld(p.expected_eval) * jagged_eval, ld(p.jagged_sc.eval))) { host_fail = V_JAGGED_EVAL_PROOF; return; }
         std::vector<uint64_t> total(nr);
         for (size_t r = 0; r < nr; r++) total[r] = round_area[r] + added_vals[r];
         observe_ext(ld(p.expected_eval));
-        return stacked(total);
+        stacked(total);
     }
 
     // StackedPcsVerifier::verify_trusted_evaluation (slop/crates/stacked/src/verifier.rs:39-99)
-    sp1b200_err stacked(const std::vector<uint64_t>& areas) {
+    void stacked(const std::vector<uint64_t>& areas) {
         const size_t npt = p.jagged_sc.polys.size();
-        if (npt < ls) { host_fail = V_INCORRECT_SHAPE; return nullptr; }
+        if (npt < ls) { host_fail = V_INCORRECT_SHAPE; return; }
         const std::vector<E4> pt = ext_vec(p.jagged_sc.point, npt);
         const std::vector<E4> batch_point(pt.begin(), pt.end() - ls), stack_point(pt.end() - ls, pt.end());
         std::vector<E4> flat;
         for (size_t r = 0; r < areas.size(); r++) {
-            if (areas[r] % ((uint64_t)1 << ls) || (areas[r] >> ls) != ncols[r]) { host_fail = V_INCORRECT_SHAPE; return nullptr; }
+            if (areas[r] % ((uint64_t)1 << ls) || (areas[r] >> ls) != ncols[r]) { host_fail = V_INCORRECT_SHAPE; return; }
             const std::vector<E4> e = ext_vec(p.batch_evals[r], ncols[r]);
             flat.insert(flat.end(), e.begin(), e.end());
         }
-        if (neq(ld(p.expected_eval), mle_eval(flat, batch_point))) { host_fail = V_STACKING; return nullptr; }
+        if (neq(ld(p.expected_eval), mle_eval(flat, batch_point))) { host_fail = V_STACKING; return; }
         for (size_t r = 0; r < areas.size(); r++) ch.observe_n(p.batch_evals[r], 4 * ncols[r]);
-        return basefold(stack_point, flat);
+        basefold(stack_point, flat);
     }
 
     // BasefoldVerifier::verify_mle_evaluations (slop/crates/basefold/src/verifier.rs:122-420)
-    sp1b200_err basefold(const std::vector<E4>& point, const std::vector<E4>& claims) {
-        if (!ch.check_witness(ctx->params.batch_pow_bits, p.batch_witness[0])) { host_fail = V_BATCH_POW; return nullptr; }
+    void basefold(const std::vector<E4>& point, const std::vector<E4>& claims) {
+        if (!ch.check_witness(prm.batch_pow_bits, p.batch_witness[0])) { host_fail = V_BATCH_POW; return; }
         const std::vector<E4> coeffs = hf::partial_lagrange(sample_point(hf::log2_ceil(claims.size())));
         E4 claim;
         for (size_t k = 0; k < claims.size(); k++) claim = claim + claims[k] * coeffs[k];
         const size_t len = ls;
-        if (point.size() != len || len == 0) { host_fail = V_FRI_LENGTH; return nullptr; }
+        if (point.size() != len || len == 0) { host_fail = V_FRI_LENGTH; return; }
         ch.observe(hf::to_monty(len));
         std::vector<E4> betas;
         for (size_t i = 0; i < len; i++) {
@@ -649,79 +656,47 @@ struct Verifier {
         E4 expected = claim;
         for (size_t i = 0; i < len; i++) {
             const E4 p0 = ld(p.univariate + 8 * i), p1 = ld(p.univariate + 8 * i + 4), x = point[len - 1 - i];
-            if (neq(expected, (E4::one() - x) * p0 + x * p1)) { host_fail = V_BASEFOLD_SUMCHECK; return nullptr; }
+            if (neq(expected, (E4::one() - x) * p0 + x * p1)) { host_fail = V_BASEFOLD_SUMCHECK; return; }
             expected = p0 + betas[i] * p1;
         }
         ch.observe_n(p.final_poly, 4);
-        if (!ch.check_witness(ctx->params.pow_bits, p.pow_witness[0])) { host_fail = V_POW; return nullptr; }
+        if (!ch.check_witness(prm.pow_bits, p.pow_witness[0])) { host_fail = V_POW; return; }
         const uint32_t log_n = (uint32_t)len + lb;
-        if (log_n > 24) { host_fail = V_TWO_ADICITY; return nullptr; }
-        std::vector<uint32_t> idx(nq);
+        if (log_n > 24) { host_fail = V_TWO_ADICITY; return; }
+        idx.resize(nq);
         for (auto& q : idx) q = ch.sample_bits(log_n);
         // device: every opening, and the fold chain of every query
-        SP1_TRY(ensure_out());
         const size_t ncomp = ncols.size();
-        std::vector<OpenJob> jobs;
-        for (size_t r = 0; r < ncomp; r++) {
+        for (size_t r = 0; r < ncomp; r++) {   // component openings are checked against the jagged round's original commitments
             const layout::Opening& o = p.component[r];
-            jobs.push_back(OpenJob{off(o.values), o.width, off(o.paths), off(o.root), 0, o.log_height, 0, 0});
+            jobs.push_back(OpenJob{off(o.values), o.width, off(o.paths), off(o.root), off(p.merkle_commits + 8 * r), o.log_height, 0, 0});
         }
         for (size_t r = 0; r < len; r++) {
             const layout::Opening& o = p.query[r];
             jobs.push_back(OpenJob{off(o.values), o.width, off(o.paths), off(o.root), off(p.fri_commits + 8 * r), o.log_height, (uint32_t)r + 1, 0});
         }
-        // component openings are checked against the jagged round's original commitments; the device reads them from the evaluation section
-        for (size_t r = 0; r < ncomp; r++) jobs[r].commit_off = off(p.merkle_commits + 8 * r);
-        std::vector<uint32_t> aux;   // idx | coeffs | betas | fold offsets, then the jobs
-        aux.insert(aux.end(), idx.begin(), idx.end());
-        const size_t coeff_at = aux.size();
-        for (size_t k = 0; k < claims.size(); k++) for (int i = 0; i < 4; i++) aux.push_back(coeffs[k].c[i]);
-        const size_t beta_at = aux.size();
-        for (auto& b : betas) for (int i = 0; i < 4; i++) aux.push_back(b.c[i]);
-        const size_t fold_off_at = aux.size();
-        for (size_t r = 0; r < len; r++) aux.push_back(off(p.query[r].values));
-        while (aux.size() % 4) aux.push_back(0);
-        const size_t jobs_at = aux.size();
-        aux.resize(aux.size() + jobs.size() * sizeof(OpenJob) / 4);
-        memcpy(&aux[jobs_at], jobs.data(), jobs.size() * sizeof(OpenJob));
-        uint32_t *d_ev, *d_aux;
-        SP1_TRY(mem.alloc((void**)&d_ev, ev_words * 4));
-        SP1_TRY(mem.alloc((void**)&d_aux, aux.size() * 4));
-        SP1_CUDA(cudaMemcpyAsync(d_ev, ev_base, ev_words * 4, cudaMemcpyHostToDevice, ctx->stream));
-        SP1_CUDA(cudaMemcpyAsync(d_aux, aux.data(), aux.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-        const uint32_t n_jobs = (uint32_t)jobs.size();
-        SP1_CUDA(cudaEventRecord(ev[0], ctx->stream));
-        SP1_LAUNCH(ctx, verify_merkle_kernel, blocks_for((uint64_t)n_jobs * (nq + 1), 128), 128, 0, reinterpret_cast<const OpenJob*>(d_aux + jobs_at),
-                   n_jobs, nq, d_ev, d_aux, d_out);
-        SP1_CUDA(cudaEventRecord(ev[1], ctx->stream));
-        FoldArgs a{};
-        a.nq = nq; a.len = (uint32_t)len; a.n_comp = (uint32_t)ncomp;
-        for (size_t r = 0; r < ncomp; r++) { a.comp_off[r] = off(p.component[r].values); a.comp_w[r] = p.component[r].width; }
-        a.log_n = log_n;
-        a.g = hf::pow(hf::to_monty(3), (uint64_t)127 << (24 - log_n));
-        a.minus1 = hf::pow(hf::to_monty(3), (uint64_t)127 << 23);
-        a.final_off = off(p.final_poly);
-        SP1_LAUNCH(ctx, verify_fold_kernel, blocks_for(nq, 128), 128, 0, a, d_ev, d_aux + fold_off_at, d_aux, d_aux + coeff_at, d_aux + beta_at,
-                   d_out + fold_at);
-        SP1_CUDA(cudaEventRecord(ev[2], ctx->stream));
-        launched = fold_launched = true;
+        for (size_t k = 0; k < claims.size(); k++) for (int i = 0; i < 4; i++) coeff_words.push_back(coeffs[k].c[i]);
+        for (auto& b : betas) for (int i = 0; i < 4; i++) beta_words.push_back(b.c[i]);
+        for (size_t r = 0; r < len; r++) fold_offs.push_back(off(p.query[r].values));
+        fa.nq = nq; fa.len = (uint32_t)len; fa.n_comp = (uint32_t)ncomp;
+        for (size_t r = 0; r < ncomp; r++) { fa.comp_off[r] = off(p.component[r].values); fa.comp_w[r] = p.component[r].width; }
+        fa.log_n = log_n;
+        fa.g = hf::pow(hf::to_monty(3), (uint64_t)127 << (24 - log_n));
+        fa.minus1 = hf::pow(hf::to_monty(3), (uint64_t)127 << 23);
+        fa.final_off = off(p.final_poly);
+        fold = true;
         // the device checks in verify_mle_evaluations' order: component openings round by round, then per fold round the opened value
         // and that round's openings, then final_poly
-        for (size_t r = 0; r < ncomp; r++) deferred.push_back(Deferred{V_TCS_COMPONENT, {(uint32_t)(r * nq), (uint32_t)((r + 1) * nq),
-                                                                                          (uint32_t)(n_jobs * nq + r), (uint32_t)(n_jobs * nq + r + 1)}});
+        for (size_t r = 0; r < ncomp; r++) deferred.push_back(Deferred{V_TCS_COMPONENT, (uint32_t)r});
         for (size_t r = 0; r < len; r++) {
-            deferred.push_back(Deferred{V_QUERY_VALUE, {(uint32_t)r}});
-            const size_t j = ncomp + r;
-            deferred.push_back(Deferred{V_TCS_QUERY, {(uint32_t)(j * nq), (uint32_t)((j + 1) * nq), (uint32_t)(n_jobs * nq + j), (uint32_t)(n_jobs * nq + j + 1)}});
+            deferred.push_back(Deferred{V_QUERY_VALUE, (uint32_t)r});
+            deferred.push_back(Deferred{V_TCS_QUERY, (uint32_t)(ncomp + r)});
         }
-        deferred.push_back(Deferred{V_QUERY_FINAL_POLY, {}});
+        deferred.push_back(Deferred{V_QUERY_FINAL_POLY, NO_JOB});
         const E4 f = ld(p.final_poly);
         if (neq(f, ld(p.univariate + 8 * (len - 1)) + betas.back() * ld(p.univariate + 8 * (len - 1) + 4))) host_fail = V_SUMCHECK_FINAL_POLY;
-        return nullptr;
     }
 
-    std::vector<Deferred> deferred;
-    uint32_t host_fail = V_ACCEPT;
 
     // the last checks of verify_shard (shard.rs:662-742): without its two dummy tables, each round lists one table per chip (per chip
     // with preprocessed columns in the preprocessed round), in chip order, with that chip's height as its row count and its width as
@@ -744,39 +719,70 @@ struct Verifier {
         return V_ACCEPT;
     }
 
-    // one copy of every device result, then the checks in order; host_fail (if set) comes after every deferred check
-    sp1b200_err resolve(uint32_t* verdict, float* kernel_ms) {
-        *kernel_ms = 0;
-        std::vector<uint32_t> out(out_words);
-        if (launched) {
-            SP1_CUDA(cudaMemcpyAsync(out.data(), d_out, out_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            SP1_CUDA(cudaStreamSynchronize(ctx->stream));
-            float ms = 0;
-            if (fold_launched && cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) { ctx->phase_ms["verify.merkle"] = ms; *kernel_ms += ms; }
-            if (fold_launched && cudaEventElapsedTime(&ms, ev[1], ev[2]) == cudaSuccess) { ctx->phase_ms["verify.fold"] = ms; *kernel_ms += ms; }
-            if (jag_pending && cudaEventElapsedTime(&ms, ev[3], ev[4]) == cudaSuccess) { ctx->phase_ms["verify.jagged_eval"] = ms; *kernel_ms += ms; }
+    // the host phase: the shard's own words enter the transcript started from `start` - public values, main commitment, chip shapes
+    // (shard.rs:437-470) - then every host check in verify_shard's order, recording the device work.  No CUDA call.
+    void run(const uint32_t* start) {
+        const size_t nch = m->chips.size();
+        ch.load(start);
+        ch.observe_n(p.pv, p.n_pv);
+        ch.observe_n(p.commit, 8);
+        ch.observe(hf::to_monty(nch));
+        if (nch && mlr + 1 >= 30) verdict = V_INVALID_SHAPE;   // a degree point of 30 or more bits (shard.rs:477)
+        for (size_t k = 0; k < nch && !verdict; k++) {
+            ch.observe(hf::to_monty(heights[k]));
+            const size_t len = strlen(names[k]);
+            ch.observe(hf::to_monty(len));
+            for (size_t i = 0; i < len; i++) ch.observe(hf::to_monty((uint8_t)names[k][i]));
         }
+        // the preprocessed round's leading column counts are the preprocessed widths (shard.rs:506-523)
+        const bool has_prep = ncols.size() == 2;
+        if (!verdict && has_prep) {
+            size_t t = 0;
+            for (size_t k = 0; k < nch && !verdict; k++) {
+                if (!m->chips[k].prep_w) continue;
+                if (t >= p.rc_cc[0].size() || p.rc_cc[0][t].second != m->chips[k].prep_w) verdict = V_PREP_WIDTHS;
+                t++;
+            }
+        }
+        if (!verdict) verdict = gkr();
+        if (!verdict) verdict = zerocheck();
+        if (!verdict) {
+            std::vector<const uint32_t*> commits;
+            if (has_prep) commits.push_back(prep_commit8);
+            commits.push_back(p.commit);
+            jagged(commits);
+        }
+        if (!verdict) tail_fail = chip_tables();
+    }
+
+    // where the device phase put this shard's results: its first opening job, its fold words, its jagged partials
+    uint32_t job0 = 0, fold_at = 0, jag_at = 0;
+
+    // the checks in order after the device phase: an immediate verdict, then the deferred checks, then host_fail, then tail_fail.
+    // out: the batch's output words; n_jobs: the batch's opening jobs
+    uint32_t resolve(const std::vector<uint32_t>& out, uint32_t n_jobs) const {
+        if (verdict) return verdict;
         uint32_t min_bad = ~0u, final_bad = 0;
-        if (fold_launched)
+        if (fold)
             for (uint32_t q = 0; q < nq; q++) { min_bad = std::min(min_bad, out[fold_at + q]); final_bad |= out[fold_at + nq + q]; }
         for (const Deferred& d : deferred) {
             bool bad = false;
             if (d.code == V_JAGGED_EVALUATION) {
                 hf::E4 acc[1];
-                sum_partials<1>(out.data() + jag_at, jag_blocks, acc);
+                sum_partials<1>(out.data() + jag_at, blocks_for(jag_cols), acc);
                 bad = neq(acc[0] * jag_bp, jag_expect);
             } else if (d.code == V_QUERY_VALUE) {
-                bad = min_bad == d.flag_ranges[0];
+                bad = min_bad == d.job;
             } else if (d.code == V_QUERY_FINAL_POLY) {
                 bad = final_bad != 0;
-            } else {
-                for (size_t i = 0; i < d.flag_ranges.size(); i += 2)
-                    for (uint32_t t = d.flag_ranges[i]; t < d.flag_ranges[i + 1]; t++) bad |= out[t] != 0;
+            } else {   // an opening job: its nq path checks and its tensor commitment
+                const size_t j = (size_t)job0 + d.job;
+                for (uint32_t q = 0; q < nq; q++) bad |= out[j * nq + q] != 0;
+                bad |= out[(size_t)n_jobs * nq + j] != 0;
             }
-            if (bad) { *verdict = d.code; return nullptr; }
+            if (bad) return d.code;
         }
-        *verdict = host_fail;
-        return nullptr;
+        return host_fail ? host_fail : tail_fail;
     }
 };
 
@@ -803,93 +809,220 @@ bool canonical_proof(const layout::ShardProof& p, const sp1b200_machine* m, uint
     return ok && canonical(p.merkle_commits, 8 * p.rc_cc.size()) && canonical(p.expected_eval, 4);
 }
 
+// the device phase of a batch: every shard's evaluation section in one buffer, every recorded input in one auxiliary buffer, one
+// launch per kernel, one copy back; then each shard's checks in order
+sp1b200_err run_device(sp1b200_ctx* ctx, const std::vector<Verifier*>& vs, uint32_t* verdicts, VerifyTimes& t) {
+    const uint32_t nq = ctx->params.num_queries;
+    std::vector<uint64_t> ev_at(vs.size());
+    uint64_t ev_words = 0;
+    std::vector<uint32_t> aux;
+    auto align = [&](size_t a) { while (aux.size() % a) aux.push_back(0); };
+    auto put = [&](const std::vector<uint32_t>& v) { const uint32_t at = (uint32_t)aux.size(); aux.insert(aux.end(), v.begin(), v.end()); return at; };
+    std::vector<OpenJob> jobs;
+    std::vector<FoldArgs> folds;
+    std::vector<JagArgs> jags;
+    unsigned jag_blocks = 0;
+    for (Verifier* v : vs) if (v->jag) jag_blocks = std::max(jag_blocks, blocks_for(v->jag_cols));
+    size_t n_fold = 0, n_jag = 0;
+    for (Verifier* v : vs) { n_fold += v->fold; n_jag += v->jag; }
+    uint64_t n_jobs = 0;
+    for (Verifier* v : vs) if (v->fold) n_jobs += v->jobs.size();
+    const size_t fold_base = (size_t)n_jobs * (nq + 1), jag_base = fold_base + 2 * (size_t)nq * n_fold;
+    const size_t out_words = jag_base + 4 * (size_t)jag_blocks * n_jag;
+    if (out_words >> 32) return sp1b200_set_error("verify: %zu device result words in one batch do not fit 32-bit offsets", out_words);
+    for (size_t s = 0; s < vs.size(); s++) {
+        Verifier& v = *vs[s];
+        if (!v.fold && !v.jag) continue;
+        ev_at[s] = ev_words;
+        const uint32_t base = (uint32_t)ev_words;
+        ev_words += v.ev_words;
+        if (v.fold) {
+            v.job0 = (uint32_t)jobs.size();
+            v.fold_at = (uint32_t)(fold_base + 2 * (size_t)nq * folds.size());
+            FoldArgs a = v.fa;
+            a.idx_at = put(v.idx);
+            for (OpenJob j : v.jobs) {
+                j.values_off += base; j.paths_off += base; j.root_off += base; j.commit_off += base; j.idx_off = a.idx_at;
+                jobs.push_back(j);
+            }
+            a.coeff_at = put(v.coeff_words);
+            a.beta_at = put(v.beta_words);
+            std::vector<uint32_t> fo(v.fold_offs);
+            for (auto& o : fo) o += base;
+            a.fold_off_at = put(fo);
+            for (uint32_t r = 0; r < a.n_comp; r++) a.comp_off[r] += base;
+            a.final_off += base;
+            a.out_at = v.fold_at;
+            folds.push_back(a);
+        }
+        if (v.jag) {
+            v.jag_at = (uint32_t)(jag_base + 4 * (size_t)jag_blocks * jags.size());
+            JagArgs j{};
+            j.n_cols = v.jag_cols; j.nb = v.jag_nb; j.partial_at = v.jag_at;
+            j.col_eq_at = put(v.col_eq);
+            j.point_at = put(v.jag_point);
+            align(2);
+            j.prefix_at = (uint32_t)(aux.size() / 2);
+            const size_t at = aux.size();
+            aux.resize(at + 2 * v.prefix.size());
+            memcpy(&aux[at], v.prefix.data(), v.prefix.size() * 8);
+            jags.push_back(j);
+        }
+    }
+    if (ev_words >> 32 || aux.size() >> 31) return sp1b200_set_error("verify: a batch of %zu shards does not fit 32-bit offsets", vs.size());
+    std::vector<uint32_t> out(out_words);
+    if (out_words) {
+        align(4);
+        const size_t jobs_at = aux.size();
+        aux.resize(jobs_at + jobs.size() * sizeof(OpenJob) / 4);
+        memcpy(aux.data() + jobs_at, jobs.data(), jobs.size() * sizeof(OpenJob));
+        const size_t folds_at = aux.size();
+        aux.resize(folds_at + folds.size() * sizeof(FoldArgs) / 4);
+        memcpy(aux.data() + folds_at, folds.data(), folds.size() * sizeof(FoldArgs));
+        const size_t jags_at = aux.size();
+        aux.resize(jags_at + jags.size() * sizeof(JagArgs) / 4);
+        memcpy(aux.data() + jags_at, jags.data(), jags.size() * sizeof(JagArgs));
+        DevFree mem(ctx);
+        uint32_t *d_ev, *d_aux, *d_out;
+        SP1_TRY(mem.alloc((void**)&d_ev, std::max<uint64_t>(ev_words, 1) * 4));
+        SP1_TRY(mem.alloc((void**)&d_aux, aux.size() * 4));
+        SP1_TRY(mem.alloc((void**)&d_out, out_words * 4));
+        for (size_t s = 0; s < vs.size(); s++)
+            if (vs[s]->fold || vs[s]->jag)
+                SP1_CUDA(cudaMemcpyAsync(d_ev + ev_at[s], vs[s]->ev_base, vs[s]->ev_words * 4, cudaMemcpyHostToDevice, ctx->stream));
+        SP1_CUDA(cudaMemcpyAsync(d_aux, aux.data(), aux.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+        SP1_CUDA(cudaMemsetAsync(d_out, 0, out_words * 4, ctx->stream));
+        cudaEvent_t ev[4] = {};
+        struct Events { cudaEvent_t* e; ~Events() { for (int i = 0; i < 4; i++) if (e[i]) cudaEventDestroy(e[i]); } } guard{ev};
+        for (auto& e : ev) SP1_CUDA(cudaEventCreate(&e));
+        SP1_CUDA(cudaEventRecord(ev[0], ctx->stream));
+        if (!jobs.empty())
+            SP1_LAUNCH(ctx, verify_merkle_kernel, blocks_for(n_jobs * (nq + 1), 128), 128, 0, reinterpret_cast<const OpenJob*>(d_aux + jobs_at),
+                       (uint32_t)n_jobs, nq, d_ev, d_aux, d_out);
+        SP1_CUDA(cudaEventRecord(ev[1], ctx->stream));
+        if (!folds.empty())
+            SP1_LAUNCH(ctx, verify_fold_kernel, dim3(blocks_for(nq, 128), (unsigned)folds.size()), 128, 0,
+                       reinterpret_cast<const FoldArgs*>(d_aux + folds_at), d_ev, d_aux, d_out);
+        SP1_CUDA(cudaEventRecord(ev[2], ctx->stream));
+        if (!jags.empty())
+            SP1_LAUNCH(ctx, verify_jagged_kernel, dim3(jag_blocks, (unsigned)jags.size()), 256, 0, reinterpret_cast<const JagArgs*>(d_aux + jags_at),
+                       d_aux, d_out);
+        SP1_CUDA(cudaEventRecord(ev[3], ctx->stream));
+        SP1_CUDA(cudaMemcpyAsync(out.data(), d_out, out_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        SP1_CUDA(cudaStreamSynchronize(ctx->stream));
+        float ms = 0;
+        if (!folds.empty()) {
+            t.fold_ran = true;
+            if (cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) t.merkle += ms;
+            if (cudaEventElapsedTime(&ms, ev[1], ev[2]) == cudaSuccess) t.fold += ms;
+        }
+        if (!jags.empty()) {
+            t.jagged_ran = true;
+            if (cudaEventElapsedTime(&ms, ev[2], ev[3]) == cudaSuccess) t.jagged += ms;
+        }
+    }
+    for (size_t s = 0; s < vs.size(); s++) verdicts[s] = vs[s]->resolve(out, (uint32_t)n_jobs);
+    return nullptr;
+}
+
 }  // namespace
+
+sp1b200_err verify_parse_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint32_t* h_prep_commit8, const uint64_t* h_heights,
+                               const char* const* chip_names, const uint32_t* h_proof, uint64_t n_words, const std::string& who_s,
+                               VerifyShardIn& out) {
+    const char* who = who_s.c_str();
+    const sp1b200_params& prm = ctx->params;
+    const uint32_t mlr = prm.max_log_row_count, ls = prm.log_stacking_height, nq = prm.num_queries;
+    if (mlr > 30 || ls > 30 || prm.log_blowup > 24 || nq == 0 || nq > (1u << 16))
+        return sp1b200_set_error("%s: context parameters out of range (max_log_row_count %u, log_stacking_height %u, num_queries %u)", who, mlr, ls, nq);
+    const size_t nch = m->chips.size();
+    out.mw.resize(nch); out.pw.resize(nch);
+    bool has_prep = false;
+    for (size_t k = 0; k < nch; k++) {
+        out.mw[k] = m->chips[k].main_w; out.pw[k] = m->chips[k].prep_w;
+        has_prep |= out.pw[k] != 0;
+        if (!chip_names[k]) return sp1b200_set_error("%s: chip %zu has no name", who, k);
+        if (h_heights[k] >> (mlr + 1)) return sp1b200_set_error("%s: chip %zu: height %llu does not fit %u bits", who, k, (unsigned long long)h_heights[k], mlr + 1);
+    }
+    if (!m->interactions || m->host.size() != nch) return sp1b200_set_error("%s: machine is not initialised", who);
+    if (has_prep && !h_prep_commit8) return sp1b200_set_error("%s: the machine has preprocessed columns but h_prep_commit8 is NULL", who);
+    out.heights = h_heights;
+    layout::Shape& shape = out.shape;
+    shape.n_chips = nch; shape.main_w = out.mw.data(); shape.prep_w = out.pw.data();
+    shape.max_log_row_count = mlr; shape.log_stacking_height = ls; shape.num_queries = nq;
+    shape.ncols = layout::round_columns(nch, h_heights, out.mw.data(), out.pw.data(), ls);
+    layout::ShardProof& p = out.p;
+    if (const char* why = layout::parse_shard_proof(h_proof, n_words, shape, p)) return sp1b200_set_error("%s: %s", who, why);
+    // the oracle's reader and BasefoldProof's shape: every opening has the height of its round's tree
+    for (size_t r = 0; r < p.component.size(); r++)
+        if (p.component[r].log_height != ls + prm.log_blowup) return sp1b200_set_error("%s: evaluation proof: commitment round %zu opening has log_height %u, the layout needs %u", who, r, p.component[r].log_height, ls + prm.log_blowup);
+    for (uint32_t r = 0; r < ls; r++)
+        if (p.query[r].log_height != ls + prm.log_blowup - r - 1) return sp1b200_set_error("%s: evaluation proof: fold round %u opening has log_height %u, the layout needs %u", who, r, p.query[r].log_height, ls + prm.log_blowup - r - 1);
+    if (!canonical_proof(p, m, mlr, ls, nq)) return sp1b200_set_error("%s: a field word of the proof is not canonical (>= p)", who);
+    for (size_t k = 0; k < nch; k++)
+        for (uint32_t pi : m->host[k].publics)
+            if (pi >= p.n_pv) return sp1b200_set_error("%s: chip %zu reads public value %u but the proof carries %u", who, k, pi, p.n_pv);
+    // the verifier reads no more GKR outputs or tables per round than a shard of this library can have (the layout reader admits
+    // more, for the wire format's sake)
+    if (p.n_out > (1u << 20)) return sp1b200_set_error("%s: LogUp-GKR section: %u outputs, more than 2^20", who, p.n_out);
+    for (auto& t : p.rc_cc)
+        if (t.size() > 4096) return sp1b200_set_error("%s: evaluation proof: %zu tables in a round, more than 4096", who, t.size());
+    return nullptr;
+}
+
+sp1b200_err verify_shards(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint32_t* h_prep_commit8, const char* const* chip_names,
+                          const std::vector<const VerifyShardIn*>& shards, const uint32_t* start34, uint32_t host_threads,
+                          uint32_t* verdicts, uint32_t* finals, VerifyTimes& t) {
+    const size_t n = shards.size();
+    std::vector<std::unique_ptr<Verifier>> vs;
+    std::vector<Verifier*> vp;
+    for (const VerifyShardIn* in : shards) {
+        vs.emplace_back(new Verifier(ctx->params, m, in->p, in->heights, chip_names, in->shape.ncols, h_prep_commit8));
+        vp.push_back(vs.back().get());
+    }
+    const auto h0 = std::chrono::steady_clock::now();
+    const size_t nt = std::min<size_t>(std::max<uint32_t>(host_threads, 1), n);
+    if (nt <= 1) {
+        for (auto& v : vs) v->run(start34);
+    } else {   // the host phases share nothing but the read-only machine; each thread takes the next shard
+        std::atomic<size_t> next{0};
+        std::vector<std::thread> pool;
+        for (size_t i = 0; i < nt; i++)
+            pool.emplace_back([&] { for (size_t s; (s = next.fetch_add(1)) < n;) vs[s]->run(start34); });
+        for (auto& th : pool) th.join();
+    }
+    t.host_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - h0).count();
+    SP1_TRY(run_device(ctx, vp, verdicts, t));
+    if (finals)
+        for (size_t s = 0; s < n; s++) if (!verdicts[s]) vs[s]->ch.store(finals + 34 * s);
+    return nullptr;
+}
 
 extern "C" {
 
-const char* sp1b200_verdict_name(uint32_t verdict) { return verdict < V_COUNT ? VERDICT_NAMES[verdict] : "Unknown"; }
+const char* sp1b200_verdict_name(uint32_t verdict) {
+    if (verdict < V_COUNT) return VERDICT_NAMES[verdict];
+    const char* core = verify_core_verdict_name(verdict);
+    return core ? core : "Unknown";
+}
 
 sp1b200_err sp1b200_verify_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint32_t* h_prep_commit8, const uint64_t* h_heights,
                                  const char* const* chip_names, const uint32_t* h_proof, uint64_t n_words, uint32_t* h_chal, uint32_t* h_verdict) {
     SP1_DEVICE_GUARD(ctx);
     if (!ctx || !m || !h_heights || !chip_names || !h_proof || !h_chal || !h_verdict) return sp1b200_set_error("verify_shard: NULL argument");
     const auto t0 = std::chrono::steady_clock::now();
-    const sp1b200_params& prm = ctx->params;
-    const uint32_t mlr = prm.max_log_row_count, ls = prm.log_stacking_height, nq = prm.num_queries;
-    if (mlr > 30 || ls > 30 || prm.log_blowup > 24 || nq == 0 || nq > (1u << 16))
-        return sp1b200_set_error("verify_shard: context parameters out of range (max_log_row_count %u, log_stacking_height %u, num_queries %u)", mlr, ls, nq);
-    const size_t nch = m->chips.size();
-    std::vector<uint32_t> mw(nch), pw(nch);
-    bool has_prep = false;
-    for (size_t k = 0; k < nch; k++) {
-        mw[k] = m->chips[k].main_w; pw[k] = m->chips[k].prep_w;
-        has_prep |= pw[k] != 0;
-        if (!chip_names[k]) return sp1b200_set_error("verify_shard: chip %zu has no name", k);
-        if (h_heights[k] >> (mlr + 1)) return sp1b200_set_error("verify_shard: chip %zu: height %llu does not fit %u bits", k, (unsigned long long)h_heights[k], mlr + 1);
-    }
-    if (!m->interactions || m->host.size() != nch) return sp1b200_set_error("verify_shard: machine is not initialised");
-    if (has_prep && !h_prep_commit8) return sp1b200_set_error("verify_shard: the machine has preprocessed columns but h_prep_commit8 is NULL");
-    layout::Shape shape;
-    shape.n_chips = nch; shape.main_w = mw.data(); shape.prep_w = pw.data();
-    shape.max_log_row_count = mlr; shape.log_stacking_height = ls; shape.num_queries = nq;
-    shape.ncols = layout::round_columns(nch, h_heights, mw.data(), pw.data(), ls);
-    layout::ShardProof p;
-    if (const char* why = layout::parse_shard_proof(h_proof, n_words, shape, p)) return sp1b200_set_error("verify_shard: %s", why);
-    // the oracle's reader and BasefoldProof's shape: every opening has the height of its round's tree
-    for (size_t r = 0; r < p.component.size(); r++)
-        if (p.component[r].log_height != ls + prm.log_blowup) return sp1b200_set_error("verify_shard: evaluation proof: commitment round %zu opening has log_height %u, the layout needs %u", r, p.component[r].log_height, ls + prm.log_blowup);
-    for (uint32_t r = 0; r < ls; r++)
-        if (p.query[r].log_height != ls + prm.log_blowup - r - 1) return sp1b200_set_error("verify_shard: evaluation proof: fold round %u opening has log_height %u, the layout needs %u", r, p.query[r].log_height, ls + prm.log_blowup - r - 1);
-    if (!canonical_proof(p, m, mlr, ls, nq)) return sp1b200_set_error("verify_shard: a field word of the proof is not canonical (>= p)");
-    for (size_t k = 0; k < nch; k++)
-        for (uint32_t pi : m->host[k].publics)
-            if (pi >= p.n_pv) return sp1b200_set_error("verify_shard: chip %zu reads public value %u but the proof carries %u", k, pi, p.n_pv);
-    // the verifier reads no more GKR outputs or tables per round than a shard of this library can have (the layout reader admits
-    // more, for the wire format's sake)
-    if (p.n_out > (1u << 20)) return sp1b200_set_error("verify_shard: LogUp-GKR section: %u outputs, more than 2^20", p.n_out);
-    for (auto& t : p.rc_cc)
-        if (t.size() > 4096) return sp1b200_set_error("verify_shard: evaluation proof: %zu tables in a round, more than 4096", t.size());
-    const uint32_t* ev_base = p.univariate;
-    const uint64_t ev_words = (uint64_t)(p.pv - ev_base);
-    Verifier v(ctx, m, p, h_heights, shape.ncols, ev_base, ev_words);
-    v.ch.load(h_chal);
-    // the shard's own words enter the transcript: public values, main commitment, chip shapes (shard.rs:437-470)
-    v.ch.observe_n(p.pv, p.n_pv);
-    v.ch.observe_n(p.commit, 8);
-    v.ch.observe(hf::to_monty(nch));
-    uint32_t verdict = V_ACCEPT;
-    if (nch && mlr + 1 >= 30) verdict = V_INVALID_SHAPE;   // a degree point of 30 or more bits (shard.rs:477)
-    for (size_t k = 0; k < nch && !verdict; k++) {
-        v.ch.observe(hf::to_monty(h_heights[k]));
-        const size_t len = strlen(chip_names[k]);
-        v.ch.observe(hf::to_monty(len));
-        for (size_t i = 0; i < len; i++) v.ch.observe(hf::to_monty((uint8_t)chip_names[k][i]));
-    }
-    // the preprocessed round's leading column counts are the preprocessed widths (shard.rs:506-523)
-    if (!verdict && has_prep) {
-        size_t t = 0;
-        for (size_t k = 0; k < nch && !verdict; k++) {
-            if (!pw[k]) continue;
-            if (t >= p.rc_cc[0].size() || p.rc_cc[0][t].second != pw[k]) verdict = V_PREP_WIDTHS;
-            t++;
-        }
-    }
-    if (!verdict) verdict = v.gkr();
-    if (!verdict) verdict = v.zerocheck();
-    if (!verdict) {
-        std::vector<const uint32_t*> commits;
-        if (has_prep) commits.push_back(h_prep_commit8);
-        commits.push_back(p.commit);
-        SP1_TRY(v.jagged(commits, &verdict));
-    }
+    VerifyShardIn in;
+    SP1_TRY(verify_parse_shard(ctx, m, h_prep_commit8, h_heights, chip_names, h_proof, n_words, "verify_shard", in));
+    uint32_t verdict = V_ACCEPT, fin[34];
+    VerifyTimes t;
+    SP1_TRY(verify_shards(ctx, m, h_prep_commit8, chip_names, {&in}, h_chal, 1, &verdict, fin, t));
     float kernel_ms = 0;
-    if (!verdict) SP1_TRY(v.resolve(&verdict, &kernel_ms));
-    else SP1_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (!verdict) verdict = v.chip_tables();
+    if (t.fold_ran) { ctx->phase_ms["verify.merkle"] = t.merkle; ctx->phase_ms["verify.fold"] = t.fold; kernel_ms += t.merkle + t.fold; }
+    if (t.jagged_ran) { ctx->phase_ms["verify.jagged_eval"] = t.jagged; kernel_ms += t.jagged; }
     ctx->phase_ms["verify.kernels"] = kernel_ms;
     ctx->phase_ms["verify.total"] = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     *h_verdict = verdict;
-    if (!verdict) v.ch.store(h_chal);
+    if (!verdict) memcpy(h_chal, fin, sizeof(fin));
     return nullptr;
 }
 

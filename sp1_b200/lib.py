@@ -14,6 +14,24 @@ SO_PATH = os.path.join(HERE, "libsp1b200.so")
 u32p = C.POINTER(C.c_uint32)
 
 
+# word offsets of PublicValues<[F; 4], [F; 3], [F; 4], F> (crates/hypercube/src/air/public_values.rs, without mprotect) in a shard's
+# public values; (offset, length).  A core proof's shards carry PV_MAX_NUM = PROOF_MAX_NUM_PVS words, the first PV_NUM_ELTS of them used.
+PV = dict(prev_committed_value_digest=(0, 32), committed_value_digest=(32, 32), prev_deferred_proofs_digest=(64, 8),
+          deferred_proofs_digest=(72, 8), pc_start=(80, 3), next_pc=(83, 3), prev_exit_code=(86, 1), exit_code=(87, 1),
+          is_execution_shard=(88, 1), previous_init_addr=(89, 3), last_init_addr=(92, 3), previous_finalize_addr=(95, 3),
+          last_finalize_addr=(98, 3), previous_init_page_idx=(101, 3), last_init_page_idx=(104, 3), previous_finalize_page_idx=(107, 3),
+          last_finalize_page_idx=(110, 3), initial_timestamp=(113, 4), last_timestamp=(117, 4), is_timestamp_high_eq=(121, 1),
+          inv_timestamp_high=(122, 1), is_timestamp_low_eq=(123, 1), inv_timestamp_low=(124, 1), global_init_count=(125, 1),
+          global_finalize_count=(126, 1), global_page_prot_init_count=(127, 1), global_page_prot_finalize_count=(128, 1),
+          global_count=(129, 1), global_cumulative_sum=(130, 14), prev_commit_syscall=(144, 1), commit_syscall=(145, 1),
+          prev_commit_deferred_syscall=(146, 1), commit_deferred_syscall=(147, 1), initial_timestamp_inv=(148, 1),
+          last_timestamp_inv=(149, 1), is_first_execution_shard=(150, 1), is_untrusted_programs_enabled=(151, 1), proof_nonce=(152, 4),
+          empty=(156, 4))
+PV_NUM_ELTS = 160
+PV_MAX_NUM = 187
+VK_TAIL_WORDS = 24   # pc_start[3] | initial_global_cumulative_sum x[7] y[7] | enable_untrusted_programs | 6 zeros
+
+
 class Params(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("log_stacking_height", "max_log_row_count", "log_blowup", "num_queries",
                                           "pow_bits", "batch_pow_bits", "gkr_pow_bits", "grind_mode")]
@@ -60,7 +78,7 @@ ERR_FUNCS = [
     "sp1b200_stacked_commit", "sp1b200_stacked_prove", "sp1b200_jagged_commit", "sp1b200_jagged_column_claims",
     "sp1b200_jagged_prove", "sp1b200_machine_create", "sp1b200_zerocheck", "sp1b200_logup_gkr", "sp1b200_prove_shard",
     "sp1b200_setup_and_prove_shard", "sp1b200_shard_proof_to_bincode", "sp1b200_shard_proof_from_bincode",
-    "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard",
+    "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard", "sp1b200_verify_core_proof",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
@@ -277,6 +295,28 @@ class Lib:
         self._chk(self.L.sp1b200_verify_shard(self.ctx, machine, _ptr(pc), H, NM, _ptr(w), C.c_uint64(w.size), _ptr(st), C.byref(verdict)))
         return int(verdict.value), st
 
+    def verify_core_proof(self, machine, prep_commit, vk_tail, heights_per_shard, names, words_per_shard, host_threads=0):
+        """SP1Prover::verify on a core proof: the shards' flat proof words (one machine, names and context parameters), chip heights
+        per shard, and the verifying key = prep_commit[8] + vk_tail[24].  -> (verdict, shard, shard_verdict, final_challengers):
+        verdict 0 accepts and final_challengers is then [n_shards, 34] (each shard verifier's final state), else None; for
+        InvalidShardProof, shard_verdict is the failing shard's verify_shard code (verdict_name names both code spaces)."""
+        n = len(words_per_shard)
+        nch = len(names)
+        H = np.ascontiguousarray(np.asarray(heights_per_shard, dtype=np.uint64).reshape(n * nch) if n else np.zeros(1, np.uint64))
+        NM = (C.c_char_p * max(1, nch))(*[s.encode() for s in names])
+        ws = [None if w is None else np.ascontiguousarray(w, dtype=np.uint32) for w in words_per_shard]
+        P = (C.c_void_p * max(1, n))(*[None if w is None else w.ctypes.data for w in ws])
+        NW = (C.c_uint64 * max(1, n))(*[0 if w is None else w.size for w in ws])
+        pc = np.ascontiguousarray(prep_commit, dtype=np.uint32)
+        tail = np.ascontiguousarray(vk_tail, dtype=np.uint32)
+        fin = np.zeros((max(1, n), 34), np.uint32)
+        verdict, shard, sv = C.c_uint32(), C.c_uint32(), C.c_uint32()
+        self._chk(self.L.sp1b200_verify_core_proof(self.ctx, machine, _ptr(pc), _ptr(tail), C.c_uint32(tail.size), C.c_uint32(n),
+                                                    C.c_void_p(H.ctypes.data), NM, P, NW, C.c_uint32(host_threads), _ptr(fin),
+                                                    C.byref(verdict), C.byref(shard), C.byref(sv)))
+        v = int(verdict.value)
+        return v, int(shard.value), int(sv.value), (fin[:n].copy() if v == 0 else None)
+
     def _debug_call(self, fn, args, cap_words):
         out = np.empty(max(1, cap_words), np.uint32)
         nw = C.c_uint64()
@@ -376,7 +416,7 @@ def parse_interaction_report(w):
 
 
 def verdict_name(verdict):
-    """the reason a verdict of verify_shard names ("Accepted" for 0)"""
+    """the reason a verdict of verify_shard or verify_core_proof names ("Accepted" for 0)"""
     return load().sp1b200_verdict_name(C.c_uint32(verdict)).decode()
 
 
