@@ -125,6 +125,46 @@ void host_poseidon2_permute(uint32_t* s) {
 uint32_t host_to_monty(uint64_t canonical) { return (uint32_t)(((canonical % kb::P) << 32) % kb::P); }
 uint32_t host_from_monty(uint32_t m) { return h_reduce(m); }
 
+void host_hash(const uint32_t* in, size_t n, uint32_t* out8) {
+    uint32_t s[16] = {0};
+    size_t fill = 0;
+    for (size_t i = 0; i < n; i++) { s[fill++] = in[i]; if (fill == 8) { host_poseidon2_permute(s); fill = 0; } }
+    if (fill) host_poseidon2_permute(s);
+    memcpy(out8, s, 32);
+}
+void host_compress(const uint32_t* l8, const uint32_t* r8, uint32_t* out8) {
+    uint32_t s[16];
+    memcpy(s, l8, 32); memcpy(s + 8, r8, 32);
+    host_poseidon2_permute(s);
+    memcpy(out8, s, 32);
+}
+
+void table_size_commitment(const uint32_t* original8, const std::vector<std::pair<uint64_t, uint64_t>>& tables, uint32_t* out8) {
+    std::vector<uint32_t> meta{host_to_monty(tables.size())};
+    for (auto& t : tables) meta.push_back(host_to_monty(t.first));
+    for (auto& t : tables) meta.push_back(host_to_monty(t.second));
+    uint32_t h[8];
+    host_hash(meta.data(), meta.size(), h);
+    host_compress(original8, h, out8);
+}
+
+void observe_chip_shapes(HostChallenger& ch, size_t n_chips, const uint64_t* heights, const char* const* names) {
+    ch.observe(host_to_monty(n_chips));
+    for (size_t k = 0; k < n_chips; k++) {
+        ch.observe(host_to_monty(heights[k]));
+        const size_t len = strlen(names[k]);
+        ch.observe(host_to_monty(len));
+        for (size_t i = 0; i < len; i++) ch.observe(host_to_monty((uint8_t)names[k][i]));
+    }
+}
+
+hf::E4 batched_opening_claim(const uint32_t* main, uint32_t main_w, const uint32_t* prep, uint32_t prep_w, const hf::E4& gamma) {
+    hf::E4 acc, g = gamma;
+    for (uint32_t j = 0; j < main_w; j++) { acc = acc + hf::E4::load(main + 4 * j) * g; g = g * gamma; }
+    for (uint32_t j = 0; j < prep_w; j++) { acc = acc + hf::E4::load(prep + 4 * j) * g; g = g * gamma; }
+    return acc;
+}
+
 void HostChallenger::duplexing() {
     for (uint32_t i = 0; i < nin; i++) sponge[i] = inbuf[i];
     nin = 0;

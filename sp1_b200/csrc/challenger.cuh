@@ -4,11 +4,19 @@
 // semantics sp1-gpu/crates/sys/include/challenger/challenger.cuh:22-112.  Only the PoW grind runs on the device.
 #pragma once
 #include "ctx.cuh"
+#include "hostfield.hpp"
 #include <cstring>
+#include <utility>
+#include <vector>
 
 uint32_t host_to_monty(uint64_t canonical);
 uint32_t host_from_monty(uint32_t m);
 void host_poseidon2_permute(uint32_t* s16);
+// PaddingFreeSponge<16, 8, 8> (overwrite mode) and the 2-to-1 compression, with the transcript's permutation
+void host_hash(const uint32_t* in, size_t n, uint32_t* out8);
+void host_compress(const uint32_t* l8, const uint32_t* r8, uint32_t* out8);
+// a jagged round's commitment: compress(original, hash(n_tables | rows of every table | columns of every table)); tables: (rows, cols)
+void table_size_commitment(const uint32_t* original8, const std::vector<std::pair<uint64_t, uint64_t>>& tables, uint32_t* out8);
 
 struct HostChallenger {
     sp1b200_ctx* ctx = nullptr;
@@ -29,3 +37,9 @@ struct HostChallenger {
     bool check_witness(uint32_t bits, uint32_t w_monty);
     sp1b200_err grind(uint32_t bits, uint32_t* w_monty);  // device search, canonical-min witness
 };
+
+// Transcript steps the shard prover and the shard verifier share.
+// The chip shapes after the main commitment (shard.rs): the chip count, then per chip its height and its name (length, then bytes).
+void observe_chip_shapes(HostChallenger& ch, size_t n_chips, const uint64_t* heights, const char* const* names);
+// A chip's γ-batched opening claim Σ_j γ^(j+1) o_j over its opened values, main columns then preprocessed ones (ext each).
+hf::E4 batched_opening_claim(const uint32_t* main, uint32_t main_w, const uint32_t* prep, uint32_t prep_w, const hf::E4& gamma);

@@ -63,6 +63,11 @@ inline E4 operator*(const E4& a, const E4& b) {
     r.c[3] = reduce4(a0 * b3 + a1 * b2 + a2 * b1 + a3 * b0);
     return r;
 }
+// the base-field names for E4, so that code templated on the value type (the constraint interpreter, machine.cuh) takes either
+inline E4 add(const E4& a, const E4& b) { return a + b; }
+inline E4 sub(const E4& a, const E4& b) { return a - b; }
+inline E4 mul(const E4& a, const E4& b) { return a * b; }
+inline E4 neg(const E4& a) { return E4() - a; }
 inline E4 inv(const E4& a) {
     // Frobenius-free inverse via the tower F[y]/(y^2-3) (y = x^2)
     const uint32_t three = to_monty(3);
@@ -89,6 +94,14 @@ inline std::vector<E4> partial_lagrange(const std::vector<E4>& point) {
         ev.swap(nx);
     }
     return ev;
+}
+
+// Σ_i eq(point, i) · vals[i] over the first min(|vals|, 2^|point|) values: the multilinear extension of vals at point
+inline E4 mle_eval(const std::vector<E4>& vals, const std::vector<E4>& point) {
+    const std::vector<E4> eq = partial_lagrange(point);
+    E4 acc;
+    for (size_t i = 0; i < vals.size() && i < eq.size(); i++) acc = acc + eq[i] * vals[i];
+    return acc;
 }
 
 // Lagrange basis over N distinct nodes, L[i][k] = coefficient of X^k in L_i(X) (degree N-1), with ONE field inversion

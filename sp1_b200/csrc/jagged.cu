@@ -24,25 +24,6 @@ namespace {
 using kb::Ext;
 using hf::E4;
 
-// ---- host sponge (PaddingFreeSponge) for the table-shape hash; a few dozen words ----------------------------------
-void host_hash(const std::vector<uint32_t>& w, uint32_t* out8) {
-    uint32_t st[16] = {0};
-    size_t i = 0;
-    while (i < w.size()) {
-        size_t k = std::min<size_t>(8, w.size() - i);
-        for (size_t j = 0; j < k; j++) st[j] = w[i + j];
-        host_poseidon2_permute(st);
-        i += k;
-    }
-    for (int j = 0; j < 8; j++) out8[j] = st[j];
-}
-void host_compress(const uint32_t* l, const uint32_t* r, uint32_t* out8) {
-    uint32_t st[16];
-    for (int j = 0; j < 8; j++) { st[j] = l[j]; st[8 + j] = r[j]; }
-    host_poseidon2_permute(st);
-    for (int j = 0; j < 8; j++) out8[j] = st[j];
-}
-
 struct SegTable {  // the virtual long base vector = concatenation of the rounds' dense buffers, then zeros
     const uint32_t* ptr[8];
     uint64_t end[8];
@@ -237,17 +218,7 @@ __global__ void __launch_bounds__(256) hadamard_fold_kernel(const uint32_t* __re
     block_reduce<2>({s0, sh}, partial, mail);
 }
 
-// ---- branching program (slop/crates/jagged/src/poly.rs:136-175, 384-470) ---------------------------------------
-// state index = carry + 2 * comparison_so_far ; returns -1 on failure
-__device__ __forceinline__ int bp_transition(int row_bit, int index_bit, int cur_bit, int next_bit, int state) {
-    int carry = state & 1, cmp = state >> 1;
-    int new_cmp = (index_bit == next_bit) ? cmp : next_bit;
-    int s = row_bit + carry + cur_bit;
-    if (index_bit != (s & 1)) return -1;
-    return (s >> 1) + 2 * new_cmp;
-}
-
-// ---- prefix / suffix form of the same evaluation -----------------------------------------------------------------
+// ---- branching program (one layer: bp_transition, sumcheck.cuh), in prefix / suffix form ----------------------------
 // The evaluation is  e0^T M_0 M_1 ... M_hl init  with one 4x4 transfer matrix per layer, M_l = M(cur_l, next_l).  In sumcheck
 // round r only ONE layer holds the free variable: layers above it still see the column's boolean prefix-sum bits (and, in
 // the second half, next-coordinates that were bound earlier and never change again), layers below it see coordinates that
@@ -409,10 +380,9 @@ sp1b200_err sp1b200_jagged_commit(sp1b200_ctx* ctx, const uint32_t* dense_any, u
     uint64_t area = 0;
     for (uint32_t t = 0; t < n_tables; t++) {
         if (rows[t] > ((uint64_t)1 << mlr)) return sp1b200_set_error("jagged_commit: table %u has %llu rows > 2^%u", t, (unsigned long long)rows[t], mlr);
-        r->row_counts.push_back(rows[t]); r->col_counts.push_back(cols[t]); area += rows[t] * cols[t];
+        r->tables.emplace_back(rows[t], cols[t]); area += rows[t] * cols[t];
     }
-    const uint64_t S = (uint64_t)1 << ls, R = (uint64_t)1 << mlr;
-    const uint64_t padded = std::max(((area + S - 1) / S) * S, S);
+    const uint64_t padded = layout::stacked_columns(area, ls) << ls;
     const uint64_t added = padded - area;
     r->area = area; r->padded_area = padded;
     SP1_CUDA(cudaMallocFromPoolAsync((void**)&r->d_dense, padded * 4, ctx->pool, ctx->stream));
@@ -420,19 +390,12 @@ sp1b200_err sp1b200_jagged_commit(sp1b200_ctx* ctx, const uint32_t* dense_any, u
     cudaError_t ce = area ? cudaMemcpyAsync(r->d_dense, dense_any, area * 4, cudaMemcpyDefault, ctx->stream) : cudaSuccess;
     sp1b200_upload_release(ctx, up_slot);                        // the slot is free once this copy has run
     if (ce == cudaSuccess && added) ce = cudaMemsetAsync(r->d_dense + area, 0, added * 4, ctx->stream);
-    sp1b200_err e = ce == cudaSuccess ? sp1b200_stacked_commit(ctx, r->d_dense, padded / S, keep_codeword, r->original_commit, &r->stacked)
+    sp1b200_err e = ce == cudaSuccess ? sp1b200_stacked_commit(ctx, r->d_dense, padded >> ls, keep_codeword, r->original_commit, &r->stacked)
                                       : sp1b200_set_error("jagged_commit: copying the dense trace: %s", cudaGetErrorString(ce));
     if (e) { cudaFreeAsync(r->d_dense, ctx->stream); r->d_dense = nullptr; return e; }
-    const uint64_t added_cols = std::max<uint64_t>((added + R - 1) / R, 1);
-    r->row_counts.push_back(R); r->row_counts.push_back(added - (added_cols - 1) * R);
-    r->col_counts.push_back(added_cols - 1); r->col_counts.push_back(1);
-    r->padding_cols = added_cols;
-    std::vector<uint32_t> meta{hf::to_monty(r->row_counts.size())};
-    for (uint64_t x : r->row_counts) meta.push_back(hf::to_monty(x));
-    for (uint64_t x : r->col_counts) meta.push_back(hf::to_monty(x));
-    uint32_t hsh[8];
-    host_hash(meta, hsh);
-    host_compress(r->original_commit, hsh, r->commit);
+    const layout::Tables pad = layout::padding_tables(area, ls, mlr);
+    r->tables.insert(r->tables.end(), pad.begin(), pad.end());
+    table_size_commitment(r->original_commit, r->tables, r->commit);
     if (h_commit8) memcpy(h_commit8, r->commit, 32);
     *out = r.release();
     return nullptr;
@@ -454,9 +417,10 @@ sp1b200_err sp1b200_jagged_column_claims(sp1b200_ctx* ctx, const sp1b200_jagged_
     std::vector<EvalTable> tabs;  // the round's tables without the two padding tables
     uint64_t off = 0;
     uint32_t nc = 0;
-    for (size_t t = 0; t + 2 < r->row_counts.size(); t++) {
-        tabs.push_back(EvalTable{r->d_dense + off, r->row_counts[t], (uint32_t)r->col_counts[t], nc});
-        off += r->row_counts[t] * r->col_counts[t]; nc += (uint32_t)r->col_counts[t];
+    for (size_t t = 0; t + 2 < r->tables.size(); t++) {
+        const auto& [rows, cols] = r->tables[t];
+        tabs.push_back(EvalTable{r->d_dense + off, rows, (uint32_t)cols, nc});
+        off += rows * cols; nc += (uint32_t)cols;
     }
     if (!nc) return nullptr;
     SP1_TRY(mem.alloc((void**)&d_z, mlr * 16));
@@ -486,14 +450,10 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     SP1_TRY(ch.init(ctx, h_chal));
     PhaseTimer t_all(ctx, "jagged.total");
 
-    // column heights over all rounds (dummy tables included) and prefix sums
-    std::vector<uint64_t> heights;
-    uint64_t total_cols = 0;
-    for (uint32_t r = 0; r < n_rounds; r++)
-        for (size_t t = 0; t < rounds[r]->row_counts.size(); t++)
-            for (uint64_t c = 0; c < rounds[r]->col_counts[t]; c++) { heights.push_back(rounds[r]->row_counts[t]); total_cols++; }
-    std::vector<uint64_t> prefix;
-    { uint64_t s = 0; for (uint64_t hgt : heights) { prefix.push_back(s); s += hgt; } prefix.push_back(prefix.back() + heights.back()); }
+    // column prefix sums over all rounds (padding tables included)
+    std::vector<uint64_t> prefix{0};
+    for (uint32_t r = 0; r < n_rounds; r++) layout::append_column_prefix(prefix, rounds[r]->tables);
+    const uint64_t total_cols = prefix.size() - 1;
     const uint32_t lm = hf::log2_ceil(prefix.back());
     if (lm < ls) return sp1b200_set_error("jagged_prove: internal: log_m < log_stacking_height");
     if (lm < 2) return sp1b200_set_error("jagged_prove: fewer than two sumcheck variables (log_m = %u)", lm);
@@ -508,15 +468,13 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     {
         size_t k = 0;
         for (uint32_t r = 0; r < n_rounds; r++) {
-            uint64_t real = 0;
-            for (size_t t = 0; t + 2 < rounds[r]->col_counts.size(); t++) real += rounds[r]->col_counts[t];
-            for (uint64_t c = 0; c < real; c++) column_claims.push_back(E4::load(h_claims + 4 * (k++)));
-            for (uint64_t c = 0; c < rounds[r]->padding_cols; c++) column_claims.push_back(E4());
+            const layout::Tables& tb = rounds[r]->tables;
+            for (size_t t = 0; t < tb.size(); t++)
+                for (uint64_t c = 0; c < tb[t].second; c++) column_claims.push_back(t + 2 < tb.size() ? E4::load(h_claims + 4 * (k++)) : E4());
         }
     }
+    const E4 claim = hf::mle_eval(column_claims, z_col);
     std::vector<E4> col_eq_full = hf::partial_lagrange(z_col);
-    E4 claim;
-    for (size_t i = 0; i < column_claims.size(); i++) claim = claim + col_eq_full[i] * column_claims[i];
 
     // K = the rounds summed straight from the base-field trace (see jagged_round_kernel): every aligned 2^K block must lie in one
     // column (2^K divides every prefix sum), in one segment (K <= log_stacking_height) and in one run of 2^lb rows (K <= lb); round
@@ -756,8 +714,8 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     for (auto& x : rhos) put(x.c, 4);
     put(je_eval.c, 4);
     for (uint32_t r = 0; r < n_rounds; r++) {
-        put1((uint32_t)rounds[r]->row_counts.size());
-        for (size_t t = 0; t < rounds[r]->row_counts.size(); t++) { put1((uint32_t)rounds[r]->row_counts[t]); put1((uint32_t)rounds[r]->col_counts[t]); }
+        put1((uint32_t)rounds[r]->tables.size());
+        for (auto& t : rounds[r]->tables) { put1((uint32_t)t.first); put1((uint32_t)t.second); }
     }
     for (uint32_t r = 0; r < n_rounds; r++) put(rounds[r]->original_commit, 8);
     put(base_eval.c, 4);

@@ -1,7 +1,10 @@
 // The machine description shared by zerocheck.cu and gkr.cu: per-chip constraint bytecode (reference layout,
 // sp1-gpu/crates/sys/include/zerocheck/sequential.cuh:13-49) and LogUp interactions.
 #pragma once
+#include "hostfield.hpp"
+#include <algorithm>
 #include <cstdint>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -18,11 +21,34 @@ struct ChipProg {  // device pointers into the machine arena
     uint32_t n_instrs, n_asserts, n_regs, main_w, prep_w, n_constraints;
     const ZcInstr* zc; uint32_t n_zc, zc_regs;  // re-scheduled program interpreted by the zerocheck kernels
 };
-struct HostProg {  // host copy for the padded-row adjustment (one evaluation on the all-zero row per proof)
+struct HostProg {  // host copy for host_eval_constraints (the prover's all-zero row, the verifier's opened values)
     std::vector<DagInstr> instrs; std::vector<LeafRef> leaves; std::vector<uint32_t> consts, publics, assert_regs, assert_alphas;
     // the same row polynomial as a sum of self-contained pieces (zc_lower.hpp): {offset into the chip's stream arena, length}
     std::vector<std::pair<uint32_t, uint32_t>> zc_pieces;
 };
+
+// The host interpreter of a chip's bytecode at one row: Σ powers[assert_alphas[i]] · regs[assert_regs[i]].  R is the register type:
+// the base field's Montgomery word (the prover's all-zero row) or hf::E4 (the verifier's opened values).  leaf(l) is the row's value
+// of leaf l; pv the public values.
+template <class R, class Leaf>
+hf::E4 host_eval_constraints(const HostProg& p, uint32_t n_regs, const uint32_t* pv, const std::vector<hf::E4>& powers, Leaf leaf) {
+    const auto base = [](uint32_t x) { if constexpr (std::is_same<R, hf::E4>::value) return hf::E4::from_base(x); else return x; };
+    std::vector<R> regs(std::max<uint32_t>(n_regs, 1));
+    for (const DagInstr& in : p.instrs) {
+        switch (in.opcode) {
+            case BC_LOAD_LEAF: regs[in.out] = leaf(p.leaves[in.a]); break;
+            case BC_LOAD_CONST: regs[in.out] = base(p.consts[in.a]); break;
+            case BC_LOAD_PUBLIC: regs[in.out] = base(pv[p.publics[in.a]]); break;
+            case BC_ADD_F: regs[in.out] = hf::add(regs[in.a], regs[in.b]); break;
+            case BC_SUB_F: regs[in.out] = hf::sub(regs[in.a], regs[in.b]); break;
+            case BC_MUL_F: regs[in.out] = hf::mul(regs[in.a], regs[in.b]); break;
+            case BC_NEG_F: regs[in.out] = hf::neg(regs[in.a]); break;
+        }
+    }
+    hf::E4 acc;
+    for (size_t i = 0; i < p.assert_regs.size(); i++) acc = acc + powers[p.assert_alphas[i]] * regs[p.assert_regs[i]];
+    return acc;
+}
 
 // LogUp interactions (crates/hypercube/src/lookup/interaction.rs:11-22), parsed from the machine blob's interaction section (gkr.cu).
 // A virtual column is constant + sum weight * column; an interaction's multiplicity is vcols[vcol_start], its values follow.

@@ -1,5 +1,7 @@
 // The flat proof words of sp1b200_prove_shard, read in one place: the wire format (wire.cu) and the shard verifier (verify.cu) both
-// walk a proof through parse_shard_proof, so the two cannot disagree about the layout.  Host code only.
+// walk a proof through parse_shard_proof, and the shard prover (shard.cu) reads the LogUp-GKR and zerocheck outputs it chains with
+// the same section readers, so none of them can disagree about the layout.  Also the jagged round's shape rules the prover and the
+// verifier share.  Host code only.
 //
 // Words: [5][len_0..len_4] then the sections
 //   0 main commitment (8)
@@ -60,17 +62,40 @@ struct Shape {
     std::vector<size_t> ncols;            // per commitment round: {preprocessed,} main
 };
 
-// ncols of a shard: ceil(area / 2^log_stacking_height), at least 1, per round (a preprocessed round only if a chip has such columns)
+// A jagged round's tables as (rows, cols) runs: its chip tables, then its two padding tables.
+using Tables = std::vector<std::pair<uint64_t, uint64_t>>;
+
+// the stacked columns of 2^log_stack cells that hold a round of `area` cells: ceil(area / 2^log_stack), at least 1
+inline uint64_t stacked_columns(uint64_t area, uint32_t log_stack) {
+    const uint64_t S = (uint64_t)1 << log_stack;
+    return std::max<uint64_t>((area + S - 1) / S, 1);
+}
+
+// The two padding tables that fill a round of `area` cells up to its stacked columns: (2^max_log_row_count rows, n - 1 columns)
+// and (the rest, 1 column), n being the fewest columns of 2^max_log_row_count rows that hold the padding (at least 1).
+inline Tables padding_tables(uint64_t area, uint32_t log_stack, uint32_t max_log_row_count) {
+    const uint64_t R = (uint64_t)1 << max_log_row_count, added = (stacked_columns(area, log_stack) << log_stack) - area;
+    const uint64_t n = std::max<uint64_t>((added + R - 1) / R, 1);
+    return {{R, n - 1}, {added - (n - 1) * R, 1}};
+}
+
+// Appends the tables' columns to the column prefix sums: prefix[c] = the rows of every column before column c, and the last entry
+// is the running total (start from {0}).
+inline void append_column_prefix(std::vector<uint64_t>& prefix, const Tables& tables) {
+    for (auto& t : tables)
+        for (uint64_t c = 0; c < t.second; c++) prefix.push_back(prefix.back() + t.first);
+}
+
+// ncols of a shard: stacked_columns per round (a preprocessed round only if a chip has such columns)
 inline std::vector<size_t> round_columns(size_t n_chips, const uint64_t* heights, const uint32_t* main_w, const uint32_t* prep_w, uint32_t log_stack) {
     uint64_t prep_area = 0, main_area = 0; bool has_prep = false;
     for (size_t k = 0; k < n_chips; k++) {
         main_area += heights[k] * main_w[k];
         if (prep_w[k]) { has_prep = true; prep_area += heights[k] * prep_w[k]; }
     }
-    const uint64_t S = (uint64_t)1 << log_stack;
     std::vector<size_t> n;
-    if (has_prep) n.push_back((size_t)std::max<uint64_t>((prep_area + S - 1) / S, 1));
-    n.push_back((size_t)std::max<uint64_t>((main_area + S - 1) / S, 1));
+    if (has_prep) n.push_back((size_t)stacked_columns(prep_area, log_stack));
+    n.push_back((size_t)stacked_columns(main_area, log_stack));
     return n;
 }
 
@@ -94,7 +119,7 @@ struct ShardProof {
     const uint32_t* pow_witness = nullptr; const uint32_t* batch_witness = nullptr;
     std::vector<const uint32_t*> batch_evals;
     Sumcheck jagged_sc, jagged_eval;
-    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> rc_cc;
+    std::vector<Tables> rc_cc;
     const uint32_t* merkle_commits = nullptr;
     const uint32_t* expected_eval = nullptr;
     uint32_t max_log_rows = 0, log_m = 0;
@@ -126,6 +151,39 @@ inline const char* read_opening(FlatReader& r, Opening& o, size_t nq, size_t wid
     return r.ok ? nullptr : "evaluation proof section: section is shorter than its layout";
 }
 
+// The LogUp-GKR section (all of r's words) into v's LogUp-GKR fields.  Returns nullptr on success, else what is wrong.
+inline const char* read_gkr(FlatReader& r, const Shape& s, ShardProof& v) {
+    const size_t nch = s.n_chips;
+    v.n_out = r.u();
+    if (!r.ok || v.n_out > MAX_GKR_OUTPUTS) return "LogUp-GKR section: output count out of range";
+    v.out_num = r.take(4 * (size_t)v.n_out); v.out_den = r.take(4 * (size_t)v.n_out);
+    const uint32_t nr = r.u();
+    if (!r.ok || nr > MAX_ROUNDS) return "LogUp-GKR section: round count out of range";
+    v.rounds.resize(nr);
+    for (auto& q : v.rounds) {
+        q.nd = r.take(16);
+        if (!read_sumcheck(r, q.sc)) return "LogUp-GKR section: malformed round sumcheck";
+    }
+    v.gkr_point = r.take(4 * (size_t)s.max_log_row_count);
+    v.gkr_main.resize(nch); v.gkr_prep.resize(nch);
+    for (size_t k = 0; k < nch; k++) { v.gkr_main[k] = r.take(4 * (size_t)s.main_w[k]); v.gkr_prep[k] = r.take(4 * (size_t)s.prep_w[k]); }
+    v.gkr_witness = r.take(1);
+    if (!r.ok) return "LogUp-GKR section: section is shorter than its layout";
+    if (r.p != r.end) return "LogUp-GKR section: trailing words";
+    return nullptr;
+}
+
+// The zerocheck section (all of r's words) into v's zerocheck fields and opened values.  Returns nullptr on success, else what is wrong.
+inline const char* read_zerocheck(FlatReader& r, const Shape& s, ShardProof& v) {
+    const size_t nch = s.n_chips;
+    if (!read_sumcheck(r, v.zc)) return "zerocheck section: malformed sumcheck";
+    v.zc_prep.resize(nch); v.zc_main.resize(nch);
+    for (size_t k = 0; k < nch; k++) { v.zc_prep[k] = r.take(4 * (size_t)s.prep_w[k]); v.zc_main[k] = r.take(4 * (size_t)s.main_w[k]); }
+    if (!r.ok) return "zerocheck section: section is shorter than its layout";
+    if (r.p != r.end) return "zerocheck section: trailing words";
+    return nullptr;
+}
+
 // Splits and walks the words.  Returns nullptr on success, else what is wrong (prefixed by the section).
 inline const char* parse_shard_proof(const uint32_t* w, uint64_t n_words, const Shape& s, ShardProof& v) {
     if (!w || n_words < 6 || w[0] != 5) return "not a shard proof (header)";
@@ -133,35 +191,11 @@ inline const char* parse_shard_proof(const uint32_t* w, uint64_t n_words, const 
     if (6 + l0 + l1 + l2 + l3 + l4 != n_words || l0 != 8) return "section lengths do not add up";
     const uint32_t* s0 = w + 6; const uint32_t* s1 = s0 + l0; const uint32_t* s2 = s1 + l1; const uint32_t* s3 = s2 + l2; const uint32_t* s4 = s3 + l3;
     v.commit = s0; v.pv = s4; v.n_pv = (uint32_t)l4;
-    const size_t nch = s.n_chips, nq = s.num_queries;
-    const uint32_t mlr = s.max_log_row_count, ls = s.log_stacking_height;
-    {   // LogUp-GKR
-        FlatReader r{s1, s2};
-        v.n_out = r.u();
-        if (!r.ok || v.n_out > MAX_GKR_OUTPUTS) return "LogUp-GKR section: output count out of range";
-        v.out_num = r.take(4 * (size_t)v.n_out); v.out_den = r.take(4 * (size_t)v.n_out);
-        const uint32_t nr = r.u();
-        if (!r.ok || nr > MAX_ROUNDS) return "LogUp-GKR section: round count out of range";
-        v.rounds.resize(nr);
-        for (auto& q : v.rounds) {
-            q.nd = r.take(16);
-            if (!read_sumcheck(r, q.sc)) return "LogUp-GKR section: malformed round sumcheck";
-        }
-        v.gkr_point = r.take(4 * (size_t)mlr);
-        v.gkr_main.resize(nch); v.gkr_prep.resize(nch);
-        for (size_t k = 0; k < nch; k++) { v.gkr_main[k] = r.take(4 * (size_t)s.main_w[k]); v.gkr_prep[k] = r.take(4 * (size_t)s.prep_w[k]); }
-        v.gkr_witness = r.take(1);
-        if (!r.ok) return "LogUp-GKR section: section is shorter than its layout";
-        if (r.p != s2) return "LogUp-GKR section: trailing words";
-    }
-    {   // zerocheck and opened values
-        FlatReader r{s2, s3};
-        if (!read_sumcheck(r, v.zc)) return "zerocheck section: malformed sumcheck";
-        v.zc_prep.resize(nch); v.zc_main.resize(nch);
-        for (size_t k = 0; k < nch; k++) { v.zc_prep[k] = r.take(4 * (size_t)s.prep_w[k]); v.zc_main[k] = r.take(4 * (size_t)s.main_w[k]); }
-        if (!r.ok) return "zerocheck section: section is shorter than its layout";
-        if (r.p != s3) return "zerocheck section: trailing words";
-    }
+    const size_t nq = s.num_queries;
+    const uint32_t ls = s.log_stacking_height;
+    FlatReader gkr{s1, s2}, zc{s2, s3};
+    if (const char* e = read_gkr(gkr, s, v)) return e;
+    if (const char* e = read_zerocheck(zc, s, v)) return e;
     {   // evaluation proof
         FlatReader r{s3, s4};
         const size_t n_rounds = s.ncols.size();

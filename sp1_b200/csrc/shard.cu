@@ -7,6 +7,7 @@
 #include "hostfield.hpp"
 #include "machine.cuh"
 #include "pcs.cuh"
+#include "proof_layout.hpp"
 #include <cstring>
 #include <memory>
 #include <string>
@@ -19,17 +20,20 @@ static sp1b200_err chip_pointers(const char* who, const sp1b200_machine* m, cons
     const size_t nch = m->chips.size();
     d_main.assign(nch, nullptr); d_prep.assign(nch, nullptr);
     uint64_t off = 0, poff = 0; size_t pt = 0;
+    // the preprocessed round's chip tables: all of its tables but the two padding tables
+    const size_t n_prep_tables = prep_round ? prep_round->tables.size() - 2 : 0;
     for (size_t k = 0; k < nch; k++) {
         d_main[k] = d_main_dense + off;
         off += h_heights[k] * m->chips[k].main_w;
         if (m->chips[k].prep_w) {
-            if (!prep_round || pt + 2 >= prep_round->row_counts.size() + 0 || prep_round->col_counts[pt] != m->chips[k].prep_w)
+            if (pt >= n_prep_tables || prep_round->tables[pt].second != m->chips[k].prep_w)
                 return sp1b200_set_error("%s: preprocessed round does not match the machine at chip %zu", who, k);
-            if (prep_round->row_counts[pt] != h_heights[k])
-                return sp1b200_set_error("%s: chip %zu: preprocessed height %llu != main height %llu", who, k,
-                                         (unsigned long long)prep_round->row_counts[pt], (unsigned long long)h_heights[k]);
+            const uint64_t rows = prep_round->tables[pt].first;
+            if (rows != h_heights[k])
+                return sp1b200_set_error("%s: chip %zu: preprocessed height %llu != main height %llu", who, k, (unsigned long long)rows,
+                                         (unsigned long long)h_heights[k]);
             d_prep[k] = prep_round->d_dense + poff;
-            poff += prep_round->row_counts[pt] * prep_round->col_counts[pt];
+            poff += rows * m->chips[k].prep_w;
             pt++;
         }
     }
@@ -121,13 +125,7 @@ sp1b200_err sp1b200_prove_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b
     }
     struct Guard { sp1b200_ctx* c; sp1b200_jagged_round* r; ~Guard() { sp1b200_jagged_round_free(c, r); } } guard{ctx, main_round};
     ch.observe_n(commit, 8);
-    ch.observe(hf::to_monty(nch));
-    for (size_t k = 0; k < nch; k++) {
-        ch.observe(hf::to_monty(h_heights[k]));
-        const size_t len = strlen(chip_names[k]);
-        ch.observe(hf::to_monty(len));
-        for (size_t i = 0; i < len; i++) ch.observe(hf::to_monty((uint8_t)chip_names[k][i]));
-    }
+    observe_chip_shapes(ch, nch, h_heights, chip_names);
     // chip column pointers inside the dense buffers
     std::vector<const uint32_t*> d_main, d_prep;
     SP1_TRY(chip_pointers("prove_shard", m, prep_round, main_round->d_dense, h_heights, d_main, d_prep));
@@ -140,55 +138,41 @@ sp1b200_err sp1b200_prove_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b
     uint32_t* gkr = ctx->shard_scratch.get();
     uint64_t n_gkr = 0;
     SP1_TRY(sp1b200_logup_gkr(ctx, m, h_heights, d_main.data(), d_prep.data(), h_replay_witnesses, st, gkr, scratch_cap, &n_gkr));
-    // tail of the gkr words: point (mlr ext) | per chip {main, prep openings} | witness
-    size_t total_w = 0;
-    for (auto& c : m->chips) total_w += c.main_w + c.prep_w;
-    if (n_gkr < 1 + 4 * total_w + 4 * (uint64_t)mlr)
-        return sp1b200_set_error("prove_shard: LogUp-GKR section has %llu words, fewer than its point + openings + witness tail", (unsigned long long)n_gkr);
-    const uint32_t* tail = gkr + n_gkr - 1 - 4 * total_w - 4 * mlr;
-    const uint32_t* gkr_point = tail;
-    const uint32_t* openings = tail + 4 * mlr;
+    // the phase outputs are read with the proof layout's section readers
+    std::vector<uint32_t> main_w(nch), prep_w(nch);
+    for (size_t k = 0; k < nch; k++) { main_w[k] = m->chips[k].main_w; prep_w[k] = m->chips[k].prep_w; }
+    layout::Shape shape;
+    shape.n_chips = nch; shape.main_w = main_w.data(); shape.prep_w = prep_w.data(); shape.max_log_row_count = mlr;
+    layout::ShardProof phases;   // its LogUp-GKR and zerocheck fields
+    layout::FlatReader gkr_words{gkr, gkr + n_gkr};
+    if (const char* why = layout::read_gkr(gkr_words, shape, phases)) return sp1b200_set_error("prove_shard: %s", why);
     ch.load(st);
     E4 alpha, gamma;
     ch.sample_ext(alpha.c); ch.sample_ext(gamma.c);
     std::vector<uint32_t> claims(nch * 4);
-    {
-        const uint32_t* o = openings;
-        for (size_t k = 0; k < nch; k++) {
-            E4 acc, g = gamma;
-            for (uint32_t j = 0; j < m->chips[k].main_w + m->chips[k].prep_w; j++, o += 4) { acc = acc + E4::load(o) * g; g = g * gamma; }
-            acc.store(&claims[4 * k]);
-        }
-    }
+    for (size_t k = 0; k < nch; k++)
+        batched_opening_claim(phases.gkr_main[k], main_w[k], phases.gkr_prep[k], prep_w[k], gamma).store(&claims[4 * k]);
     ch.store(st);
     uint32_t* zc = gkr + scratch_cap;
     uint64_t n_zc = 0;
-    SP1_TRY(sp1b200_zerocheck(ctx, m, h_heights, d_main.data(), d_prep.data(), h_pv, n_pv, gkr_point, alpha.c, gamma.c, claims.data(), st, zc,
-                              scratch_cap, &n_zc));
-    // zerocheck words: [mlr] { [5] coeffs(20) } x mlr | claimed_sum 4 | point 4 mlr | eval 4 | per chip {prep evals, main evals}
-    if (n_zc != 1 + (uint64_t)mlr * 21 + 4 + 4 * (uint64_t)mlr + 4 + 4 * total_w || zc[0] != mlr)
-        return sp1b200_set_error("prove_shard: zerocheck section has %llu words, layout expects %llu", (unsigned long long)n_zc,
-                                 (unsigned long long)(1 + (uint64_t)mlr * 21 + 4 + 4 * (uint64_t)mlr + 4 + 4 * total_w));
-    const uint32_t* zpoint = zc + 1 + (size_t)mlr * 21 + 4;
-    const uint32_t* zopen = zpoint + 4 * mlr + 4;
+    SP1_TRY(sp1b200_zerocheck(ctx, m, h_heights, d_main.data(), d_prep.data(), h_pv, n_pv, phases.gkr_point, alpha.c, gamma.c, claims.data(), st,
+                              zc, scratch_cap, &n_zc));
+    layout::FlatReader zc_words{zc, zc + n_zc};
+    if (const char* why = layout::read_zerocheck(zc_words, shape, phases)) return sp1b200_set_error("prove_shard: %s", why);
+    if (phases.zc.polys.size() != mlr)
+        return sp1b200_set_error("prove_shard: zerocheck section: %zu rounds, the point needs %u", phases.zc.polys.size(), mlr);
+    // the jagged claims: the opened values of the preprocessed round's columns, then the main round's, in chip order
     std::vector<uint32_t> jclaims;
-    {
-        std::vector<uint32_t> pc, mc;
-        const uint32_t* o = zopen;
-        for (size_t k = 0; k < nch; k++) {
-            pc.insert(pc.end(), o, o + 4 * m->chips[k].prep_w); o += 4 * m->chips[k].prep_w;
-            mc.insert(mc.end(), o, o + 4 * m->chips[k].main_w); o += 4 * m->chips[k].main_w;
-        }
-        if (prep_round) jclaims.insert(jclaims.end(), pc.begin(), pc.end());
-        jclaims.insert(jclaims.end(), mc.begin(), mc.end());
-    }
+    if (prep_round)
+        for (size_t k = 0; k < nch; k++) jclaims.insert(jclaims.end(), phases.zc_prep[k], phases.zc_prep[k] + 4 * prep_w[k]);
+    for (size_t k = 0; k < nch; k++) jclaims.insert(jclaims.end(), phases.zc_main[k], phases.zc_main[k] + 4 * main_w[k]);
     std::vector<sp1b200_jagged_round*> rounds;
     if (prep_round) rounds.push_back(prep_round);
     rounds.push_back(main_round);
     uint32_t* ev = gkr + 2 * scratch_cap;
     uint64_t n_ev = 0;
-    SP1_TRY(sp1b200_jagged_prove(ctx, rounds.data(), (uint32_t)rounds.size(), zpoint, jclaims.data(), h_replay_witnesses ? h_replay_witnesses + 1 : nullptr,
-                                 st, ev, scratch_cap, &n_ev));
+    SP1_TRY(sp1b200_jagged_prove(ctx, rounds.data(), (uint32_t)rounds.size(), phases.zc.point, jclaims.data(),
+                                 h_replay_witnesses ? h_replay_witnesses + 1 : nullptr, st, ev, scratch_cap, &n_ev));
     const uint64_t total = 6 + 8 + n_gkr + n_zc + n_ev + n_pv;
     t_all.stop();
     if (h_words) *h_words = total;

@@ -31,6 +31,16 @@ __device__ __forceinline__ uint32_t root_pow(const uint32_t* __restrict__ TH, co
     return lo ? kb::mul(hi, __ldg(TL + lo)) : hi;
 }
 
+// One layer of the jagged branching program (slop/crates/jagged/src/poly.rs:136-175, 384-470), for the prover's kernels
+// (jagged.cu) and the verifier's host evaluation (verify.cu).  state = carry + 2 * comparison_so_far; returns -1 on failure.
+__host__ __device__ __forceinline__ int bp_transition(int row_bit, int index_bit, int cur_bit, int next_bit, int state) {
+    int carry = state & 1, cmp = state >> 1;
+    int new_cmp = (index_bit == next_bit) ? cmp : next_bit;
+    int s = row_bit + carry + cur_bit;
+    if (index_bit != (s & 1)) return -1;
+    return (s >> 1) + 2 * new_cmp;
+}
+
 // E[j] = prod_t (bit (k-1-t) of j ? x_t : 1 - x_t) for j < 2^k, point[0] <-> most significant bit of j (sumcheck.cu)
 sp1b200_err launch_eq_table(sp1b200_ctx* ctx, const uint32_t* d_point, int k, uint32_t* d_out);
 // E'[j] = E[2j] + E[2j+1], j < n_out: drops the last coordinate of the eq point (sumcheck.cu)

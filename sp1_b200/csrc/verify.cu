@@ -23,24 +23,10 @@
 #include <atomic>
 #include <chrono>
 #include <cstring>
+#include <iterator>
 #include <memory>
 #include <thread>
 #include <vector>
-
-// Poseidon2 sponge / 2-to-1 compression on the host (the transcript's permutation), for the verifier's few table-size hashes
-static void host_hash(const uint32_t* in, size_t n, uint32_t* out8) {
-    uint32_t s[16] = {0};
-    size_t fill = 0;
-    for (size_t i = 0; i < n; i++) { s[fill++] = in[i]; if (fill == 8) { host_poseidon2_permute(s); fill = 0; } }
-    if (fill) host_poseidon2_permute(s);
-    memcpy(out8, s, 32);
-}
-static void host_compress(const uint32_t* l8, const uint32_t* r8, uint32_t* out8) {
-    uint32_t s[16];
-    memcpy(s, l8, 32); memcpy(s + 8, r8, 32);
-    host_poseidon2_permute(s);
-    memcpy(out8, s, 32);
-}
 
 namespace {
 
@@ -189,61 +175,7 @@ __global__ void __launch_bounds__(256) verify_jagged_kernel(const JagArgs* __res
 
 // ---- host part ------------------------------------------------------------------------------------------------------------------
 
-enum : uint32_t {
-    V_ACCEPT = 0, V_POW, V_INVALID_SHAPE, V_ZERO_DENOMINATOR, V_CUMULATIVE_SUM, V_INVALID_SHAPE_ROUNDS, V_INCONSISTENT_SUMCHECK_CLAIM,
-    V_SC_PROOF_SHAPE, V_SC_CLAIMED_SUM, V_SC_ROUND, V_SC_POINT, V_SC_EVAL, V_INCONSISTENT_EVALUATION, V_LAST_LAYER_DIMENSION,
-    V_TRACE_POINT, V_INVALID_SHAPE_OPENINGS, V_NUMERATOR_EVAL, V_DENOMINATOR_EVAL, V_OPENING_SHAPE, V_HEIGHT_BITS, V_HEIGHT_TOO_LARGE,
-    V_CONSTRAINTS_EVAL, V_CONSTRAINTS_CLAIMED_SUM, V_INCORRECT_SHAPE, V_INCORRECT_TABLE_SIZES, V_AREA_OUT_OF_BOUNDS, V_DUMMY_TABLES,
-    V_SUMCHECK_CLAIM_MISMATCH, V_MONOTONICITY, V_JAGGED_EVALUATION, V_JAGGED_EVAL_PROOF, V_STACKING, V_BATCH_POW, V_FRI_LENGTH,
-    V_BASEFOLD_SUMCHECK, V_TWO_ADICITY, V_TCS_COMPONENT, V_QUERY_VALUE, V_TCS_QUERY, V_QUERY_FINAL_POLY, V_SUMCHECK_FINAL_POLY,
-    V_PREP_WIDTHS, V_CHIP_TABLES, V_COUNT
-};
-// every code is the one include/sp1b200.h documents
-static_assert(V_ACCEPT == SP1B200_VERDICT_ACCEPT, "verdict code differs from include/sp1b200.h");
-static_assert(V_POW == SP1B200_VERDICT_POW, "verdict code differs from include/sp1b200.h");
-static_assert(V_INVALID_SHAPE == SP1B200_VERDICT_INVALID_SHAPE, "verdict code differs from include/sp1b200.h");
-static_assert(V_ZERO_DENOMINATOR == SP1B200_VERDICT_ZERO_DENOMINATOR, "verdict code differs from include/sp1b200.h");
-static_assert(V_CUMULATIVE_SUM == SP1B200_VERDICT_CUMULATIVE_SUM_MISMATCH, "verdict code differs from include/sp1b200.h");
-static_assert(V_INVALID_SHAPE_ROUNDS == SP1B200_VERDICT_INVALID_SHAPE_ROUNDS, "verdict code differs from include/sp1b200.h");
-static_assert(V_INCONSISTENT_SUMCHECK_CLAIM == SP1B200_VERDICT_INCONSISTENT_SUMCHECK_CLAIM, "verdict code differs from include/sp1b200.h");
-static_assert(V_SC_PROOF_SHAPE == SP1B200_VERDICT_SUMCHECK_PROOF_SHAPE, "verdict code differs from include/sp1b200.h");
-static_assert(V_SC_CLAIMED_SUM == SP1B200_VERDICT_SUMCHECK_CLAIMED_SUM, "verdict code differs from include/sp1b200.h");
-static_assert(V_SC_ROUND == SP1B200_VERDICT_SUMCHECK_ROUND, "verdict code differs from include/sp1b200.h");
-static_assert(V_SC_POINT == SP1B200_VERDICT_SUMCHECK_POINT, "verdict code differs from include/sp1b200.h");
-static_assert(V_SC_EVAL == SP1B200_VERDICT_SUMCHECK_EVAL, "verdict code differs from include/sp1b200.h");
-static_assert(V_INCONSISTENT_EVALUATION == SP1B200_VERDICT_INCONSISTENT_EVALUATION, "verdict code differs from include/sp1b200.h");
-static_assert(V_LAST_LAYER_DIMENSION == SP1B200_VERDICT_LAST_LAYER_DIMENSION, "verdict code differs from include/sp1b200.h");
-static_assert(V_TRACE_POINT == SP1B200_VERDICT_TRACE_POINT_MISMATCH, "verdict code differs from include/sp1b200.h");
-static_assert(V_INVALID_SHAPE_OPENINGS == SP1B200_VERDICT_INVALID_SHAPE_OPENINGS, "verdict code differs from include/sp1b200.h");
-static_assert(V_NUMERATOR_EVAL == SP1B200_VERDICT_NUMERATOR_EVALUATION, "verdict code differs from include/sp1b200.h");
-static_assert(V_DENOMINATOR_EVAL == SP1B200_VERDICT_DENOMINATOR_EVALUATION, "verdict code differs from include/sp1b200.h");
-static_assert(V_OPENING_SHAPE == SP1B200_VERDICT_OPENING_SHAPE, "verdict code differs from include/sp1b200.h");
-static_assert(V_HEIGHT_BITS == SP1B200_VERDICT_HEIGHT_BITS, "verdict code differs from include/sp1b200.h");
-static_assert(V_HEIGHT_TOO_LARGE == SP1B200_VERDICT_HEIGHT_TOO_LARGE, "verdict code differs from include/sp1b200.h");
-static_assert(V_CONSTRAINTS_EVAL == SP1B200_VERDICT_CONSTRAINTS_EVAL, "verdict code differs from include/sp1b200.h");
-static_assert(V_CONSTRAINTS_CLAIMED_SUM == SP1B200_VERDICT_CONSTRAINTS_CLAIMED_SUM, "verdict code differs from include/sp1b200.h");
-static_assert(V_INCORRECT_SHAPE == SP1B200_VERDICT_INCORRECT_SHAPE, "verdict code differs from include/sp1b200.h");
-static_assert(V_INCORRECT_TABLE_SIZES == SP1B200_VERDICT_INCORRECT_TABLE_SIZES, "verdict code differs from include/sp1b200.h");
-static_assert(V_AREA_OUT_OF_BOUNDS == SP1B200_VERDICT_AREA_OUT_OF_BOUNDS, "verdict code differs from include/sp1b200.h");
-static_assert(V_DUMMY_TABLES == SP1B200_VERDICT_DUMMY_TABLES, "verdict code differs from include/sp1b200.h");
-static_assert(V_SUMCHECK_CLAIM_MISMATCH == SP1B200_VERDICT_SUMCHECK_CLAIM_MISMATCH, "verdict code differs from include/sp1b200.h");
-static_assert(V_MONOTONICITY == SP1B200_VERDICT_MONOTONICITY, "verdict code differs from include/sp1b200.h");
-static_assert(V_JAGGED_EVALUATION == SP1B200_VERDICT_JAGGED_EVALUATION, "verdict code differs from include/sp1b200.h");
-static_assert(V_JAGGED_EVAL_PROOF == SP1B200_VERDICT_JAGGED_EVAL_PROOF, "verdict code differs from include/sp1b200.h");
-static_assert(V_STACKING == SP1B200_VERDICT_STACKING, "verdict code differs from include/sp1b200.h");
-static_assert(V_BATCH_POW == SP1B200_VERDICT_BATCH_POW, "verdict code differs from include/sp1b200.h");
-static_assert(V_FRI_LENGTH == SP1B200_VERDICT_FRI_LENGTH, "verdict code differs from include/sp1b200.h");
-static_assert(V_BASEFOLD_SUMCHECK == SP1B200_VERDICT_BASEFOLD_SUMCHECK, "verdict code differs from include/sp1b200.h");
-static_assert(V_TWO_ADICITY == SP1B200_VERDICT_TWO_ADICITY, "verdict code differs from include/sp1b200.h");
-static_assert(V_TCS_COMPONENT == SP1B200_VERDICT_TCS_COMPONENT, "verdict code differs from include/sp1b200.h");
-static_assert(V_QUERY_VALUE == SP1B200_VERDICT_QUERY_VALUE, "verdict code differs from include/sp1b200.h");
-static_assert(V_TCS_QUERY == SP1B200_VERDICT_TCS_QUERY, "verdict code differs from include/sp1b200.h");
-static_assert(V_QUERY_FINAL_POLY == SP1B200_VERDICT_QUERY_FINAL_POLY, "verdict code differs from include/sp1b200.h");
-static_assert(V_SUMCHECK_FINAL_POLY == SP1B200_VERDICT_SUMCHECK_FINAL_POLY, "verdict code differs from include/sp1b200.h");
-static_assert(V_PREP_WIDTHS == SP1B200_VERDICT_PREPROCESSED_WIDTHS, "verdict code differs from include/sp1b200.h");
-static_assert(V_CHIP_TABLES == SP1B200_VERDICT_CHIP_TABLES, "verdict code differs from include/sp1b200.h");
-static_assert(V_COUNT == SP1B200_VERDICT_EMPTY_PROOF, "the core-proof verdicts follow the shard verdicts");
-const char* const VERDICT_NAMES[V_COUNT] = {
+const char* const VERDICT_NAMES[] = {
     "Accepted", "Pow", "InvalidShape", "ZeroDenominator", "CumulativeSumMismatch", "InvalidShape(rounds)", "InconsistentSumcheckClaim",
     "InvalidProofShape", "InconsistencyWithClaimedSum", "SumcheckRoundInconsistency", "InvalidProofShape(point)", "InconsistencyWithEval",
     "InconsistentEvaluation", "InvalidLastLayerDimension", "TracePointMismatch", "InvalidShape(openings)", "NumeratorEvaluationMismatch",
@@ -253,6 +185,8 @@ const char* const VERDICT_NAMES[V_COUNT] = {
     "JaggedEvaluationFailed", "JaggedEvalProofVerificationFailed", "StackingError", "BatchPow", "SumcheckFriLengthMismatch", "Sumcheck",
     "TwoAdicityOverflow", "TcsError(component)", "QueryValueMismatch", "TcsError(query)", "QueryFinalPolyMismatch",
     "SumcheckFinalPolyMismatch", "InvalidShape(preprocessed widths)", "InvalidShape(chip tables)"};
+// indexed by the shard verdict codes of include/sp1b200.h; the core-proof verdicts follow them (verify_core.cu)
+static_assert(std::size(VERDICT_NAMES) == SP1B200_VERDICT_EMPTY_PROOF, "one name per shard verdict code of include/sp1b200.h");
 
 inline bool neq(const E4& a, const E4& b) { return !(a == b); }
 inline E4 ld(const uint32_t* p) { return E4::load(p); }
@@ -260,12 +194,6 @@ inline E4 eqf(const E4& a, const E4& b) { return a * b + (E4::one() - a) * (E4::
 inline E4 base(uint64_t canonical) { return E4::from_base(hf::to_monty(canonical)); }
 
 std::vector<E4> ext_vec(const uint32_t* p, size_t n) { std::vector<E4> v(n); for (size_t i = 0; i < n; i++) v[i] = ld(p + 4 * i); return v; }
-E4 mle_eval(const std::vector<E4>& vals, const std::vector<E4>& point) {
-    const std::vector<E4> eq = hf::partial_lagrange(point);
-    E4 acc;
-    for (size_t i = 0; i < vals.size() && i < eq.size(); i++) acc = acc + eq[i] * vals[i];
-    return acc;
-}
 std::vector<E4> point_from_usize(uint64_t x, unsigned dim) {
     std::vector<E4> p(dim);
     for (unsigned i = 0; i < dim; i++) p[i] = base((x >> (dim - 1 - i)) & 1);
@@ -284,13 +212,6 @@ E4 full_geq(const std::vector<E4>& threshold, const std::vector<E4>& point) {
 struct BranchingProgram {
     const std::vector<E4>& z_row; const std::vector<E4>& z_index; size_t num_vars;
     static E4 lsb(const std::vector<E4>& p, size_t i) { return p.size() <= i ? E4() : p[p.size() - 1 - i]; }
-    static int transition(int row_bit, int index_bit, int cur_bit, int next_bit, int state) {   // state = carry + 2 * comparison
-        const int carry = state & 1, cmp = state >> 1;
-        const int new_cmp = index_bit == next_bit ? cmp : next_bit;
-        const int s = row_bit + carry + cur_bit;
-        if (index_bit != (s & 1)) return -1;
-        return (s >> 1) + 2 * new_cmp;
-    }
     E4 eval(const std::vector<E4>& prefix, const std::vector<E4>& next) const {
         E4 res[4]; res[2] = E4::one();
         for (size_t layer = num_vars + 1; layer-- > 0;) {
@@ -299,7 +220,7 @@ struct BranchingProgram {
             for (int st = 0; st < 4; st++) {
                 E4 acc[4];
                 for (int i = 0; i < 16; i++) {
-                    const int o = transition((i >> 3) & 1, (i >> 2) & 1, (i >> 1) & 1, i & 1, st);
+                    const int o = bp_transition((i >> 3) & 1, (i >> 2) & 1, (i >> 1) & 1, i & 1, st);
                     if (o >= 0) acc[o] = acc[o] + eq[i];
                 }
                 for (int k = 0; k < 4; k++) nres[st] = nres[st] + acc[k] * res[k];
@@ -331,7 +252,7 @@ struct Verifier {
 
     // outcome of the host phase: `verdict` is a failure found before any device check; otherwise the deferred checks, then host_fail,
     // then tail_fail (the chip-table check) decide
-    uint32_t verdict = V_ACCEPT, host_fail = V_ACCEPT, tail_fail = V_ACCEPT;
+    uint32_t verdict = SP1B200_VERDICT_ACCEPT, host_fail = SP1B200_VERDICT_ACCEPT, tail_fail = SP1B200_VERDICT_ACCEPT;
     std::vector<Deferred> deferred;
     // recorded device work.  Jagged column sum: the column prefix sums, eq(z_col, c) and the jagged-eval point; acc * jag_bp ==
     // jag_expect is checked after the copy
@@ -363,25 +284,25 @@ struct Verifier {
     // partially_verify_sumcheck_proof (slop/crates/sumcheck/src/verifier.rs:21-107)
     uint32_t sumcheck(const layout::Sumcheck& s, size_t nvars, size_t degree) {
         const size_t n = s.polys.size();
-        if (n != nvars || nvars == 0) return V_SC_PROOF_SHAPE;
+        if (n != nvars || nvars == 0) return SP1B200_VERDICT_SUMCHECK_PROOF_SHAPE;
         auto eval = [&](size_t i, const E4& x) { E4 r; for (size_t k = s.n_coeffs[i]; k-- > 0;) r = r * x + ld(s.polys[i] + 4 * k); return r; };
         auto sum01 = [&](size_t i) { E4 r = s.n_coeffs[i] ? ld(s.polys[i]) : E4(); for (size_t k = 0; k < s.n_coeffs[i]; k++) r = r + ld(s.polys[i] + 4 * k); return r; };
-        if (neq(sum01(0), ld(s.claimed_sum))) return V_SC_CLAIMED_SUM;
-        if (s.n_coeffs[0] != degree + 1) return V_SC_PROOF_SHAPE;
+        if (neq(sum01(0), ld(s.claimed_sum))) return SP1B200_VERDICT_SUMCHECK_CLAIMED_SUM;
+        if (s.n_coeffs[0] != degree + 1) return SP1B200_VERDICT_SUMCHECK_PROOF_SHAPE;
         ch.observe_n(s.polys[0], 4 * (size_t)s.n_coeffs[0]);
         std::vector<E4> alphas;   // most recent first
         for (size_t i = 1; i < n; i++) {
-            if (s.n_coeffs[i] != degree + 1) return V_SC_PROOF_SHAPE;
+            if (s.n_coeffs[i] != degree + 1) return SP1B200_VERDICT_SUMCHECK_PROOF_SHAPE;
             const E4 a = sample_ext();
             alphas.insert(alphas.begin(), a);
-            if (neq(eval(i - 1, a), sum01(i))) return V_SC_ROUND;
+            if (neq(eval(i - 1, a), sum01(i))) return SP1B200_VERDICT_SUMCHECK_ROUND;
             ch.observe_n(s.polys[i], 4 * (size_t)s.n_coeffs[i]);
         }
         const E4 a = sample_ext();
         alphas.insert(alphas.begin(), a);
-        for (size_t i = 0; i < n; i++) if (neq(alphas[i], ld(s.point + 4 * i))) return V_SC_POINT;
-        if (neq(eval(n - 1, a), ld(s.eval))) return V_SC_EVAL;
-        return V_ACCEPT;
+        for (size_t i = 0; i < n; i++) if (neq(alphas[i], ld(s.point + 4 * i))) return SP1B200_VERDICT_SUMCHECK_POINT;
+        if (neq(eval(n - 1, a), ld(s.eval))) return SP1B200_VERDICT_SUMCHECK_EVAL;
+        return SP1B200_VERDICT_ACCEPT;
     }
 
     E4 vcol(const VColDev& v, const E4* prep, const E4* main) const {
@@ -400,31 +321,31 @@ struct Verifier {
         size_t arity = 1, ni = 0;
         for (auto& c : H.per_chip) { ni += c.size(); for (auto& in : c) arity = std::max<size_t>(arity, in.n_values + 1); }
         const unsigned bdim = hf::log2_ceil(arity);
-        if (!ch.check_witness(prm.gkr_pow_bits, p.gkr_witness[0])) return V_POW;
+        if (!ch.check_witness(prm.gkr_pow_bits, p.gkr_witness[0])) return SP1B200_VERDICT_POW;
         const E4 alpha = sample_ext();
         const std::vector<E4> beta_seed = sample_point(bdim);
         (void)sample_ext();
         const unsigned v = hf::log2_ceil(ni);
         const size_t expected = (size_t)1 << (v + 1);
-        if (p.n_out != expected) return V_INVALID_SHAPE;
+        if (p.n_out != expected) return SP1B200_VERDICT_INVALID_SHAPE;
         observe_var_ext(p.out_num, p.n_out);
         observe_var_ext(p.out_den, p.n_out);
         const std::vector<E4> num = ext_vec(p.out_num, expected), den = ext_vec(p.out_den, expected);
         E4 cum;
-        for (size_t i = 0; i < expected; i++) { if (den[i].is_zero()) return V_ZERO_DENOMINATOR; cum = cum + num[i] * hf::inv(den[i]); }
-        if (!cum.is_zero()) return V_CUMULATIVE_SUM;
+        for (size_t i = 0; i < expected; i++) { if (den[i].is_zero()) return SP1B200_VERDICT_ZERO_DENOMINATOR; cum = cum + num[i] * hf::inv(den[i]); }
+        if (!cum.is_zero()) return SP1B200_VERDICT_CUMULATIVE_SUM_MISMATCH;
         std::vector<E4> point = sample_point(v + 1);
-        E4 num_eval = mle_eval(num, point), den_eval = mle_eval(den, point);
-        if (p.rounds.size() + 1 != mlr) return V_INVALID_SHAPE_ROUNDS;
+        E4 num_eval = hf::mle_eval(num, point), den_eval = hf::mle_eval(den, point);
+        if (p.rounds.size() + 1 != mlr) return SP1B200_VERDICT_INVALID_SHAPE_ROUNDS;
         for (size_t i = 0; i < p.rounds.size(); i++) {
             const layout::GkrRound& r = p.rounds[i];
             const E4 lambda = sample_ext();
-            if (neq(ld(r.sc.claimed_sum), num_eval * lambda + den_eval)) return V_INCONSISTENT_SUMCHECK_CLAIM;
+            if (neq(ld(r.sc.claimed_sum), num_eval * lambda + den_eval)) return SP1B200_VERDICT_INCONSISTENT_SUMCHECK_CLAIM;
             if (uint32_t e = sumcheck(r.sc, i + v + 1, 3)) return e;
             const E4 n0 = ld(r.nd), n1 = ld(r.nd + 4), d0 = ld(r.nd + 8), d1 = ld(r.nd + 12);
             E4 eqv = E4::one();
             for (size_t k = 0; k < point.size(); k++) eqv = eqv * eqf(ld(r.sc.point + 4 * k), point[k]);
-            if (neq(ld(r.sc.eval), eqv * ((n0 * d1 + n1 * d0) * lambda + d0 * d1))) return V_INCONSISTENT_EVALUATION;
+            if (neq(ld(r.sc.eval), eqv * ((n0 * d1 + n1 * d0) * lambda + d0 * d1))) return SP1B200_VERDICT_INCONSISTENT_EVALUATION;
             ch.observe_n(r.nd, 16);
             point = ext_vec(r.sc.point, r.sc.polys.size());
             const E4 lc = sample_ext();
@@ -433,8 +354,8 @@ struct Verifier {
             den_eval = d0 + (d1 - d0) * lc;
         }
         const std::vector<E4> ipt(point.begin(), point.begin() + v), tpt(point.begin() + v, point.end());
-        if (tpt.size() != mlr) return V_LAST_LAYER_DIMENSION;
-        for (uint32_t k = 0; k < mlr; k++) if (neq(tpt[k], ld(p.gkr_point + 4 * k))) return V_TRACE_POINT;
+        if (tpt.size() != mlr) return SP1B200_VERDICT_LAST_LAYER_DIMENSION;
+        for (uint32_t k = 0; k < mlr; k++) if (neq(tpt[k], ld(p.gkr_point + 4 * k))) return SP1B200_VERDICT_TRACE_POINT_MISMATCH;
         const std::vector<E4> betas = hf::partial_lagrange(beta_seed);
         std::vector<E4> pe{E4()};
         pe.insert(pe.end(), tpt.begin(), tpt.end());
@@ -461,36 +382,23 @@ struct Verifier {
             }
         }
         nv.resize((size_t)1 << v, E4()); dv.resize((size_t)1 << v, E4::one());
-        if (neq(num_eval, mle_eval(nv, ipt))) return V_NUMERATOR_EVAL;
-        if (neq(den_eval, mle_eval(dv, ipt))) return V_DENOMINATOR_EVAL;
-        return V_ACCEPT;
+        if (neq(num_eval, hf::mle_eval(nv, ipt))) return SP1B200_VERDICT_NUMERATOR_EVALUATION;
+        if (neq(den_eval, hf::mle_eval(dv, ipt))) return SP1B200_VERDICT_DENOMINATOR_EVALUATION;
+        return SP1B200_VERDICT_ACCEPT;
     }
 
-    // the chip's constraints folded with the reversed α powers (the verifier folder's Horner order) at one row of extension values
+    // the chip's constraints folded with the reversed α powers (the verifier folder's Horner order) at one row of extension values;
+    // null columns: the all-zero row
     E4 eval_air(size_t k, const E4* prep, const E4* main, const std::vector<E4>& powers) const {
-        const HostProg& hp = m->host[k];
-        std::vector<E4> regs(std::max<uint32_t>(m->chips[k].n_regs, 1));
-        for (const DagInstr& in : hp.instrs) {
-            switch (in.opcode) {
-                case BC_LOAD_LEAF: { const LeafRef& l = hp.leaves[in.a]; regs[in.out] = main ? (l.source == LEAF_MAIN ? main : prep)[l.col] : E4(); break; }
-                case BC_LOAD_CONST: regs[in.out] = E4::from_base(hp.consts[in.a]); break;
-                case BC_LOAD_PUBLIC: regs[in.out] = E4::from_base(p.pv[hp.publics[in.a]]); break;
-                case BC_ADD_F: regs[in.out] = regs[in.a] + regs[in.b]; break;
-                case BC_SUB_F: regs[in.out] = regs[in.a] - regs[in.b]; break;
-                case BC_MUL_F: regs[in.out] = regs[in.a] * regs[in.b]; break;
-                case BC_NEG_F: regs[in.out] = E4() - regs[in.a]; break;
-            }
-        }
-        E4 acc;
-        for (size_t i = 0; i < hp.assert_regs.size(); i++) acc = acc + powers[hp.assert_alphas[i]] * regs[hp.assert_regs[i]];
-        return acc;
+        return host_eval_constraints<E4>(m->host[k], m->chips[k].n_regs, p.pv, powers,
+                                         [&](const LeafRef& l) { return main ? (l.source == LEAF_MAIN ? main : prep)[l.col] : E4(); });
     }
 
     // ShardVerifier::verify_zerocheck (crates/hypercube/src/verifier/shard.rs:288-434)
     uint32_t zerocheck() {
         const size_t nch = m->chips.size();
         const E4 alpha = sample_ext(), gkr_c = sample_ext(), lambda = sample_ext();
-        if (p.zc.polys.size() != mlr) return V_INVALID_SHAPE;
+        if (p.zc.polys.size() != mlr) return SP1B200_VERDICT_INVALID_SHAPE;
         const std::vector<E4> zp = ext_vec(p.zc.point, mlr);
         E4 eqv = E4::one();
         for (uint32_t i = 0; i < mlr; i++) eqv = eqv * eqf(ld(p.gkr_point + 4 * i), zp[i]);
@@ -500,7 +408,7 @@ struct Verifier {
         for (size_t k = 0; k < nch; k++) {
             const ChipProg& c = m->chips[k];
             const std::vector<E4> degree = point_from_usize(heights[k], mlr + 1);
-            for (size_t i = 1; i < degree.size(); i++) if (!(degree[i] * degree[0]).is_zero()) return V_HEIGHT_TOO_LARGE;
+            for (size_t i = 1; i < degree.size(); i++) if (!(degree[i] * degree[0]).is_zero()) return SP1B200_VERDICT_HEIGHT_TOO_LARGE;
             const E4 geq = full_geq(degree, pt);
             std::vector<E4> rev(c.n_constraints);
             E4 pw = E4::one();
@@ -508,89 +416,73 @@ struct Verifier {
             const std::vector<E4> mo = ext_vec(p.zc_main[k], c.main_w), po = ext_vec(p.zc_prep[k], c.prep_w);
             const E4 pra = eval_air(k, nullptr, nullptr, rev);
             const E4 ce = eval_air(k, po.data(), mo.data(), rev) - pra * geq;
-            E4 ob, g = gkr_c;
-            for (auto& x : mo) { ob = ob + x * g; g = g * gkr_c; }
-            for (auto& x : po) { ob = ob + x * g; g = g * gkr_c; }
+            const E4 ob = batched_opening_claim(p.zc_main[k], c.main_w, p.zc_prep[k], c.prep_w, gkr_c);
             rlc = rlc * lambda + eqv * (ce + ob);
         }
-        if (neq(ld(p.zc.eval), rlc)) return V_CONSTRAINTS_EVAL;
+        if (neq(ld(p.zc.eval), rlc)) return SP1B200_VERDICT_CONSTRAINTS_EVAL;
         E4 mod;
-        for (size_t k = 0; k < nch; k++) {
-            E4 s, g = gkr_c;
-            for (uint32_t j = 0; j < m->chips[k].main_w; j++) { s = s + ld(p.gkr_main[k] + 4 * j) * g; g = g * gkr_c; }
-            for (uint32_t j = 0; j < m->chips[k].prep_w; j++) { s = s + ld(p.gkr_prep[k] + 4 * j) * g; g = g * gkr_c; }
-            mod = lambda * mod + s;
-        }
-        if (neq(ld(p.zc.claimed_sum), mod)) return V_CONSTRAINTS_CLAIMED_SUM;
+        for (size_t k = 0; k < nch; k++)
+            mod = lambda * mod + batched_opening_claim(p.gkr_main[k], m->chips[k].main_w, p.gkr_prep[k], m->chips[k].prep_w, gkr_c);
+        if (neq(ld(p.zc.claimed_sum), mod)) return SP1B200_VERDICT_CONSTRAINTS_CLAIMED_SUM;
         if (uint32_t e = sumcheck(p.zc, mlr, 4)) return e;
         ch.observe(hf::to_monty(nch));
         for (size_t k = 0; k < nch; k++) { observe_var_ext(p.zc_prep[k], m->chips[k].prep_w); observe_var_ext(p.zc_main[k], m->chips[k].main_w); }
-        return V_ACCEPT;
+        return SP1B200_VERDICT_ACCEPT;
     }
 
     // JaggedPcsVerifier::verify_trusted_evaluations (slop/crates/jagged/src/verifier.rs:113-384) with the stacked and BaseFold verifiers
     // behind it; commitments = {preprocessed,} main
     void jagged(const std::vector<const uint32_t*>& commitments) {
         const size_t nr = commitments.size();
-        for (auto& v : p.rc_cc) if (v.empty()) { verdict = V_INCORRECT_SHAPE; return; }
+        for (auto& v : p.rc_cc) if (v.empty()) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
         // column heights as (rows, cols) runs; totals in 128 bits so that no count in the words can wrap them
         unsigned __int128 total_cols = 0, total_area = 0;
         for (auto& v : p.rc_cc) for (auto& rc : v) { total_cols += rc.second; total_area += (unsigned __int128)rc.first * rc.second; }
-        if (total_cols == 0) { verdict = V_INCORRECT_SHAPE; return; }
+        if (total_cols == 0) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
         const uint64_t area64 = total_area >> 63 ? ~(uint64_t)0 : (uint64_t)total_area;
-        if (p.max_log_rows != mlr || p.log_m != hf::log2_ceil(area64) || total_area >> 63) { verdict = V_INCORRECT_SHAPE; return; }
+        if (p.max_log_rows != mlr || p.log_m != hf::log2_ceil(area64) || total_area >> 63) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
         // log_m matches the area, so the columns with rows are few; a column count that is absurd only through empty tables cannot be
         // laid out
-        if (total_cols > ((uint64_t)1 << 24)) { verdict = V_INCORRECT_SHAPE; return; }
+        if (total_cols > ((uint64_t)1 << 24)) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
         const size_t n_cols = (size_t)total_cols;
-        std::vector<uint64_t> prefix;
+        std::vector<uint64_t> prefix{0};
         prefix.reserve(n_cols + 1);
-        {
-            uint64_t s = 0;
-            for (auto& v : p.rc_cc) for (auto& rc : v) for (uint32_t c = 0; c < rc.second; c++) { prefix.push_back(s); s += rc.first; }
-            prefix.push_back(s);
-        }
+        for (auto& v : p.rc_cc) layout::append_column_prefix(prefix, v);
         const std::vector<E4> z_col = sample_point(hf::log2_ceil(n_cols));
-        const uint64_t R = (uint64_t)1 << mlr, S = (uint64_t)1 << ls;
-        std::vector<uint64_t> round_area(nr), added_vals(nr), added_cols(nr);
+        const uint64_t R = (uint64_t)1 << mlr;
+        std::vector<uint64_t> padded_area(nr), added_cols(nr);
         std::vector<std::vector<E4>> claims(nr);
         for (size_t r = 0; r < nr; r++) {
             const auto& v = p.rc_cc[r];
-            if (v.size() < 2) { verdict = V_INCORRECT_SHAPE; return; }
+            if (v.size() < 2) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
             uint64_t expect = 0, area = 0;
             for (size_t t = 0; t + 2 < v.size(); t++) { expect += v[t].second; area += (uint64_t)v[t].first * v[t].second; }
             // the claims of round r are the zerocheck's opened values of that round's columns, in chip order
             size_t have = 0;
             for (size_t k = 0; k < m->chips.size(); k++) have += (nr == 2 && r == 0) ? m->chips[k].prep_w : m->chips[k].main_w;
-            if (have != expect) { verdict = V_INCORRECT_SHAPE; return; }
+            if (have != expect) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
             for (size_t k = 0; k < m->chips.size(); k++) {
                 const bool prep = nr == 2 && r == 0;
                 const uint32_t w = prep ? m->chips[k].prep_w : m->chips[k].main_w;
                 const uint32_t* o = prep ? p.zc_prep[k] : p.zc_main[k];
                 for (uint32_t j = 0; j < w; j++) claims[r].push_back(ld(o + 4 * j));
             }
-            std::vector<uint32_t> meta{hf::to_monty(v.size())};
-            for (auto& rc : v) meta.push_back(hf::to_monty(rc.first));
-            for (auto& rc : v) meta.push_back(hf::to_monty(rc.second));
-            uint32_t h[8], cm[8];
-            host_hash(meta.data(), meta.size(), h);
-            host_compress(p.merkle_commits + 8 * r, h, cm);
-            if (memcmp(cm, commitments[r], 32)) { verdict = V_INCORRECT_TABLE_SIZES; return; }
-            if (area == 0 || area >= ((uint64_t)1 << 30)) { verdict = V_AREA_OUT_OF_BOUNDS; return; }
-            const uint64_t next = ((area + S - 1) / S) * S, av = next - area, ac = std::max<uint64_t>((av + R - 1) / R, 1);
-            if (v[v.size() - 2].second + 1 != ac || v.back().second != 1 || v[v.size() - 2].first != R || v.back().first != av - (ac - 1) * R) {
-                verdict = V_DUMMY_TABLES; return;
-            }
-            for (auto& rc : v) if (rc.first > R) { verdict = V_INCORRECT_SHAPE; return; }
-            round_area[r] = area; added_vals[r] = av; added_cols[r] = ac;
+            uint32_t cm[8];
+            table_size_commitment(p.merkle_commits + 8 * r, v, cm);
+            if (memcmp(cm, commitments[r], 32)) { verdict = SP1B200_VERDICT_INCORRECT_TABLE_SIZES; return; }
+            if (area == 0 || area >= ((uint64_t)1 << 30)) { verdict = SP1B200_VERDICT_AREA_OUT_OF_BOUNDS; return; }
+            const layout::Tables pad = layout::padding_tables(area, ls, mlr);
+            if (!std::equal(pad.begin(), pad.end(), v.end() - 2)) { verdict = SP1B200_VERDICT_DUMMY_TABLES; return; }
+            for (auto& rc : v) if (rc.first > R) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
+            padded_area[r] = layout::stacked_columns(area, ls) << ls; added_cols[r] = pad[0].second + pad[1].second;
         }
-        if (p.log_m >= 30) { verdict = V_AREA_OUT_OF_BOUNDS; return; }
+        if (p.log_m >= 30) { verdict = SP1B200_VERDICT_AREA_OUT_OF_BOUNDS; return; }
         std::vector<E4> column_claims;
         for (size_t r = 0; r < nr; r++) { column_claims.insert(column_claims.end(), claims[r].begin(), claims[r].end()); column_claims.resize(column_claims.size() + added_cols[r]); }
-        if (prefix.size() != column_claims.size() + 1) { verdict = V_INCORRECT_SHAPE; return; }
-        if (neq(mle_eval(column_claims, z_col), ld(p.jagged_sc.claimed_sum))) { verdict = V_SUMCHECK_CLAIM_MISMATCH; return; }
+        if (prefix.size() != column_claims.size() + 1) { verdict = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
+        if (neq(hf::mle_eval(column_claims, z_col), ld(p.jagged_sc.claimed_sum))) { verdict = SP1B200_VERDICT_SUMCHECK_CLAIM_MISMATCH; return; }
         if ((verdict = sumcheck(p.jagged_sc, p.log_m, 2))) return;
-        for (size_t c = 0; c + 1 < prefix.size(); c++) if (prefix[c] > prefix[c + 1]) { verdict = V_MONOTONICITY; return; }
+        for (size_t c = 0; c + 1 < prefix.size(); c++) if (prefix[c] > prefix[c + 1]) { verdict = SP1B200_VERDICT_MONOTONICITY; return; }
         // JaggedEvalSumcheckConfig::jagged_evaluation (slop/crates/jagged/src/jagged_eval/sumcheck_eval.rs:45-155)
         const uint32_t lm = p.log_m;
         observe_ext(ld(p.jagged_eval.claimed_sum));
@@ -613,39 +505,37 @@ struct Verifier {
         }
         const E4 jagged_eval = ld(p.jagged_eval.claimed_sum);
         // (the check acc == eval of the jagged-eval sumcheck is resolved with the device flags; nothing below reads acc)
-        deferred.push_back(Deferred{V_JAGGED_EVALUATION, NO_JOB});
-        if (neq(ld(p.expected_eval) * jagged_eval, ld(p.jagged_sc.eval))) { host_fail = V_JAGGED_EVAL_PROOF; return; }
-        std::vector<uint64_t> total(nr);
-        for (size_t r = 0; r < nr; r++) total[r] = round_area[r] + added_vals[r];
+        deferred.push_back(Deferred{SP1B200_VERDICT_JAGGED_EVALUATION, NO_JOB});
+        if (neq(ld(p.expected_eval) * jagged_eval, ld(p.jagged_sc.eval))) { host_fail = SP1B200_VERDICT_JAGGED_EVAL_PROOF; return; }
         observe_ext(ld(p.expected_eval));
-        stacked(total);
+        stacked(padded_area);
     }
 
     // StackedPcsVerifier::verify_trusted_evaluation (slop/crates/stacked/src/verifier.rs:39-99)
     void stacked(const std::vector<uint64_t>& areas) {
         const size_t npt = p.jagged_sc.polys.size();
-        if (npt < ls) { host_fail = V_INCORRECT_SHAPE; return; }
+        if (npt < ls) { host_fail = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
         const std::vector<E4> pt = ext_vec(p.jagged_sc.point, npt);
         const std::vector<E4> batch_point(pt.begin(), pt.end() - ls), stack_point(pt.end() - ls, pt.end());
         std::vector<E4> flat;
         for (size_t r = 0; r < areas.size(); r++) {
-            if (areas[r] % ((uint64_t)1 << ls) || (areas[r] >> ls) != ncols[r]) { host_fail = V_INCORRECT_SHAPE; return; }
+            if (areas[r] % ((uint64_t)1 << ls) || (areas[r] >> ls) != ncols[r]) { host_fail = SP1B200_VERDICT_INCORRECT_SHAPE; return; }
             const std::vector<E4> e = ext_vec(p.batch_evals[r], ncols[r]);
             flat.insert(flat.end(), e.begin(), e.end());
         }
-        if (neq(ld(p.expected_eval), mle_eval(flat, batch_point))) { host_fail = V_STACKING; return; }
+        if (neq(ld(p.expected_eval), hf::mle_eval(flat, batch_point))) { host_fail = SP1B200_VERDICT_STACKING; return; }
         for (size_t r = 0; r < areas.size(); r++) ch.observe_n(p.batch_evals[r], 4 * ncols[r]);
         basefold(stack_point, flat);
     }
 
     // BasefoldVerifier::verify_mle_evaluations (slop/crates/basefold/src/verifier.rs:122-420)
     void basefold(const std::vector<E4>& point, const std::vector<E4>& claims) {
-        if (!ch.check_witness(prm.batch_pow_bits, p.batch_witness[0])) { host_fail = V_BATCH_POW; return; }
+        if (!ch.check_witness(prm.batch_pow_bits, p.batch_witness[0])) { host_fail = SP1B200_VERDICT_BATCH_POW; return; }
         const std::vector<E4> coeffs = hf::partial_lagrange(sample_point(hf::log2_ceil(claims.size())));
         E4 claim;
         for (size_t k = 0; k < claims.size(); k++) claim = claim + claims[k] * coeffs[k];
         const size_t len = ls;
-        if (point.size() != len || len == 0) { host_fail = V_FRI_LENGTH; return; }
+        if (point.size() != len || len == 0) { host_fail = SP1B200_VERDICT_FRI_LENGTH; return; }
         ch.observe(hf::to_monty(len));
         std::vector<E4> betas;
         for (size_t i = 0; i < len; i++) {
@@ -656,13 +546,13 @@ struct Verifier {
         E4 expected = claim;
         for (size_t i = 0; i < len; i++) {
             const E4 p0 = ld(p.univariate + 8 * i), p1 = ld(p.univariate + 8 * i + 4), x = point[len - 1 - i];
-            if (neq(expected, (E4::one() - x) * p0 + x * p1)) { host_fail = V_BASEFOLD_SUMCHECK; return; }
+            if (neq(expected, (E4::one() - x) * p0 + x * p1)) { host_fail = SP1B200_VERDICT_BASEFOLD_SUMCHECK; return; }
             expected = p0 + betas[i] * p1;
         }
         ch.observe_n(p.final_poly, 4);
-        if (!ch.check_witness(prm.pow_bits, p.pow_witness[0])) { host_fail = V_POW; return; }
+        if (!ch.check_witness(prm.pow_bits, p.pow_witness[0])) { host_fail = SP1B200_VERDICT_POW; return; }
         const uint32_t log_n = (uint32_t)len + lb;
-        if (log_n > 24) { host_fail = V_TWO_ADICITY; return; }
+        if (log_n > 24) { host_fail = SP1B200_VERDICT_TWO_ADICITY; return; }
         idx.resize(nq);
         for (auto& q : idx) q = ch.sample_bits(log_n);
         // device: every opening, and the fold chain of every query
@@ -687,14 +577,15 @@ struct Verifier {
         fold = true;
         // the device checks in verify_mle_evaluations' order: component openings round by round, then per fold round the opened value
         // and that round's openings, then final_poly
-        for (size_t r = 0; r < ncomp; r++) deferred.push_back(Deferred{V_TCS_COMPONENT, (uint32_t)r});
+        for (size_t r = 0; r < ncomp; r++) deferred.push_back(Deferred{SP1B200_VERDICT_TCS_COMPONENT, (uint32_t)r});
         for (size_t r = 0; r < len; r++) {
-            deferred.push_back(Deferred{V_QUERY_VALUE, (uint32_t)r});
-            deferred.push_back(Deferred{V_TCS_QUERY, (uint32_t)(ncomp + r)});
+            deferred.push_back(Deferred{SP1B200_VERDICT_QUERY_VALUE, (uint32_t)r});
+            deferred.push_back(Deferred{SP1B200_VERDICT_TCS_QUERY, (uint32_t)(ncomp + r)});
         }
-        deferred.push_back(Deferred{V_QUERY_FINAL_POLY, NO_JOB});
+        deferred.push_back(Deferred{SP1B200_VERDICT_QUERY_FINAL_POLY, NO_JOB});
         const E4 f = ld(p.final_poly);
-        if (neq(f, ld(p.univariate + 8 * (len - 1)) + betas.back() * ld(p.univariate + 8 * (len - 1) + 4))) host_fail = V_SUMCHECK_FINAL_POLY;
+        if (neq(f, ld(p.univariate + 8 * (len - 1)) + betas.back() * ld(p.univariate + 8 * (len - 1) + 4)))
+            host_fail = SP1B200_VERDICT_SUMCHECK_FINAL_POLY;
     }
 
 
@@ -712,11 +603,11 @@ struct Verifier {
                 if (!prep || w) want.emplace_back(heights[k], w);
             }
             const auto& v = p.rc_cc[r];
-            if (v.size() != want.size() + 2) return V_CHIP_TABLES;
+            if (v.size() != want.size() + 2) return SP1B200_VERDICT_CHIP_TABLES;
             for (size_t t = 0; t < want.size(); t++)
-                if (v[t].first != want[t].first || v[t].second != want[t].second) return V_CHIP_TABLES;
+                if (v[t].first != want[t].first || v[t].second != want[t].second) return SP1B200_VERDICT_CHIP_TABLES;
         }
-        return V_ACCEPT;
+        return SP1B200_VERDICT_ACCEPT;
     }
 
     // the host phase: the shard's own words enter the transcript started from `start` - public values, main commitment, chip shapes
@@ -726,21 +617,15 @@ struct Verifier {
         ch.load(start);
         ch.observe_n(p.pv, p.n_pv);
         ch.observe_n(p.commit, 8);
-        ch.observe(hf::to_monty(nch));
-        if (nch && mlr + 1 >= 30) verdict = V_INVALID_SHAPE;   // a degree point of 30 or more bits (shard.rs:477)
-        for (size_t k = 0; k < nch && !verdict; k++) {
-            ch.observe(hf::to_monty(heights[k]));
-            const size_t len = strlen(names[k]);
-            ch.observe(hf::to_monty(len));
-            for (size_t i = 0; i < len; i++) ch.observe(hf::to_monty((uint8_t)names[k][i]));
-        }
+        observe_chip_shapes(ch, nch, heights, names);
+        if (nch && mlr + 1 >= 30) verdict = SP1B200_VERDICT_INVALID_SHAPE;   // a degree point of 30 or more bits (shard.rs:477)
         // the preprocessed round's leading column counts are the preprocessed widths (shard.rs:506-523)
         const bool has_prep = ncols.size() == 2;
         if (!verdict && has_prep) {
             size_t t = 0;
             for (size_t k = 0; k < nch && !verdict; k++) {
                 if (!m->chips[k].prep_w) continue;
-                if (t >= p.rc_cc[0].size() || p.rc_cc[0][t].second != m->chips[k].prep_w) verdict = V_PREP_WIDTHS;
+                if (t >= p.rc_cc[0].size() || p.rc_cc[0][t].second != m->chips[k].prep_w) verdict = SP1B200_VERDICT_PREPROCESSED_WIDTHS;
                 t++;
             }
         }
@@ -767,13 +652,13 @@ struct Verifier {
             for (uint32_t q = 0; q < nq; q++) { min_bad = std::min(min_bad, out[fold_at + q]); final_bad |= out[fold_at + nq + q]; }
         for (const Deferred& d : deferred) {
             bool bad = false;
-            if (d.code == V_JAGGED_EVALUATION) {
+            if (d.code == SP1B200_VERDICT_JAGGED_EVALUATION) {
                 hf::E4 acc[1];
                 sum_partials<1>(out.data() + jag_at, blocks_for(jag_cols), acc);
                 bad = neq(acc[0] * jag_bp, jag_expect);
-            } else if (d.code == V_QUERY_VALUE) {
+            } else if (d.code == SP1B200_VERDICT_QUERY_VALUE) {
                 bad = min_bad == d.job;
-            } else if (d.code == V_QUERY_FINAL_POLY) {
+            } else if (d.code == SP1B200_VERDICT_QUERY_FINAL_POLY) {
                 bad = final_bad != 0;
             } else {   // an opening job: its nq path checks and its tensor commitment
                 const size_t j = (size_t)job0 + d.job;
@@ -1001,7 +886,7 @@ sp1b200_err verify_shards(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint
 extern "C" {
 
 const char* sp1b200_verdict_name(uint32_t verdict) {
-    if (verdict < V_COUNT) return VERDICT_NAMES[verdict];
+    if (verdict < std::size(VERDICT_NAMES)) return VERDICT_NAMES[verdict];
     const char* core = verify_core_verdict_name(verdict);
     return core ? core : "Unknown";
 }
@@ -1013,7 +898,7 @@ sp1b200_err sp1b200_verify_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, con
     const auto t0 = std::chrono::steady_clock::now();
     VerifyShardIn in;
     SP1_TRY(verify_parse_shard(ctx, m, h_prep_commit8, h_heights, chip_names, h_proof, n_words, "verify_shard", in));
-    uint32_t verdict = V_ACCEPT, fin[34];
+    uint32_t verdict = SP1B200_VERDICT_ACCEPT, fin[34];
     VerifyTimes t;
     SP1_TRY(verify_shards(ctx, m, h_prep_commit8, chip_names, {&in}, h_chal, 1, &verdict, fin, t));
     float kernel_ms = 0;

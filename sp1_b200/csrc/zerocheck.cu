@@ -34,6 +34,15 @@ constexpr int ZC_GLOBAL_REGS = 1024;  // last tier: register file in a global-me
 constexpr unsigned ZC_GLOBAL_MAXB = 132 * 2;  // blocks of a global-tier job: bounds the workspace (blocks x regs x 3 nodes x 128 x 16 B)
 constexpr size_t ZC_MAX_PIECES = 16;
 
+// The register-file tier of a program with `regs` live registers per thread, in the sumcheck and in the constraint check: 0 / 1 / 2
+// a shared-memory file of 8 / 16 / 32 registers (per block: 48 / 96 / 192 KiB in the sumcheck's extension-field rounds, 3 nodes x
+// 16 B x 128 threads; 4 / 8 / 16 KiB in the constraint check, one base-field node), 3 local memory, 4 the global workspace.
+inline int zc_tier(uint32_t regs) {
+    constexpr uint32_t TIER_REGS[3] = {8, 16, 32};
+    for (int t = 0; t < 3; t++) if (regs <= TIER_REGS[t]) return t;
+    return regs <= (uint32_t)ZC_LOCAL_REGS ? 3 : 4;
+}
+
 template <class K> struct Ops;
 template <> struct Ops<uint32_t> {
     static __device__ __forceinline__ uint32_t zero() { return 0; }
@@ -394,25 +403,6 @@ __global__ void __launch_bounds__(32) zc_debug_select_kernel(const ZcDbgSelect* 
     }
 }
 
-// host interpreter on the all-zero row (padded_row_adjustment, shard.rs:520-537): Σ powers[alpha_idx] * reg
-E4 host_eval_zero_row(const HostProg& p, const uint32_t* pv, const std::vector<E4>& powers, uint32_t n_regs) {
-    std::vector<uint32_t> regs(n_regs ? n_regs : 1, 0);
-    for (const DagInstr& in : p.instrs) {
-        switch (in.opcode) {
-            case BC_LOAD_LEAF: regs[in.out] = 0; break;
-            case BC_LOAD_CONST: regs[in.out] = p.consts[in.a]; break;
-            case BC_LOAD_PUBLIC: regs[in.out] = pv[p.publics[in.a]]; break;
-            case BC_ADD_F: regs[in.out] = hf::add(regs[in.a], regs[in.b]); break;
-            case BC_SUB_F: regs[in.out] = hf::sub(regs[in.a], regs[in.b]); break;
-            case BC_MUL_F: regs[in.out] = hf::mul(regs[in.a], regs[in.b]); break;
-            case BC_NEG_F: regs[in.out] = hf::neg(regs[in.a]); break;
-        }
-    }
-    E4 acc;
-    for (size_t i = 0; i < p.assert_regs.size(); i++) acc = acc + powers[p.assert_alphas[i]] * regs[p.assert_regs[i]];
-    return acc;
-}
-
 struct VGeq {
     uint32_t threshold = 0; E4 geq_c, eq_c;
     VGeq fix_last(const E4& a) const {
@@ -591,7 +581,8 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         ap_off[k] = all_ap.size();
         all_ap.insert(all_ap.end(), rev.begin(), rev.end());
         if (rev.empty()) all_ap.push_back(E4());
-        s.pra = host_eval_zero_row(m->host[k], h_pv, rev, p.n_regs);
+        // the all-zero row (padded_row_adjustment, shard.rs:520-537)
+        s.pra = host_eval_constraints<uint32_t>(m->host[k], p.n_regs, h_pv, rev, [](const LeafRef&) { return 0u; });
         s.vg.threshold = (uint32_t)s.h; s.vg.geq_c = E4::one();
         const uint64_t nh = (s.h + 1) / 2;
         const size_t w = p.main_w + p.prep_w;
@@ -615,9 +606,6 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
     int ecur = 0;
 
     // ---- the whole launch plan is known up front (heights halve deterministically): job tables of every round, one upload ----
-    // tiers of the shared-memory register file (registers per thread); chips above the last tier use the local-memory kernel
-    static const uint32_t TIER_REGS[3] = {8, 16, 32};  // x 3 nodes x 16 B x 128 threads = 48 / 96 / 192 KiB per block (EF rounds)
-    auto tier_of = [&](uint32_t regs) { for (int t = 0; t < 3; t++) if (regs <= TIER_REGS[t]) return t; return regs <= (uint32_t)ZC_LOCAL_REGS ? 3 : 4; };
     size_t ws_bytes = 0;  // global register-file workspace: worst launch of the last tier (EF rounds: 16 B per register and node)
     struct Launch { size_t job0; uint32_t n_jobs, blocks, regs; int tier; };
     struct RoundPlan { std::vector<Launch> sums; size_t fix0; uint32_t fix_jobs, fix_blocks; std::vector<uint32_t> chip_of_job; size_t job0; };
@@ -653,7 +641,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
                 Launch Lc{jobs.size(), 0, 0, 0, tier};
                 for (size_t k = 0; k < nchips; k++) {
                     const ChipProg& p = m->chips[k];
-                    if (!hcur[k] || tier_of(p.zc_regs) != tier) continue;
+                    if (!hcur[k] || zc_tier(p.zc_regs) != tier) continue;
                     unsigned nb = blocks_for((hcur[k] + 1) / 2, ZC_BLOCK);
                     if (nb > MAXB) nb = MAXB;
                     if (tier == 4 && nb > ZC_GLOBAL_MAXB) nb = ZC_GLOBAL_MAXB;
@@ -884,8 +872,6 @@ sp1b200_err sp1b200_debug_constraints_device(sp1b200_ctx* ctx, const sp1b200_mac
     uint32_t* d_pv;
     SP1_TRY(mem.alloc((void**)&d_pv, (n_pv ? n_pv : 1) * 4));
     if (n_pv) SP1_CUDA(cudaMemcpyAsync(d_pv, h_pv, n_pv * 4, cudaMemcpyHostToDevice, st));
-    static const uint32_t TIER_REGS[3] = {8, 16, 32};   // the zerocheck kernels' tiers (one node: 4 / 8 / 16 KiB per block)
-    auto tier_of = [&](uint32_t regs) { for (int t = 0; t < 3; t++) if (regs <= TIER_REGS[t]) return t; return regs <= (uint32_t)ZC_LOCAL_REGS ? 3 : 4; };
     struct Launch { size_t job0; uint32_t n_jobs, blocks, regs; int tier; };
     // one launch per register-file tier over every chip of that tier; n_of(k) = work items of chip k (0: no job)
     auto plan = [&](std::vector<ZcDbgJob>& jobs, std::vector<Launch>& launches, size_t& ws_bytes, auto n_of, auto fill) {
@@ -893,7 +879,7 @@ sp1b200_err sp1b200_debug_constraints_device(sp1b200_ctx* ctx, const sp1b200_mac
             Launch Lc{jobs.size(), 0, 0, 0, tier};
             for (size_t k = 0; k < nchips; k++) {
                 const uint64_t n = n_of(k);
-                if (!n || tier_of(m->chips[k].zc_regs) != tier) continue;
+                if (!n || zc_tier(m->chips[k].zc_regs) != tier) continue;
                 unsigned nb = std::min<unsigned>(blocks_for(n, ZC_BLOCK), 132 * 4);
                 if (tier == 4) nb = std::min(nb, ZC_GLOBAL_MAXB);
                 ZcDbgJob j{};

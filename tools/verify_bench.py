@@ -40,6 +40,8 @@ def full_size_proof(lib, workload, dev):
     d_main = torch.cat(mains).contiguous()
     d_prep = torch.cat(preps).contiguous()
     del mains, preps
+    # the library reads the traces on its own stream: torch's kernels that wrote them must have finished
+    torch.cuda.current_stream(dev).synchronize()
     machine = lib.machine_create(mach["blob"])
     pc, h_prep = lib.jagged_commit_dense(d_prep, [s.h for s in specs if s.wp], [1 + s.extra_prep for s in specs if s.wp])
     st = HostChallenger().st.copy()

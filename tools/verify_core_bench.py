@@ -45,12 +45,13 @@ def prove_chain(lib, workload, n, dev, seed=900):
             if sp.wp:
                 preps.append(p_)
         d_main = torch.cat(mains).contiguous()
-        del mains
-        if prep_round is None and preps:
-            d_prep = torch.cat(preps).contiguous()
+        d_prep = torch.cat(preps).contiguous() if prep_round is None and preps else None
+        del mains, preps
+        # the library reads the traces on its own stream: torch's kernels that wrote them must have finished
+        torch.cuda.current_stream(dev).synchronize()
+        if d_prep is not None:
             pc, prep_round = lib.jagged_commit_dense(d_prep, [s_.h for s_ in specs if s_.wp], [1 + s_.extra_prep for s_ in specs if s_.wp])
             del d_prep
-        del preps
         hc = HostChallenger(); hc.observe(pc); hc.observe(tail)
         st = hc.st.copy()
         words.append(lib.prove_shard(machine, prep_round, d_main, heights, names, SA.to_monty(np.array(pv)), st))
