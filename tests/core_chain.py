@@ -5,10 +5,12 @@ The chain: timestamps from [0, 0, 0, 1]; program counters from the key's pc_star
 shard (shard 0); optionally one non-execution shard (timestamps, pc and exit code unchanged across it); the commit-syscall flags at 1
 from the first shard on; non-zero init / finalize addresses; one proof nonce; and global cumulative sums zero + k_i · dummy whose k_i
 cancel against the key's initial sum zero - (Σ k_i) · dummy.  Everything is canonical integers; the synthetic chips read public value
-0 = prev_committed_value_digest[0][0], so shard i's traces are built with pv0_of(pvs[i])."""
+0 = prev_committed_value_digest[0][0], so shard i's traces are built with pv0_of(pvs[i]).
+
+PV_CASES: one chain fault per reason the public-value checks across shards give, with the verdict and shard the reference's loop stops at."""
 import numpy as np
 
-from tests.test_septic import DUMMY, ZERO, curve_add, curve_neg, sadd, sinv, smul, ssub
+from tests.septic import DUMMY, START, ZERO, curve_add, curve_neg, multiples
 
 P = 0x7F000001
 PV_MAX_NUM = 187
@@ -29,17 +31,6 @@ def setf(pv, name, vals):
 def getf(pv, name):
     at, n = _off(name)
     return list(pv[at:at + n])
-
-
-def multiples(base, k):
-    """[base, 2 base, ..., k base]: the doubling by the tangent, then incomplete additions"""
-    x, y = base
-    s = smul(sadd(smul([3, 0, 0, 0, 0, 0, 0], smul(x, x)), [45, 0, 0, 0, 0, 0, 0]), sinv(sadd(y, y)))
-    x2 = ssub(ssub(smul(s, s), x), x)
-    out = [base, (x2, ssub(smul(s, ssub(x, x2)), y))]
-    while len(out) < k:
-        out.append(curve_add(out[-1], base))
-    return out[:k]
 
 
 def vk_tail(pc_start, initial_sum, untrusted=0):
@@ -97,3 +88,98 @@ def chain(n, seed, non_execution=None, untrusted=0):
 
 def pv0_of(pv):
     return int(pv[0])
+
+
+# (name, mutation of the valid 3-shard chain with a non-execution shard 1, expected verdict, expected shard)
+def _set(s, name, vals):
+    return lambda pvs, tail: setf(pvs[s], name, vals)
+
+
+def _m_len(pvs, tail):
+    pvs[1][:] = pvs[1][:186]
+
+
+def _m_never(field):
+    def f(pvs, tail):
+        for pv in pvs:
+            setf(pv, "previous_" + field, [0, 0, 0]); setf(pv, "last_" + field, [0, 0, 0])
+    return f
+
+
+def _m_commit(field):
+    def f(pvs, tail):
+        for pv in pvs:
+            setf(pv, "prev_" + field, 0); setf(pv, field, 0)
+    return f
+
+
+def _m_ts_changed(pvs, tail):
+    last = getf(pvs[1], "last_timestamp"); last[3] += 1
+    setf(pvs[1], "last_timestamp", last); setf(pvs[2], "initial_timestamp", last)
+
+
+def _m_pc_nonexec(pvs, tail):
+    setf(pvs[1], "next_pc", [7, 7, 7]); setf(pvs[2], "pc_start", [7, 7, 7])
+
+
+def _m_exit_nonexec(pvs, tail):
+    setf(pvs[1], "exit_code", 3); setf(pvs[2], "prev_exit_code", 3); setf(pvs[2], "exit_code", 3)
+
+
+def _m_exit_changed(pvs, tail):
+    setf(pvs[0], "exit_code", 3)
+    for s in (1, 2):
+        setf(pvs[s], "prev_exit_code", 3); setf(pvs[s], "exit_code", 3)
+    setf(pvs[2], "exit_code", 4)
+
+
+def _m_digest(pvs, tail):
+    g = getf(pvs[1], "global_cumulative_sum")
+    p = (g[:7], g[7:])
+    q = curve_add(p, DUMMY)
+    setf(pvs[1], "global_cumulative_sum", list(q[0]) + list(q[1]))
+
+
+def _m_exceptional(pvs, tail):
+    tail[3:17] = list(START[0]) + list(START[1])
+
+
+def _m_bump(s, name, k=0):
+    def f(pvs, tail):
+        v = getf(pvs[s], name); v[k] = (v[k] + 1) % P
+        setf(pvs[s], name, v)
+    return f
+
+
+PV_CASES = [
+    ("length", _m_len, 46, 1),
+    ("first shard twice", _set(2, "is_first_execution_shard", 1), 47, 2),
+    ("first shard not boolean", _set(1, "is_first_execution_shard", 2), 48, 1),
+    ("first shard not set", _set(0, "is_first_execution_shard", 0), 49, 3),
+    ("initial timestamp", _m_bump(2, "initial_timestamp", 3), 50, 2),
+    ("timestamp unchanged on an execution shard", _set(1, "is_execution_shard", 1), 51, 1),
+    ("timestamp changed on a non-execution shard", _m_ts_changed, 52, 1),
+    ("pc_start != vk.pc_start", _m_bump(0, "pc_start", 1), 53, 0),
+    ("pc_start != prev_next_pc", _m_bump(2, "pc_start", 0), 54, 2),
+    ("pc changed on a non-execution shard", _m_pc_nonexec, 55, 1),
+    ("not halted", _set(2, "next_pc", [5, 0, 0]), 56, 3),
+    ("prev_exit_code", _set(0, "prev_exit_code", 1), 57, 0),
+    ("exit code changed on a non-execution shard", _m_exit_nonexec, 58, 1),
+    ("exit code changed twice", _m_exit_changed, 59, 2),
+    ("proof nonce", _m_bump(2, "proof_nonce", 1), 60, 2),
+    ("previous_init_addr", _m_bump(1, "previous_init_addr"), 61, 1),
+    ("previous_finalize_addr", _m_bump(1, "previous_finalize_addr", 2), 62, 1),
+    ("previous_init_page_idx", _m_bump(2, "previous_init_page_idx"), 63, 2),
+    ("previous_finalize_page_idx", _m_bump(2, "previous_finalize_page_idx", 1), 64, 2),
+    ("untrusted programs flag", _set(0, "is_untrusted_programs_enabled", 1), 65, 0),
+    ("zero address never initialized", _m_never("init_addr"), 66, 3),
+    ("zero address never finalized", _m_never("finalize_addr"), 67, 3),
+    ("committed value digest", _m_bump(1, "prev_committed_value_digest", 5), 68, 1),
+    ("deferred proofs digest", _m_bump(2, "prev_deferred_proofs_digest", 7), 69, 2),
+    ("commit syscall", _set(0, "prev_commit_syscall", 1), 70, 0),
+    ("commit deferred syscall", _set(1, "prev_commit_deferred_syscall", 0), 71, 1),
+    ("COMMIT never called", _m_commit("commit_syscall"), 72, 3),
+    ("COMMIT_DEFERRED_PROOFS never called", _m_commit("commit_deferred_syscall"), 73, 3),
+    ("global cumulative sum", _m_digest, 74, 3),
+    ("exceptional point addition", _m_exceptional, 75, 0),
+]

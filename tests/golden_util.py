@@ -5,8 +5,8 @@ import os
 
 import numpy as np
 
+from tests import machines as M
 from tests import oracle_lib as O
-from tests.test_oracle import _synth_machine_gkr
 
 PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "shard_proofs.json")
 
@@ -16,14 +16,9 @@ def cases():
 
 
 def inputs_of(case):
-    """re-create the seeded inputs of a golden case (same generator the fixture script used)"""
-    rng = np.random.default_rng(case["seed"])
-    spec = [tuple(s) for s in case["spec"]]
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger()
-    ch.observe(O.rand_field(rng, 9))
-    return blob, heights, mains, preps, pv, names, ch
+    """re-create the seeded inputs of a golden case (same generator the fixture script used)
+    -> (blob, heights, mains, preps, pv, names, challenger)"""
+    return M.shard_inputs(case["spec"], case["seed"])
 
 
 def check_words(case, prep_commit, words, final_state):
@@ -43,7 +38,6 @@ def check_words(case, prep_commit, words, final_state):
 
 # ---- BASELINE-size goldens (tests/golden/shard_proofs_fullsize.json): workloads S1 / S2 with the core protocol parameters ------------
 FULL_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "shard_proofs_fullsize.json")
-FULL_PV0 = 12345
 
 
 def fullsize_cases():
@@ -52,16 +46,9 @@ def fullsize_cases():
 
 def fullsize_inputs(workload, seed):
     """the seeded full-size inputs of a golden case: the bench machine of `workload` (sp1_b200.workload.synthetic_machine) with numpy
-    traces (so that the CPU generator and the GPU test see the same words).  -> (mach, heights, mains, preps, pv, challenger)"""
-    from sp1_b200 import synth_air as SA
-    from sp1_b200 import workload as W
-    mach = W.synthetic_machine(workload, seed=42)
+    traces (so that the CPU generator and the GPU test see the same words).  -> (blob, heights, mains, preps, pv, names, challenger)"""
     rng = np.random.default_rng(seed)
-    mains, preps = [], []
-    for sp in mach["specs"]:
-        m_, p_ = SA.synth_trace(rng, sp.h, sp.g, sp.wp, FULL_PV0, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        mains.append(m_); preps.append(p_)
-    pv = O.to_monty(np.array([FULL_PV0, 5, 6, 7]))
+    inp = M.workload_machine(workload, rng)
     ch = O.Challenger()
     ch.observe(O.rand_field(rng, 9))
-    return mach, [s_[0] for s_ in mach["specs"]], mains, preps, pv, ch
+    return inp + (ch,)

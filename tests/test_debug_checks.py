@@ -1,95 +1,24 @@
 """The shard checks on the CPU: the restated debug_constraints_all_chips / debug_interactions_with_all_chips (oracle/debug.hpp) on
 satisfiable and corrupted machines, the interaction check's key fingerprint (linear, so colliding keys can be built from it), and
-the code ptxas generates for the constraint-check kernel.  Helpers here build the machines tests/test_gpu_debug.py checks on the GPU."""
-import ctypes as C
+the code ptxas generates for the constraint-check kernel."""
 import os
 import re
 
 import numpy as np
 import pytest
 
-from sp1_b200 import synth_air as SA
-from sp1_b200 import workload as W
 from sp1_b200.lib import parse_constraint_report, parse_interaction_report
-from tests import hostcheck_lib
 from tests import debug_oracle_lib as DO
+from tests import machines as M
 from tests import oracle_lib as O
+from tests.machines import colliding_keys, cross_chip_machine, fingerprint
 
 P = O.P
-PV = O.to_monty(np.array([12345, 5, 6, 7]))
-
-
-def _inter_words(inters):
-    """inters: [(is_send, kind, mult vcol words, [value vcol words])] -> the chip's interaction words"""
-    w = [len(inters)]
-    for is_send, kind, mult, vals in inters:
-        w += [is_send, kind, len(vals)] + mult
-        for v in vals:
-            w += v
-    return w
-
-
-def cross_chip_machine(rng, h=64, mult_col_kind4=False):
-    """two one-group chips whose sends (chip 0) and receives (chip 1) sit in different chips: chip 1's trace is chip 0's with the rows
-    reversed.  Interactions (sends in chip 0, receives in chip 1, same order): kind 4 (a, 9) with multiplicity 1 (or column d when
-    mult_col_kind4), kind 6 (b) with multiplicity d."""
-    w, _, _ = SA.synth_chip(1, False)
-    m0, _ = SA.synth_trace(rng, h, 1, False, 12345)
-    m1 = np.ascontiguousarray(m0[:, ::-1])
-    a, b, d = (SA.LEAF_MAIN, 0, 1), (SA.LEAF_MAIN, 1, 1), (SA.LEAF_MAIN, 3, 1)
-    mult4 = SA._vcol([d]) if mult_col_kind4 else SA._vcol([], constant=1)
-    inter = lambda s: [(s, 4, mult4, [SA._vcol([a]), SA._vcol([], constant=9)]), (s, 6, SA._vcol([d]), [SA._vcol([b])])]
-    blob = SA.machine_blob_with_interactions([w, w], [_inter_words(inter(1)), _inter_words(inter(0))])
-    return blob, [h, h], [m0, m1], [None, None]
-
-
-def fingerprint(kind, values):
-    L = hostcheck_lib.load()
-    f = L.sp1b200_hostcheck_fingerprint
-    f.restype = C.c_uint64
-    v = np.ascontiguousarray(values, dtype=np.uint32)
-    return int(f(C.c_uint32(kind), C.c_uint32(v.size), v.ctypes.data_as(C.POINTER(C.c_uint32)) if v.size else None))
-
-
-def colliding_keys(rng, kind=5):
-    """two different 3-value keys (canonical values) with equal fingerprints, from the two linear forms read off basis vectors"""
-    def forms(vals):
-        x = fingerprint(kind, O.to_monty(np.array(vals)))
-        return x >> 31, x & 0x7fffffff
-    base = forms([0, 0, 0])
-    c = []
-    for t in range(3):
-        e = [0, 0, 0]; e[t] = 1
-        f = forms(e)
-        c.append(((f[0] - base[0]) % P, (f[1] - base[1]) % P))
-    # d = c0 x c1 (componentwise forms over the three values) is in the kernel of both forms
-    u, v = [x[0] for x in c], [x[1] for x in c]
-    d = [(u[1] * v[2] - u[2] * v[1]) % P, (u[2] * v[0] - u[0] * v[2]) % P, (u[0] * v[1] - u[1] * v[0]) % P]
-    A = [int(x) for x in rng.integers(0, P, 3)]
-    B = [(x + y) % P for x, y in zip(A, d)]
-    assert A != B
-    return A, B
-
-
-def constant_key_machine(rng, chip_inters, heights):
-    """one-group chips whose interactions have constant values: chip_inters[k] = [(is_send, kind, canonical values)], multiplicity 1"""
-    words, iws, mains = [], [], []
-    for inters, h in zip(chip_inters, heights):
-        w, _, _ = SA.synth_chip(1, False)
-        words.append(w)
-        iws.append(_inter_words([(s, k, SA._vcol([], constant=1), [SA._vcol([], constant=x) for x in vals]) for s, k, vals in inters]))
-        mains.append(SA.synth_trace(rng, h, 1, False, 12345)[0])
-    return SA.machine_blob_with_interactions(words, iws), list(heights), mains, [None] * len(heights)
+PV = M.PV
 
 
 def _small_workload(name):
-    m = W.synthetic_machine(name, seed=42, scale=1 / 256)
-    rng = np.random.default_rng(3)
-    mains, preps = [], []
-    for sp in m["specs"]:
-        a, p = SA.synth_trace(rng, sp.h, sp.g, sp.wp, 12345, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        mains.append(a); preps.append(p)
-    return m["blob"], [sp.h for sp in m["specs"]], mains, preps
+    return M.workload_machine(name, seed=3, scale=1 / 256)[:4]
 
 
 @pytest.mark.parametrize("workload", ["tiny", "tinyc", "tinyr"])

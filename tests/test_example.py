@@ -29,23 +29,15 @@ def test_wire_example_host_on_the_cpu(tmp_path):
     bytes it writes are the committed golden wire bytes"""
     import hashlib
     import json
-    from tests.test_wire import _proof
+    from tests import machines as M
     from tools import gen_golden_proofs as GG
     _build()
     name, spec, log_stack, mlr, seed, nq, pw, bpw, gpw = GG.CASES[2]
     rng_case = GG.bincode_case(*GG.CASES[2])
-    # the same seeded proof as the golden generator (tools/gen_golden_proofs.py run_case)
-    rng = np.random.default_rng(seed)
-    from tests import oracle_lib as O
-    from tests.test_oracle import _synth_machine_gkr
-    from tests.test_wire import _widths
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger(); ch.observe(O.rand_field(rng, 9))
-    _, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, ch, num_queries=nq, pow_bits=pw, batch_pow_bits=bpw,
-                                    gkr_pow_bits=gpw)
+    # the same seeded proof as the golden generator
+    blob, heights, _, _, names, _, words, _ = GG.prove_case(spec, log_stack, mlr, seed, nq, pw, bpw, gpw)
     job = _u32(log_stack, mlr, 2, nq, len(names))
-    for nm, h, (a, b) in zip(names, heights, _widths(blob)):
+    for nm, h, (a, b) in zip(names, heights, M.widths(blob)):
         raw = nm.encode()
         job += _u32(len(raw)) + raw + b"\0" * (-len(raw) % 4) + _u32(h & 0xffffffff, h >> 32, a, b)
     job += _u32(words.size) + words.astype("<u4").tobytes()

@@ -6,30 +6,27 @@ import pytest
 
 from sp1_b200 import synth_air as SA
 from sp1_b200.lib import parse_constraint_report, parse_interaction_report
-from tests import machines as M
 from tests import debug_oracle_lib as DO
+from tests import gpu_prove as GP
+from tests import machines as M
 from tests import oracle_lib as O
-from tests.test_debug_checks import colliding_keys, constant_key_machine, cross_chip_machine
-from tests.test_oracle import _synth_machine
+from tests.machines import Chip, colliding_keys, constant_key_machine, cross_chip_machine
 
 pytestmark = pytest.mark.gpu
 P = O.P
 
 TIER_SPECS = [
     ([(5, 1, False), (0, 2, False), (6, 1, True)], 3),
-    ([(512, 6, False, True), (300, 14, True, True), (1024, 28, False, True), (96, 40, False, True), (2047, 3, True)], 12),
-    ([(192, 250, False, True), (64, 500, True, True), (8191, 3, True), (96, 1000, False, True), (600, 300, False, True)], 13),
+    ([Chip(512, 6, False, deep=True), Chip(300, 14, True, deep=True), Chip(1024, 28, False, deep=True), Chip(96, 40, False, deep=True),
+      (2047, 3, True)], 12),
+    ([Chip(192, 250, False, deep=True), Chip(64, 500, True, deep=True), (8191, 3, True), Chip(96, 1000, False, deep=True),
+      Chip(600, 300, False, deep=True)], 13),
 ]
 
 
 def _lib(mlr):
     from sp1_b200 import Lib
     return Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21))
-
-
-def _prep_round(lib, preps):
-    ps = [p for p in preps if p is not None]
-    return lib.jagged_commit(ps)[1] if ps else None
 
 
 def _check(lib, mach, prep_round, blob, heights, mains, preps, pv, max_rows=3, max_keys=16, inter=True):
@@ -56,10 +53,10 @@ def _corrupt_cells(rng, mains, n_chips=3):
 @pytest.mark.parametrize("spec,mlr", TIER_SPECS)
 def test_constraint_report_register_tiers(spec, mlr):
     rng = np.random.default_rng(1700 + mlr)
-    blob, heights, mains, preps, pv = _synth_machine(rng, spec)
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, spec, interactions=False)
     lib = _lib(mlr)
     mach = lib.machine_create(blob)
-    pr = _prep_round(lib, preps)
+    pr = GP.commit_prep(lib, preps)[1]
     assert _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False) == {}
     _corrupt_cells(rng, mains)
     assert _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False)
@@ -92,7 +89,7 @@ def test_reports_on_calibrated_and_workload_machines(case):
         mlr = 12
     lib = _lib(mlr)
     mach = lib.machine_create(blob)
-    pr = _prep_round(lib, preps)
+    pr = GP.commit_prep(lib, preps)[1]
     _check(lib, mach, pr, blob, heights, mains, preps, pv)
     words = lib.debug_interactions_words(mach, pr, M.dense_main(mains), heights)
     assert words.tolist() == [0, 0, 0]
@@ -107,7 +104,7 @@ def test_reports_on_calibrated_and_workload_machines(case):
 def _inter_case(blob, heights, mains, preps, max_keys=16, mlr=8):
     lib = _lib(mlr)
     mach = lib.machine_create(blob)
-    pr = _prep_round(lib, preps)
+    pr = GP.commit_prep(lib, preps)[1]
     got = lib.debug_interactions_words(mach, pr, M.dense_main(mains), heights, max_keys)
     want = DO.debug_interactions(blob, heights, mains, preps, max_keys)
     if pr is not None:
@@ -136,21 +133,8 @@ def test_interaction_report_cross_chip():
 
 def _blob_segments(blob):
     """-> (per chip program words, per chip interaction words) of a machine blob"""
-    b = [int(x) for x in blob]
-    progs, inters, p = [], [], 1
-    for _ in range(b[0]):
-        ni, nl, nc, npub, na = b[p + 4:p + 9]
-        ln = 9 + 2 * ni + 2 * nl + nc + npub + 2 * na
-        progs.append(b[p:p + ln]); p += ln
-    for _ in range(b[0]):
-        q = p + 1
-        for _ in range(b[p]):
-            nv = b[q + 2]; q += 3
-            for _ in range(nv + 1):
-                q += 2 + 3 * b[q]
-        inters.append(b[p:q]); p = q
-    assert p == len(b)
-    return progs, inters
+    segs = M.chip_segments(blob)
+    return [s[2] for s in segs], [s[3] for s in segs]
 
 
 def _bump_first_receive(iw):
@@ -197,12 +181,11 @@ def test_pointer_kinds_errors_memory_and_proof_unchanged():
     import torch
     rng = np.random.default_rng(2000)
     spec = [(1024, 2, True), (256 + 32, 3, False), (0, 1, False), (2048, 1, True)]
-    from tests.test_oracle import _synth_machine_gkr
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
+    blob, heights, mains, preps, pv, names = M.spec_machine(rng, spec, names="Chip{:02d}")
     mains[1][2, 7] = (int(mains[1][2, 7]) + 3) % P
     lib = _lib(11)
     mach = lib.machine_create(blob)
-    pr = _prep_round(lib, preps)
+    pr = GP.commit_prep(lib, preps)[1]
     dense = M.dense_main(mains)
     ref_c = lib.debug_constraints_words(mach, pr, dense, heights, pv)
     ref_i = lib.debug_interactions_words(mach, pr, dense, heights)
@@ -235,7 +218,6 @@ def test_pointer_kinds_errors_memory_and_proof_unchanged():
     # a proof after either check equals the proof without it (clean trace)
     mains[1][2, 7] = (int(mains[1][2, 7]) - 3) % P
     dense = M.dense_main(mains)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
     proofs = []
     for pre in (None, "c", "i"):
         if pre == "c":
@@ -243,47 +225,56 @@ def test_pointer_kinds_errors_memory_and_proof_unchanged():
         if pre == "i":
             assert lib.debug_interactions_words(mach, pr, dense, heights).tolist() == [0, 0, 0]
         st = O.Challenger().st.copy()
-        proofs.append(lib.prove_shard(mach, pr, dense, heights, names, pv, st))
+        proofs.append(GP.prove(lib, mach, pr, mains, heights, names, pv, st))
     assert all((p_.size == proofs[0].size and (p_ == proofs[0]).all()) for p_ in proofs)
     lib.jagged_round_free(pr)
     lib.machine_free(mach)
     lib.close()
 
 
+def _write_cell(dense, cell, value):
+    """a torch write into a trace the library reads next: the library runs on its own stream, so the write must have finished"""
+    import torch
+    dense[cell] = value
+    torch.cuda.current_stream(dense.device).synchronize()
+
+
 def test_full_size_s2c_shard():
     """one full-size S2c shard built on the device: clean -> both reports empty; one corrupted cell -> that (chip, row) with the
     constraints the oracle finds for that row alone; one chip's receive made unbalanced in the blob -> the oracle's report for that chip"""
-    import torch
     from sp1_b200 import Lib
     from sp1_b200 import workload as W
+    from tools.device_traces import device_traces
     mach_d = W.synthetic_machine("S2c", seed=42)
     specs, blob = mach_d["specs"], mach_d["blob"]
     heights = [sp.h for sp in specs]
-    parts, preps = [], []
-    for i, sp in enumerate(specs):
-        m, p = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, 12345, 500 + i, 0, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        parts.append(m); preps.append(p)
-    dense = torch.cat(parts).contiguous()
-    pv = O.to_monty(np.array([12345, 5, 6, 7]))
+    dense, d_prep, prep_rows, prep_cols = device_traces(specs, M.PV0, lambda i: 500 + i, 0)
+    wd = M.widths(blob)
+
+    def chip_table(d, k, side):
+        """chip k's main (side 0) or preprocessed (side 1) table on the device, [cols, rows]"""
+        off = sum(h * w[side] for h, w in zip(heights[:k], wd[:k]))
+        return d[off:off + heights[k] * wd[k][side]].view(-1, heights[k])
+
+    def host(t):
+        return np.ascontiguousarray(t.cpu().numpy().view(np.uint32))
+    pv = M.PV
     lib = Lib(0)
     mach = lib.machine_create(blob)
-    pts = [(p.view(-1, sp.h).cpu().numpy().view(np.uint32)) for p, sp in zip(preps, specs) if p is not None]
-    pr = lib.jagged_commit(pts)[1] if pts else None
+    pr = lib.jagged_commit_dense(d_prep, prep_rows, prep_cols)[1] if d_prep is not None else None
     assert lib.debug_constraints_words(mach, pr, dense, heights, pv).tolist() == [0]
     assert lib.debug_interactions_words(mach, pr, dense, heights).tolist() == [0, 0, 0]
     k = int(np.argmax(heights)); row = heights[k] - 5
-    off = sum(h * (6 * sp.g + (1 if sp.wp else 0) + sp.extra) for h, sp in zip(heights[:k], specs[:k]))
-    cell = off + 2 * heights[k] + row
-    dense[cell] = int((int(dense[cell].item()) + 1) % P)
+    cell = sum(h * w[0] for h, w in zip(heights[:k], wd[:k])) + 2 * heights[k] + row
+    _write_cell(dense, cell, int((int(dense[cell].item()) + 1) % P))
     rep = parse_constraint_report(lib.debug_constraints_words(mach, pr, dense, heights, pv))
-    main_k = dense[off:off + heights[k] * (6 * specs[k].g + (1 if specs[k].wp else 0) + specs[k].extra)].view(-1, heights[k])
-    one_row = np.ascontiguousarray(main_k[:, row:row + 1].cpu().numpy().view(np.uint32))
-    prep_row = None if preps[k] is None else np.ascontiguousarray(preps[k].view(-1, heights[k])[:, row:row + 1].cpu().numpy().view(np.uint32))
+    one_row = host(chip_table(dense, k, 0)[:, row:row + 1])
+    prep_row = host(chip_table(d_prep, k, 1)[:, row:row + 1]) if wd[k][1] else None
     # the oracle on chip k's row alone (a one-chip machine with that chip's program)
-    alone = DO.debug_constraints(_one_chip_blob(blob, k), [1], [one_row], [prep_row], pv)
+    alone = DO.debug_constraints(SA.machine_blob([M.chip_segments(blob)[k][2]]), [1], [one_row], [prep_row], pv)
     want = parse_constraint_report(alone)
     assert list(rep) == [k] and rep[k]["n_failing_rows"] == 1 and rep[k]["rows"] == {row: want[0]["rows"][0]}
-    dense[cell] = int((int(dense[cell].item()) - 1) % P)
+    _write_cell(dense, cell, int((int(dense[cell].item()) - 1) % P))
     # one chip's receive made unbalanced in the blob (the smallest chip with interactions, so that the oracle runs on it alone)
     progs, inters = _blob_segments(blob)
     c = min((i for i in range(len(specs)) if heights[i] and inters[i][0]), key=lambda i: heights[i])
@@ -291,11 +282,9 @@ def test_full_size_s2c_shard():
     mach2 = lib.machine_create(SA.machine_blob_with_interactions(progs, inters2))
     got = parse_interaction_report(lib.debug_interactions_words(mach2, pr, dense, heights, max_keys=1 << 17))
     lib.machine_free(mach2)
-    offc = sum(h * (6 * sp.g + (1 if sp.wp else 0) + sp.extra) for h, sp in zip(heights[:c], specs[:c]))
-    main_c = dense[offc:offc + heights[c] * (6 * specs[c].g + (1 if specs[c].wp else 0) + specs[c].extra)].view(-1, heights[c])
-    prep_c = None if preps[c] is None else preps[c].view(-1, heights[c]).cpu().numpy().view(np.uint32)
+    prep_c = host(chip_table(d_prep, c, 1)) if wd[c][1] else None
     want = parse_interaction_report(DO.debug_interactions(SA.machine_blob_with_interactions([progs[c]], [inters2[c]]), [heights[c]],
-                                                         [main_c.cpu().numpy().view(np.uint32)], [prep_c], max_keys=1 << 17))
+                                                         [host(chip_table(dense, c, 0))], [prep_c], max_keys=1 << 17))
     # the same unbalanced keys and nets; chip c carries the whole net.  A key can also occur (balanced) in other chips - the synthetic
     # traces share small values such as 0 between chips - and those chips are listed with net 0, possibly as the first occurrence.
     assert 0 < want["n_unbalanced"] == got["n_unbalanced"] == len(want["keys"]) == len(got["keys"])
@@ -310,8 +299,3 @@ def test_full_size_s2c_shard():
     lib.jagged_round_free(pr) if pr is not None else None
     lib.machine_free(mach)
     lib.close()
-
-
-def _one_chip_blob(blob, k):
-    """chip k's constraint program as a one-chip machine without interactions"""
-    return SA.machine_blob([_blob_segments(blob)[0][k]])

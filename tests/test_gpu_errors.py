@@ -3,8 +3,9 @@ of reading out of bounds, hanging or silently accepting bad input — the refere
 import numpy as np
 import pytest
 
+from tests import gpu_prove as GP
+from tests import machines as M
 from tests import oracle_lib as O
-from tests.test_oracle import _synth_machine_gkr
 
 pytestmark = pytest.mark.gpu
 
@@ -19,7 +20,7 @@ def lib():
 
 def _machine(rng):
     spec = [(1024, 2, True), (256 + 32, 3, False), (2048, 1, True)]
-    return _synth_machine_gkr(rng, spec)
+    return M.spec_machine(rng, spec, names="Chip{:02d}")
 
 
 def test_machine_create_rejects_malformed_blobs(lib):
@@ -63,11 +64,10 @@ def test_prove_shard_capacity_error_leaves_the_transcript_untouched(lib):
     proves from the same transcript)"""
     from sp1_b200.lib import Sp1B200Error
     rng = np.random.default_rng(2)
-    blob, heights, mains, preps, pv = _machine(rng)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
+    blob, heights, mains, preps, pv, names = _machine(rng)
     mach = lib.machine_create(blob)
-    _, prep_round = lib.jagged_commit([p for p in preps if p is not None])
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+    _, prep_round = GP.commit_prep(lib, preps)
+    dense = M.dense_main(mains)
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 5))
     st = ch.st.copy()
     with pytest.raises(Sp1B200Error, match="capacity"):
@@ -84,10 +84,9 @@ def test_prove_shard_capacity_error_leaves_the_transcript_untouched(lib):
 def test_shape_errors_are_reported(lib):
     from sp1_b200.lib import Sp1B200Error
     rng = np.random.default_rng(3)
-    blob, heights, mains, preps, pv = _machine(rng)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
+    blob, heights, mains, preps, pv, names = _machine(rng)
     mach = lib.machine_create(blob)
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+    dense = M.dense_main(mains)
     st = O.Challenger().st.copy()
     # preprocessed round missing although the machine has preprocessed columns
     with pytest.raises(Sp1B200Error, match="preprocessed"):
@@ -96,7 +95,7 @@ def test_shape_errors_are_reported(lib):
     with pytest.raises(Sp1B200Error, match="rows"):
         lib.jagged_commit_dense(np.zeros(8, np.uint32), [1 << 12], [1])
     # too few public values for the programs' LOAD_PUBLIC indices
-    _, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+    _, prep_round = GP.commit_prep(lib, preps)
     with pytest.raises(Sp1B200Error, match="public value"):
         lib.prove_shard(mach, prep_round, dense, heights, names, pv[:0], st)
     lib.jagged_round_free(prep_round)
@@ -116,16 +115,15 @@ def test_repeated_contexts_and_proofs_do_not_leak_device_memory():
     import torch
     from sp1_b200 import Lib
     rng = np.random.default_rng(4)
-    blob, heights, mains, preps, pv = _machine(rng)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+    blob, heights, mains, preps, pv, names = _machine(rng)
+    dense = M.dense_main(mains)
     torch.cuda.synchronize()
     used = []
     ref = None
     for it in range(6):
         L = Lib(0, log_stacking_height=10, max_log_row_count=11, num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
         mach = L.machine_create(blob)
-        _, prep_round = L.jagged_commit([p for p in preps if p is not None])
+        _, prep_round = GP.commit_prep(L, preps)
         for _ in range(3):
             w = L.prove_shard(mach, prep_round, dense, heights, names, pv, O.Challenger().st.copy())
             if ref is None:

@@ -2,9 +2,9 @@
 protocol parameters: stacking height 2^21, 124 queries, 16 + 5 + 12 proof-of-work bits): the oracle cannot PROVE this size in test
 time, but the restated reference verifier (ShardVerifier::verify_shard, run by the oracle from the proof words alone) must accept the
 proof the CUDA library produces, end in the prover's challenger state, and reject it after a one-bit change."""
-import numpy as np
 import pytest
 
+from tests import machines as M
 from tests import oracle_lib as O
 
 pytestmark = pytest.mark.gpu
@@ -14,30 +14,19 @@ pytestmark = pytest.mark.gpu
 def test_full_size_gpu_proof_is_accepted_by_the_restated_reference_verifier(workload):
     import torch
     from sp1_b200 import Lib
-    from sp1_b200 import synth_air as SA
     from sp1_b200 import workload as W
     from sp1_b200.lib import HostChallenger
+    from tools.device_traces import device_traces
 
-    dev = torch.device("cuda", 0)
     mach = W.synthetic_machine(workload, seed=42)
     specs, names = mach["specs"], mach["names"]
-    heights = [s_[0] for s_ in specs]
-    pv0 = 12345
-    pv = O.to_monty(np.array([pv0, 5, 6, 7]))
-    mains, preps = [], []
-    for i, sp in enumerate(specs):
-        m_, p_ = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, pv0, 7000 + i, dev, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        mains.append(m_)
-        if sp.wp:
-            preps.append(p_)
-    d_main = torch.cat(mains).contiguous()
-    d_prep = torch.cat(preps).contiguous()
-    del mains, preps
+    heights = [s_.h for s_ in specs]
+    pv = M.PV
+    d_main, d_prep, prep_rows, prep_cols = device_traces(specs, M.PV0, lambda i: 7000 + i, torch.device("cuda", 0))
     prm = W.params_of(workload)                           # core parameters, or the recursion ones for the compress-shape shard
     lib = Lib(device=0, **prm)
     machine = lib.machine_create(mach["blob"])
-    prep_rows = [s_.h for s_ in specs if s_.wp]
-    pc, h_prep = lib.jagged_commit_dense(d_prep, prep_rows, [1 + s_.extra_prep for s_ in specs if s_.wp])
+    pc, h_prep = lib.jagged_commit_dense(d_prep, prep_rows, prep_cols)
     st0 = HostChallenger().st.copy()
     st = st0.copy()
     words = lib.prove_shard(machine, h_prep, d_main, heights, names, pv, st)

@@ -3,9 +3,10 @@ the restated LogUpGkrVerifier::verify_logup_gkr on its own proof).  Bit-exact, i
 import numpy as np
 import pytest
 
+from tests import gpu_prove as GP
+from tests import machines as M
 from tests import oracle_lib as O
-from tests.machines import Chip, first_diff, n_interactions, spec_machine
-from tests.test_oracle import _synth_machine_gkr
+from tests.machines import Chip, first_diff, full_table_spec, n_interactions, shard_diff, spec_machine
 
 pytestmark = pytest.mark.gpu
 
@@ -18,18 +19,15 @@ pytestmark = pytest.mark.gpu
     ([(4096, 2, True), (1000, 3, False), (0, 1, False), (2048 + 32, 5, False)], 13),
 ])
 def test_logup_gkr_matches_oracle(spec, mlr):
-    import torch
     from sp1_b200 import Lib
     rng = np.random.default_rng(950 + mlr)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
+    blob, heights, mains, preps, pv, _ = spec_machine(rng, spec)
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
     och = ch.clone()
     owords = O.gkr_prove_verify(blob, heights, mains, preps, mlr, och, gkr_pow_bits=6)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21), gkr_pow_bits=6)
     mach = lib.machine_create(blob)
-    d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
-    d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
-    torch.cuda.synchronize()
+    d_mains, d_preps = _upload(mains, preps)
     st = ch.st.copy()
     words = lib.logup_gkr(mach, heights, d_mains, d_preps, st)
     assert words.size == owords.size, (words.size, owords.size)
@@ -42,39 +40,30 @@ def test_logup_gkr_matches_oracle(spec, mlr):
 
 def test_logup_gkr_and_whole_shard_with_silent_chips():
     """chips that carry constraints but no LogUp interactions, absent chips, tiny heights: GKR alone and the whole shard proof"""
-    import torch
     from sp1_b200 import Lib
-    from tests.test_oracle import GKR_EDGE_CASES, _synth_machine_gkr_custom
-    for spec, silent, mlr in GKR_EDGE_CASES:
+    for spec, silent, mlr in M.GKR_EDGE_CASES:
         rng = np.random.default_rng(960 + mlr)
-        blob, heights, mains, preps, pv = _synth_machine_gkr_custom(rng, spec, silent)
+        blob, heights, mains, preps, pv, names = spec_machine(rng, M.silent(spec, silent), names="Chip{:02d}")
         ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
         och = ch.clone()
         owords = O.gkr_prove_verify(blob, heights, mains, preps, mlr, och, gkr_pow_bits=4)
         log_stack = min(mlr, 4)
         lib = Lib(0, max_log_row_count=mlr, log_stacking_height=log_stack, gkr_pow_bits=4, num_queries=4, pow_bits=3, batch_pow_bits=2)
         mach = lib.machine_create(blob)
-        d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
-        d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
-        torch.cuda.synchronize()
+        d_mains, d_preps = _upload(mains, preps)
         st = ch.st.copy()
         words = lib.logup_gkr(mach, heights, d_mains, d_preps, st)
         assert words.size == owords.size and (words == owords).all()
         assert (st == och.st).all()
         # whole shard on the same machine
-        names = [f"Chip{i:02d}" for i in range(len(heights))]
         c2 = O.Challenger(); c2.observe(O.rand_field(rng, 5))
         oc2 = c2.clone()
         opc, ow = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, oc2, num_queries=4, pow_bits=3,
                                        batch_pow_bits=2, gkr_pow_bits=4)
-        prep_tabs = [p for p in preps if p is not None]
-        prep_round = None
-        if prep_tabs:
-            pc, prep_round = lib.jagged_commit(prep_tabs)
-            assert (pc == opc).all()
-        dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+        pc, prep_round = GP.commit_prep(lib, preps)
+        assert (pc == opc).all()
         st2 = c2.st.copy()
-        w2 = lib.prove_shard(mach, prep_round, dense, heights, names, pv, st2)
+        w2 = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st2)
         assert w2.size == ow.size and (w2 == ow).all() and (st2 == oc2.st).all()
         if prep_round is not None:
             lib.jagged_round_free(prep_round)
@@ -168,7 +157,6 @@ def test_logup_gkr_and_whole_shard_two_row_variables(case):
     """max_log_row_count = 2 is the only use of gkr_fix2_kernel<uint32_t, false>, of gkr_sum2_kernel<uint32_t> with two = 0 and of
     gkr_first_level_kernel without level 2: LogUp-GKR alone and the whole shard"""
     from sp1_b200 import Lib
-    from tests.machines import dense_main, shard_diff
     mlr, log_stack = 2, 2
     seed = 990 + case
     blob, heights, mains, preps, pv, names = spec_machine(np.random.default_rng(seed), MLR2_CASES[case])
@@ -179,28 +167,15 @@ def test_logup_gkr_and_whole_shard_two_row_variables(case):
     ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(seed + 2), 9))
     och = ch.clone()
     opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, **prm)
-    pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+    pc, prep_round = GP.commit_prep(lib, preps)
     assert (pc == opc).all(), "preprocessed commitment differs from the oracle"
     st = ch.st.copy()
-    words = lib.prove_shard(mach, prep_round, dense_main(mains), heights, names, pv, st)
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st)
     assert words.size == owords.size and (words == owords).all(), shard_diff(words, owords)
     assert (st == och.st).all(), "final challenger state differs from the oracle"
     lib.jagged_round_free(prep_round)
     lib.machine_free(mach)
     lib.close()
-
-
-def full_table_spec(n_chips, seed, absent=True):
-    """n_chips tiny chips with varied heights (1 included, and 0 when `absent`), some with preprocessed columns or filler columns,
-    light and calibrated interactions.  With absent=False every chip takes a slot of the GKR batch table."""
-    rng = np.random.default_rng(seed)
-    heights = ([0] if absent else []) + [1, 2, 3, 32]
-    heights += [int(x) for x in rng.integers(0 if absent else 1, 33, n_chips - len(heights))]
-    spec = []
-    for k, h in enumerate(heights):
-        vps = None if k % 3 == 0 else [int(x) for x in rng.integers(1, 13, 1 + k % 4)]
-        spec.append(Chip(h, 1 + k % 2, k % 4 == 1, None, int(k % 5 == 2), 1 if k % 8 == 5 else 0, vps))
-    return spec
 
 
 def test_logup_gkr_full_batch_table_then_one_chip_too_many():

@@ -1,9 +1,9 @@
 """GPU path against the committed golden fixtures (tests/golden/shard_proofs.json): no oracle call on this path — the CUDA
 library alone must reproduce the commitments, every proof word (SHA-256) and the final challenger state."""
-import numpy as np
 import pytest
 
 from tests import golden_util as G
+from tests import gpu_prove as GP
 
 pytestmark = pytest.mark.gpu
 
@@ -16,13 +16,9 @@ def test_gpu_reproduces_golden_shard_proofs(case):
               num_queries=case["num_queries"], pow_bits=case["pow_bits"], batch_pow_bits=case["batch_pow_bits"],
               gkr_pow_bits=case["gkr_pow_bits"])
     mach = lib.machine_create(blob)
-    prep_tabs = [p for p in preps if p is not None]
-    pc, prep_round = lib.jagged_commit(prep_tabs) if prep_tabs else (np.zeros(8, np.uint32), None)
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+    pc, prep_round = GP.commit_prep(lib, preps)
     st = ch.st.copy()
-    words = lib.prove_shard(mach, prep_round, dense, heights, names, pv, st)
-    if not prep_tabs:
-        pc = np.array(case["prep_commit"], np.uint32)   # no preprocessed round: nothing to compare
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st)
     G.check_words(case, pc, words, st)
     if prep_round is not None:
         lib.jagged_round_free(prep_round)
@@ -35,15 +31,12 @@ def test_gpu_reproduces_baseline_size_golden(case):
     """BASELINE-size bit parity (workloads S1 / S2, CORE protocol parameters): the code paths that only run at scale (fast RS-encode
     tiles, flat compress layers above 2^16, zerocheck pieces, 96-job GKR batches) against the oracle's committed proof."""
     from sp1_b200 import Lib
-    mach, heights, mains, preps, pv, ch = G.fullsize_inputs(case["workload"], case["seed"])
+    blob, heights, mains, preps, pv, names, ch = G.fullsize_inputs(case["workload"], case["seed"])
     lib = Lib(0)   # sp1b200_default_core_params
-    m = lib.machine_create(mach["blob"])
-    prep_tabs = [p for p in preps if p is not None]
-    pc, prep_round = lib.jagged_commit(prep_tabs)
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(x).reshape(-1) for x in mains if x.size]))
-    del mains
+    m = lib.machine_create(blob)
+    pc, prep_round = GP.commit_prep(lib, preps)
     st = ch.st.copy()
-    words = lib.prove_shard(m, prep_round, dense, heights, mach["names"], pv, st)
+    words = GP.prove(lib, m, prep_round, mains, heights, names, pv, st)
     G.check_words(case, pc, words, st)
     lib.jagged_round_free(prep_round)
     lib.machine_free(m)

@@ -1,42 +1,10 @@
 """GPU parity tests (jagged PCS): commit of chip tables, column claims, Hadamard + branching-program sumchecks and the
 stacked/BaseFold proof through the C ABI vs the oracle (which also runs the restated JaggedPcsVerifier)."""
-import numpy as np
 import pytest
 
-from tests import oracle_lib as O
+from tests.gpu_prove import check_jagged
 
 pytestmark = pytest.mark.gpu
-
-
-def _run(shapes_rounds, log_stack, max_log_rows, seed, nq=8, pow_bits=4, batch_bits=2):
-    from sp1_b200 import Lib
-    rng = np.random.default_rng(seed)
-    rounds = [O.random_tables(rng, s) for s in shapes_rounds]
-    z_row = O.rand_field(rng, (max_log_rows, 4))
-    ch = O.Challenger()
-    ch.observe(O.rand_field(rng, 3))
-    och = ch.clone()
-    ocommits, oclaims, oproof = O.jagged_prove_verify(rounds, log_stack, max_log_rows, z_row, och, num_queries=nq,
-                                                      pow_bits=pow_bits, batch_pow_bits=batch_bits)
-    lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=max_log_rows, num_queries=nq, pow_bits=pow_bits,
-              batch_pow_bits=batch_bits)
-    handles, claims = [], []
-    for i, tabs in enumerate(rounds):
-        commit, h = lib.jagged_commit(tabs)
-        assert (commit == ocommits[i]).all(), f"round {i} jagged commitment differs"
-        handles.append(h)
-        claims.append(lib.jagged_column_claims(h, z_row, sum(t.shape[0] for t in tabs)))
-    claims = np.concatenate(claims)
-    assert (claims == oclaims).all(), "column claims differ"
-    st = ch.st.copy()
-    proof = lib.jagged_prove(handles, z_row, claims, st)
-    assert proof.size == oproof.size, (proof.size, oproof.size)
-    bad = np.nonzero(proof != oproof)[0]
-    assert bad.size == 0, f"first differing proof words {bad[:8]} of {proof.size}"
-    assert (st == och.st).all()
-    for h in handles:
-        lib.jagged_round_free(h)
-    lib.close()
 
 
 @pytest.mark.parametrize("shapes,log_stack,mlr", [
@@ -46,10 +14,10 @@ def _run(shapes_rounds, log_stack, max_log_rows, seed, nq=8, pow_bits=4, batch_b
     ([[(32, 5), (17, 3)], [(20, 7)]], 4, 5),
 ])
 def test_jagged_matches_oracle_small(shapes, log_stack, mlr):
-    _run(shapes, log_stack, mlr, seed=600 + log_stack + mlr)
+    check_jagged(shapes, log_stack, mlr, seed=600 + log_stack + mlr)
 
 
 def test_jagged_matches_oracle_medium():
     # heights that are multiples of 32 (the reference's trace heights), two rounds, empty chips, 2^12 stacking height
     shapes = [[(4096, 3), (96, 17), (0, 5)], [(8192, 9), (2048 + 32, 40), (0, 3), (64, 13), (8192, 2)]]
-    _run(shapes, 12, 13, seed=77, nq=16, pow_bits=8, batch_bits=5)
+    check_jagged(shapes, 12, 13, seed=77, nq=16, pow_bits=8, batch_bits=5)

@@ -2,10 +2,10 @@
 rounds that never materialise the extension-field arrays, chosen by the library from the column alignment (2^K divides every
 column prefix sum), log_stacking_height and log_m.  K = 0 (some column starts at an odd index) is the same path with no trace
 rounds: the fold pass to level 0 sums round 0.  Each case names the K it reaches and is checked word for word against the
-oracle through the same harness as tests/test_gpu_jagged.py."""
+oracle through the same harness as tests/test_gpu_jagged.py (gpu_prove.check_jagged)."""
 import pytest
 
-from tests.test_gpu_jagged import _run
+from tests.gpu_prove import check_jagged
 
 pytestmark = pytest.mark.gpu
 
@@ -59,7 +59,7 @@ CASES = [
 @pytest.mark.parametrize("name,shapes,log_stack,mlr,k", CASES, ids=[c[0] for c in CASES])
 def test_jagged_trace_rounds_match_oracle(name, shapes, log_stack, mlr, k):
     assert trace_rounds_k(shapes, log_stack, mlr) == k, name
-    _run(shapes, log_stack, mlr, seed=900 + log_stack + mlr + k)
+    check_jagged(shapes, log_stack, mlr, seed=900 + log_stack + mlr + k)
 
 
 @pytest.mark.parametrize("shapes,log_stack,mlr,k", [
@@ -71,4 +71,4 @@ def test_jagged_trace_rounds_grid_loops(shapes, log_stack, mlr, k):
     # the fold pass to level K writes 2^(log_m - K) entries: 2^20 pairs for k0 and 2^19 for k1 and k5, so each of its 132 x 8
     # blocks of 256 threads loops over the grid; every warp of the trace-round passes walks a span of many blocks
     assert trace_rounds_k(shapes, log_stack, mlr) == k
-    _run(shapes, log_stack, mlr, seed=913 + k)
+    check_jagged(shapes, log_stack, mlr, seed=913 + k)

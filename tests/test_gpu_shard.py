@@ -4,34 +4,26 @@ must be identical."""
 import numpy as np
 import pytest
 
-from tests import oracle_lib as O
+from tests import gpu_prove as GP
 from tests import machines as M
-from tests.test_oracle import SHARD_SPECS, _synth_machine_gkr
+from tests import oracle_lib as O
 
 pytestmark = pytest.mark.gpu
 
 
 def _run(spec, log_stack, mlr, seed, nq=8, pow_bits=4, batch_bits=2, gkr_bits=3):
     from sp1_b200 import Lib
-    rng = np.random.default_rng(seed)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger(); ch.observe(O.rand_field(rng, 9))
+    blob, heights, mains, preps, pv, names, ch = M.shard_inputs(spec, seed)
     och = ch.clone()
     opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, num_queries=nq, pow_bits=pow_bits,
                                        batch_pow_bits=batch_bits, gkr_pow_bits=gkr_bits)
     lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, num_queries=nq, pow_bits=pow_bits, batch_pow_bits=batch_bits,
               gkr_pow_bits=gkr_bits)
     mach = lib.machine_create(blob)
-    prep_tabs = [p for p in preps if p is not None]
-    prep_round = None
-    if prep_tabs:
-        pc, prep_round = lib.jagged_commit(prep_tabs)
-        assert (pc == opc).all(), "preprocessed commitment differs"
-    parts = [np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]
-    main_dense = np.ascontiguousarray(np.concatenate(parts))
+    pc, prep_round = GP.commit_prep(lib, preps)
+    assert (pc == opc).all(), "preprocessed commitment differs"
     st = ch.st.copy()
-    words = lib.prove_shard(mach, prep_round, main_dense, heights, names, pv, st)
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st)
     assert words.size == owords.size, (words.size, owords.size, words[:6], owords[:6])
     bad = np.nonzero(words != owords)[0]
     assert bad.size == 0, f"first differing words {bad[:8]} of {words.size} (sections {owords[:6]})"
@@ -40,8 +32,7 @@ def _run(spec, log_stack, mlr, seed, nq=8, pow_bits=4, batch_bits=2, gkr_bits=3)
     # the same words, names and heights (tests/test_wire.py covers the format itself on the CPU)
     from sp1_b200 import lib as PL
     from tests import bincode_ref as BR
-    from tests.test_wire import _widths
-    w = _widths(blob)
+    w = M.widths(blob)
     prm = dict(log_stacking_height=log_stack, max_log_row_count=mlr, num_queries=nq, pow_bits=pow_bits, batch_pow_bits=batch_bits, gkr_pow_bits=gkr_bits)
     data = PL.shard_proof_to_bincode(words, names, heights, [a for a, _ in w], [b for _, b in w], **prm)
     flat, dn, dh = BR.flatten(BR.decode_shard_proof(data))
@@ -52,7 +43,7 @@ def _run(spec, log_stack, mlr, seed, nq=8, pow_bits=4, batch_bits=2, gkr_bits=3)
     lib.close()
 
 
-@pytest.mark.parametrize("spec,log_stack,mlr", SHARD_SPECS)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
 def test_prove_shard_matches_oracle(spec, log_stack, mlr):
     _run(spec, log_stack, mlr, seed=1200 + mlr)
 
@@ -68,12 +59,11 @@ def test_prove_shard_from_upload_slots_is_identical():
     from sp1_b200 import Lib
     rng = np.random.default_rng(4242)
     spec = [(2048, 2, True), (512 + 32, 3, False), (4096, 1, False)]
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    lib = Lib(0, log_stacking_height=11, max_log_row_count=12, num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
+    blob, heights, mains, preps, pv, names = M.spec_machine(rng, spec, names="Chip{:02d}")
+    lib = Lib(0, log_stacking_height=11, max_log_row_count=12, **M.SMALL)
     mach = lib.machine_create(blob)
-    _, prep_round = lib.jagged_commit([p for p in preps if p is not None])
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+    _, prep_round = GP.commit_prep(lib, preps)
+    dense = M.dense_main(mains)
     st0 = O.Challenger().st.copy()
     ref = lib.prove_shard(mach, prep_round, dense, heights, names, pv, st0.copy())
     pinned = torch.from_numpy(dense.view(np.int32)).pin_memory()
@@ -99,10 +89,7 @@ def test_prove_shard_replays_non_minimal_witnesses(skip):
     from sp1_b200 import Lib
     spec = [(1024, 2, True), (256 + 32, 3, False), (0, 1, False), (2048, 1, True)]
     log_stack, mlr, nq, pw, bpw, gpw = 10, 11, 8, 4, 2, 3
-    rng = np.random.default_rng(5150 + skip)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger(); ch.observe(O.rand_field(rng, 9))
+    blob, heights, mains, preps, pv, names, ch = M.shard_inputs(spec, 5150 + skip)
     L = O.lib()
     omin = ch.clone()
     _, wmin = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, omin, num_queries=nq, pow_bits=pw,
@@ -121,11 +108,10 @@ def test_prove_shard_replays_non_minimal_witnesses(skip):
     lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, num_queries=nq, pow_bits=pw, batch_pow_bits=bpw, gkr_pow_bits=gpw,
               grind_mode=1)
     mach = lib.machine_create(blob)
-    pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+    pc, prep_round = GP.commit_prep(lib, preps)
     assert (pc == opc).all()
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
     st = ch.st.copy()
-    words = lib.prove_shard(mach, prep_round, dense, heights, names, pv, st, replay=wl[:3])
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st, replay=wl[:3])
     assert words.size == owords.size
     bad = np.nonzero(words != owords)[0]
     assert bad.size == 0, f"first differing words {bad[:8]} of {words.size}"
@@ -144,15 +130,14 @@ def test_setup_and_prove_shard_equals_setup_then_prove():
     spec = [(1024, 2, True), (256 + 32, 3, False), (0, 1, False), (2048, 1, True)]
     log_stack, mlr, nq, pw, bpw, gpw = 10, 11, 8, 4, 2, 3
     rng = np.random.default_rng(8080)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
+    blob, heights, mains, preps, pv, names = M.spec_machine(rng, spec, names="Chip{:02d}")
     vk_tail = np.concatenate([O.rand_field(rng, 3 + 7 + 7), O.to_monty(np.array([0])), np.zeros(6, np.uint32)])   # pc_start, cumulative sum x, y, flag, padding
     lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, num_queries=nq, pow_bits=pw, batch_pow_bits=bpw, gkr_pow_bits=gpw)
     mach = lib.machine_create(blob)
     prep_tabs = [p for p in preps if p is not None]
     prep_dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in prep_tabs]))
     rows, cols = [p.shape[1] for p in prep_tabs], [p.shape[0] for p in prep_tabs]
-    dense = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m).reshape(-1) for m in mains if m.size]))
+    dense = M.dense_main(mains)
     st = HostChallenger().st.copy()
     pc, prep_round, words = lib.setup_and_prove_shard(mach, prep_dense, rows, cols, vk_tail, dense, heights, names, pv, st)
     # by hand
@@ -177,14 +162,11 @@ def test_setup_and_prove_shard_equals_setup_then_prove():
 
 # ---- the benchmark's shapes at reduced size, a full GKR batch table, and several contexts proving at once ------------------------------
 
-SMALL_PRM = dict(num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
-
-
 def _oracle_shard(inp, log_stack, mlr, seed):
     blob, heights, mains, preps, pv, names = inp
     ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(seed), 9))
     och = ch.clone()
-    opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, **SMALL_PRM)
+    opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, **M.SMALL)
     return ch.st.copy(), opc, owords, och.st.copy()
 
 
@@ -192,12 +174,12 @@ def _prove_and_compare(inp, log_stack, mlr, seed):
     from sp1_b200 import Lib
     blob, heights, mains, preps, pv, names = inp
     st0, opc, owords, ost = _oracle_shard(inp, log_stack, mlr, seed)
-    lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **SMALL_PRM)
+    lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **M.SMALL)
     mach = lib.machine_create(blob)
-    pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+    pc, prep_round = GP.commit_prep(lib, preps)
     assert (pc == opc).all(), "preprocessed commitment differs from the oracle"
     st = st0.copy()
-    words = lib.prove_shard(mach, prep_round, M.dense_main(mains), heights, names, pv, st)
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st)
     assert words.size == owords.size and (words == owords).all(), M.shard_diff(words, owords)
     assert (st == ost).all(), "final challenger state differs from the oracle"
     lib.jagged_round_free(prep_round)
@@ -217,8 +199,7 @@ def test_prove_shard_workload_machines_match_oracle(workload, mlr, log_stack):
 def test_prove_shard_full_batch_table():
     """96 chips, the most the LogUp-GKR batch table takes (tests/test_gpu_gkr.py checks that 97 is an error): every phase of the shard
     proof at that chip count, with tiny heights (0 and 1 included)"""
-    from tests.test_gpu_gkr import full_table_spec
-    inp = M.spec_machine(np.random.default_rng(1311), full_table_spec(96, 1321, absent=True))
+    inp = M.spec_machine(np.random.default_rng(1311), M.full_table_spec(96, 1321, absent=True))
     _prove_and_compare(inp, 5, 5, 1330)
 
 
@@ -242,9 +223,9 @@ def test_concurrent_contexts_prove_their_own_shards():
     oracle = [_oracle_shard(inp, ls, mlr, 1410 + k) for k, (inp, mlr, ls) in enumerate(jobs)]
     ctxs = []
     for (blob, heights, mains, preps, pv, names), mlr, ls in jobs:
-        lib = Lib(0, log_stacking_height=ls, max_log_row_count=mlr, **SMALL_PRM)
+        lib = Lib(0, log_stacking_height=ls, max_log_row_count=mlr, **M.SMALL)
         mach = lib.machine_create(blob)
-        pc, prep_round = lib.jagged_commit([p for p in preps if p is not None])
+        pc, prep_round = GP.commit_prep(lib, preps)
         ctxs.append((lib, mach, pc, prep_round))
     # half the contexts read their trace from device memory, half through the double-buffered upload slots from pinned host memory
     dense = [M.dense_main(inp[2]) for inp in inputs]

@@ -6,13 +6,13 @@ import threading
 import numpy as np
 import pytest
 
+from tests import gpu_prove as GP
 from tests import machines as M
 from tests import oracle_lib as O
-from tests.test_oracle import SHARD_SPECS, _synth_machine_gkr
+from tests.machines import ORACLE_LACKS, SMALL
 
 pytestmark = pytest.mark.gpu
 
-SMALL = dict(num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
 P = 0x7F000001
 
 
@@ -23,12 +23,13 @@ def _prove(inp, log_stack, mlr, seed, prm=SMALL, replay=None, **ctx):
     ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(seed), 9))
     lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **prm, **ctx)
     mach = lib.machine_create(blob)
-    prep_tabs = [p for p in preps if p is not None]
-    pc, prep_round = lib.jagged_commit(prep_tabs) if prep_tabs else (None, None)
+    pc, prep_round = GP.commit_prep(lib, preps)
     st = ch.st.copy()
-    words = lib.prove_shard(mach, prep_round, M.dense_main(mains), heights, names, pv, st, replay=replay)
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st, replay=replay)
     if prep_round is not None:
         lib.jagged_round_free(prep_round)
+    else:
+        pc = None   # the verifier takes no preprocessed commitment for a machine without preprocessed columns
     return dict(lib=lib, mach=mach, blob=blob, heights=list(heights), names=names, pc=pc, words=words, start=ch.st.copy(), final=st,
                 log_stack=log_stack, mlr=mlr, prm=prm)
 
@@ -39,8 +40,7 @@ def _close(c):
 
 
 def _spec_inp(spec, seed):
-    blob, heights, mains, preps, pv = _synth_machine_gkr(np.random.default_rng(seed), spec)
-    return blob, heights, mains, preps, pv, [f"Chip{i:02d}" for i in range(len(heights))]
+    return M.spec_machine(np.random.default_rng(seed), spec, names="Chip{:02d}")
 
 
 def _accept(c):
@@ -80,12 +80,7 @@ def _agree(c, capfd, words, heights=None, start=None, pc="same", what=""):
     return reason
 
 
-# verify_shard's checks of the jagged table shapes against the chips (shard.rs:506-523, :662-742): the oracle's restated verifier does
-# not make them, so where the library stops at one of them the oracle can only be required to reject as well
-ORACLE_LACKS = ("InvalidShape(preprocessed widths)", "InvalidShape(chip tables)")
-
-
-@pytest.mark.parametrize("spec,log_stack,mlr", SHARD_SPECS)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
 def test_accepts_small_machines(spec, log_stack, mlr):
     """max_log_row_count 3 and 7, machines with and without preprocessed columns, absent chips"""
     c = _prove(_spec_inp(spec, 2100 + mlr), log_stack, mlr, 2101)
@@ -108,8 +103,7 @@ def test_accepts_workload_machines(workload):
 
 
 def test_accepts_the_96_chip_machine():
-    from tests.test_gpu_gkr import full_table_spec
-    c = _prove(M.spec_machine(np.random.default_rng(2130), full_table_spec(96, 2131, absent=True)), 5, 5, 2132)
+    c = _prove(M.spec_machine(np.random.default_rng(2130), M.full_table_spec(96, 2131, absent=True)), 5, 5, 2132)
     _accept(c)
     _close(c)
 
@@ -221,7 +215,7 @@ def test_other_context_parameters_reject_or_fail_to_parse(other):
 
 
 def test_four_contexts_on_four_threads():
-    cases = [_prove(_spec_inp(spec, 2180 + k), ls, mlr, 2190 + k) for k, (spec, ls, mlr) in enumerate(SHARD_SPECS + [SHARD_SPECS[2]])]
+    cases = [_prove(_spec_inp(spec, 2180 + k), ls, mlr, 2190 + k) for k, (spec, ls, mlr) in enumerate(M.SHARD_SPECS + [M.SHARD_SPECS[2]])]
     bad = cases[3]["words"].copy(); bad[_sections(bad)[3][0] + 5] = (int(bad[_sections(bad)[3][0] + 5]) + 1) % P
     inputs = [c["words"] for c in cases[:3]] + [bad]
     results, errors = [None] * 4, []
@@ -280,11 +274,10 @@ def test_accepts_the_golden_shard_proofs(case):
     lib = Lib(0, log_stacking_height=case["log_stacking_height"], max_log_row_count=case["max_log_row_count"], num_queries=case["num_queries"],
               pow_bits=case["pow_bits"], batch_pow_bits=case["batch_pow_bits"], gkr_pow_bits=case["gkr_pow_bits"])
     mach = lib.machine_create(blob)
-    prep_tabs = [p for p in preps if p is not None]
-    pc, prep_round = lib.jagged_commit(prep_tabs) if prep_tabs else (None, None)
+    pc, prep_round = GP.commit_prep(lib, preps)
     st = ch.st.copy()
-    words = lib.prove_shard(mach, prep_round, M.dense_main(mains), heights, names, pv, st)
-    G.check_words(case, pc if pc is not None else np.array(case["prep_commit"], np.uint32), words, st)
+    words = GP.prove(lib, mach, prep_round, mains, heights, names, pv, st)
+    G.check_words(case, pc, words, st)
     verdict, vst = lib.verify_shard(mach, pc, heights, names, words, ch.st.copy())
     assert verdict == 0
     assert [int(x) for x in vst] == case["final_challenger"]
@@ -296,9 +289,8 @@ def test_accepts_the_golden_shard_proofs(case):
 
 def _eval_fields(w, c):
     """word offsets of the evaluation proof's fields (layout: sp1_b200/csrc/proof_layout.hpp)"""
-    from tests.test_wire import _widths
     ls, nq = c["log_stack"], c["prm"]["num_queries"]
-    wd = _widths(c["blob"])
+    wd = M.widths(c["blob"])
     S = 1 << ls
     areas = [sum(h * p for h, (_, p) in zip(c["heights"], wd)), sum(h * m for h, (m, _) in zip(c["heights"], wd))]
     ncols = ([max(1, -(-areas[0] // S))] if any(p for _, p in wd) else []) + [max(1, -(-areas[1] // S))]
@@ -373,11 +365,10 @@ def test_rejects_a_jagged_layout_other_than_the_chip_heights():
     import torch
     from sp1_b200.lib import HostChallenger, verdict_name
     from tests.ext_field import EF
-    from tests.test_wire import _widths
     ls, mlr = 7, 8
     inp = _spec_inp([(32, 2, True), (96, 1, False), (100, 1, False)], 2210)
     blob, heights, mains, preps, pv, names = inp
-    wd = _widths(blob)
+    wd = M.widths(blob)
     area, S = sum(h * m for h, (m, _) in zip(heights, wd)), 1 << ls
     # a chip whose extra row keeps the main round's stacked column count (and so every section length) unchanged
     k = next(i for i in range(len(heights)) if not wd[i][1] and -(-(area + wd[i][0]) // S) == -(-area // S) and heights[i] < 1 << mlr)
@@ -386,8 +377,7 @@ def test_rejects_a_jagged_layout_other_than_the_chip_heights():
     lib, mach = c["lib"], c["mach"]
     tabs = [np.ascontiguousarray(m) for m in mains]
     tabs[k] = np.concatenate([tabs[k], np.zeros((tabs[k].shape[0], 1), np.uint32)], axis=1)   # [cols, rows + 1]
-    prep_tabs = [p for p in preps if p is not None]
-    pc, prep_round = lib.jagged_commit(prep_tabs)
+    pc, prep_round = GP.commit_prep(lib, preps)
     commit, main_round = lib.jagged_commit(tabs)
     st = HostChallenger(c["start"])
     st.observe(pv); st.observe(commit); st.observe(O.to_monty(np.array([len(names)])))

@@ -9,55 +9,37 @@ import numpy as np
 import pytest
 
 from tests import core_chain as CC
+from tests import gpu_prove as GP
 from tests import machines as M
 from tests import oracle_lib as O
-from tests.test_septic import START, curve_add
 
 pytestmark = pytest.mark.gpu
-
-SMALL = dict(num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
-WITH_PREP = [M.Chip(256, 2, True), M.Chip(64 + 8, 3, False), M.Chip(0, 1, False), M.Chip(128, 1, True)]
-NO_PREP = [M.Chip(128, 2, False), M.Chip(32, 1, False)]
 
 V_INVALID_SHARD_PROOF = 45
 
 
-def _specs_machine(chips, mlr):
+def _specs_machine(chips):
+    """-> (blob, heights, names, chips); every shard draws its traces with M.traces"""
     blob, heights, _, _, _, names = M.spec_machine(np.random.default_rng(1), chips)
-    specs = [(c.h, c.g, c.wp, c.extra, c.extra_prep) for c in (M.Chip(*c) for c in chips)]
-    return blob, heights, names, specs
+    return blob, heights, names, chips
 
 
 def _workload_machine(workload, mlr, scale):
     from sp1_b200 import workload as W
     mach = W.synthetic_machine(workload, seed=42, max_log_rows=mlr, scale=scale)
-    specs = [(s.h, s.g, s.wp, s.extra, s.extra_prep) for s in mach["specs"]]
-    return mach["blob"], [s.h for s in mach["specs"]], list(mach["names"]), specs
-
-
-def _traces(specs, seed, pv0):
-    """the same traces for every shard (so the preprocessed tables agree), with the shard's own public value 0"""
-    from sp1_b200 import synth_air as SA
-    rng = np.random.default_rng(seed)
-    mains, preps = [], []
-    for h, g, wp, extra, extra_prep in specs:
-        m, p = SA.synth_trace(rng, h, g, wp, pv0, extra_cols=extra, extra_prep=extra_prep)
-        mains.append(m); preps.append(p)
-    return mains, preps
+    return mach["blob"], [s.h for s in mach["specs"]], list(mach["names"]), mach["specs"]
 
 
 class Core:
     """a context + machine proving shards of one program under one verifying key"""
 
-    def __init__(self, machine, log_stack, mlr, prm=SMALL, seed=5, **ctx):
+    def __init__(self, machine, log_stack, mlr, prm=M.SMALL, seed=5, **ctx):
         from sp1_b200 import Lib
         self.blob, self.heights, self.names, self.specs = machine
         self.log_stack, self.mlr, self.prm, self.seed = log_stack, mlr, prm, seed
         self.lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **prm, **ctx)
         self.mach = self.lib.machine_create(self.blob)
-        _, preps = _traces(self.specs, seed, 0)
-        tabs = [p for p in preps if p is not None]
-        self.pc, self.prep_round = self.lib.jagged_commit(tabs) if tabs else (np.zeros(8, np.uint32), None)
+        self.pc, self.prep_round = GP.commit_prep(self.lib, M.traces(self.specs, seed, 0)[1])
 
     def start(self, tail):
         from sp1_b200.lib import HostChallenger
@@ -69,10 +51,9 @@ class Core:
         tail = O.to_monty(np.array(tail))
         words, finals = [], []
         for pv in pvs:
-            mains, _ = _traces(self.specs, self.seed, CC.pv0_of(pv))
+            mains, _ = M.traces(self.specs, self.seed, CC.pv0_of(pv))
             st = self.start(tail)
-            words.append(self.lib.prove_shard(self.mach, self.prep_round, M.dense_main(mains), self.heights, self.names,
-                                              O.to_monty(np.array(pv)), st))
+            words.append(GP.prove(self.lib, self.mach, self.prep_round, mains, self.heights, self.names, O.to_monty(np.array(pv)), st))
             finals.append(st)
         return words, finals, tail
 
@@ -101,14 +82,14 @@ def _accept(c, n, seed, **kw):
 
 @pytest.mark.parametrize("n", [1, 2, 5])
 def test_accepts_with_preprocessed_columns(n):
-    c = Core(_specs_machine(WITH_PREP, 9), 8, 9)
+    c = Core(_specs_machine(M.WITH_PREP), 8, 9)
     _accept(c, n, 100 + n)
     c.close()
 
 
 @pytest.mark.parametrize("n", [1, 2, 5])
 def test_accepts_without_preprocessed_columns(n):
-    c = Core(_specs_machine(NO_PREP, 8), 7, 8)
+    c = Core(_specs_machine(M.NO_PREP), 7, 8)
     assert not c.pc.any()
     _accept(c, n, 110 + n, non_execution=1 if n > 2 else None)
     c.close()
@@ -121,108 +102,12 @@ def test_accepts_workload_machines(workload, n):
     c.close()
 
 
-# (name, mutation of the valid 3-shard chain with a non-execution shard 1, expected verdict, expected shard)
-def _set(s, name, vals):
-    return lambda pvs, tail: CC.setf(pvs[s], name, vals)
-
-
-def _m_len(pvs, tail):
-    pvs[1][:] = pvs[1][:186]
-
-
-def _m_never(field):
-    def f(pvs, tail):
-        for pv in pvs:
-            CC.setf(pv, "previous_" + field, [0, 0, 0]); CC.setf(pv, "last_" + field, [0, 0, 0])
-    return f
-
-
-def _m_commit(field):
-    def f(pvs, tail):
-        for pv in pvs:
-            CC.setf(pv, "prev_" + field, 0); CC.setf(pv, field, 0)
-    return f
-
-
-def _m_ts_changed(pvs, tail):
-    last = CC.getf(pvs[1], "last_timestamp"); last[3] += 1
-    CC.setf(pvs[1], "last_timestamp", last); CC.setf(pvs[2], "initial_timestamp", last)
-
-
-def _m_pc_nonexec(pvs, tail):
-    CC.setf(pvs[1], "next_pc", [7, 7, 7]); CC.setf(pvs[2], "pc_start", [7, 7, 7])
-
-
-def _m_exit_nonexec(pvs, tail):
-    CC.setf(pvs[1], "exit_code", 3); CC.setf(pvs[2], "prev_exit_code", 3); CC.setf(pvs[2], "exit_code", 3)
-
-
-def _m_exit_changed(pvs, tail):
-    CC.setf(pvs[0], "exit_code", 3)
-    for s in (1, 2):
-        CC.setf(pvs[s], "prev_exit_code", 3); CC.setf(pvs[s], "exit_code", 3)
-    CC.setf(pvs[2], "exit_code", 4)
-
-
-def _m_digest(pvs, tail):
-    from tests.test_septic import DUMMY
-    g = CC.getf(pvs[1], "global_cumulative_sum")
-    p = (g[:7], g[7:])
-    q = curve_add(p, DUMMY)
-    CC.setf(pvs[1], "global_cumulative_sum", list(q[0]) + list(q[1]))
-
-
-def _m_exceptional(pvs, tail):
-    tail[3:17] = list(START[0]) + list(START[1])
-
-
-def _m_bump(s, name, k=0):
-    def f(pvs, tail):
-        v = CC.getf(pvs[s], name); v[k] = (v[k] + 1) % O.P
-        CC.setf(pvs[s], name, v)
-    return f
-
-
-PV_CASES = [
-    ("length", _m_len, 46, 1),
-    ("first shard twice", _set(2, "is_first_execution_shard", 1), 47, 2),
-    ("first shard not boolean", _set(1, "is_first_execution_shard", 2), 48, 1),
-    ("first shard not set", _set(0, "is_first_execution_shard", 0), 49, 3),
-    ("initial timestamp", _m_bump(2, "initial_timestamp", 3), 50, 2),
-    ("timestamp unchanged on an execution shard", _set(1, "is_execution_shard", 1), 51, 1),
-    ("timestamp changed on a non-execution shard", _m_ts_changed, 52, 1),
-    ("pc_start != vk.pc_start", _m_bump(0, "pc_start", 1), 53, 0),
-    ("pc_start != prev_next_pc", _m_bump(2, "pc_start", 0), 54, 2),
-    ("pc changed on a non-execution shard", _m_pc_nonexec, 55, 1),
-    ("not halted", _set(2, "next_pc", [5, 0, 0]), 56, 3),
-    ("prev_exit_code", _set(0, "prev_exit_code", 1), 57, 0),
-    ("exit code changed on a non-execution shard", _m_exit_nonexec, 58, 1),
-    ("exit code changed twice", _m_exit_changed, 59, 2),
-    ("proof nonce", _m_bump(2, "proof_nonce", 1), 60, 2),
-    ("previous_init_addr", _m_bump(1, "previous_init_addr"), 61, 1),
-    ("previous_finalize_addr", _m_bump(1, "previous_finalize_addr", 2), 62, 1),
-    ("previous_init_page_idx", _m_bump(2, "previous_init_page_idx"), 63, 2),
-    ("previous_finalize_page_idx", _m_bump(2, "previous_finalize_page_idx", 1), 64, 2),
-    ("untrusted programs flag", _set(0, "is_untrusted_programs_enabled", 1), 65, 0),
-    ("zero address never initialized", _m_never("init_addr"), 66, 3),
-    ("zero address never finalized", _m_never("finalize_addr"), 67, 3),
-    ("committed value digest", _m_bump(1, "prev_committed_value_digest", 5), 68, 1),
-    ("deferred proofs digest", _m_bump(2, "prev_deferred_proofs_digest", 7), 69, 2),
-    ("commit syscall", _set(0, "prev_commit_syscall", 1), 70, 0),
-    ("commit deferred syscall", _set(1, "prev_commit_deferred_syscall", 0), 71, 1),
-    ("COMMIT never called", _m_commit("commit_syscall"), 72, 3),
-    ("COMMIT_DEFERRED_PROOFS never called", _m_commit("commit_deferred_syscall"), 73, 3),
-    ("global cumulative sum", _m_digest, 74, 3),
-    ("exceptional point addition", _m_exceptional, 75, 0),
-]
-
-
 def test_every_public_value_check():
     """one chain per reason, proved with the faulty public values (not patched after proving): exactly that verdict at that shard"""
     from sp1_b200.lib import verdict_name
-    c = Core(_specs_machine(NO_PREP, 8), 7, 8)
+    c = Core(_specs_machine(M.NO_PREP), 7, 8)
     seen = set()
-    for name, mutate, want, shard in PV_CASES:
+    for name, mutate, want, shard in CC.PV_CASES:
         pvs, tail = CC.chain(3, 140, non_execution=1)
         mutate(pvs, tail)
         words, _, mtail = c.prove(pvs, tail)
@@ -248,7 +133,6 @@ def test_corrupted_shard_matches_verify_shard_and_the_oracle(capfd):
     InvalidShardProof at shard 1 with the inner verdict sp1b200_verify_shard gives on that shard alone (and the oracle's first
     failing check), or a parse error from both calls"""
     from sp1_b200.lib import Sp1B200Error, verdict_name
-    from tests.test_gpu_verify import ORACLE_LACKS
     c, words, _, tail = _tinyc_chain()
     start = c.start(tail)
     assert c.verify(words, tail)[0] == 0
@@ -272,10 +156,10 @@ def test_corrupted_shard_matches_verify_shard_and_the_oracle(capfd):
             continue
         assert (v, s, sv) == (V_INVALID_SHARD_PROOF, 1, single), (i, verdict_name(v), s, verdict_name(sv), verdict_name(single))
         outcomes.add(verdict_name(single))
-        if len(outcomes) <= 6 and verdict_name(single) not in ORACLE_LACKS:
+        if len(outcomes) <= 6 and verdict_name(single) not in M.ORACLE_LACKS:
             capfd.readouterr()
             o = O.Challenger(); o.st[:] = start
-            r = O.verify_shard(c.blob, c.heights, c.names, c.log_stack, c.mlr, o, c.pc if c.prep_round is not None else None, bad, **c.prm)
+            r = O.verify_shard(c.blob, c.heights, c.names, c.log_stack, c.mlr, o, c.pc, bad, **c.prm)
             assert r == -1 and capfd.readouterr().err.strip().rsplit(": ", 1)[-1] == verdict_name(single), i
     assert len(outcomes) >= 4, outcomes
     c.close()
@@ -321,7 +205,7 @@ def test_threads_and_batching_do_not_change_results():
 def test_malformed_arguments_are_errors_and_leave_the_context_usable():
     import ctypes as C
     from sp1_b200.lib import Sp1B200Error, _ptr
-    c = Core(_specs_machine(NO_PREP, 8), 7, 8)
+    c = Core(_specs_machine(M.NO_PREP), 7, 8)
     pvs, tail = CC.chain(2, 170)
     words, _, mtail = c.prove(pvs, tail)
     with pytest.raises(Sp1B200Error, match="n_vk_tail"):
@@ -339,7 +223,7 @@ def test_malformed_arguments_are_errors_and_leave_the_context_usable():
 
 
 def test_two_contexts_on_two_threads():
-    cores = [Core(_specs_machine(WITH_PREP, 9), 8, 9), Core(_specs_machine(NO_PREP, 8), 7, 8)]
+    cores = [Core(_specs_machine(M.WITH_PREP), 8, 9), Core(_specs_machine(M.NO_PREP), 7, 8)]
     jobs = []
     for i, c in enumerate(cores):
         pvs, tail = CC.chain(3, 180 + i)

@@ -4,7 +4,6 @@ import numpy as np
 import pytest
 
 from tests.machines import Chip, oracle_zerocheck, product_zerocheck, spec_machine, workload_machine
-from tests.test_oracle import _synth_machine
 
 pytestmark = pytest.mark.gpu
 
@@ -17,19 +16,21 @@ pytestmark = pytest.mark.gpu
     ([(4096, 2, True), (1000, 12, False), (0, 1, False), (2048 + 32, 5, False)], 13),
     # long-lived intermediates: register pressure ~ groups -> every register-file tier (<= 8, <= 16, <= 32 in shared memory,
     # local-memory fallback above) in one proof, next to a flat chip
-    ([(512, 6, False, True), (300, 14, True, True), (1024, 28, False, True), (96, 40, False, True), (2048, 3, True)], 12),
+    ([Chip(512, 6, False, deep=True), Chip(300, 14, True, deep=True), Chip(1024, 28, False, deep=True), Chip(96, 40, False, deep=True),
+      (2048, 3, True)], 12),
     # the reference's largest register tiers (sys/lib/zerocheck/sequential.cu:298-335: 256 / 512 / 1024 registers): programs whose
     # re-scheduled live set is ~250, ~500 and ~1000 registers -> the global-memory register file, next to a shared-memory chip;
     # heights on both sides of the "pieces" threshold (<= 16 blocks of 128 row pairs)
-    ([(192, 250, False, True), (64, 500, True, True), (8192, 3, True), (96, 1000, False, True), (6000, 300, False, True)], 13),
+    ([Chip(192, 250, False, deep=True), Chip(64, 500, True, deep=True), (8192, 3, True), Chip(96, 1000, False, deep=True),
+      Chip(6000, 300, False, deep=True)], 13),
 ])
 def test_zerocheck_matches_oracle(spec, mlr):
     from sp1_b200 import Lib
     rng = np.random.default_rng(900 + mlr)
-    blob, heights, mains, preps, pv = _synth_machine(rng, spec)
+    blob, heights, mains, preps, pv, _ = spec_machine(rng, spec, interactions=False)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21))
     mach = lib.machine_create(blob)
-    if any(len(s_) > 3 and s_[1] >= 250 for s_ in spec):
+    if any(Chip(*s_).deep and s_[1] >= 250 for s_ in spec):
         regs = [lib.machine_chip_regs(mach, k) for k in range(len(spec))]
         assert max(regs) > 900 and sorted(regs)[-2] > 450 and min(regs) <= 32, regs   # the tiers the case is meant to exercise
     _check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr)

@@ -5,6 +5,7 @@ import os
 import numpy as np
 import pytest
 
+from tests import machines as M
 from tests import oracle_lib as O
 
 P = O.P
@@ -236,19 +237,6 @@ def test_jagged_pcs_roundtrip(shapes_rounds, log_stack, max_log_rows):
     assert (proof == proof2).all() and (c1.st == c2.st).all() and (commits == commits2).all()
 
 
-def _synth_machine(rng, spec, pv0=12345):
-    """spec: list of (height, groups, with_prep[, deep])"""
-    from sp1_b200 import synth_air as SA
-    words, mains, preps, heights = [], [], [], []
-    for h, g, wp, *rest in spec:
-        w, _, _ = SA.synth_chip(g, wp, deep=bool(rest and rest[0]))
-        words.append(w)
-        m, p = SA.synth_trace(rng, h, g, wp, pv0)
-        mains.append(m); preps.append(p); heights.append(h)
-    pv = O.to_monty(np.array([pv0, 5, 6, 7]))
-    return SA.machine_blob(words), heights, mains, preps, pv
-
-
 @pytest.mark.parametrize("spec,mlr", [
     ([(8, 1, False)], 3),                                  # full-height chip
     ([(5, 1, False), (0, 2, False), (6, 1, True)], 3),     # odd height, empty chip, preprocessed column
@@ -258,7 +246,7 @@ def _synth_machine(rng, spec, pv0=12345):
 def test_zerocheck_roundtrip(spec, mlr):
     """zerocheck over synthetic satisfiable AIRs (reference GPU bytecode format) -> restated verify_zerocheck accepts"""
     rng = np.random.default_rng(41)
-    blob, heights, mains, preps, pv = _synth_machine(rng, spec)
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, spec, interactions=False)
     gp = O.rand_field(rng, (mlr, 4))
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
     c1 = ch.clone()
@@ -271,24 +259,12 @@ def test_zerocheck_roundtrip(spec, mlr):
 
 def test_zerocheck_rejects_violated_constraint():
     rng = np.random.default_rng(42)
-    blob, heights, mains, preps, pv = _synth_machine(rng, [(8, 1, False)])
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, [(8, 1, False)], interactions=False)
     mains[0][2, 3] ^= 1  # break c = a*b on one row
     gp = O.rand_field(rng, (3, 4))
     ch = O.Challenger()
     with pytest.raises(RuntimeError):
         O.zerocheck_prove_verify(blob, heights, mains, preps, pv, 3, gp, ch)
-
-
-def _synth_machine_gkr(rng, spec, pv0=12345):
-    from sp1_b200 import synth_air as SA
-    words, iwords, mains, preps, heights = [], [], [], [], []
-    for h, g, wp in spec:
-        w, _, _ = SA.synth_chip(g, wp)
-        words.append(w); iwords.append(SA.synth_interactions(g, wp))
-        m, p = SA.synth_trace(rng, h, g, wp, pv0)
-        mains.append(m); preps.append(p); heights.append(h)
-    pv = O.to_monty(np.array([pv0, 5, 6, 7]))
-    return SA.machine_blob_with_interactions(words, iwords), heights, mains, preps, pv
 
 
 @pytest.mark.parametrize("spec,mlr", [
@@ -300,7 +276,7 @@ def _synth_machine_gkr(rng, spec, pv0=12345):
 def test_logup_gkr_roundtrip(spec, mlr):
     """LogUp-GKR over synthetic balanced interactions -> restated verify_logup_gkr accepts (cumulative sum 0)"""
     rng = np.random.default_rng(51)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, spec)
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
     c1 = ch.clone()
     words = O.gkr_prove_verify(blob, heights, mains, preps, mlr, c1, gkr_pow_bits=4)
@@ -309,51 +285,19 @@ def test_logup_gkr_roundtrip(spec, mlr):
     assert words.size > 50 and (words == words2).all() and (c1.st == c2.st).all()
 
 
-SHARD_SPECS = [
-    ([(8, 1, False)], 3, 3),
-    ([(5, 1, False), (0, 2, False), (6, 1, True)], 3, 3),
-    ([(32, 2, True), (96, 1, False), (128, 1, False), (0, 1, True)], 5, 7),
-]
-
-
-@pytest.mark.parametrize("spec,log_stack,mlr", SHARD_SPECS)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
 def test_whole_shard_roundtrip(spec, log_stack, mlr):
     """commit -> LogUp-GKR -> zerocheck -> jagged/stacked/BaseFold open in one transcript; restated verify_shard accepts"""
-    rng = np.random.default_rng(61)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger(); ch.observe(O.rand_field(rng, 9))
+    blob, heights, mains, preps, pv, names, ch = M.shard_inputs(spec, 61)
     c1 = ch.clone()
-    pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, c1, num_queries=8, pow_bits=4,
-                                     batch_pow_bits=2, gkr_pow_bits=3)
+    pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, c1, **M.SMALL)
     assert words[0] == 5 and words.size == 6 + int(words[1:6].sum())
 
 
-def _synth_machine_gkr_custom(rng, spec, no_interactions=(), pv0=12345):
-    """like _synth_machine_gkr, but the chips listed in `no_interactions` carry no LogUp interactions at all"""
-    from sp1_b200 import synth_air as SA
-    words, iwords, mains, preps, heights = [], [], [], [], []
-    for k, (h, g, wp) in enumerate(spec):
-        w, _, _ = SA.synth_chip(g, wp)
-        words.append(w); iwords.append([0] if k in no_interactions else SA.synth_interactions(g, wp))
-        m, p = SA.synth_trace(rng, h, g, wp, pv0)
-        mains.append(m); preps.append(p); heights.append(h)
-    pv = O.to_monty(np.array([pv0, 5, 6, 7]))
-    return SA.machine_blob_with_interactions(words, iwords), heights, mains, preps, pv
-
-
-GKR_EDGE_CASES = [
-    # spec, chips without interactions, max_log_rows
-    ([(64, 1, False), (32, 2, False), (16, 1, True)], (1,), 7),       # a chip with constraints but no interactions
-    ([(2, 1, False), (1, 1, False)], (0,), 3),                          # 4 interactions in all, heights 2 and 1
-    ([(8, 3, False), (0, 1, False), (8, 1, True)], (2,), 4),            # absent chip + silent chip with preprocessed columns
-]
-
-
-@pytest.mark.parametrize("spec,silent,mlr", GKR_EDGE_CASES)
+@pytest.mark.parametrize("spec,silent,mlr", M.GKR_EDGE_CASES)
 def test_logup_gkr_roundtrip_with_silent_chips(spec, silent, mlr):
     rng = np.random.default_rng(53)
-    blob, heights, mains, preps, pv = _synth_machine_gkr_custom(rng, spec, silent)
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, M.silent(spec, silent))
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
     c1 = ch.clone()
     words = O.gkr_prove_verify(blob, heights, mains, preps, mlr, c1, gkr_pow_bits=4)
@@ -367,7 +311,6 @@ def test_workload_shard_roundtrip_and_tamper(workload, mlr, log_stack):
     """a calibrated core shard (36 chips, 640 interactions, messages of up to 12 values, a 682-column precompile table) and a
     compress-shape shard (recursion chips with up to 36 preprocessed columns), both at a quarter of their size: the restated verifier
     accepts the oracle's proof and ends in the prover's state, and rejects it after one flipped bit in the LogUp-GKR or zerocheck section"""
-    from tests import machines as M
     blob, heights, mains, preps, pv, names = M.workload_machine(workload, seed=71, max_log_rows=mlr, scale=0.25)
     assert max(heights) <= 1 << mlr
     prm = dict(num_queries=8, pow_bits=4, batch_pow_bits=2, gkr_pow_bits=3)
@@ -389,11 +332,10 @@ def test_workload_shard_roundtrip_and_tamper(workload, mlr, log_stack):
 def test_logup_gkr_roundtrip_calibrated_interactions():
     """calibrated interactions (synth_interactions_calibrated): a 12-value message (four beta-power bits), constant-1 and column
     multiplicities, 3-term linear combinations, filler columns and three further preprocessed columns"""
-    from tests.machines import Chip, n_interactions, spec_machine
     rng = np.random.default_rng(54)
-    blob, heights, mains, preps, pv, _ = spec_machine(rng, [Chip(40, 2, False, 12, 3, 0, [12, 4, 9]), Chip(17, 1, True, None, 0, 3, [5, 12]),
-                                                            Chip(0, 1, False, None, 0, 0, [1]), Chip(64, 3, False, 20, 0, 0, [2, 11, 7, 3])])
-    assert n_interactions(blob) == 2 * (3 + 2 + 1 + 4) + 2
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, [M.Chip(40, 2, False, 12, 3, 0, [12, 4, 9]), M.Chip(17, 1, True, None, 0, 3, [5, 12]),
+                                                              M.Chip(0, 1, False, None, 0, 0, [1]), M.Chip(64, 3, False, 20, 0, 0, [2, 11, 7, 3])])
+    assert M.n_interactions(blob) == 2 * (3 + 2 + 1 + 4) + 2
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
     c1 = ch.clone()
     words = O.gkr_prove_verify(blob, heights, mains, preps, 6, c1, gkr_pow_bits=4)

@@ -8,11 +8,10 @@ import os
 
 import numpy as np
 
-from tests import core_chain as CC
 from tests import core_oracle_lib as CO
 from tests import oracle_lib as O
 from tests import ref_golden as RG
-from tests import test_septic as S
+from tests import septic as S
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STORE = RG.Store("ref_septic", "tests/test_ref_septic.py")
@@ -24,7 +23,7 @@ def _inputs():
     n = 32
     a = np.stack([S.mont([int(x) for x in rng.integers(0, O.P, 7)]) for _ in range(n)])
     b = np.stack([S.mont([int(x) for x in rng.integers(0, O.P, 7)]) for _ in range(n)])
-    mult = CC.multiples(S.DUMMY, 40)
+    mult = S.multiples(S.DUMMY, 40)
     pairs = [(mult[i], mult[j]) for i in range(10) for j in range(10) if i != j and (i + j) % 3 == 0]
     p = np.stack([S.pt_words(x) for x, _ in pairs]); q = np.stack([S.pt_words(y) for _, y in pairs])
     ks = [int(k) for k in rng.integers(1, 8, 5)]
@@ -64,7 +63,7 @@ def test_mul_and_reciprocal_match_the_reference():
     a, b, _, _, _ = _inputs()
     n = a.shape[0]
     lm, li = np.zeros(7 * n, np.uint32), np.zeros(7 * n, np.uint32)
-    S._lib().sp1b200_hostcheck_septic(S._p(a), S._p(b), S._p(lm), S._p(li), C.c_uint64(n))
+    S.lib().sp1b200_hostcheck_septic(S.ptr(a), S.ptr(b), S.ptr(lm), S.ptr(li), C.c_uint64(n))
     R = ref()
     assert (lm == R["mul"]).all() and (li == R["inv"]).all()
     assert (CO.septic_mul(a, b).reshape(-1) == R["mul"]).all() and (CO.septic_inv(a).reshape(-1) == R["inv"]).all()
@@ -74,7 +73,7 @@ def test_curve_addition_matches_the_reference():
     _, _, p, q, _ = _inputs()
     n = p.shape[0]
     out, ok = np.zeros(14 * n, np.uint32), np.zeros(n, np.uint32)
-    S._lib().sp1b200_hostcheck_septic_curve_add(S._p(p), S._p(q), S._p(out), S._p(ok), C.c_uint64(n))
+    S.lib().sp1b200_hostcheck_septic_curve_add(S.ptr(p), S.ptr(q), S.ptr(out), S.ptr(ok), C.c_uint64(n))
     R = ref()
     assert ok.all() and (out == R["add"]).all()
     oo, ook = CO.curve_add(p, q)
@@ -86,14 +85,14 @@ def test_constant_points_and_chains_match_the_reference():
     the reference's `+` is the chord) is the library's incomplete addition of (k-1)·P and P"""
     R = ref()
     const = np.zeros(42, np.uint32)
-    S._lib().sp1b200_hostcheck_septic_constants(S._p(const))
+    S.lib().sp1b200_hostcheck_septic_constants(S.ptr(const))
     cd, cs = R["chain_dummy"].reshape(K, 14), R["chain_start"].reshape(K, 14)
     assert (cd[0] == const[28:42]).all() and (cs[0] == const[0:14]).all()
     for chain in (cd, cs):
         n = K - 2
         pw, qw = np.ascontiguousarray(chain[1:K - 1]), np.ascontiguousarray(np.repeat(chain[:1], n, 0))
         out, ok = np.zeros(14 * n, np.uint32), np.zeros(n, np.uint32)
-        S._lib().sp1b200_hostcheck_septic_curve_add(S._p(pw), S._p(qw), S._p(out), S._p(ok), C.c_uint64(n))
+        S.lib().sp1b200_hostcheck_septic_curve_add(S.ptr(pw), S.ptr(qw), S.ptr(out), S.ptr(ok), C.c_uint64(n))
         assert ok.all() and (out == chain[2:].reshape(-1)).all()
         for w in chain:
             assert S.on_curve(S.words_pt(w))
@@ -102,11 +101,11 @@ def test_constant_points_and_chains_match_the_reference():
 def test_digest_sum_matches_the_reference():
     """the SepticDigest additions of the core verifier (pairwise, as verify.rs:498-505 adds them) give the reference's group sum"""
     _, _, _, _, pts = _inputs()
-    L = S._lib()
+    L = S.lib()
     acc, oacc = pts[0].copy(), pts[0].copy()
     for d in pts[1:]:
         out = np.zeros(14, np.uint32)
-        assert L.sp1b200_hostcheck_septic_digest_add(S._p(acc), S._p(np.ascontiguousarray(d)), S._p(out)) == 1
+        assert L.sp1b200_hostcheck_septic_digest_add(S.ptr(acc), S.ptr(np.ascontiguousarray(d)), S.ptr(out)) == 1
         acc = out
         oacc = CO.digest_add(oacc, d)
     R = ref()

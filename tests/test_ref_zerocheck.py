@@ -26,7 +26,7 @@ import pytest
 from sp1_b200 import synth_air as SA
 from tests import oracle_lib as O
 from tests.ext_field import EF, ONE, ZERO, efs, eval_at, interpolate, parse_partial_sumcheck
-from tests.machines import PV0, Chip, oracle_zerocheck, product_zerocheck, spec_machine, workload_machine
+from tests.machines import Chip, chip_segments, oracle_zerocheck, product_zerocheck, spec_machine, workload_machine
 from tests.ref_golden import Ref, Store
 
 STORE = Store("ref_zerocheck", "tests/test_ref_zerocheck.py")
@@ -185,13 +185,12 @@ def _vanishing_chip():
 
 def _synth(rng, spec):
     """spec: list of (height, groups, with_prep, kind), kind "flat", "deep" (long-lived intermediates) or "vanishing" (one group)"""
-    words, mains, preps, heights = [], [], [], []
-    for h, g, wp, kind in spec:
-        assert kind != "vanishing" or (g, wp) == (1, False), "the vanishing chip has one group and no preprocessed column"
-        words.append(_vanishing_chip() if kind == "vanishing" else SA.synth_chip(g, wp, deep=kind == "deep")[0])
-        m, p = SA.synth_trace(rng, h, g, wp, PV0)
-        mains.append(m); preps.append(p); heights.append(h)
-    return SA.machine_blob(words), heights, mains, preps, O.to_monty(np.array([PV0, 5, 6, 7]))
+    assert all(kind != "vanishing" or (g, wp) == (1, False) for _, g, wp, kind in spec), \
+        "the vanishing chip has one group and no preprocessed column"
+    blob, heights, mains, preps, pv, _ = spec_machine(rng, [Chip(h, g, wp, deep=kind == "deep") for h, g, wp, kind in spec],
+                                                      interactions=False)
+    progs = [_vanishing_chip() if kind == "vanishing" else seg[2] for seg, (_, _, _, kind) in zip(chip_segments(blob), spec)]
+    return SA.machine_blob(progs), heights, mains, preps, pv
 
 
 # (name, kind, spec, max_log_row_count)

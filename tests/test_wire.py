@@ -10,40 +10,22 @@ import pytest
 
 from sp1_b200 import lib as PL
 from tests import bincode_ref as BR
+from tests import machines as M
 from tests import oracle_lib as O
-from tests.test_oracle import _synth_machine_gkr
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
-def _widths(blob):
-    """(main_w, prep_w) per chip from the machine blob (layout: include/sp1b200.h, sp1b200_machine_create)"""
-    b = [int(x) for x in blob]
-    n, o, out = b[0], 1, []
-    for _ in range(n):
-        main_w, prep_w, _nc, _nr, ni, nl, ncst, npub, na = b[o:o + 9]
-        out.append((main_w, prep_w))
-        o += 9 + 2 * ni + 2 * nl + ncst + npub + 2 * na
-    return out
-
-
-CASES = [
-    # spec (height, groups, preprocessed), log_stack, max_log_rows
-    ([(8, 1, False)], 3, 3),
-    ([(5, 1, False), (0, 2, False), (6, 1, True)], 3, 3),
-    ([(32, 2, True), (96, 1, False), (128, 1, False), (0, 1, True)], 5, 7),
-]
 PARAMS = dict(log_blowup=2, num_queries=6, pow_bits=3, batch_pow_bits=2, gkr_pow_bits=3)
 
 
 def _proof(spec, log_stack, mlr, seed=71):
     rng = np.random.default_rng(seed)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
+    blob, heights, mains, preps, pv, names = M.spec_machine(rng, spec, names="Chip{:02d}")
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 5))
     start = ch.clone()
     pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, ch, **PARAMS)
-    w = _widths(blob)
+    w = M.widths(blob)
     return dict(blob=blob, heights=heights, names=names, words=words, main_w=[a for a, _ in w], prep_w=[b for _, b in w], start=start,
                 final=ch, prep_commit=pc, params=dict(PARAMS, log_stacking_height=log_stack, max_log_row_count=mlr))
 
@@ -63,7 +45,7 @@ def test_leaf_encoding_pins():
     assert k0 < k1 and pins["vk_map"]["max_word"] < BR.P
 
 
-@pytest.mark.parametrize("spec,log_stack,mlr", CASES)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
 def test_bincode_matches_the_struct_definitions(spec, log_stack, mlr):
     p = _proof(spec, log_stack, mlr)
     data = PL.shard_proof_to_bincode(p["words"], p["names"], p["heights"], p["main_w"], p["prep_w"], **p["params"])
@@ -80,7 +62,7 @@ def test_bincode_matches_the_struct_definitions(spec, log_stack, mlr):
     assert tree["public_values"] == [int(x) for x in O.from_monty(p["words"][-len(tree["public_values"]):])]
 
 
-@pytest.mark.parametrize("spec,log_stack,mlr", CASES)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
 def test_bincode_round_trip_and_verifier(spec, log_stack, mlr):
     p = _proof(spec, log_stack, mlr)
     data = PL.shard_proof_to_bincode(p["words"], p["names"], p["heights"], p["main_w"], p["prep_w"], **p["params"])
@@ -93,7 +75,7 @@ def test_bincode_round_trip_and_verifier(spec, log_stack, mlr):
 
 
 def test_bincode_rejects_malformed_input():
-    spec, log_stack, mlr = CASES[1]
+    spec, log_stack, mlr = M.SHARD_SPECS[1]
     p = _proof(spec, log_stack, mlr)
     args = (p["names"], p["main_w"], p["prep_w"])
     data = bytearray(PL.shard_proof_to_bincode(p["words"], p["names"], p["heights"], p["main_w"], p["prep_w"], **p["params"]))
@@ -129,7 +111,7 @@ def test_bincode_rejects_malformed_input():
 def test_bincode_reader_survives_random_corruption():
     """memory safety of the byte reader: random byte flips, length-prefix overwrites and truncations must end in an error message or a
     parsed proof - never in a crash or an over-read (every length prefix is checked against the bytes that remain)"""
-    spec, log_stack, mlr = CASES[2]
+    spec, log_stack, mlr = M.SHARD_SPECS[2]
     p = _proof(spec, log_stack, mlr)
     args = (p["names"], p["main_w"], p["prep_w"])
     data = PL.shard_proof_to_bincode(p["words"], p["names"], p["heights"], p["main_w"], p["prep_w"], **p["params"])
@@ -172,7 +154,7 @@ def test_bincode_reader_under_sanitizers(tmp_path):
                          f"{root}/sp1_b200/csrc/wire.cu", "-o", exe], capture_output=True, text=True)
     if cc.returncode != 0:
         pytest.skip("sanitizer build unavailable here: " + cc.stderr[-300:])
-    spec, log_stack, mlr = CASES[2]
+    spec, log_stack, mlr = M.SHARD_SPECS[2]
     p = _proof(spec, log_stack, mlr)
     data = PL.shard_proof_to_bincode(p["words"], p["names"], p["heights"], p["main_w"], p["prep_w"], **p["params"])
     f = tmp_path / "proof.bin"

@@ -4,8 +4,8 @@ in name order — and the synthetic traces satisfy their own constraints and bal
 import numpy as np
 import pytest
 
-from sp1_b200 import synth_air as SA
 from sp1_b200 import workload as W
+from tests import machines as M
 from tests import oracle_lib as O
 
 
@@ -37,17 +37,10 @@ def test_synthetic_machine_is_consistent():
 def test_synthetic_traces_satisfy_constraints_and_interactions(workload):
     """a scaled-down copy of the bench machine (light and calibrated + precompile table): the oracle proves it and its restated
     verifier accepts (constraints hold on every real row, the LogUp cumulative sum is zero)"""
-    m = W.synthetic_machine(workload, seed=42, scale=1 / 256)
-    rng = np.random.default_rng(3)
-    mains, preps = [], []
-    for sp in m["specs"]:
-        a, p = SA.synth_trace(rng, sp.h, sp.g, sp.wp, 12345, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        mains.append(a); preps.append(p)
-    pv = O.to_monty(np.array([12345, 5, 6, 7]))
-    heights = [s_[0] for s_ in m["specs"]]
+    blob, heights, mains, preps, pv, names = M.workload_machine(workload, seed=3, scale=1 / 256)
     mlr = max(5, int(np.ceil(np.log2(max(heights + [2])))))
     ch = O.Challenger()
-    pc, words = O.prove_shard_verify(m["blob"], heights, mains, preps, m["names"], pv, min(mlr, 6), mlr, ch, num_queries=4, pow_bits=2,
+    pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, min(mlr, 6), mlr, ch, num_queries=4, pow_bits=2,
                                      batch_pow_bits=1, gkr_pow_bits=2)
     assert words[0] == 5 and words.size > 100
 

@@ -22,34 +22,27 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", required=True, help="directory for debug_bench.json")
     args = ap.parse_args()
-    import numpy as np
     import torch
     from sp1_b200 import Lib
-    from sp1_b200 import synth_air as SA
     from sp1_b200 import workload as W
+    from tests import machines as M
+    from tools.device_traces import device_traces
 
     assert torch.cuda.is_available(), "debug_bench needs a GPU"
     card = torch.cuda.get_device_name(0)
     q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     power = q.stdout.strip() if q.returncode == 0 else "unknown"
-    pv = SA.to_monty(np.array([12345, 5, 6, 7]))
+    pv = M.PV
     results = []
     for wl in args.workloads:
         m = W.synthetic_machine(wl, seed=42)
-        specs = m["specs"]
-        heights = [sp.h for sp in specs]
-        parts, preps = [], []
-        for i, sp in enumerate(specs):
-            a, p = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, 12345, 700 + i, 0, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-            parts.append(a); preps.append(p)
-        dense = torch.cat(parts).contiguous()
-        torch.cuda.synchronize()
+        heights = [sp.h for sp in m["specs"]]
+        dense, d_prep, prep_rows, prep_cols = device_traces(m["specs"], M.PV0, lambda i: 700 + i, 0)
         lib = Lib(0, **W.params_of(wl))
         mach = lib.machine_create(m["blob"])
-        pts = [p.view(-1, sp.h).cpu().numpy().view(np.uint32) for p, sp in zip(preps, specs) if p is not None]
-        pr = lib.jagged_commit(pts)[1] if pts else None
-        cells = int(dense.numel()) + sum(int(p.numel()) for p in preps if p is not None)
-        pairs = sum(int(h) * int(n) for h, n in zip(heights, _interactions_per_chip(m["blob"])))
+        pr = lib.jagged_commit_dense(d_prep, prep_rows, prep_cols)[1] if d_prep is not None else None
+        cells = int(dense.numel()) + (int(d_prep.numel()) if d_prep is not None else 0)
+        pairs = sum(int(h) * int(n) for h, n in zip(heights, m["interactions"]))
         row = {"workload": wl, "card": card, "power_limit_and_max_sm_clock": power, "trace_cells": cells, "interaction_pairs": pairs}
         for name, call in (("constraints", lambda: lib.debug_constraints_words(mach, pr, dense, heights, pv)),
                            ("interactions", lambda: lib.debug_interactions_words(mach, pr, dense, heights))):
@@ -72,27 +65,11 @@ def main():
             lib.jagged_round_free(pr)
         lib.machine_free(mach)
         lib.close()
-        del dense, parts, preps
+        del dense, d_prep
         torch.cuda.empty_cache()
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "debug_bench.json"), "w") as f:
         json.dump(results, f, indent=1)
-
-
-def _interactions_per_chip(blob):
-    b = [int(x) for x in blob]
-    p = 1
-    for _ in range(b[0]):
-        ni, nl, nc, npub, na = b[p + 4:p + 9]
-        p += 9 + 2 * ni + 2 * nl + nc + npub + 2 * na
-    out = []
-    for _ in range(b[0]):
-        k = b[p]; out.append(k); p += 1
-        for _ in range(k):
-            nv = b[p + 2]; p += 3
-            for _ in range(nv + 1):
-                p += 2 + 3 * b[p]
-    return out
 
 
 if __name__ == "__main__":

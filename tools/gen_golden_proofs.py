@@ -12,13 +12,11 @@ import json
 import os
 import sys
 
-import numpy as np
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tests import golden_util as G  # noqa: E402
 from tests import oracle_lib as O  # noqa: E402
-from tests.test_oracle import _synth_machine_gkr  # noqa: E402
 
 CASES = [
     # name, spec [(height, groups, with_prep)], log_stack, max_log_rows, seed, queries, pow, batch_pow, gkr_pow
@@ -29,29 +27,21 @@ CASES = [
 ]
 
 
-def run_case(name, spec, log_stack, mlr, seed, nq, pw, bpw, gpw):
-    rng = np.random.default_rng(seed)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger()
-    ch.observe(O.rand_field(rng, 9))
+def prove_case(spec, log_stack, mlr, seed, nq, pw, bpw, gpw):
+    """the oracle's proof of a case's seeded inputs (golden_util.inputs_of) -> (blob, heights, mains, preps, names, prep commitment,
+    words, final challenger)"""
+    blob, heights, mains, preps, pv, names, ch = G.inputs_of({"spec": spec, "seed": seed})
     pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, ch, num_queries=nq, pow_bits=pw,
                                      batch_pow_bits=bpw, gkr_pow_bits=gpw)
-    n_sec = int(words[0])
-    lens = [int(x) for x in words[1:1 + n_sec]]
-    off = 1 + n_sec
-    heads = []
-    for ln in lens:
-        sec = words[off:off + ln]
-        heads.append({"first": [int(x) for x in sec[:8]], "last": [int(x) for x in sec[-8:]]})
-        off += ln
-    return {
-        "name": name, "spec": [list(s) for s in spec], "log_stacking_height": log_stack, "max_log_row_count": mlr, "seed": seed,
-        "num_queries": nq, "pow_bits": pw, "batch_pow_bits": bpw, "gkr_pow_bits": gpw,
-        "prep_commit": [int(x) for x in pc], "main_commit": [int(x) for x in words[1 + n_sec:1 + n_sec + 8]],
-        "final_challenger": [int(x) for x in ch.st], "section_lengths": lens, "n_words": int(words.size),
-        "sha256": hashlib.sha256(words.astype("<u4").tobytes()).hexdigest(), "sections": heads,
-    }
+    return blob, heights, mains, preps, names, pc, words, ch
+
+
+def run_case(name, spec, log_stack, mlr, seed, nq, pw, bpw, gpw):
+    *_, pc, words, ch = prove_case(spec, log_stack, mlr, seed, nq, pw, bpw, gpw)
+    d = {"name": name, "spec": [list(s) for s in spec], "log_stacking_height": log_stack, "max_log_row_count": mlr, "seed": seed,
+         "num_queries": nq, "pow_bits": pw, "batch_pow_bits": bpw, "gkr_pow_bits": gpw}
+    d.update(summarize(name, pc, words, ch, {}))   # the case's parameters first, as the fixture lists them
+    return d
 
 
 def summarize(name, pc, words, ch, extra):
@@ -75,14 +65,13 @@ def full_size(workloads):
     bits), proven once by the oracle (minutes on 8 cores) -> tests/golden/shard_proofs_fullsize.json.  Also stores the three grinding
     witnesses so that the replay-mode test can reproduce the same proof with grind_mode = 1."""
     import time
-    from tests import golden_util as G
     path = G.FULL_PATH
     old = {c["name"]: c for c in (json.load(open(path))["cases"] if os.path.exists(path) else [])}
     for wl in workloads:
         seed = 9000 + sum(ord(c) for c in wl)
-        mach, heights, mains, preps, pv, ch = G.fullsize_inputs(wl, seed)
+        blob, heights, mains, preps, pv, names, ch = G.fullsize_inputs(wl, seed)
         t0 = time.time()
-        pc, words = O.prove_shard_verify(mach["blob"], heights, mains, preps, mach["names"], pv, 21, 22, ch)
+        pc, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, 21, 22, ch)
         print(f"{wl}: oracle proved + verified in {time.time() - t0:.0f}s, {words.size} words", flush=True)
         old[wl] = summarize(wl, pc, words, ch, {"workload": wl, "seed": seed, "log_stacking_height": 21, "max_log_row_count": 22,
                                                 "num_queries": 124, "pow_bits": 16, "batch_pow_bits": 5, "gkr_pow_bits": 12})
@@ -96,16 +85,9 @@ def full_size(workloads):
 def bincode_case(name, spec, log_stack, mlr, seed, nq, pw, bpw, gpw):
     """the wire bytes of the same seeded proof: bincode(ShardProof) written by the product's host-only converter"""
     from sp1_b200 import lib as PL
-    from tests.test_wire import _widths
-    rng = np.random.default_rng(seed)
-    blob, heights, mains, preps, pv = _synth_machine_gkr(rng, spec)
-    names = [f"Chip{i:02d}" for i in range(len(heights))]
-    ch = O.Challenger()
-    ch.observe(O.rand_field(rng, 9))
-    _, words = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, ch, num_queries=nq, pow_bits=pw, batch_pow_bits=bpw,
-                                    gkr_pow_bits=gpw)
-    w = _widths(blob)
-    data = PL.shard_proof_to_bincode(words, names, heights, [a for a, _ in w], [b for _, b in w], log_stacking_height=log_stack,
+    _, heights, mains, preps, names, _, words, _ = prove_case(spec, log_stack, mlr, seed, nq, pw, bpw, gpw)
+    main_w, prep_w = [m.shape[0] for m in mains], [0 if p is None else p.shape[0] for p in preps]
+    data = PL.shard_proof_to_bincode(words, names, heights, main_w, prep_w, log_stacking_height=log_stack,
                                      max_log_row_count=mlr, num_queries=nq, pow_bits=pw, batch_pow_bits=bpw, gkr_pow_bits=gpw)
     return {"name": name, "words_sha256": hashlib.sha256(words.astype("<u4").tobytes()).hexdigest(), "bincode_bytes": len(data),
             "bincode_sha256": hashlib.sha256(data).hexdigest(), "head_hex": data[:64].hex()}

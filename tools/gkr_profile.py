@@ -97,13 +97,13 @@ def main():
     ap.add_argument("--out", default=None, help="also write the table to this file")
     args = ap.parse_args()
 
-    import numpy as np
     import torch
     from torch.profiler import ProfilerActivity, profile
     from sp1_b200 import Lib
     from sp1_b200.lib import HostChallenger
-    from sp1_b200 import synth_air as SA
     from sp1_b200 import shards as SH
+    from tests import machines as M
+    from tools.device_traces import device_traces
 
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
@@ -113,25 +113,12 @@ def main():
     inters = mach["interactions"]
     specs, names = mach["specs"], mach["names"]
     heights = [s_[0] for s_ in specs]
-    pv0 = 12345
-    pv = ((np.array([pv0, 5, 6, 7], dtype=np.uint64) << np.uint64(32)) % np.uint64(W.P)).astype(np.uint32)
-    mains, preps = [], []
-    prep_heights, main_heights = [], []
-    for i, sp in enumerate(specs):
-        m_, p_ = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, pv0, SH.shard_seed(0, 0) + i, dev, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        if sp.h:
-            main_heights += [sp.h] * (m_.numel() // sp.h)
-            if sp.wp:
-                prep_heights += [sp.h] * (p_.numel() // sp.h)
-        mains.append(m_)
-        if sp.wp:
-            preps.append(p_)
-    d_main = torch.cat(mains).contiguous()
-    d_prep = torch.cat(preps).contiguous()
-    del mains, preps
-    torch.cuda.synchronize()
+    main_heights = [h for h, cols in mach["main_shapes"] if h for _ in range(cols)]
+    prep_heights = [h for h, cols in mach["prep_shapes"] if h for _ in range(cols)]
+    d_main, d_prep, prep_rows, prep_cols = device_traces(specs, M.PV0, lambda i: SH.shard_seed(0, 0) + i, dev)
+    pv = M.PV
     machine = lib.machine_create(mach["blob"])
-    _, h_prep = lib.jagged_commit_dense(d_prep, [s_.h for s_ in specs if s_.wp], [1 + s_.extra_prep for s_ in specs if s_.wp])
+    _, h_prep = lib.jagged_commit_dense(d_prep, prep_rows, prep_cols)
     chal0 = HostChallenger().st.copy()
 
     def step():

@@ -21,31 +21,20 @@ if ROOT not in sys.path:
 
 def full_size_proof(lib, workload, dev):
     """prove the full-size synthetic shard `workload` on `lib`'s context (fresh transcript) -> machine handle, commitment, proof"""
-    import numpy as np
     import torch
-    from sp1_b200 import synth_air as SA
     from sp1_b200 import workload as W
     from sp1_b200.lib import HostChallenger
+    from tests import machines as M
+    from tests import oracle_lib as O
+    from tools.device_traces import device_traces
     mach = W.synthetic_machine(workload, seed=42)
     specs, names = mach["specs"], mach["names"]
     heights = [s.h for s in specs]
-    pv0 = 12345
-    pv = SA.to_monty(np.array([pv0, 5, 6, 7]))
-    mains, preps = [], []
-    for i, sp in enumerate(specs):
-        m_, p_ = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, pv0, 7000 + i, dev, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-        mains.append(m_)
-        if sp.wp:
-            preps.append(p_)
-    d_main = torch.cat(mains).contiguous()
-    d_prep = torch.cat(preps).contiguous()
-    del mains, preps
-    # the library reads the traces on its own stream: torch's kernels that wrote them must have finished
-    torch.cuda.current_stream(dev).synchronize()
+    d_main, d_prep, prep_rows, prep_cols = device_traces(specs, M.PV0, lambda i: 7000 + i, dev)
     machine = lib.machine_create(mach["blob"])
-    pc, h_prep = lib.jagged_commit_dense(d_prep, [s.h for s in specs if s.wp], [1 + s.extra_prep for s in specs if s.wp])
+    pc, h_prep = lib.jagged_commit_dense(d_prep, prep_rows, prep_cols)
     st = HostChallenger().st.copy()
-    words = lib.prove_shard(machine, h_prep, d_main, heights, names, pv, st)
+    words = lib.prove_shard(machine, h_prep, d_main, heights, names, O.to_monty([M.PV0, 5, 6, 7]), st)
     lib.jagged_round_free(h_prep)
     del d_main, d_prep
     torch.cuda.empty_cache()

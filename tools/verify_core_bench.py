@@ -25,36 +25,28 @@ def prove_chain(lib, workload, n, dev, seed=900):
     """n full-size shards of `workload` with the public values of a valid core proof -> dict for the verifiers"""
     import numpy as np
     import torch
-    from sp1_b200 import synth_air as SA
     from sp1_b200 import workload as W
     from sp1_b200.lib import HostChallenger
     from tests import core_chain as CC
+    from tests import oracle_lib as O
+    from tools.device_traces import device_traces
     mach = W.synthetic_machine(workload, seed=42)
     specs, names = mach["specs"], mach["names"]
     heights = [s.h for s in specs]
     machine = lib.machine_create(mach["blob"])
     pvs, tail = CC.chain(n, seed)
-    tail = SA.to_monty(np.array(tail))
+    tail = O.to_monty(np.array(tail))
     prep_round, pc = None, np.zeros(8, np.uint32)
     words, finals = [], []
-    for s, pv in enumerate(pvs):
-        mains, preps = [], []
-        for i, sp in enumerate(specs):   # the same seeds for every shard: identical preprocessed tables, each shard's own pv0
-            m_, p_ = SA.synth_trace_cuda(sp.h, sp.g, sp.wp, CC.pv0_of(pv), 7000 + i, dev, extra_cols=sp.extra, extra_prep=sp.extra_prep)
-            mains.append(m_)
-            if sp.wp:
-                preps.append(p_)
-        d_main = torch.cat(mains).contiguous()
-        d_prep = torch.cat(preps).contiguous() if prep_round is None and preps else None
-        del mains, preps
-        # the library reads the traces on its own stream: torch's kernels that wrote them must have finished
-        torch.cuda.current_stream(dev).synchronize()
-        if d_prep is not None:
-            pc, prep_round = lib.jagged_commit_dense(d_prep, [s_.h for s_ in specs if s_.wp], [1 + s_.extra_prep for s_ in specs if s_.wp])
-            del d_prep
+    for pv in pvs:
+        # the same seeds for every shard: identical preprocessed tables, each shard's own pv0
+        d_main, d_prep, prep_rows, prep_cols = device_traces(specs, CC.pv0_of(pv), lambda i: 7000 + i, dev)
+        if prep_round is None and d_prep is not None:
+            pc, prep_round = lib.jagged_commit_dense(d_prep, prep_rows, prep_cols)
+        del d_prep
         hc = HostChallenger(); hc.observe(pc); hc.observe(tail)
         st = hc.st.copy()
-        words.append(lib.prove_shard(machine, prep_round, d_main, heights, names, SA.to_monty(np.array(pv)), st))
+        words.append(lib.prove_shard(machine, prep_round, d_main, heights, names, O.to_monty(np.array(pv)), st))
         finals.append(st)
         del d_main
         torch.cuda.empty_cache()
