@@ -17,6 +17,7 @@
 #include "debug_fp.cuh"
 #include "hostfield.hpp"
 #include "kb31.cuh"
+#include "proof_layout.hpp"
 #include "sumcheck.cuh"
 #include <algorithm>
 #include <map>
@@ -611,9 +612,7 @@ extern "C" {
 // GkrProverImpl::prove_logup_gkr (crates/hypercube/src/logup_gkr/prover.rs:70-215).
 // d_main[k]/d_prep[k]: chip columns (column-major [w x h_heights[k]]), interactions from the machine blob.
 // h_replay_witness: the GKR grinding witness when params.grind_mode == 1.
-// Output words: n_out | numerator[n_out] ext | denominator[n_out] ext | n_rounds | per round {numerator_0, numerator_1,
-//   denominator_0, denominator_1 ext, sumcheck {n_polys, per poly {n_coeffs, coeffs}, claimed_sum, point, eval}} |
-//   evaluation point (max_log_row_count ext) | per chip {main openings, preprocessed openings} | witness
+// Output words: the LogUp-GKR section of a shard proof (proof_layout.hpp).
 sp1b200_err sp1b200_logup_gkr(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint64_t* h_heights, const uint32_t* const* d_main,
                               const uint32_t* const* d_prep, const uint32_t* h_replay_witness, uint32_t* h_chal, uint32_t* h_out, uint64_t cap,
                               uint64_t* h_words);

@@ -436,9 +436,8 @@ sp1b200_err sp1b200_jagged_column_claims(sp1b200_ctx* ctx, const sp1b200_jagged_
 
 // JaggedProver::prove_trusted_evaluations (slop/crates/jagged/src/prover.rs:162-328).
 // h_claims: for each round, the evaluations at z_row of that round's table columns (ext each), back to back.
-// Proof words: stacked proof | sumcheck {n_polys, per poly {n_coeffs, coeffs}, claimed_sum, point, eval} |
-// jagged_eval (same layout) | per round {n_tables, (rows, cols)...} | original commitments | expected_eval |
-// max_log_row_count | log_m        (field order of JaggedPcsProof, slop/crates/jagged/src/verifier.rs:17-27)
+// Proof words: the evaluation proof section of a shard proof (proof_layout.hpp), the stacked proof first
+// (field order of JaggedPcsProof, slop/crates/jagged/src/verifier.rs:17-27).
 sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* rounds, uint32_t n_rounds, const uint32_t* h_z_row,
                                  const uint32_t* h_claims, const uint32_t* h_replay, uint32_t* h_chal, uint32_t* h_proof, uint64_t cap,
                                  uint64_t* h_words) { SP1_DEVICE_GUARD(ctx);
@@ -525,7 +524,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     { uint64_t e = 0; for (uint32_t r = 0; r < n_rounds; r++) { seg.ptr[r] = rounds[r]->d_dense; e += rounds[r]->padded_area; seg.end[r] = e; } }
 
     // ---- Hadamard sumcheck (lambda = 1, t = 1) ---------------------------------------------------------------------
-    std::vector<uint32_t> sc_words;     // univariate polys
+    layout::SumcheckWriter sc;
     std::vector<E4> point;              // most recent challenge first
     E4 round_claim = claim;
     PhaseTimer t_sc(ctx, "jagged.sumcheck");
@@ -576,9 +575,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         E4 c[3];
         interp_0_1_half(e0, e1, eh * hf::inv(hf::to_monty(4)), c);
         for (int i = 0; i < 3; i++) ch.observe_n(c[i].c, 4);
-        uint32_t three = 3;
-        sc_words.push_back(three);
-        for (int i = 0; i < 3; i++) sc_words.insert(sc_words.end(), c[i].c, c[i].c + 4);
+        sc.poly(c, 3);
         E4 alpha; ch.sample_ext(alpha.c);
         point.insert(point.begin(), alpha);
         round_claim = eval3(c, alpha);
@@ -599,7 +596,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     t_sc.stop();
 
     // ---- jagged evaluation (branching program) sumcheck --------------------------------------------------------------
-    std::vector<uint32_t> je_words;
+    layout::SumcheckWriter je;
     std::vector<E4> rhos;
     E4 je_claimed, je_eval;
     {
@@ -661,7 +658,6 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         }
         ch.observe_n(je_claimed.c, 4);
         E4 cl = je_claimed;
-        je_words.push_back(dim);
         const bool bp_mail = (size_t)nblk * 8 <= SP1_MAIL_WORDS;  // otherwise fall back to copy + synchronise
         for (uint32_t round = 0; round < dim; round++) {
             if (round == hl) SP1_LAUNCH(ctx, bp_suffix_kernel, blocks_for(nk, 128), 128, 0, d_bits, nk, dim, 1, d_rho_pos, d_ri, d_T);
@@ -676,8 +672,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             E4 c[3];
             interp_0_1_half(y0, y1, yh, c);
             for (int i = 0; i < 3; i++) ch.observe_n(c[i].c, 4);
-            je_words.push_back(3);
-            for (int i = 0; i < 3; i++) je_words.insert(je_words.end(), c[i].c, c[i].c + 4);
+            je.poly(c, 3);
             E4 alpha; ch.sample_ext(alpha.c);
             rhos.insert(rhos.begin(), alpha);
             cl = eval3(c, alpha);
@@ -699,34 +694,17 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
     // the stacked proof is written straight into the caller's buffer; the jagged sections are appended after it
     uint64_t nw = 0;
     SP1_TRY(sp1b200_stacked_prove(ctx, handles.data(), n_rounds, pt.data(), (uint32_t)point.size(), h_replay, chal, h_proof, cap, &nw));
-    std::vector<uint32_t> proof;
-    auto put = [&](const uint32_t* p, size_t n) { proof.insert(proof.end(), p, p + n); };
-    auto put1 = [&](uint32_t v) { proof.push_back(v); };
-    // sumcheck proof
-    put1(lm);
-    put(sc_words.data(), sc_words.size());
-    put(claim.c, 4);
-    put(pt.data(), pt.size());
-    put(round_claim.c, 4);
-    // jagged eval proof
-    put(je_words.data(), je_words.size());
-    put(je_claimed.c, 4);
-    for (auto& x : rhos) put(x.c, 4);
-    put(je_eval.c, 4);
-    for (uint32_t r = 0; r < n_rounds; r++) {
-        put1((uint32_t)rounds[r]->tables.size());
-        for (auto& t : rounds[r]->tables) { put1((uint32_t)t.first); put1((uint32_t)t.second); }
-    }
-    for (uint32_t r = 0; r < n_rounds; r++) put(rounds[r]->original_commit, 8);
-    put(base_eval.c, 4);
-    put1(mlr);
-    put1(lm);
+    layout::FlatWriter proof;
+    sc.write(proof, claim, point.data(), round_claim);
+    je.write(proof, je_claimed, rhos.data(), je_eval);
+    for (uint32_t r = 0; r < n_rounds; r++) layout::write_tables(proof, rounds[r]->tables);
+    for (uint32_t r = 0; r < n_rounds; r++) proof.put(rounds[r]->original_commit, 8);
+    proof.ext(base_eval);
+    proof.u(mlr);
+    proof.u(lm);
     t_all.stop();
     memcpy(h_chal, chal, sizeof(chal));
-    if (h_words) *h_words = nw + proof.size();
-    if (nw + proof.size() > cap) return sp1b200_set_error("jagged_prove: proof needs %llu words, capacity %llu", (unsigned long long)(nw + proof.size()), (unsigned long long)cap);
-    if (h_proof) memcpy(h_proof + nw, proof.data(), proof.size() * 4);
-    return nullptr;
+    return layout::deliver("jagged_prove", "proof", proof.words, h_proof, cap, h_words, nw);
 }
 
 }  // extern "C"

@@ -13,6 +13,7 @@
 #include "hostfield.hpp"
 #include "kb31.cuh"
 #include "poseidon2.cuh"
+#include "proof_layout.hpp"
 #include "sumcheck.cuh"
 #include <array>
 #include <memory>
@@ -244,8 +245,7 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
     DevFree mem(ctx);
     HostChallenger ch;
     SP1_TRY(ch.init(ctx, h_chal));
-    std::vector<uint32_t> proof;
-    auto put = [&](const uint32_t* p, size_t n) { proof.insert(proof.end(), p, p + n); };
+    layout::FlatWriter proof;
 
     // stack point (last log_h coordinates) on device + eq table
     uint32_t *d_point, *d_E, *d_E2;
@@ -397,8 +397,8 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
     for (auto& q : idx) q = ch.sample_bits(log_h + b);
 
     // ---- assemble: univariate messages, fri commitments -----------------------------------------------------------
-    put(uni.data(), uni.size());
-    put(fri_commits.data(), fri_commits.size());
+    proof.put(uni.data(), uni.size());
+    proof.put(fri_commits.data(), fri_commits.size());
 
     // ---- query phase -------------------------------------------------------------------------------------------------
     PhaseTimer t_q(ctx, "open.queries");
@@ -423,11 +423,7 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         SP1_CUDA(cudaMemcpyAsync(vals.data(), d_vals, vals.size() * 4, cudaMemcpyDeviceToHost, st));
         SP1_CUDA(cudaMemcpyAsync(paths.data(), d_paths, paths.size() * 4, cudaMemcpyDeviceToHost, st));
         SP1_CUDA(cudaStreamSynchronize(st));
-        put(vals.data(), vals.size());
-        put(c->root, 8);
-        uint32_t meta[2] = {LH, (uint32_t)c->ncols};
-        put(meta, 2);
-        put(paths.data(), paths.size());
+        layout::write_opening(proof, vals.data(), nq, (uint32_t)c->ncols, c->root, LH, paths.data());
     }
     for (uint32_t r = 0; r < log_h; r++) {
         for (auto& q : idx) q >>= 1;
@@ -443,24 +439,17 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         SP1_CUDA(cudaMemcpyAsync(vals.data(), d_vals, vals.size() * 4, cudaMemcpyDeviceToHost, st));
         if (lh) SP1_CUDA(cudaMemcpyAsync(paths.data(), d_paths, paths.size() * 4, cudaMemcpyDeviceToHost, st));
         SP1_CUDA(cudaStreamSynchronize(st));
-        put(vals.data(), vals.size());
-        put(fri_roots[r].data(), 8);
-        uint32_t meta[2] = {lh, 8};
-        put(meta, 2);
-        put(paths.data(), paths.size());
+        layout::write_opening(proof, vals.data(), nq, 8, fri_roots[r].data(), lh, paths.data());
     }
     t_q.stop();
-    put(fin, 4);
-    put(&pow_w, 1);
-    put(&batch_w, 1);
-    put(evals.data(), evals.size());
+    proof.put(fin, 4);
+    proof.u(pow_w);
+    proof.u(batch_w);
+    proof.put(evals.data(), evals.size());
     t_all.stop();
 
     ch.store(h_chal);
-    if (h_words) *h_words = proof.size();
-    if (proof.size() > cap) return sp1b200_set_error("stacked_prove: proof needs %zu words, capacity %llu", proof.size(), (unsigned long long)cap);
-    if (h_proof) memcpy(h_proof, proof.data(), proof.size() * 4);
-    return nullptr;
+    return layout::deliver("stacked_prove", "proof", proof.words, h_proof, cap, h_words);
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
-// The flat proof words of sp1b200_prove_shard, read in one place: the wire format (wire.cu) and the shard verifier (verify.cu) both
-// walk a proof through parse_shard_proof, and the shard prover (shard.cu) reads the LogUp-GKR and zerocheck outputs it chains with
-// the same section readers, so none of them can disagree about the layout.  Also the jagged round's shape rules the prover and the
-// verifier share.  Host code only.
+// The flat proof words of sp1b200_prove_shard, read and written in one place.  The wire format (wire.cu) and the shard verifier
+// (verify.cu) walk a proof through parse_shard_proof, and the shard prover (shard.cu) reads the LogUp-GKR and zerocheck outputs it
+// chains with the same section readers.  The phase provers and the wire format write the sections through the writers next to those
+// readers, so no reader or writer can disagree about the layout.  Also the jagged round's shape rules the prover and the verifier
+// share, and the copy-out of an entry point's words.  Host code only.
 //
 // Words: [5][len_0..len_4] then the sections
 //   0 main commitment (8)
@@ -17,11 +18,15 @@
 // opening  = values[num_queries][width] | root digest | log_height | width | paths digest[num_queries][log_height]
 // Every length read from the words is checked against the words that remain before it is used.
 #pragma once
+#include "hostfield.hpp"
 #include <algorithm>
 #include <cstddef>
 #include <cstdint>
+#include <cstring>
 #include <utility>
 #include <vector>
+
+const char* sp1b200_set_error(const char* fmt, ...);   // ctx.cu
 
 namespace layout {
 
@@ -37,6 +42,13 @@ struct FlatReader {
     const uint32_t* p; const uint32_t* end; bool ok = true;
     uint32_t u() { if (p >= end) { ok = false; return 0; } return *p++; }
     const uint32_t* take(size_t n) { if ((size_t)(end - p) < n) { ok = false; p = end; return nullptr; } const uint32_t* r = p; p += n; return r; }
+};
+
+struct FlatWriter {
+    std::vector<uint32_t> words;
+    void u(uint32_t x) { words.push_back(x); }
+    void put(const uint32_t* p, size_t n) { words.insert(words.end(), p, p + n); }
+    void ext(const hf::E4& e) { put(e.c, 4); }
 };
 
 struct Sumcheck {
@@ -64,6 +76,12 @@ struct Shape {
 
 // A jagged round's tables as (rows, cols) runs: its chip tables, then its two padding tables.
 using Tables = std::vector<std::pair<uint64_t, uint64_t>>;
+
+// n_tables | (rows, cols) per table: one round of the evaluation proof's row and column counts
+inline void write_tables(FlatWriter& w, const Tables& tables) {
+    w.u((uint32_t)tables.size());
+    for (auto& t : tables) { w.u((uint32_t)t.first); w.u((uint32_t)t.second); }
+}
 
 // the stacked columns of 2^log_stack cells that hold a round of `area` cells: ceil(area / 2^log_stack), at least 1
 inline uint64_t stacked_columns(uint64_t area, uint32_t log_stack) {
@@ -141,6 +159,25 @@ inline bool read_sumcheck(FlatReader& r, Sumcheck& s) {
     return r.ok;
 }
 
+// A sumcheck as its prover emits it: poly() once per round polynomial, between transcript steps, then write() once the point and
+// the evaluation are known.  The point has one coordinate per round polynomial, the most recent challenge first.
+struct SumcheckWriter {
+    FlatWriter polys;
+    uint32_t n_polys = 0;
+    void poly(const hf::E4* coeffs, uint32_t n_coeffs) {
+        polys.u(n_coeffs);
+        for (uint32_t i = 0; i < n_coeffs; i++) polys.ext(coeffs[i]);
+        n_polys++;
+    }
+    void write(FlatWriter& w, const hf::E4& claimed_sum, const hf::E4* point, const hf::E4& eval) const {
+        w.u(n_polys);
+        w.put(polys.words.data(), polys.words.size());
+        w.ext(claimed_sum);
+        for (uint32_t i = 0; i < n_polys; i++) w.ext(point[i]);
+        w.ext(eval);
+    }
+};
+
 // nullptr, or what is wrong with the opening
 inline const char* read_opening(FlatReader& r, Opening& o, size_t nq, size_t width) {
     o.values = r.take(nq * width);
@@ -149,6 +186,15 @@ inline const char* read_opening(FlatReader& r, Opening& o, size_t nq, size_t wid
     if (r.ok && (o.width != width || o.log_height > MAX_LOG_HEIGHT)) return "evaluation proof section: opening width / height words do not match the layout";
     if (r.ok) o.paths = r.take(nq * (size_t)o.log_height * 8);
     return r.ok ? nullptr : "evaluation proof section: section is shorter than its layout";
+}
+
+// values: [nq][width]; paths: [nq][log_height] digests
+inline void write_opening(FlatWriter& w, const uint32_t* values, size_t nq, uint32_t width, const uint32_t* root, uint32_t log_height,
+                          const uint32_t* paths) {
+    w.put(values, nq * width);
+    w.put(root, 8);
+    w.u(log_height); w.u(width);
+    w.put(paths, nq * (size_t)log_height * 8);
 }
 
 // The LogUp-GKR section (all of r's words) into v's LogUp-GKR fields.  Returns nullptr on success, else what is wrong.
@@ -225,6 +271,28 @@ inline const char* parse_shard_proof(const uint32_t* w, uint64_t n_words, const 
         if (!r.ok) return "evaluation proof section: section is shorter than its layout";
         if (r.p != s4) return "evaluation proof section: trailing words";
     }
+    return nullptr;
+}
+
+// The words of a shard proof whose sections 1..4 have these lengths.
+inline uint64_t shard_proof_words(uint64_t n_gkr, uint64_t n_zc, uint64_t n_ev, uint64_t n_pv) { return 6 + 8 + n_gkr + n_zc + n_ev + n_pv; }
+
+// The mirror of parse_shard_proof's split: [5][len_0..len_4] and the five sections into out (shard_proof_words of room).
+inline void write_shard_proof(uint32_t* out, const uint32_t* commit, const uint32_t* gkr, uint64_t n_gkr, const uint32_t* zc, uint64_t n_zc,
+                              const uint32_t* ev, uint64_t n_ev, const uint32_t* pv, uint64_t n_pv) {
+    const uint32_t hdr[6] = {5, 8, (uint32_t)n_gkr, (uint32_t)n_zc, (uint32_t)n_ev, (uint32_t)n_pv};
+    const std::pair<const uint32_t*, uint64_t> sections[6] = {{hdr, 6}, {commit, 8}, {gkr, n_gkr}, {zc, n_zc}, {ev, n_ev}, {pv, n_pv}};
+    for (auto& s : sections) { memcpy(out, s.first, s.second * 4); out += s.second; }
+}
+
+// Copies an entry point's words to h_out (if not NULL) after the `at` words it already wrote there.  *h_words (if not NULL) gets the
+// total either way; a total above cap is the error "<who>: <what> needs N words, capacity C" and copies nothing.
+inline const char* deliver(const char* who, const char* what, const std::vector<uint32_t>& words, uint32_t* h_out, uint64_t cap,
+                           uint64_t* h_words, uint64_t at = 0) {
+    const uint64_t total = at + words.size();
+    if (h_words) *h_words = total;
+    if (total > cap) return sp1b200_set_error("%s: %s needs %llu words, capacity %llu", who, what, (unsigned long long)total, (unsigned long long)cap);
+    if (h_out) memcpy(h_out + at, words.data(), words.size() * 4);
     return nullptr;
 }
 

@@ -64,13 +64,6 @@ static sp1b200_err with_shard_inputs(const char* who, sp1b200_ctx* ctx, const sp
     return e;
 }
 
-static sp1b200_err deliver(const char* who, const std::vector<uint32_t>& words, uint32_t* h_out, uint64_t cap, uint64_t* h_words) {
-    if (h_words) *h_words = words.size();
-    if (words.size() > cap) return sp1b200_set_error("%s: report needs %zu words, capacity %llu", who, words.size(), (unsigned long long)cap);
-    if (h_out) memcpy(h_out, words.data(), words.size() * 4);
-    return nullptr;
-}
-
 extern "C" {
 
 // debug_constraints_all_chips (crates/hypercube/src/debug.rs:27-130) on the device: report words in include/sp1b200.h
@@ -83,7 +76,7 @@ sp1b200_err sp1b200_debug_constraints(sp1b200_ctx* ctx, const sp1b200_machine* m
                                   return sp1b200_debug_constraints_device(ctx, m, h_heights, d_main.data(), d_prep.data(), h_pv, n_pv,
                                                                           max_rows_per_chip, words);
                               }));
-    return deliver("debug_constraints", words, h_out, out_cap_words, h_out_words);
+    return layout::deliver("debug_constraints", "report", words, h_out, out_cap_words, h_out_words);
 }
 
 // debug_interactions_with_all_chips (crates/hypercube/src/lookup/debug.rs:48-200) on the device: report words in include/sp1b200.h
@@ -95,13 +88,11 @@ sp1b200_err sp1b200_debug_interactions(sp1b200_ctx* ctx, const sp1b200_machine* 
                               [&](const std::vector<const uint32_t*>& d_main, const std::vector<const uint32_t*>& d_prep) {
                                   return sp1b200_debug_interactions_device(ctx, m, h_heights, d_main.data(), d_prep.data(), max_keys, words);
                               }));
-    return deliver("debug_interactions", words, h_out, out_cap_words, h_out_words);
+    return layout::deliver("debug_interactions", "report", words, h_out, out_cap_words, h_out_words);
 }
 
-// Proof words: [5][len_0..len_4] then the sections
-//   0 main commitment (8) | 1 LogUp-GKR proof (sp1b200_logup_gkr words) | 2 zerocheck proof + opened values (sp1b200_zerocheck words) |
-//   3 evaluation proof (sp1b200_jagged_prove words) | 4 public values
-// = the fields of ShardProof (crates/hypercube/src/verifier/proof.rs:47-61); chip degrees are the heights the caller passed.
+// Proof words (proof_layout.hpp): the main commitment, the sp1b200_logup_gkr, sp1b200_zerocheck and sp1b200_jagged_prove words, the
+// public values = the fields of ShardProof (crates/hypercube/src/verifier/proof.rs:47-61); chip degrees are the heights the caller passed.
 // h_replay_witnesses (grind_mode == 1): {gkr witness, batch grinding witness, pow witness}.
 sp1b200_err sp1b200_prove_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b200_jagged_round* prep_round, const uint32_t* main_dense_any,
                                 const uint64_t* h_heights, const char* const* chip_names, const uint32_t* h_pv, uint32_t n_pv,
@@ -173,23 +164,14 @@ sp1b200_err sp1b200_prove_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, sp1b
     uint64_t n_ev = 0;
     SP1_TRY(sp1b200_jagged_prove(ctx, rounds.data(), (uint32_t)rounds.size(), phases.zc.point, jclaims.data(),
                                  h_replay_witnesses ? h_replay_witnesses + 1 : nullptr, st, ev, scratch_cap, &n_ev));
-    const uint64_t total = 6 + 8 + n_gkr + n_zc + n_ev + n_pv;
+    const uint64_t total = layout::shard_proof_words(n_gkr, n_zc, n_ev, n_pv);
     t_all.stop();
     if (h_words) *h_words = total;
     // the caller's challenger is advanced only together with a delivered proof: on a capacity error h_chal is untouched and
     // *h_words holds the size to retry with
     if (h_proof && total > cap) return sp1b200_set_error("prove_shard: proof needs %llu words, capacity %llu", (unsigned long long)total, (unsigned long long)cap);
     memcpy(h_chal, st, sizeof(st));
-    if (h_proof) {
-        uint32_t* o = h_proof;
-        const uint32_t hdr[6] = {5, 8, (uint32_t)n_gkr, (uint32_t)n_zc, (uint32_t)n_ev, n_pv};
-        memcpy(o, hdr, 24); o += 6;
-        memcpy(o, commit, 32); o += 8;
-        memcpy(o, gkr, n_gkr * 4); o += n_gkr;
-        memcpy(o, zc, n_zc * 4); o += n_zc;
-        memcpy(o, ev, n_ev * 4); o += n_ev;
-        memcpy(o, h_pv, n_pv * 4);
-    }
+    if (h_proof) layout::write_shard_proof(h_proof, commit, gkr, n_gkr, zc, n_zc, ev, n_ev, h_pv, n_pv);
     return nullptr;
 }
 

@@ -87,12 +87,11 @@ struct BinReader {
     void fail(const char* m) { if (ok) { ok = false; why = m; } }
     // a length that is about to be used to read at least `unit` bytes per element
     uint64_t len(size_t unit) { const uint64_t n = u64(); if (ok && unit && n > (uint64_t)(end - p) / unit) fail("length prefix exceeds the input"); return ok ? n : 0; }
-};
-
-struct FlatWriter {
-    std::vector<uint32_t> w;
-    void u(uint64_t v, BinReader& r) { if (v > 0xffffffffull) r.fail("count does not fit the flat layout"); w.push_back((uint32_t)v); }
-    void fs(BinReader& r, size_t n) { for (size_t i = 0; i < n && r.ok; i++) w.push_back(r.f()); }
+    // a count about to become one flat word
+    uint32_t narrow(uint64_t v) { if (v > 0xffffffffull) fail("count does not fit the flat layout"); return (uint32_t)v; }
+    // n field elements onto o / as n extension elements (zero after a failure); reading stops at the first failure
+    void fs(layout::FlatWriter& o, uint64_t n) { for (uint64_t i = 0; i < n && ok; i++) o.u(f()); }
+    std::vector<hf::E4> exts(uint64_t n) { std::vector<hf::E4> v(n); for (auto& x : v) for (int i = 0; i < 4 && ok; i++) x.c[i] = f(); return v; }
 };
 
 void get_dims(BinReader& r, std::initializer_list<uint64_t> want) {
@@ -101,41 +100,43 @@ void get_dims(BinReader& r, std::initializer_list<uint64_t> want) {
     for (uint64_t x : want) if (r.u64() != x) r.fail("tensor dimensions do not match its storage");
 }
 
-void get_sumcheck(BinReader& r, FlatWriter& o) {
+void get_sumcheck(BinReader& r, layout::FlatWriter& o) {
     const uint64_t n = r.len(8);
-    o.u(n, r);
-    for (uint64_t i = 0; i < n && r.ok; i++) { const uint64_t m = r.len(16); o.u(m, r); o.fs(r, 4 * m); }
-    o.fs(r, 4);
+    r.narrow(n);
+    layout::SumcheckWriter s;
+    for (uint64_t i = 0; i < n && r.ok; i++) { const uint32_t m = r.narrow(r.len(16)); s.poly(r.exts(m).data(), m); }
+    const hf::E4 claimed_sum = r.exts(1)[0];
     if (r.len(16) != n) r.fail("sumcheck point dimension differs from the number of round polynomials");
-    o.fs(r, 4 * n);
-    o.fs(r, 4);
+    const std::vector<hf::E4> point = r.exts(n);   // at least n_polys coordinates
+    s.write(o, claimed_sum, point.data(), r.exts(1)[0]);
 }
 
 // MleEval<EF>; returns the number of evaluations
-uint64_t get_mle_eval(BinReader& r, FlatWriter& o) {
+uint64_t get_mle_eval(BinReader& r, layout::FlatWriter& o) {
     const uint64_t n = r.len(16);
-    o.fs(r, 4 * n);
+    r.fs(o, 4 * n);
     get_dims(r, {n});
     return n;
 }
 
-void get_opening(BinReader& r, FlatWriter& o) {
+void get_opening(BinReader& r, layout::FlatWriter& o) {
     const uint64_t nv = r.len(4);
-    const size_t at = o.w.size();
-    o.fs(r, nv);
+    layout::FlatWriter values, root, paths;
+    r.fs(values, nv);
     const uint64_t nd = r.len(8);
     if (nd != 2) { r.fail("opening values are not a 2-D tensor"); return; }
     const uint64_t nq = r.u64(), width = r.u64();
     if (nq * width != nv) r.fail("opening values: dimensions do not match the storage");
-    (void)at;
-    o.fs(r, 8);
+    r.fs(root, 8);
     const uint64_t lh = r.u64(), wd = r.u64();
     if (wd != width) r.fail("opening: proof width differs from the width of the values");
-    o.u(lh, r); o.u(wd, r);
+    r.narrow(lh); r.narrow(wd);
     const uint64_t np = r.len(32);
     if (np != nq * lh) r.fail("opening: number of path digests is not queries x log_height");
-    o.fs(r, 8 * np);
+    r.fs(paths, 8 * np);
     get_dims(r, {nq, lh});
+    // only an intact opening has the words its dimensions promise
+    if (r.ok) layout::write_opening(o, values.words.data(), nq, (uint32_t)wd, root.words.data(), (uint32_t)lh, paths.words.data());
 }
 
 bool names_sorted(const char* const* names, size_t n) {
@@ -232,7 +233,7 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
     if (mlr > 62) return sp1b200_set_error("shard_proof_from_bincode: parameters out of range");
     if (!names_sorted(chip_names, nch)) return sp1b200_set_error("shard_proof_from_bincode: chip names must be strictly ascending (BTreeMap order)");
     BinReader r{h_bytes, h_bytes + n_bytes};
-    FlatWriter pv, gkr, zc, ev;
+    layout::FlatWriter pv, gkr, zc, ev;
     uint32_t commit[8];
     auto chip_name = [&](size_t k) {
         const uint64_t n = r.len(1);
@@ -241,21 +242,21 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
         r.p += n;
     };
     const uint64_t n_pv = r.len(4);
-    pv.fs(r, n_pv);
+    r.fs(pv, n_pv);
     for (int i = 0; i < 8; i++) commit[i] = r.f();
     {   // logup_gkr_proof
         uint64_t n_out = 0;
         for (int side = 0; side < 2 && r.ok; side++) {
             const uint64_t n = r.len(16);
-            if (side == 0) { n_out = n; gkr.u(n, r); } else if (n != n_out) r.fail("circuit output: numerator and denominator lengths differ");
-            gkr.fs(r, 4 * n);
+            if (side == 0) { n_out = n; gkr.u(r.narrow(n)); } else if (n != n_out) r.fail("circuit output: numerator and denominator lengths differ");
+            r.fs(gkr, 4 * n);
             get_dims(r, {n, 1});
         }
         const uint64_t nr = r.len(64);
-        gkr.u(nr, r);
-        for (uint64_t i = 0; i < nr && r.ok; i++) { gkr.fs(r, 16); get_sumcheck(r, gkr); }
+        gkr.u(r.narrow(nr));
+        for (uint64_t i = 0; i < nr && r.ok; i++) { r.fs(gkr, 16); get_sumcheck(r, gkr); }
         if (r.len(16) != mlr) r.fail("LogUp evaluation point is not max_log_row_count long");
-        gkr.fs(r, 4 * (size_t)mlr);
+        r.fs(gkr, 4 * (size_t)mlr);
         if (r.len(8) != nch) r.fail("chip_openings: number of chips differs from the machine's");
         for (size_t k = 0; k < nch && r.ok; k++) {
             chip_name(k);
@@ -265,16 +266,16 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
             if ((tag == 1) != (h_prep_w[k] != 0)) r.fail("chip_openings: preprocessed openings present/absent against the machine");
             if (tag == 1 && get_mle_eval(r, gkr) != h_prep_w[k]) r.fail("chip_openings: preprocessed width differs from the machine's");
         }
-        gkr.fs(r, 1);
+        r.fs(gkr, 1);
     }
     get_sumcheck(r, zc);
     if (r.len(8) != nch) r.fail("opened_values: number of chips differs from the machine's");
     for (size_t k = 0; k < nch && r.ok; k++) {
         chip_name(k);
         if (r.len(16) != h_prep_w[k]) r.fail("opened_values: preprocessed width differs from the machine's");
-        zc.fs(r, 4 * (size_t)h_prep_w[k]);
+        r.fs(zc, 4 * (size_t)h_prep_w[k]);
         if (r.len(16) != h_main_w[k]) r.fail("opened_values: main width differs from the machine's");
-        zc.fs(r, 4 * (size_t)h_main_w[k]);
+        r.fs(zc, 4 * (size_t)h_main_w[k]);
         if (r.len(4) != mlr + 1) r.fail("opened_values: degree is not max_log_row_count + 1 bits");
         uint64_t h = 0;
         for (uint32_t i = 0; i <= mlr && r.ok; i++) { const uint32_t bit = r.u32(); if (bit > 1) r.fail("opened_values: degree coordinate is not a bit"); h = (h << 1) | bit; }
@@ -282,43 +283,37 @@ sp1b200_err sp1b200_shard_proof_from_bincode(const sp1b200_params* params, uint3
     }
     {   // evaluation_proof
         const uint64_t n_um = r.len(32);
-        ev.fs(r, 8 * n_um);
+        r.fs(ev, 8 * n_um);
         if (r.len(32) != n_um) r.fail("fri_commitments and univariate_messages differ in length");
-        ev.fs(r, 8 * n_um);
+        r.fs(ev, 8 * n_um);
         if (n_um != params->log_stacking_height) r.fail("BaseFold proof does not have log_stacking_height rounds");
         const uint64_t n_rounds = r.len(64);
         for (uint64_t q = 0; q < n_rounds && r.ok; q++) get_opening(r, ev);
         if (r.len(64) != n_um) r.fail("query phase does not have one opening per fold round");
         for (uint64_t q = 0; q < n_um && r.ok; q++) get_opening(r, ev);
-        ev.fs(r, 6);
+        r.fs(ev, 6);
         if (r.len(24) != n_rounds) r.fail("batch_evaluations: number of rounds differs");
         for (uint64_t q = 0; q < n_rounds && r.ok; q++) get_mle_eval(r, ev);
         get_sumcheck(r, ev); get_sumcheck(r, ev);
         if (r.len(8) != n_rounds) r.fail("row/column counts: number of rounds differs");
         for (uint64_t q = 0; q < n_rounds && r.ok; q++) {
-            const uint64_t cnt = r.len(16);
-            ev.u(cnt, r);
-            for (uint64_t i = 0; i < cnt && r.ok; i++) { ev.u(r.u64(), r); ev.u(r.u64(), r); }
+            layout::Tables t(r.narrow(r.len(16)));
+            for (auto& rc : t) if (r.ok) { rc.first = r.narrow(r.u64()); rc.second = r.narrow(r.u64()); }
+            layout::write_tables(ev, t);
         }
         if (r.len(32) != n_rounds) r.fail("merkle_tree_commitments: number of rounds differs");
-        ev.fs(r, 8 * n_rounds);
-        ev.fs(r, 4);
-        ev.u(r.u64(), r); ev.u(r.u64(), r);
+        r.fs(ev, 8 * n_rounds);
+        r.fs(ev, 4);
+        ev.u(r.narrow(r.u64())); ev.u(r.narrow(r.u64()));
     }
     if (r.ok && r.p != r.end) r.fail("trailing bytes");
     if (!r.ok) return sp1b200_set_error("shard_proof_from_bincode: %s (at byte %llu of %llu)", r.why, (unsigned long long)(r.p - h_bytes), (unsigned long long)n_bytes);
-    const uint64_t total = 6 + 8 + gkr.w.size() + zc.w.size() + ev.w.size() + pv.w.size();
+    const uint64_t total = layout::shard_proof_words(gkr.words.size(), zc.words.size(), ev.words.size(), pv.words.size());
     if (h_words) *h_words = total;
     if (h_proof) {
         if (total > cap_words) return sp1b200_set_error("shard_proof_from_bincode: needs %llu words, capacity %llu", (unsigned long long)total, (unsigned long long)cap_words);
-        uint32_t* o = h_proof;
-        const uint32_t hdr[6] = {5, 8, (uint32_t)gkr.w.size(), (uint32_t)zc.w.size(), (uint32_t)ev.w.size(), (uint32_t)pv.w.size()};
-        memcpy(o, hdr, 24); o += 6;
-        memcpy(o, commit, 32); o += 8;
-        memcpy(o, gkr.w.data(), gkr.w.size() * 4); o += gkr.w.size();
-        memcpy(o, zc.w.data(), zc.w.size() * 4); o += zc.w.size();
-        memcpy(o, ev.w.data(), ev.w.size() * 4); o += ev.w.size();
-        memcpy(o, pv.w.data(), pv.w.size() * 4);
+        layout::write_shard_proof(h_proof, commit, gkr.words.data(), gkr.words.size(), zc.words.data(), zc.words.size(), ev.words.data(),
+                                  ev.words.size(), pv.words.data(), pv.words.size());
     }
     return nullptr;
 }

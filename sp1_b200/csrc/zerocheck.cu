@@ -14,6 +14,7 @@
 #include "challenger.cuh"
 #include "hostfield.hpp"
 #include "kb31.cuh"
+#include "proof_layout.hpp"
 #include <algorithm>
 #include <memory>
 #include <vector>
@@ -524,7 +525,7 @@ uint32_t sp1b200_machine_num_chips(const sp1b200_machine* m) { return (uint32_t)
 // d_main[k] / d_prep[k]: device pointers, column-major [w x heights[k]] base-field columns (prep may be NULL when prep_w == 0);
 // h_alpha / h_gamma: the constraint- and opening-batching challenges already sampled by the caller (shard.rs:707-709);
 // h_claims: per chip Σ_j gamma^(j+1) opening_j (main then preprocessed) from LogUp-GKR; h_gkr_point: max_log_row_count ext.
-// Output words: sumcheck proof {n_polys, per poly {n_coeffs, coeffs}, claimed_sum, point, eval} | per chip {prep evals, main evals}.
+// Output words: the zerocheck section of a shard proof (proof_layout.hpp).
 sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint64_t* h_heights, const uint32_t* const* d_main,
                               const uint32_t* const* d_prep, const uint32_t* h_pv, uint32_t n_pv, const uint32_t* h_gkr_point,
                               const uint32_t* h_alpha, const uint32_t* h_gamma, const uint32_t* h_claims, uint32_t* h_chal, uint32_t* h_out,
@@ -725,8 +726,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
     std::vector<E4> round_claims(nchips);
     E4 claimed_sum;
     for (size_t k = 0; k < nchips; k++) { round_claims[k] = E4::load(h_claims + 4 * k); claimed_sum = claimed_sum * lambda + round_claims[k]; }
-    std::vector<uint32_t> words;
-    words.push_back(mlr);
+    layout::SumcheckWriter sc;
     std::vector<E4> point;
     std::vector<E4> ys((size_t)nchips * 4);  // per chip: round polynomial values at the nodes 0, 1, 2, 4
     std::vector<uint32_t> hs((size_t)max_jobs * 36);
@@ -795,8 +795,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         E4 rlc[5];
         for (int c5 = 0; c5 < 5; c5++) for (int i = 0; i < 4; i++) rlc[c5] = rlc[c5] + basis[i][c5] * Y[i];
         for (auto& c : rlc) ch.observe_n(c.c, 4);
-        words.push_back(5);
-        for (auto& c : rlc) words.insert(words.end(), c.c, c.c + 4);
+        sc.poly(rlc, 5);
         E4 a; ch.sample_ext(a.c);
         point.insert(point.begin(), a);
         const Ext da = to_ext(a);
@@ -826,9 +825,8 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
     }
     E4 final_eval;
     for (auto& c : round_claims) final_eval = final_eval * lambda + c;
-    words.insert(words.end(), claimed_sum.c, claimed_sum.c + 4);
-    for (auto& x : point) words.insert(words.end(), x.c, x.c + 4);
-    words.insert(words.end(), final_eval.c, final_eval.c + 4);
+    layout::FlatWriter proof;
+    sc.write(proof, claimed_sum, point.data(), final_eval);
     // opened values: one EF row per chip (main columns then preprocessed, zeros for absent chips), fetched with one copy;
     // observed and emitted prep-first as the reference does
     std::vector<uint32_t> fin((wsum ? wsum : 1) * 4);
@@ -841,15 +839,12 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         const uint32_t* pvv = mv + 4 * (size_t)p.main_w;
         ch.observe(hf::to_monty(p.prep_w)); ch.observe_n(pvv, (size_t)p.prep_w * 4);
         ch.observe(hf::to_monty(p.main_w)); ch.observe_n(mv, (size_t)p.main_w * 4);
-        words.insert(words.end(), pvv, pvv + (size_t)p.prep_w * 4);
-        words.insert(words.end(), mv, mv + (size_t)p.main_w * 4);
+        proof.put(pvv, (size_t)p.prep_w * 4);
+        proof.put(mv, (size_t)p.main_w * 4);
     }
     t_all.stop();
     ch.store(h_chal);
-    if (h_words) *h_words = words.size();
-    if (words.size() > cap) return sp1b200_set_error("zerocheck: output needs %zu words, capacity %llu", words.size(), (unsigned long long)cap);
-    if (h_out) memcpy(h_out, words.data(), words.size() * 4);
-    return nullptr;
+    return layout::deliver("zerocheck", "output", proof.words, h_out, cap, h_words);
 }
 
 }  // extern "C"
