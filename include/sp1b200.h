@@ -439,6 +439,76 @@ sp1b200_err sp1b200_verify_core_proof(sp1b200_ctx* ctx, const sp1b200_machine* m
                                       uint32_t host_threads, uint32_t* h_final_challengers, uint32_t* h_verdict, uint32_t* h_shard,
                                       uint32_t* h_shard_verdict);
 
+/* ---- recursion keys, public values and the recursion vk map (host only unless a context is taken) ---------------------------------
+ * MachineVerifyingKey::hash_koalabear without mprotect (crates/hypercube/src/verifier/hashable_key.rs:94-118): poseidon2_hash of the 26
+ * words prep_commit[8] | pc_start[3] | initial_global_cumulative_sum x[7] y[7] | enable_untrusted_programs, i.e. the commitment and the
+ * first 18 words of the 24-word vk_tail that sp1b200_setup_and_prove_shard takes (its 6 padding words are observed, not hashed).
+ * n_vk_tail must be 24. */
+sp1b200_err sp1b200_vk_hash(const uint32_t* h_prep_commit8, const uint32_t* h_vk_tail, uint32_t n_vk_tail, uint32_t* h_out8);
+/* koalabears_to_bn254 (hashable_key.rs:23-33) as 32 big-endian bytes, the vk.bytes32() value: the canonical words concatenated 31 bits
+ * apart, first word most significant (248 bits < r, so no reduction; byte 0 is zero). */
+sp1b200_err sp1b200_digest_bytes32(const uint32_t* h_digest8, uint8_t* h_out32);
+/* recursion_public_values_digest (crates/prover/src/utils.rs:22-28): the sponge over the first NUM_PV_ELMS_TO_HASH = 175 words of the 187
+ * words of RecursionPublicValues (crates/recursion/executor/src/public_values.rs:39-143; sp1_vk_digest at 136, vk_root at 144,
+ * is_complete at 168, digest at 175, proof_nonce at 183). */
+sp1b200_err sp1b200_recursion_pv_digest(const uint32_t* h_pv187, uint32_t* h_out8);
+
+/* RecursionVks::from_map (crates/prover/src/recursion.rs:59-87): the digests (n x 8 words) deduplicated and sorted in canonical
+ * lexicographic order, [i; 8] added for every index i below pad_to the keys do not reach (as the development map is padded), then
+ * MerkleTree::commit (crates/recursion/circuit/src/basefold/merkle_tree.rs:24-64): key i is leaf i, padded with zero digests to a power
+ * of two, leaves stored bit-reversed, layers compressed pairwise on the device (the tree kernels of sp1b200_merkle_commit; memory from the
+ * context's pool, returned before the call ends).  The layers are then kept on the host.  Fewer than two keys, more than 2^26, or a
+ * non-canonical word is an error.  vk_verification: whether sp1b200_verify_compressed checks a proof's key against the map. */
+typedef struct sp1b200_recursion_vks sp1b200_recursion_vks;
+sp1b200_err sp1b200_recursion_vks_create(sp1b200_ctx* ctx, const uint32_t* h_digests, uint64_t n, uint64_t pad_to, int vk_verification,
+                                         sp1b200_recursion_vks** out);
+void sp1b200_recursion_vks_free(sp1b200_recursion_vks* vks);
+void sp1b200_recursion_vks_root(const sp1b200_recursion_vks* vks, uint32_t* h_out8);
+uint64_t sp1b200_recursion_vks_num_keys(const sp1b200_recursion_vks* vks);
+/* RecursionVks::open / MerkleTree::open (recursion.rs:141-170, merkle_tree.rs:66-88): the index of digest8 in the map and its Merkle path
+ * (*h_n_path = the tree height digests of 8 words into h_path, path_cap digests of room).  A digest outside the map is an error ("vk not
+ * allowed").  The path verifies as verify_merkle_proof (crates/hypercube/src/verifier/proof.rs:121-143) does: reverse_bits_len(index,
+ * path length) - index bits above the path length are ignored - then one compression per sibling, the sibling on the left when the low
+ * bit is one. */
+sp1b200_err sp1b200_recursion_vks_open(const sp1b200_recursion_vks* vks, const uint32_t* h_digest8, uint64_t* h_index, uint32_t* h_path,
+                                       uint32_t path_cap, uint32_t* h_n_path);
+
+/* ---- compressed / shrink proof verifier (SP1Prover::verify_compressed / verify_shrink, crates/prover/src/verify.rs:527-642) ---------
+ * Verifies n_proofs recursion proofs of one machine at the context's parameters.  Proof s has its own verifying key
+ * h_vks[s * 32 ..]: preprocessed commitment[8] | vk_tail[24] (as sp1b200_vk_hash), its chip heights h_heights[s * n_chips ..], its
+ * flat proof words (sp1b200_prove_shard words), its vk_merkle_proof (h_vk_index[s], h_vk_path_len[s] <= 64 digests at h_vk_paths[s]) and
+ * the digest of the SP1 program key the proof must be for (h_sp1_vk_digests[s * 8 ..], the reference's vk.hash_koalabear()).
+ * mode SP1B200_COMPRESSED takes no shrink key (h_shrink_vk must be NULL); mode SP1B200_SHRINK compares every proof's key with
+ * h_shrink_vk (32 words as above, NULL = not initialised) word for word.  The Rust key's chip information is not compared: here it is
+ * fixed by the machine and heights passed in.  Checks per proof, in the reference's order:
+ *   shrink only: UninitializedVerificationKey (h_shrink_vk NULL), InvalidVerificationKey (key differs);
+ *   InvalidPublicValues(invalid public values length) (not 187 public values; code 46);
+ *   InvalidShardProof (code 45; h_shard_verdicts[s] = the verify_shard code), from a fresh transcript that observed the proof's key;
+ *   the public values' digest (words 175..182) is not the digest of words 0..174; vk_root (144..151) is not the map's root;
+ *   InvalidVerificationKey when the map has vk_verification on and the Merkle proof of sp1b200_vk_hash(key) does not reach the root;
+ *   is_complete (168) is not 1; sp1_vk_digest (136..143) differs from the expected digest.
+ * h_verdicts[s] = 0 accepts (h_final_challengers[s * 34 ..], optional, then holds the verifier's final transcript state), else the first
+ * failing check (sp1b200_verdict_name).  The host phases run on host_threads threads (0 = the hardware concurrency); the device work of
+ * all proofs runs in one launch per kernel for each batch of at most 2^26 proof words (SP1B200_VERIFY_BATCH_WORDS can lower the cap;
+ * batching never changes a verdict).  Errors: a proof that does not parse (as sp1b200_verify_shard), a vk Merkle path longer than 64, a
+ * non-canonical word in a key, path or expected digest, NULL pointers, n_proofs = 0.  A rejection is not an error; the context stays
+ * usable after either. */
+#define SP1B200_COMPRESSED 0u
+#define SP1B200_SHRINK 1u
+#define SP1B200_VERDICT_RECURSION_PV_DIGEST 77u         /* InvalidPublicValues(recursion public values are invalid) */
+#define SP1B200_VERDICT_VK_ROOT 78u                     /* InvalidPublicValues(vk_root mismatch) */
+#define SP1B200_VERDICT_INVALID_VERIFICATION_KEY 79u    /* InvalidVerificationKey: shrink key differs, or the key is not in the vk map */
+#define SP1B200_VERDICT_IS_COMPLETE 80u                 /* InvalidPublicValues(is_complete is not 1) */
+#define SP1B200_VERDICT_SP1_VK_DIGEST 81u               /* InvalidPublicValues(sp1 vk hash mismatch) */
+#define SP1B200_VERDICT_UNINITIALIZED_VERIFICATION_KEY 82u /* UninitializedVerificationKey: shrink mode without a shrink key */
+#define SP1B200_VERDICT_COMPRESSED_COUNT 83u            /* one past the last code */
+sp1b200_err sp1b200_verify_compressed(sp1b200_ctx* ctx, const sp1b200_machine* machine, const sp1b200_recursion_vks* vks, uint32_t mode,
+                                      const uint32_t* h_shrink_vk, uint32_t n_proofs, const uint32_t* h_vks, const uint64_t* h_heights,
+                                      const char* const* chip_names, const uint32_t* const* h_proofs, const uint64_t* h_n_words,
+                                      const uint64_t* h_vk_index, const uint32_t* const* h_vk_paths, const uint32_t* h_vk_path_len,
+                                      const uint32_t* h_sp1_vk_digests, uint32_t host_threads, uint32_t* h_final_challengers,
+                                      uint32_t* h_verdicts, uint32_t* h_shard_verdicts);
+
 #ifdef __cplusplus
 }
 #endif

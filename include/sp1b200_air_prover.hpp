@@ -237,6 +237,61 @@ class AirProver {
         return v;
     }
 
+    // SP1Prover::verify_compressed / verify_shrink (crates/prover/src/verify.rs:527-642) of recursion proofs of this machine
+    // (sp1b200_verify_compressed): each with its own key (prep_commit[8] | vk_tail[24]), chip heights, proof words, vk Merkle proof
+    // (sp1b200_recursion_vks_open) and the SP1 program key digest it must be for.  shrink_vk != nullptr selects shrink mode, checked
+    // against *shrink_vk; shrink mode without a key is SP1B200_SHRINK with shrink_vk_missing = true.  Proofs that do not parse throw.
+    struct RecursionProof {
+        std::vector<uint32_t> vk;                       // 32 words
+        std::vector<uint64_t> heights;
+        std::vector<uint32_t> words;
+        uint64_t vk_index = 0;
+        std::vector<Digest> vk_path;
+        Digest sp1_vk_digest{};
+    };
+    struct CompressedVerdict {
+        uint32_t code = SP1B200_VERDICT_ACCEPT, shard_code = SP1B200_VERDICT_ACCEPT;
+        std::string reason, shard_reason;
+        Challenger final_challenger{};
+        bool accepted() const { return code == SP1B200_VERDICT_ACCEPT; }
+    };
+    std::vector<CompressedVerdict> verify_compressed(const sp1b200_recursion_vks* vks, const std::vector<RecursionProof>& proofs,
+                                                     const std::vector<uint32_t>* shrink_vk = nullptr, bool shrink_vk_missing = false,
+                                                     uint32_t host_threads = 0) {
+        std::vector<const char*> names;
+        for (const Chip& c : chips_) names.push_back(c.name.c_str());
+        std::vector<uint32_t> keys, digests, path_len;
+        std::vector<uint64_t> h, nw, index;
+        std::vector<const uint32_t*> words, paths;
+        for (const RecursionProof& p : proofs) {
+            if (p.heights.size() != chips_.size()) throw Error("verify_compressed: one height per chip expected");
+            if (p.vk.size() != 32) throw Error("verify_compressed: a verifying key has 32 words");
+            keys.insert(keys.end(), p.vk.begin(), p.vk.end());
+            h.insert(h.end(), p.heights.begin(), p.heights.end());
+            words.push_back(p.words.data());
+            nw.push_back(p.words.size());
+            index.push_back(p.vk_index);
+            paths.push_back(p.vk_path.empty() ? nullptr : p.vk_path[0].data());
+            path_len.push_back((uint32_t)p.vk_path.size());
+            digests.insert(digests.end(), p.sp1_vk_digest.begin(), p.sp1_vk_digest.end());
+        }
+        const bool shrink = shrink_vk || shrink_vk_missing;
+        if (shrink_vk && shrink_vk->size() != 32) throw Error("verify_compressed: the shrink key has 32 words");
+        std::vector<uint32_t> fin(34 * proofs.size()), code(proofs.size()), shard_code(proofs.size());
+        check(sp1b200_verify_compressed(ctx_, machine_, vks, shrink ? SP1B200_SHRINK : SP1B200_COMPRESSED, shrink_vk ? shrink_vk->data() : nullptr,
+                                        (uint32_t)proofs.size(), keys.data(), h.data(), names.data(), words.data(), nw.data(), index.data(),
+                                        paths.data(), path_len.data(), digests.data(), host_threads, fin.data(), code.data(), shard_code.data()));
+        std::vector<CompressedVerdict> out(proofs.size());
+        for (size_t s = 0; s < proofs.size(); s++) {
+            out[s].code = code[s];
+            out[s].shard_code = shard_code[s];
+            out[s].reason = sp1b200_verdict_name(code[s]);
+            out[s].shard_reason = sp1b200_verdict_name(shard_code[s]);
+            if (out[s].accepted()) std::copy(fin.begin() + 34 * s, fin.begin() + 34 * (s + 1), out[s].final_challenger.data());
+        }
+        return out;
+    }
+
     // bincode(ShardProof) of a proof returned by prove_shard_with_pk / setup_and_prove_shard: the bytes the reference's workers, recursion
     // tree and verifier exchange (crates/hypercube/src/verifier/proof.rs:47-61; sp1b200_shard_proof_to_bincode)
     std::vector<uint8_t> to_bincode(const std::vector<uint32_t>& proof_words, const std::vector<uint64_t>& heights) const {

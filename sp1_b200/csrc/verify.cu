@@ -1,5 +1,6 @@
 // ShardVerifier::verify_shard (crates/hypercube/src/verifier/shard.rs:437-750) on the flat proof words of sp1b200_prove_shard, for one
-// shard (sp1b200_verify_shard) or for every shard of a core proof (sp1b200_verify_core_proof, verify_core.cu).
+// shard (sp1b200_verify_shard), for every shard of a core proof (sp1b200_verify_core_proof, verify_core.cu) or for a list of recursion
+// proofs (sp1b200_verify_compressed, recursion_vks.cu).
 // A shard is verified in two phases.  The host phase - the transcript, the PoW checks, the GKR / zerocheck / jagged sumcheck rounds, the
 // branching program and every chip's constraints at the zerocheck point (a few thousand extension-field operations) - touches no CUDA
 // API: it records the device work the queries need (ShardWork), so the host phases of many shards can run on as many threads.  The
@@ -832,6 +833,7 @@ sp1b200_err verify_parse_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, const
     if (!m->interactions || m->host.size() != nch) return sp1b200_set_error("%s: machine is not initialised", who);
     if (has_prep && !h_prep_commit8) return sp1b200_set_error("%s: the machine has preprocessed columns but h_prep_commit8 is NULL", who);
     out.heights = h_heights;
+    out.prep_commit8 = h_prep_commit8;
     layout::Shape& shape = out.shape;
     shape.n_chips = nch; shape.main_w = out.mw.data(); shape.prep_w = out.pw.data();
     shape.max_log_row_count = mlr; shape.log_stacking_height = ls; shape.num_queries = nq;
@@ -855,25 +857,25 @@ sp1b200_err verify_parse_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, const
     return nullptr;
 }
 
-sp1b200_err verify_shards(sp1b200_ctx* ctx, const sp1b200_machine* m, const uint32_t* h_prep_commit8, const char* const* chip_names,
-                          const std::vector<const VerifyShardIn*>& shards, const uint32_t* start34, uint32_t host_threads,
+sp1b200_err verify_shards(sp1b200_ctx* ctx, const sp1b200_machine* m, const char* const* chip_names,
+                          const std::vector<const VerifyShardIn*>& shards, const std::vector<const uint32_t*>& starts, uint32_t host_threads,
                           uint32_t* verdicts, uint32_t* finals, VerifyTimes& t) {
     const size_t n = shards.size();
     std::vector<std::unique_ptr<Verifier>> vs;
     std::vector<Verifier*> vp;
     for (const VerifyShardIn* in : shards) {
-        vs.emplace_back(new Verifier(ctx->params, m, in->p, in->heights, chip_names, in->shape.ncols, h_prep_commit8));
+        vs.emplace_back(new Verifier(ctx->params, m, in->p, in->heights, chip_names, in->shape.ncols, in->prep_commit8));
         vp.push_back(vs.back().get());
     }
     const auto h0 = std::chrono::steady_clock::now();
     const size_t nt = std::min<size_t>(std::max<uint32_t>(host_threads, 1), n);
     if (nt <= 1) {
-        for (auto& v : vs) v->run(start34);
+        for (size_t s = 0; s < n; s++) vs[s]->run(starts[s]);
     } else {   // the host phases share nothing but the read-only machine; each thread takes the next shard
         std::atomic<size_t> next{0};
         std::vector<std::thread> pool;
         for (size_t i = 0; i < nt; i++)
-            pool.emplace_back([&] { for (size_t s; (s = next.fetch_add(1)) < n;) vs[s]->run(start34); });
+            pool.emplace_back([&] { for (size_t s; (s = next.fetch_add(1)) < n;) vs[s]->run(starts[s]); });
         for (auto& th : pool) th.join();
     }
     t.host_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - h0).count();
@@ -888,6 +890,7 @@ extern "C" {
 const char* sp1b200_verdict_name(uint32_t verdict) {
     if (verdict < std::size(VERDICT_NAMES)) return VERDICT_NAMES[verdict];
     const char* core = verify_core_verdict_name(verdict);
+    if (!core) core = verify_compressed_verdict_name(verdict);
     return core ? core : "Unknown";
 }
 
@@ -900,7 +903,7 @@ sp1b200_err sp1b200_verify_shard(sp1b200_ctx* ctx, const sp1b200_machine* m, con
     SP1_TRY(verify_parse_shard(ctx, m, h_prep_commit8, h_heights, chip_names, h_proof, n_words, "verify_shard", in));
     uint32_t verdict = SP1B200_VERDICT_ACCEPT, fin[34];
     VerifyTimes t;
-    SP1_TRY(verify_shards(ctx, m, h_prep_commit8, chip_names, {&in}, h_chal, 1, &verdict, fin, t));
+    SP1_TRY(verify_shards(ctx, m, chip_names, {&in}, {h_chal}, 1, &verdict, fin, t));
     float kernel_ms = 0;
     if (t.fold_ran) { ctx->phase_ms["verify.merkle"] = t.merkle; ctx->phase_ms["verify.fold"] = t.fold; kernel_ms += t.merkle + t.fold; }
     if (t.jagged_ran) { ctx->phase_ms["verify.jagged_eval"] = t.jagged; kernel_ms += t.jagged; }

@@ -175,14 +175,14 @@ uint32_t check_public_values(const std::vector<const uint32_t*>& pvs, const std:
     return SP1B200_VERDICT_ACCEPT;
 }
 
-uint64_t batch_words_cap() {
+}  // namespace
+
+uint64_t verify_batch_words_cap() {
     const char* e = getenv("SP1B200_VERIFY_BATCH_WORDS");
     if (!e || !*e) return DEFAULT_BATCH_WORDS;
     const unsigned long long v = strtoull(e, nullptr, 10);
     return v ? std::min<uint64_t>(v, DEFAULT_BATCH_WORDS) : DEFAULT_BATCH_WORDS;
 }
-
-}  // namespace
 
 const char* verify_core_verdict_name(uint32_t verdict) {
     if (verdict < SP1B200_VERDICT_EMPTY_PROOF || verdict >= SP1B200_VERDICT_CORE_COUNT) return nullptr;
@@ -234,9 +234,9 @@ sp1b200_err sp1b200_verify_core_proof(sp1b200_ctx* ctx, const sp1b200_machine* m
         ch.observe_n(h_vk_tail, n_vk_tail);
         ch.store(start);
         if (!host_threads) host_threads = std::max(1u, std::thread::hardware_concurrency());
-        // batches of consecutive shards with at most batch_words_cap() proof words (at least one shard each), in order: the first
-        // failing shard of the first failing batch is the lowest failing shard
-        const uint64_t cap = batch_words_cap();
+        // batches of consecutive shards with at most verify_batch_words_cap() proof words (at least one shard each), in order: the
+        // first failing shard of the first failing batch is the lowest failing shard
+        const uint64_t cap = verify_batch_words_cap();
         std::vector<uint32_t> verdicts(n_shards);
         for (uint32_t a = 0; a < n_shards && !verdict;) {
             uint32_t b = a + 1;
@@ -244,8 +244,8 @@ sp1b200_err sp1b200_verify_core_proof(sp1b200_ctx* ctx, const sp1b200_machine* m
             while (b < n_shards && words + h_n_words[b] <= cap) words += h_n_words[b++];
             std::vector<const VerifyShardIn*> batch;
             for (uint32_t s = a; s < b; s++) batch.push_back(in[s].get());
-            SP1_TRY(verify_shards(ctx, m, has_prep ? h_prep_commit8 : nullptr, chip_names, batch, start, host_threads, verdicts.data() + a,
-                                  finals.data() + 34 * (size_t)a, t));
+            SP1_TRY(verify_shards(ctx, m, chip_names, batch, std::vector<const uint32_t*>(batch.size(), start), host_threads,
+                                  verdicts.data() + a, finals.data() + 34 * (size_t)a, t));
             for (uint32_t s = a; s < b; s++)
                 if (verdicts[s]) { verdict = SP1B200_VERDICT_INVALID_SHARD_PROOF; shard = s; *h_shard_verdict = verdicts[s]; break; }
             a = b;

@@ -30,6 +30,11 @@ PV = dict(prev_committed_value_digest=(0, 32), committed_value_digest=(32, 32), 
 PV_NUM_ELTS = 160
 PV_MAX_NUM = 187
 VK_TAIL_WORDS = 24   # pc_start[3] | initial_global_cumulative_sum x[7] y[7] | enable_untrusted_programs | 6 zeros
+# word offsets of RecursionPublicValues<F> (crates/recursion/executor/src/public_values.rs:39-143) that verify_compressed reads; the first
+# RPV_NUM_TO_HASH words are hashed into `digest`
+RPV = dict(sp1_vk_digest=(136, 8), vk_root=(144, 8), is_complete=(168, 1), digest=(175, 8), proof_nonce=(183, 4))
+RPV_NUM_TO_HASH = 175
+COMPRESSED, SHRINK = 0, 1
 
 
 class Params(C.Structure):
@@ -65,6 +70,7 @@ def load():
         L.sp1b200_machine_num_chips.restype = C.c_uint32
         L.sp1b200_machine_chip_regs.restype = C.c_uint32
         L.sp1b200_verdict_name.restype = C.c_char_p
+        L.sp1b200_recursion_vks_num_keys.restype = C.c_uint64
         for name in ERR_FUNCS:
             getattr(L, name).restype = C.c_char_p
         _cdll = L
@@ -79,12 +85,14 @@ ERR_FUNCS = [
     "sp1b200_jagged_prove", "sp1b200_machine_create", "sp1b200_zerocheck", "sp1b200_logup_gkr", "sp1b200_prove_shard",
     "sp1b200_setup_and_prove_shard", "sp1b200_shard_proof_to_bincode", "sp1b200_shard_proof_from_bincode",
     "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard", "sp1b200_verify_core_proof",
+    "sp1b200_vk_hash", "sp1b200_digest_bytes32", "sp1b200_recursion_pv_digest", "sp1b200_recursion_vks_create", "sp1b200_recursion_vks_open",
+    "sp1b200_verify_compressed",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
                "sp1b200_launch_count", "sp1b200_last_phase_ms", "sp1b200_commit_free", "sp1b200_jagged_round_free",
                "sp1b200_machine_free", "sp1b200_machine_num_chips", "sp1b200_machine_chip_regs",
-               "sp1b200_verdict_name"]
+               "sp1b200_verdict_name", "sp1b200_recursion_vks_free", "sp1b200_recursion_vks_root", "sp1b200_recursion_vks_num_keys"]
 
 
 def _ptr(a):
@@ -317,6 +325,40 @@ class Lib:
         v = int(verdict.value)
         return v, int(shard.value), int(sv.value), (fin[:n].copy() if v == 0 else None)
 
+    def recursion_vks(self, digests, pad_to=0, vk_verification=True):
+        """RecursionVks::from_map over the digests ([n, 8] Montgomery words), the tree built on the device -> RecursionVks"""
+        d = np.ascontiguousarray(np.asarray(digests, dtype=np.uint32).reshape(-1, 8))
+        h = C.c_void_p()
+        self._chk(self.L.sp1b200_recursion_vks_create(self.ctx, _ptr(d) if d.size else None, C.c_uint64(d.shape[0]), C.c_uint64(pad_to),
+                                                      C.c_int(int(vk_verification)), C.byref(h)))
+        return RecursionVks(self.L, h, vk_verification)
+
+    def verify_compressed(self, machine, vks, keys, heights_per_proof, names, words_per_proof, merkle_proofs, sp1_vk_digests,
+                          mode=COMPRESSED, shrink_vk=None, host_threads=0):
+        """SP1Prover::verify_compressed (mode COMPRESSED) or verify_shrink (mode SHRINK) of n recursion proofs of one machine.
+        keys: per proof its verifying key, 32 words (prep_commit[8] | vk_tail[24]); merkle_proofs: per proof (index, path [k, 8]);
+        sp1_vk_digests: per proof the expected SP1 program key digest (8 words); shrink_vk: 32 words or None.
+        -> (verdicts, shard_verdicts, final_challengers): verdict 0 accepts and final_challengers[s] is then the verifier's final state."""
+        n, nch = len(words_per_proof), len(names)
+        K = np.ascontiguousarray(np.asarray(keys, dtype=np.uint32).reshape(-1))
+        H = np.ascontiguousarray(np.asarray(heights_per_proof, dtype=np.uint64).reshape(-1) if n else np.zeros(1, np.uint64))
+        NM = (C.c_char_p * max(1, nch))(*[s.encode() for s in names])
+        ws = [None if w is None else np.ascontiguousarray(w, dtype=np.uint32) for w in words_per_proof]
+        P = (C.c_void_p * max(1, n))(*[None if w is None else w.ctypes.data for w in ws])
+        NW = (C.c_uint64 * max(1, n))(*[0 if w is None else w.size for w in ws])
+        paths = [np.ascontiguousarray(np.asarray(p, dtype=np.uint32).reshape(-1)) for _, p in merkle_proofs]
+        IDX = (C.c_uint64 * max(1, n))(*[int(i) for i, _ in merkle_proofs])
+        PP = (C.c_void_p * max(1, n))(*[p.ctypes.data if p.size else None for p in paths])
+        PL = (C.c_uint32 * max(1, n))(*[p.size // 8 for p in paths])
+        D = np.ascontiguousarray(np.asarray(sp1_vk_digests, dtype=np.uint32).reshape(-1))
+        sv = None if shrink_vk is None else np.ascontiguousarray(shrink_vk, dtype=np.uint32)
+        fin = np.zeros((max(1, n), 34), np.uint32)
+        verdicts, shard_verdicts = np.zeros(max(1, n), np.uint32), np.zeros(max(1, n), np.uint32)
+        self._chk(self.L.sp1b200_verify_compressed(self.ctx, machine, vks.h, C.c_uint32(mode), _ptr(sv), C.c_uint32(n), _ptr(K) if K.size else None,
+                                                    C.c_void_p(H.ctypes.data), NM, P, NW, IDX, PP, PL, _ptr(D) if D.size else None,
+                                                    C.c_uint32(host_threads), _ptr(fin), _ptr(verdicts), _ptr(shard_verdicts)))
+        return [int(v) for v in verdicts[:n]], [int(v) for v in shard_verdicts[:n]], fin[:n].copy()
+
     def _debug_call(self, fn, args, cap_words):
         out = np.empty(max(1, cap_words), np.uint32)
         nw = C.c_uint64()
@@ -416,8 +458,76 @@ def parse_interaction_report(w):
 
 
 def verdict_name(verdict):
-    """the reason a verdict of verify_shard or verify_core_proof names ("Accepted" for 0)"""
+    """the reason a verdict of verify_shard, verify_core_proof or verify_compressed names ("Accepted" for 0)"""
     return load().sp1b200_verdict_name(C.c_uint32(verdict)).decode()
+
+
+class RecursionVks:
+    """the recursion vk map of Lib.recursion_vks: root, key count and openings are host lookups"""
+
+    def __init__(self, L, h, vk_verification):
+        self.L, self.h, self.vk_verification = L, h, vk_verification
+
+    def root(self):
+        out = np.zeros(8, np.uint32)
+        self.L.sp1b200_recursion_vks_root(self.h, _ptr(out))
+        return out
+
+    def num_keys(self):
+        return int(self.L.sp1b200_recursion_vks_num_keys(self.h))
+
+    def open(self, digest):
+        """-> (index, path [height, 8]); a digest outside the map raises"""
+        d = np.ascontiguousarray(digest, dtype=np.uint32)
+        path = np.zeros((64, 8), np.uint32)
+        idx, n = C.c_uint64(), C.c_uint32()
+        err = self.L.sp1b200_recursion_vks_open(self.h, _ptr(d), C.byref(idx), _ptr(path), C.c_uint32(64), C.byref(n))
+        if err:
+            raise Sp1B200Error(err.decode())
+        return int(idx.value), path[:n.value].copy()
+
+    def close(self):
+        if self.h:
+            self.L.sp1b200_recursion_vks_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _host_call(fn, *args):
+    err = fn(*args)
+    if err:
+        raise Sp1B200Error(err.decode())
+
+
+def vk_hash(prep_commit, vk_tail):
+    """MachineVerifyingKey::hash_koalabear (without mprotect) of prep_commit[8] + vk_tail[24] -> 8 words"""
+    pc = np.ascontiguousarray(prep_commit, dtype=np.uint32)
+    tail = np.ascontiguousarray(vk_tail, dtype=np.uint32)
+    out = np.zeros(8, np.uint32)
+    _host_call(load().sp1b200_vk_hash, _ptr(pc), _ptr(tail), C.c_uint32(tail.size), _ptr(out))
+    return out
+
+
+def digest_bytes32(digest):
+    """koalabears_to_bn254 of a digest as 32 big-endian bytes (vk.bytes32())"""
+    d = np.ascontiguousarray(digest, dtype=np.uint32)
+    out = np.zeros(32, np.uint8)
+    _host_call(load().sp1b200_digest_bytes32, _ptr(d), C.c_void_p(out.ctypes.data))
+    return out.tobytes()
+
+
+def recursion_pv_digest(pv):
+    """recursion_public_values_digest of the 187 words of RecursionPublicValues -> 8 words"""
+    p = np.ascontiguousarray(pv, dtype=np.uint32)
+    assert p.size == PV_MAX_NUM
+    out = np.zeros(8, np.uint32)
+    _host_call(load().sp1b200_recursion_pv_digest, _ptr(p), _ptr(out))
+    return out
 
 
 class HostChallenger:
