@@ -79,6 +79,11 @@ float sp1b200_last_phase_ms(sp1b200_ctx* ctx, const char* phase);
 
 /* ---- kernel-level entry points (replace the per-kernel FFI of sp1-gpu/crates/sys/src/{all}.rs) ------------- */
 
+/* Alignment of caller device buffers: the Poseidon2 states of sp1b200_poseidon2_permute, the output of sp1b200_rs_encode and the
+ * d_layers_out digests of sp1b200_merkle_commit are read or written with 16-byte vector accesses, so a device pointer passed there
+ * must be 16-byte aligned.  A pointer from sp1b200_malloc or cudaMalloc (256-byte aligned), or one a multiple of 4 words into
+ * such a buffer, is. */
+
 /* Poseidon2 permutation of n independent 16-word states (poseidon2.cuh:46-80). */
 sp1b200_err sp1b200_poseidon2_permute(sp1b200_ctx* ctx, uint32_t* states_any, uint64_t n);
 

@@ -18,9 +18,10 @@ def prove(lib, mach, prep_round, mains, heights, names, pv, state, replay=None):
     return lib.prove_shard(mach, prep_round, M.dense_main(mains), heights, names, pv, state, replay=replay)
 
 
-def check_jagged(shapes_rounds, log_stack, max_log_rows, seed, nq=8, pow_bits=4, batch_bits=2):
+def check_jagged(shapes_rounds, log_stack, max_log_rows, seed, nq=8, pow_bits=4, batch_bits=2, between=None):
     """jagged PCS on random tables of the given (rows, cols) shapes per round: every commitment, column claim and proof word and the
-    final challenger state equal the oracle's"""
+    final challenger state equal the oracle's.  between(lib): called before every call into the library and once after the proof"""
+    between = between or (lambda lib: None)
     from sp1_b200 import Lib
     rng = np.random.default_rng(seed)
     rounds = [O.random_tables(rng, s) for s in shapes_rounds]
@@ -34,14 +35,18 @@ def check_jagged(shapes_rounds, log_stack, max_log_rows, seed, nq=8, pow_bits=4,
               batch_pow_bits=batch_bits)
     handles, claims = [], []
     for i, tabs in enumerate(rounds):
+        between(lib)
         commit, h = lib.jagged_commit(tabs)
         assert (commit == ocommits[i]).all(), f"round {i} jagged commitment differs"
         handles.append(h)
+        between(lib)
         claims.append(lib.jagged_column_claims(h, z_row, sum(t.shape[0] for t in tabs)))
     claims = np.concatenate(claims)
     assert (claims == oclaims).all(), "column claims differ"
     st = ch.st.copy()
+    between(lib)
     proof = lib.jagged_prove(handles, z_row, claims, st)
+    between(lib)
     assert proof.size == oproof.size, (proof.size, oproof.size)
     bad = np.nonzero(proof != oproof)[0]
     assert bad.size == 0, f"first differing proof words {bad[:8]} of {proof.size}"

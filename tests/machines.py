@@ -242,9 +242,10 @@ def _ext_add(a, b):
     return ((a.astype(np.uint64) + b) % O.P).astype(np.uint32)
 
 
-def product_zerocheck(lib, mach, heights, mains, preps, pv, gp, st0, openings):
+def product_zerocheck(lib, mach, heights, mains, preps, pv, gp, st0, openings, device=None):
     """the product's zerocheck (Lib.zerocheck) on the inputs of oracle_zerocheck: alpha and gamma sampled from st0 as the oracle samples
-    them, the per-chip claims sum_j gamma^(j+1) * opening_j (main then prep).  -> (proof words, challenger state after the proof)"""
+    them, the per-chip claims sum_j gamma^(j+1) * opening_j (main then prep).  device: (per chip main, per chip preprocessed) device
+    tensors holding mains / preps, or None to upload them here.  -> (proof words, challenger state after the proof)"""
     import torch
     from sp1_b200.lib import HostChallenger
     hc = HostChallenger(st0.copy())
@@ -257,9 +258,12 @@ def product_zerocheck(lib, mach, heights, mains, preps, pv, gp, st0, openings):
             acc = _ext_add(acc, _ext_mul(openings[k + j], g))
             g = _ext_mul(g, gamma)
         claims.append(acc); k += w
-    d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
-    d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
-    torch.cuda.synchronize()
+    if device is None:
+        d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
+        d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
+        torch.cuda.synchronize()
+    else:
+        d_mains, d_preps = device
     words = lib.zerocheck(mach, heights, d_mains, d_preps, pv, gp, alpha, gamma, np.stack(claims), hc.st)
     return words, hc.st
 

@@ -8,91 +8,14 @@ import os
 import numpy as np
 import pytest
 
-from tests import gpu_prove as GP
 from tests import machines as M
 from tests import oracle_lib as O
 from tests import recursion_ref as RR
+from tests.provers import Rec, specs_machine, workload_specs_machine
 
 pytestmark = pytest.mark.gpu
 
 SHRINK = 1
-
-
-def _specs_machine(chips):
-    blob, heights, _, _, _, names = M.spec_machine(np.random.default_rng(1), chips)
-    return blob, heights, names, chips
-
-
-def _workload_machine(workload, mlr, scale):
-    from sp1_b200 import workload as W
-    mach = W.synthetic_machine(workload, seed=42, max_log_rows=mlr, scale=scale)
-    return mach["blob"], [s.h for s in mach["specs"]], list(mach["names"]), mach["specs"]
-
-
-class Rec:
-    """a context + recursion machine proving shards under distinct verifying keys, with a vk map over those keys"""
-
-    def __init__(self, machine, log_stack, mlr, n_keys=6, prm=M.SMALL, seed=5, extra_keys=20):
-        from sp1_b200 import Lib
-        from sp1_b200 import lib as B
-        self.blob, self.heights, self.names, self.specs = machine
-        self.log_stack, self.mlr, self.prm, self.seed = log_stack, mlr, prm, seed
-        self.lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **prm)
-        self.mach = self.lib.machine_create(self.blob)
-        self.pc, self.prep_round = GP.commit_prep(self.lib, M.traces(self.specs, seed, 0)[1])
-        rng = np.random.default_rng(300 + seed)
-        self.keys = [np.concatenate([self.pc, O.rand_field(rng, 18), np.zeros(6, np.uint32)]) for _ in range(n_keys + 1)]
-        self.outsider = self.keys.pop()   # a key the map does not hold
-        self.digests = np.concatenate([np.stack([B.vk_hash(k[:8], k[8:]) for k in self.keys]), O.rand_field(rng, (extra_keys, 8))])
-        self.vks = self.lib.recursion_vks(self.digests)
-        self.vks_off = self.lib.recursion_vks(self.digests, vk_verification=False)
-        self.root = self.vks.root()
-        self.sp1 = O.rand_field(rng, 8)
-        self.rng = rng
-
-    def pv(self, **faults):
-        """valid recursion public values, then the faults: vk_root, is_complete, digest (a word of the digest changed after hashing)"""
-        from sp1_b200 import lib as B
-        pv = O.rand_field(self.rng, 187)
-        pv[0] = O.to_monty(int(self.rng.integers(1, 1 << 20)))
-        pv[136:144] = self.sp1
-        pv[144:152] = self.root
-        pv[168] = RR.ONE
-        if faults.get("vk_root"):
-            pv[147] = (int(pv[147]) + 1) % O.P
-        if faults.get("is_complete"):
-            pv[168] = 0
-        pv[175:183] = B.recursion_pv_digest(pv)
-        if faults.get("digest"):
-            pv[176] = (int(pv[176]) + 1) % O.P
-        return pv
-
-    def prove(self, key, pv):
-        from sp1_b200.lib import HostChallenger
-        mains, _ = M.traces(self.specs, self.seed, int(O.from_monty(pv[:1])[0]))
-        hc = HostChallenger(); hc.observe(key)
-        st = hc.st.copy()
-        return GP.prove(self.lib, self.mach, self.prep_round, mains, self.heights, self.names, pv, st), st
-
-    def merkle(self, key):
-        from sp1_b200 import lib as B
-        return self.vks.open(B.vk_hash(key[:8], key[8:]))
-
-    def verify(self, cases, vks=None, **kw):
-        """cases: list of (key, words, merkle proof, expected sp1 digest)"""
-        return self.lib.verify_compressed(self.mach, vks or self.vks, [c[0] for c in cases], [self.heights] * len(cases), self.names,
-                                          [c[1] for c in cases], [c[2] for c in cases], [c[3] for c in cases], **kw)
-
-    def oracle(self, key, words, n_pv, merkle, sp1, vk_verification=True, **kw):
-        return RR.verify_compressed(self.blob, self.heights, self.names, self.log_stack, self.mlr, self.prm, key, words, n_pv, self.root,
-                                    vk_verification, merkle, sp1, **kw)[0]
-
-    def close(self):
-        self.vks.close(); self.vks_off.close()
-        if self.prep_round is not None:
-            self.lib.jagged_round_free(self.prep_round)
-        self.lib.machine_free(self.mach)
-        self.lib.close()
 
 
 # ---- the vk tree --------------------------------------------------------------------------------------------------------------------
@@ -129,7 +52,7 @@ def test_vk_tree_matches_the_restatement(n, pad_to):
 # ---- acceptance ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("which", ["tinyr", "no_prep"])
 def test_accepts_recursion_proofs(which):
-    m = _workload_machine("tinyr", 12, 0.25) if which == "tinyr" else _specs_machine(M.NO_PREP)
+    m = workload_specs_machine("tinyr", 12, 0.25) if which == "tinyr" else specs_machine(M.NO_PREP)
     c = Rec(m, 10, 12) if which == "tinyr" else Rec(m, 7, 8)
     if which == "no_prep":
         assert not c.pc.any()
@@ -187,7 +110,7 @@ def _faulty_cases(c):
 
 @pytest.fixture(scope="module")
 def faulty():
-    c = Rec(_specs_machine(M.NO_PREP), 7, 8)
+    c = Rec(specs_machine(M.NO_PREP), 7, 8)
     yield c, _faulty_cases(c)
     c.close()
 
@@ -255,7 +178,7 @@ def test_threads_and_batching_do_not_change_results(faulty):
 
 def test_corrupted_proof_matches_verify_shard_and_the_oracle(capfd):
     from sp1_b200.lib import HostChallenger, Sp1B200Error, verdict_name
-    c = Rec(_workload_machine("tinyr", 12, 0.25), 10, 12, n_keys=2)
+    c = Rec(workload_specs_machine("tinyr", 12, 0.25), 10, 12, n_keys=2)
     key = c.keys[0]
     words, _ = c.prove(key, c.pv())
     hc = HostChallenger(); hc.observe(key)

@@ -9,63 +9,13 @@ import numpy as np
 import pytest
 
 from tests import core_chain as CC
-from tests import gpu_prove as GP
 from tests import machines as M
 from tests import oracle_lib as O
+from tests.provers import Core, specs_machine, workload_specs_machine
 
 pytestmark = pytest.mark.gpu
 
 V_INVALID_SHARD_PROOF = 45
-
-
-def _specs_machine(chips):
-    """-> (blob, heights, names, chips); every shard draws its traces with M.traces"""
-    blob, heights, _, _, _, names = M.spec_machine(np.random.default_rng(1), chips)
-    return blob, heights, names, chips
-
-
-def _workload_machine(workload, mlr, scale):
-    from sp1_b200 import workload as W
-    mach = W.synthetic_machine(workload, seed=42, max_log_rows=mlr, scale=scale)
-    return mach["blob"], [s.h for s in mach["specs"]], list(mach["names"]), mach["specs"]
-
-
-class Core:
-    """a context + machine proving shards of one program under one verifying key"""
-
-    def __init__(self, machine, log_stack, mlr, prm=M.SMALL, seed=5, **ctx):
-        from sp1_b200 import Lib
-        self.blob, self.heights, self.names, self.specs = machine
-        self.log_stack, self.mlr, self.prm, self.seed = log_stack, mlr, prm, seed
-        self.lib = Lib(0, log_stacking_height=log_stack, max_log_row_count=mlr, **prm, **ctx)
-        self.mach = self.lib.machine_create(self.blob)
-        self.pc, self.prep_round = GP.commit_prep(self.lib, M.traces(self.specs, seed, 0)[1])
-
-    def start(self, tail):
-        from sp1_b200.lib import HostChallenger
-        hc = HostChallenger(); hc.observe(self.pc); hc.observe(tail)
-        return hc.st.copy()
-
-    def prove(self, pvs, tail):
-        """-> (words per shard, final prover state per shard); tail, pvs: canonical"""
-        tail = O.to_monty(np.array(tail))
-        words, finals = [], []
-        for pv in pvs:
-            mains, _ = M.traces(self.specs, self.seed, CC.pv0_of(pv))
-            st = self.start(tail)
-            words.append(GP.prove(self.lib, self.mach, self.prep_round, mains, self.heights, self.names, O.to_monty(np.array(pv)), st))
-            finals.append(st)
-        return words, finals, tail
-
-    def verify(self, words, tail, heights=None, threads=0):
-        hs = [self.heights] * len(words) if heights is None else heights
-        return self.lib.verify_core_proof(self.mach, self.pc, tail, hs, self.names, words, host_threads=threads)
-
-    def close(self):
-        if self.prep_round is not None:
-            self.lib.jagged_round_free(self.prep_round)
-        self.lib.machine_free(self.mach)
-        self.lib.close()
 
 
 def _accept(c, n, seed, **kw):
@@ -82,14 +32,14 @@ def _accept(c, n, seed, **kw):
 
 @pytest.mark.parametrize("n", [1, 2, 5])
 def test_accepts_with_preprocessed_columns(n):
-    c = Core(_specs_machine(M.WITH_PREP), 8, 9)
+    c = Core(specs_machine(M.WITH_PREP), 8, 9)
     _accept(c, n, 100 + n)
     c.close()
 
 
 @pytest.mark.parametrize("n", [1, 2, 5])
 def test_accepts_without_preprocessed_columns(n):
-    c = Core(_specs_machine(M.NO_PREP), 7, 8)
+    c = Core(specs_machine(M.NO_PREP), 7, 8)
     assert not c.pc.any()
     _accept(c, n, 110 + n, non_execution=1 if n > 2 else None)
     c.close()
@@ -97,7 +47,7 @@ def test_accepts_without_preprocessed_columns(n):
 
 @pytest.mark.parametrize("workload,n", [("tinyc", 3), ("tinyr", 2)])
 def test_accepts_workload_machines(workload, n):
-    c = Core(_workload_machine(workload, 12, 0.25), 10, 12)
+    c = Core(workload_specs_machine(workload, 12, 0.25), 10, 12)
     _accept(c, n, 120 + n)
     c.close()
 
@@ -105,7 +55,7 @@ def test_accepts_workload_machines(workload, n):
 def test_every_public_value_check():
     """one chain per reason, proved with the faulty public values (not patched after proving): exactly that verdict at that shard"""
     from sp1_b200.lib import verdict_name
-    c = Core(_specs_machine(M.NO_PREP), 7, 8)
+    c = Core(specs_machine(M.NO_PREP), 7, 8)
     seen = set()
     for name, mutate, want, shard in CC.PV_CASES:
         pvs, tail = CC.chain(3, 140, non_execution=1)
@@ -122,7 +72,7 @@ def test_every_public_value_check():
 
 
 def _tinyc_chain(n=3, seed=150, **ctx):
-    c = Core(_workload_machine("tinyc", 12, 0.25), 10, 12, **ctx)
+    c = Core(workload_specs_machine("tinyc", 12, 0.25), 10, 12, **ctx)
     pvs, tail = CC.chain(n, seed)
     words, finals, mtail = c.prove(pvs, tail)
     return c, words, finals, mtail
@@ -205,7 +155,7 @@ def test_threads_and_batching_do_not_change_results():
 def test_malformed_arguments_are_errors_and_leave_the_context_usable():
     import ctypes as C
     from sp1_b200.lib import Sp1B200Error, _ptr
-    c = Core(_specs_machine(M.NO_PREP), 7, 8)
+    c = Core(specs_machine(M.NO_PREP), 7, 8)
     pvs, tail = CC.chain(2, 170)
     words, _, mtail = c.prove(pvs, tail)
     with pytest.raises(Sp1B200Error, match="n_vk_tail"):
@@ -223,7 +173,7 @@ def test_malformed_arguments_are_errors_and_leave_the_context_usable():
 
 
 def test_two_contexts_on_two_threads():
-    cores = [Core(_specs_machine(M.WITH_PREP), 8, 9), Core(_specs_machine(M.NO_PREP), 7, 8)]
+    cores = [Core(specs_machine(M.WITH_PREP), 8, 9), Core(specs_machine(M.NO_PREP), 7, 8)]
     jobs = []
     for i, c in enumerate(cores):
         pvs, tail = CC.chain(3, 180 + i)
