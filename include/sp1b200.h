@@ -264,6 +264,24 @@ sp1b200_err sp1b200_setup_and_prove_shard(sp1b200_ctx* ctx, const sp1b200_machin
                                           sp1b200_jagged_round** prep_round_out, uint32_t* h_proof, uint64_t proof_cap_words,
                                           uint64_t* h_proof_words);
 
+/* ---- program setup (the part of AirProver::setup that depends on the program, crates/hypercube/src/prover/shard.rs:259-290) --------
+ * MachineProgram::pc_start + initial_global_cumulative_sum + untrusted_config for a core program (crates/core/executor/src/program.rs:
+ * 161-229), as the 24-word vk_tail that sp1b200_setup_and_prove_shard, sp1b200_verify_core_proof and sp1b200_vk_hash take:
+ *   pc_start = the 16-bit limbs 0..16 / 16..32 / 32..48 of pc_start_abs | initial_global_cumulative_sum x[7] y[7] |
+ *   enable_untrusted_programs | 6 zeros (Montgomery words).
+ * The sum is SepticDigest::zero() plus the negation of SepticCurve::lift_x of one message per memory entry (address mem_addrs_any[i],
+ * word mem_words_any[i]: [Memory << 24, 0, address limbs 0..16 / 16..32 / 32..48, (w & 0xFFFF) + 2^16 ((w >> 32) & 0xFF),
+ * ((w >> 16) & 0xFFFF) + 2^16 ((w >> 40) & 0xFF), w >> 48]) and, only when enable_untrusted_programs is 1, one per page entry (index
+ * page_idx_any[i], protection page_prot_any[i]: [PageProtAccess << 24, 0, index bits 0..4 / 4..20 / 20..36, prot, 0, 0]), summed under
+ * the complete addition law; with enable_untrusted_programs 0 the page image is not read.  An empty image gives SepticDigest::zero().
+ * The arrays are host or device memory; device memory comes from the context's pool and is returned before the call ends.
+ * Errors: a duplicate memory address or page index (the image is a map; the message names the key), an entry none of whose 256 lift
+ * offsets gives a point, a sum at infinity, NULL arrays with a non-zero count, enable_untrusted_programs other than 0 or 1, 2^31 - 1
+ * entries or more.  The context stays usable after an error.  Phases: "program_vk_tail", "program_vk_tail.lift", ".sum". */
+sp1b200_err sp1b200_program_vk_tail(sp1b200_ctx* ctx, uint64_t pc_start_abs, const uint64_t* mem_addrs_any, const uint64_t* mem_words_any,
+                                    uint64_t n_mem, const uint64_t* page_idx_any, const uint8_t* page_prot_any, uint64_t n_pages,
+                                    int enable_untrusted_programs, uint32_t* h_vk_tail24);
+
 /* ---- shard checks (the reference's cfg(sp1_debug_constraints) build; nothing of the transcript is touched) -------------------------
  * Both take the shard inputs of sp1b200_prove_shard (same validation: prep_round = the round committed at setup or NULL, its heights
  * equal to the main heights, every height <= 2^max_log_row_count; main_dense_any = host pointer, device pointer or upload slot), so a

@@ -3,6 +3,7 @@
 // Mirrors the trait the reference selects its shard prover through, `sp1_hypercube::prover::AirProver<GC, SC>`
 // (crates/hypercube/src/prover/shard.rs:45-101): same method names, argument meaning and error behaviour
 //   machine()                       -> the chips (name order) this prover was built for
+//   setup(...)                      -> setup_from_vk plus the verifying key's words computed from the program's memory image
 //   setup_from_vk(...)              -> commits the preprocessed traces once per program, returns the proving key
 //                                      (`PreprocessedData<ProvingKey>`) and the preprocessed commitment of the verifying key
 //   setup_and_prove_shard(...)      -> setup, observe the verifying key, prove (the vk-less path of the first shard of a program)
@@ -71,6 +72,26 @@ class ProvingKey {
     sp1b200_jagged_round* round_ = nullptr;
 };
 
+// What setup needs of a program (MachineProgram: pc_start_abs, memory_image and page_prot_image as parallel arrays in any order, host or
+// device memory, enable_untrusted_programs)
+struct ProgramImage {
+    uint64_t pc_start_abs = 0;
+    const uint64_t* mem_addrs = nullptr;
+    const uint64_t* mem_words = nullptr;
+    uint64_t n_mem = 0;
+    const uint64_t* page_idx = nullptr;
+    const uint8_t* page_prot = nullptr;
+    uint64_t n_pages = 0;
+    bool enable_untrusted_programs = false;
+};
+
+// MachineVerifyingKey as the library's calls take it: the preprocessed commitment and the 24 words observed after it
+// (pc_start[3], initial_global_cumulative_sum x[7] y[7], enable_untrusted_programs, six zeros)
+struct VerifyingKeyWords {
+    Digest preprocessed_commit{};
+    std::vector<uint32_t> tail;
+};
+
 class AirProver {
   public:
     // chips in name order; machine_blob = the constraint bytecode + interactions of every chip (sp1b200_machine_create)
@@ -115,6 +136,19 @@ class AirProver {
         if (!rows.empty())
             check(sp1b200_jagged_commit(ctx_, prep_dense_any, (uint32_t)rows.size(), rows.data(), cols.data(), 1, pk.commit.data(), &pk.round_));
         return pk;
+    }
+
+    // AirProver::setup (shard.rs:88-95 -> setup_from_vk(program, None), shard.rs:259-290): the proving key as setup_from_vk makes it and
+    // the verifying key, whose initial global cumulative sum is computed from the program's memory image on the device
+    // (sp1b200_program_vk_tail).  The image is checked before anything is committed.
+    std::pair<ProvingKey, VerifyingKeyWords> setup(const uint32_t* prep_dense_any, const std::vector<uint64_t>& heights, const ProgramImage& program) {
+        VerifyingKeyWords vk;
+        vk.tail.resize(24);
+        check(sp1b200_program_vk_tail(ctx_, program.pc_start_abs, program.mem_addrs, program.mem_words, program.n_mem, program.page_idx,
+                                      program.page_prot, program.n_pages, program.enable_untrusted_programs ? 1 : 0, vk.tail.data()));
+        ProvingKey pk = setup_from_vk(prep_dense_any, heights);
+        vk.preprocessed_commit = pk.commit;
+        return {std::move(pk), std::move(vk)};
     }
 
     // AirProver::preprocessed_table_heights

@@ -6,6 +6,7 @@
 #include "debug_fp.cuh"
 #include "hostfield.hpp"
 #include "septic.hpp"
+#include "septic.cuh"
 #include "zc_lower.hpp"
 #include <cstring>
 #include <type_traits>
@@ -193,5 +194,38 @@ int sp1b200_hostcheck_septic_digest_add(const uint32_t* a, const uint32_t* b, ui
 void sp1b200_hostcheck_septic_constants(uint32_t* out42) {
     const sep::Point pts[3] = {sep::digest_zero(), sep::digest_start(), sep::dummy_point()};
     for (int i = 0; i < 3; i++) { pts[i].x.store(out42 + 14 * i); pts[i].y.store(out42 + 14 * i + 7); }
+}
+// The program setup's device septic code (septic.cuh), Montgomery words: lift_x of n messages (8 words each) -> offsets[i] (-1 when
+// none of the 256 offsets gives a point) and points (x then y, 14 words); square roots of n septic elements (ok[i] = 0 for a
+// non-square, out left zero); n complete additions of points (infinity = 14 zero words).
+void sp1b200_hostcheck_lift_x(const uint32_t* msgs, int32_t* offsets, uint32_t* pts, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        uint32_t m[8];
+        for (int k = 0; k < 8; k++) m[k] = msgs[8 * i + k];
+        s7::Pt p = s7::infinity();
+        offsets[i] = s7::lift_x(m, p);
+        for (int k = 0; k < 7; k++) { pts[14 * i + k] = p.x.c[k]; pts[14 * i + 7 + k] = p.y.c[k]; }
+    }
+}
+void sp1b200_hostcheck_septic_sqrt(const uint32_t* a, uint32_t* out, uint32_t* ok, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        s7::E7 x;
+        for (int k = 0; k < 7; k++) x.c[k] = a[7 * i + k];
+        const uint32_t nrm = s7::pow_r(x);
+        ok[i] = s7::is_zero(x) || s7::base_is_square(nrm);
+        const s7::E7 r = ok[i] ? s7::sqrt(x, nrm) : s7::zero();
+        for (int k = 0; k < 7; k++) out[7 * i + k] = r.c[k];
+    }
+}
+void sp1b200_hostcheck_curve_add_complete(const uint32_t* p, const uint32_t* q, uint32_t* out, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        s7::Pt a, b;
+        for (int k = 0; k < 7; k++) {
+            a.x.c[k] = p[14 * i + k]; a.y.c[k] = p[14 * i + 7 + k];
+            b.x.c[k] = q[14 * i + k]; b.y.c[k] = q[14 * i + 7 + k];
+        }
+        const s7::Pt r = s7::add_complete(a, b);
+        for (int k = 0; k < 7; k++) { out[14 * i + k] = r.x.c[k]; out[14 * i + 7 + k] = r.y.c[k]; }
+    }
 }
 }

@@ -86,7 +86,7 @@ ERR_FUNCS = [
     "sp1b200_setup_and_prove_shard", "sp1b200_shard_proof_to_bincode", "sp1b200_shard_proof_from_bincode",
     "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard", "sp1b200_verify_core_proof",
     "sp1b200_vk_hash", "sp1b200_digest_bytes32", "sp1b200_recursion_pv_digest", "sp1b200_recursion_vks_create", "sp1b200_recursion_vks_open",
-    "sp1b200_verify_compressed",
+    "sp1b200_verify_compressed", "sp1b200_program_vk_tail",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
@@ -406,6 +406,29 @@ class Lib:
                                                        _ptr(main_dense), H, NM, _ptr(pv), C.c_uint32(pv.size), _ptr(rw), _ptr(challenger_state),
                                                        _ptr(pc), C.byref(h), _ptr(out), C.c_uint64(cap_words), C.byref(nw)))
         return pc, h, out[:nw.value].copy()
+
+    def program_vk_tail(self, pc_start_abs, mem_addrs, mem_words, page_idx=None, page_prot=None, enable_untrusted_programs=0):
+        """MachineProgram::pc_start + initial_global_cumulative_sum + untrusted_config of a program's memory image (and page image) ->
+        the 24-word vk_tail (Montgomery words).  Addresses, words and page indices are 64-bit, protections 8-bit: numpy arrays or
+        torch tensors on the host or the device (torch int64 / uint8)."""
+        def arr(a, dtype):
+            if a is None:
+                return None, 0
+            if hasattr(a, "data_ptr"):
+                assert a.is_contiguous() and a.element_size() == np.dtype(dtype).itemsize
+                return C.c_void_p(a.data_ptr() if a.numel() else None), a.numel()
+            a = np.ascontiguousarray(a, dtype=dtype)
+            return a, a.size
+        a, n_mem = arr(mem_addrs, np.uint64)
+        w, n_w = arr(mem_words, np.uint64)
+        pi, n_pages = arr(page_idx, np.uint64)
+        pp, n_p = arr(page_prot, np.uint8)
+        assert n_mem == n_w and n_pages == n_p, "one word per address and one protection per page index"
+        p = lambda x: x if x is None or isinstance(x, C.c_void_p) else (C.c_void_p(x.ctypes.data) if x.size else None)
+        out = np.zeros(VK_TAIL_WORDS, np.uint32)
+        self._chk(self.L.sp1b200_program_vk_tail(self.ctx, C.c_uint64(pc_start_abs), p(a), p(w), C.c_uint64(n_mem), p(pi), p(pp),
+                                                 C.c_uint64(n_pages), C.c_int(enable_untrusted_programs), _ptr(out)))
+        return out
 
     def pack_row_major(self, rows_any, shapes, d_dense_out):
         """tables back to back, each row-major [rows x cols] -> device buffer with each table column-major"""
