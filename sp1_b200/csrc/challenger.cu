@@ -75,34 +75,26 @@ sp1b200_err sp1b200_grind_device(sp1b200_ctx* ctx, uint32_t* d_state, uint32_t b
 // ---- host challenger -----------------------------------------------------------------------------------------
 namespace {
 using p2::RC_HOST;
-inline uint32_t h_reduce(uint64_t x) {
-    uint32_t m = (uint32_t)x * kb::MPRIME;
-    uint64_t u = x + (uint64_t)m * kb::P;
-    uint32_t r = (uint32_t)(u >> 32);
-    return r >= kb::P ? r - kb::P : r;
-}
-inline uint32_t h_add(uint32_t a, uint32_t b) { uint32_t s = a + b; return s >= kb::P ? s - kb::P : s; }
-inline uint32_t h_mul(uint32_t a, uint32_t b) { return h_reduce((uint64_t)a * b); }
-inline uint32_t h_cube(uint32_t x) { return h_mul(h_mul(x, x), x); }
+inline uint32_t h_cube(uint32_t x) { return kb::mul(kb::sqr(x), x); }
 inline void h_ext_layer(uint32_t* s) {
     for (int q = 0; q < 16; q += 4) {
         uint32_t a = s[q], b = s[q + 1], c = s[q + 2], d = s[q + 3];
-        uint32_t t = h_add(h_add(a, b), h_add(c, d));
+        uint32_t t = kb::add(kb::add(a, b), kb::add(c, d));
         // rows of [[2,3,1,1],[1,2,3,1],[1,1,2,3],[3,1,1,2]]
-        s[q] = h_add(t, h_add(a, h_add(b, b)));
-        s[q + 1] = h_add(t, h_add(b, h_add(c, c)));
-        s[q + 2] = h_add(t, h_add(c, h_add(d, d)));
-        s[q + 3] = h_add(t, h_add(d, h_add(a, a)));
+        s[q] = kb::add(t, kb::add(a, kb::add(b, b)));
+        s[q + 1] = kb::add(t, kb::add(b, kb::add(c, c)));
+        s[q + 2] = kb::add(t, kb::add(c, kb::add(d, d)));
+        s[q + 3] = kb::add(t, kb::add(d, kb::add(a, a)));
     }
     uint32_t col[4];
-    for (int j = 0; j < 4; j++) col[j] = h_add(h_add(s[j], s[4 + j]), h_add(s[8 + j], s[12 + j]));
-    for (int i = 0; i < 16; i++) s[i] = h_add(s[i], col[i & 3]);
+    for (int j = 0; j < 4; j++) col[j] = kb::add(kb::add(s[j], s[4 + j]), kb::add(s[8 + j], s[12 + j]));
+    for (int i = 0; i < 16; i++) s[i] = kb::add(s[i], col[i & 3]);
 }
 inline void h_int_layer(uint32_t* s) {
     uint64_t sum = 0;
     for (int i = 0; i < 16; i++) sum += s[i];
-    uint32_t o0 = h_reduce(sum - s[0] + (kb::P - s[0]));
-    for (int i = 1; i < 16; i++) s[i] = h_reduce(sum + ((uint64_t)s[i] << (i == 15 ? 15 : i - 1)));
+    uint32_t o0 = kb::monty_reduce(sum - s[0] + (kb::P - s[0]));
+    for (int i = 1; i < 16; i++) s[i] = kb::monty_reduce(sum + ((uint64_t)s[i] << (i == 15 ? 15 : i - 1)));
     s[0] = o0;
 }
 }  // namespace
@@ -110,20 +102,18 @@ inline void h_int_layer(uint32_t* s) {
 void host_poseidon2_permute(uint32_t* s) {
     h_ext_layer(s);
     for (int r = 0; r < 4; r++) {
-        for (int i = 0; i < 16; i++) s[i] = h_cube(h_add(s[i], RC_HOST.ext[r * 16 + i]));
+        for (int i = 0; i < 16; i++) s[i] = h_cube(kb::add(s[i], RC_HOST.ext[r * 16 + i]));
         h_ext_layer(s);
     }
     for (int r = 0; r < 20; r++) {
-        s[0] = h_cube(h_add(s[0], RC_HOST.inr[r]));
+        s[0] = h_cube(kb::add(s[0], RC_HOST.inr[r]));
         h_int_layer(s);
     }
     for (int r = 4; r < 8; r++) {
-        for (int i = 0; i < 16; i++) s[i] = h_cube(h_add(s[i], RC_HOST.ext[r * 16 + i]));
+        for (int i = 0; i < 16; i++) s[i] = h_cube(kb::add(s[i], RC_HOST.ext[r * 16 + i]));
         h_ext_layer(s);
     }
 }
-uint32_t host_to_monty(uint64_t canonical) { return (uint32_t)(((canonical % kb::P) << 32) % kb::P); }
-uint32_t host_from_monty(uint32_t m) { return h_reduce(m); }
 
 void host_hash(const uint32_t* in, size_t n, uint32_t* out8) {
     uint32_t s[16] = {0};
@@ -140,21 +130,21 @@ void host_compress(const uint32_t* l8, const uint32_t* r8, uint32_t* out8) {
 }
 
 void table_size_commitment(const uint32_t* original8, const std::vector<std::pair<uint64_t, uint64_t>>& tables, uint32_t* out8) {
-    std::vector<uint32_t> meta{host_to_monty(tables.size())};
-    for (auto& t : tables) meta.push_back(host_to_monty(t.first));
-    for (auto& t : tables) meta.push_back(host_to_monty(t.second));
+    std::vector<uint32_t> meta{kb::to_monty_c(tables.size())};
+    for (auto& t : tables) meta.push_back(kb::to_monty_c(t.first));
+    for (auto& t : tables) meta.push_back(kb::to_monty_c(t.second));
     uint32_t h[8];
     host_hash(meta.data(), meta.size(), h);
     host_compress(original8, h, out8);
 }
 
 void observe_chip_shapes(HostChallenger& ch, size_t n_chips, const uint64_t* heights, const char* const* names) {
-    ch.observe(host_to_monty(n_chips));
+    ch.observe(kb::to_monty_c(n_chips));
     for (size_t k = 0; k < n_chips; k++) {
-        ch.observe(host_to_monty(heights[k]));
+        ch.observe(kb::to_monty_c(heights[k]));
         const size_t len = strlen(names[k]);
-        ch.observe(host_to_monty(len));
-        for (size_t i = 0; i < len; i++) ch.observe(host_to_monty((uint8_t)names[k][i]));
+        ch.observe(kb::to_monty_c(len));
+        for (size_t i = 0; i < len; i++) ch.observe(kb::to_monty_c((uint8_t)names[k][i]));
     }
 }
 
@@ -200,7 +190,7 @@ uint32_t HostChallenger::sample() {
     return outbuf[--nout];
 }
 void HostChallenger::sample_ext(uint32_t* out4) { for (int i = 0; i < 4; i++) out4[i] = sample(); }
-uint32_t HostChallenger::sample_bits(uint32_t bits) { return host_from_monty(sample()) & ((1u << bits) - 1u); }
+uint32_t HostChallenger::sample_bits(uint32_t bits) { return kb::to_canonical(sample()) & ((1u << bits) - 1u); }
 bool HostChallenger::check_witness(uint32_t bits, uint32_t w_monty) { observe(w_monty); return sample_bits(bits) == 0; }
 sp1b200_err HostChallenger::grind(uint32_t bits, uint32_t* w_monty) {
     uint32_t st[34];
@@ -211,7 +201,7 @@ sp1b200_err HostChallenger::grind(uint32_t bits, uint32_t* w_monty) {
     SP1_CUDA(cudaMemcpyAsync(st, d_scratch, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
     SP1_CUDA(cudaStreamSynchronize(ctx->stream));
     load(st);
-    *w_monty = host_to_monty(wc);
+    *w_monty = kb::to_monty_c(wc);
     return nullptr;
 }
 

@@ -9,8 +9,6 @@
 #include <utility>
 #include <vector>
 
-uint32_t host_to_monty(uint64_t canonical);
-uint32_t host_from_monty(uint32_t m);
 void host_poseidon2_permute(uint32_t* s16);
 // PaddingFreeSponge<16, 8, 8> (overwrite mode) and the 2-to-1 compression, with the transcript's permutation
 void host_hash(const uint32_t* in, size_t n, uint32_t* out8);

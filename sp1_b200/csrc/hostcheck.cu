@@ -5,7 +5,6 @@
 #include "rs_twiddles.cuh"
 #include "debug_fp.cuh"
 #include "hostfield.hpp"
-#include "septic.hpp"
 #include "septic.cuh"
 #include "zc_lower.hpp"
 #include <cstring>
@@ -87,10 +86,10 @@ int sp1b200_hostcheck_zc_lower(const uint32_t* chip, const uint32_t* main_row, c
                 case BC_LOAD_LEAF: regs[in.out] = leaf(hp.leaves[in.a]); break;
                 case BC_LOAD_CONST: regs[in.out] = hp.consts[in.a]; break;
                 case BC_LOAD_PUBLIC: regs[in.out] = pv[hp.publics[in.a]]; break;
-                case BC_ADD_F: regs[in.out] = hf::add(regs[in.a], regs[in.b]); break;
-                case BC_SUB_F: regs[in.out] = hf::sub(regs[in.a], regs[in.b]); break;
-                case BC_MUL_F: regs[in.out] = hf::mul(regs[in.a], regs[in.b]); break;
-                case BC_NEG_F: regs[in.out] = hf::neg(regs[in.a]); break;
+                case BC_ADD_F: regs[in.out] = kb::add(regs[in.a], regs[in.b]); break;
+                case BC_SUB_F: regs[in.out] = kb::sub(regs[in.a], regs[in.b]); break;
+                case BC_MUL_F: regs[in.out] = kb::mul(regs[in.a], regs[in.b]); break;
+                case BC_NEG_F: regs[in.out] = kb::neg(regs[in.a]); break;
             }
         }
         E4 acc;
@@ -106,10 +105,10 @@ int sp1b200_hostcheck_zc_lower(const uint32_t* chip, const uint32_t* main_row, c
                 case ZC_LOAD_PREP: rf[in.out] = prep_row[(uint32_t)in.a | ((uint32_t)in.b << 16)]; break;
                 case ZC_CONST: rf[in.out] = hp.consts[in.a]; break;
                 case ZC_PUBLIC: rf[in.out] = pv[hp.publics[in.a]]; break;
-                case ZC_ADD: { uint32_t x = rf[in.a], y = rf[in.b]; rf[in.out] = hf::add(x, y); break; }
-                case ZC_SUB: { uint32_t x = rf[in.a], y = rf[in.b]; rf[in.out] = hf::sub(x, y); break; }
-                case ZC_MUL: { uint32_t x = rf[in.a], y = rf[in.b]; rf[in.out] = hf::mul(x, y); break; }
-                case ZC_NEG: rf[in.out] = hf::neg(rf[in.a]); break;
+                case ZC_ADD: { uint32_t x = rf[in.a], y = rf[in.b]; rf[in.out] = kb::add(x, y); break; }
+                case ZC_SUB: { uint32_t x = rf[in.a], y = rf[in.b]; rf[in.out] = kb::sub(x, y); break; }
+                case ZC_MUL: { uint32_t x = rf[in.a], y = rf[in.b]; rf[in.out] = kb::mul(x, y); break; }
+                case ZC_NEG: rf[in.out] = kb::neg(rf[in.a]); break;
                 case ZC_ASSERT: a = a + E4::load(alpha_pows + 4 * in.b) * rf[in.a]; break;
             }
         }
@@ -140,13 +139,13 @@ uint64_t sp1b200_hostcheck_fingerprint(uint32_t kind, uint32_t n_values, const u
     return dbgfp::fingerprint(kind, n_values, values);
 }
 
-// Host transcript arithmetic (hostfield.hpp): product, inverse, and the batched-inversion Lagrange interpolation through 4 / 5 nodes
+// Host transcript arithmetic (hostfield.hpp, kb31.cuh): product, inverse, and the batched-inversion Lagrange interpolation through 4 / 5 nodes
 // that the sumcheck drivers use.  coeffs_out: n ext elements = coefficients of the polynomial through (x_i, y_i).
 void sp1b200_hostcheck_e4(const uint32_t* a, const uint32_t* b, uint32_t* mul_out, uint32_t* inv_out, uint64_t n) {
     using hf::E4;
     for (uint64_t i = 0; i < n; i++) {
         (E4::load(a + 4 * i) * E4::load(b + 4 * i)).store(mul_out + 4 * i);
-        hf::inv(E4::load(a + 4 * i)).store(inv_out + 4 * i);
+        E4(kb::ext_inv(E4::load(a + 4 * i))).store(inv_out + 4 * i);
     }
 }
 int sp1b200_hostcheck_interpolate(const uint32_t* xs, const uint32_t* ys, uint32_t n, uint32_t* coeffs_out) {
@@ -166,34 +165,34 @@ int sp1b200_hostcheck_interpolate(const uint32_t* xs, const uint32_t* ys, uint32
     return 0;
 }
 
-// The core-proof verifier's septic arithmetic (septic.hpp), Montgomery words: n products and inverses of septic elements (7 words
+// The core-proof verifier's septic arithmetic (septic.cuh), Montgomery words: n products and inverses of septic elements (7 words
 // each); n curve additions add_incomplete(p, q) of points (14 words: x then y), ok[i] = 0 on the exceptional case; SepticDigest
 // addition; and the three constant points zero, starting digest, dummy (42 words).
 void sp1b200_hostcheck_septic(const uint32_t* a, const uint32_t* b, uint32_t* mul_out, uint32_t* inv_out, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) {
-        const sep::E7 x = sep::E7::load(a + 7 * i), y = sep::E7::load(b + 7 * i);
-        (x * y).store(mul_out + 7 * i);
-        sep::inv(x).store(inv_out + 7 * i);
+        s7::E7 x, y;
+        for (int k = 0; k < 7; k++) { x.c[k] = a[7 * i + k]; y.c[k] = b[7 * i + k]; }
+        const s7::E7 m = s7::mul(x, y), v = s7::inv(x);
+        for (int k = 0; k < 7; k++) { mul_out[7 * i + k] = m.c[k]; inv_out[7 * i + k] = v.c[k]; }
     }
 }
 void sp1b200_hostcheck_septic_curve_add(const uint32_t* p, const uint32_t* q, uint32_t* out, uint32_t* ok, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) {
-        const sep::Point a{sep::E7::load(p + 14 * i), sep::E7::load(p + 14 * i + 7)}, b{sep::E7::load(q + 14 * i), sep::E7::load(q + 14 * i + 7)};
-        sep::Point r{};
-        ok[i] = sep::add_incomplete(a, b, r);
-        r.x.store(out + 14 * i); r.y.store(out + 14 * i + 7);
+        s7::Pt r = s7::infinity();
+        ok[i] = s7::add_incomplete(s7::load_point(p + 14 * i), s7::load_point(q + 14 * i), r);
+        s7::store_point(r, out + 14 * i);
     }
 }
 int sp1b200_hostcheck_septic_digest_add(const uint32_t* a, const uint32_t* b, uint32_t* out) {
-    const sep::Point x{sep::E7::load(a), sep::E7::load(a + 7)}, y{sep::E7::load(b), sep::E7::load(b + 7)};
-    sep::Point r{};
-    if (!sep::digest_add(x, y, r)) return 0;
-    r.x.store(out); r.y.store(out + 7);
+    s7::Pt r;
+    if (!s7::digest_add(s7::load_point(a), s7::load_point(b), r)) return 0;
+    s7::store_point(r, out);
     return 1;
 }
 void sp1b200_hostcheck_septic_constants(uint32_t* out42) {
-    const sep::Point pts[3] = {sep::digest_zero(), sep::digest_start(), sep::dummy_point()};
-    for (int i = 0; i < 3; i++) { pts[i].x.store(out42 + 14 * i); pts[i].y.store(out42 + 14 * i + 7); }
+    s7::store_point(s7::digest_zero(), out42);
+    s7::store_point(s7::digest_start(), out42 + 14);
+    s7::store_point(s7::dummy_point(), out42 + 28);
 }
 // The program setup's device septic code (septic.cuh), Montgomery words: lift_x of n messages (8 words each) -> offsets[i] (-1 when
 // none of the 256 offsets gives a point) and points (x then y, 14 words); square roots of n septic elements (ok[i] = 0 for a
@@ -204,7 +203,7 @@ void sp1b200_hostcheck_lift_x(const uint32_t* msgs, int32_t* offsets, uint32_t* 
         for (int k = 0; k < 8; k++) m[k] = msgs[8 * i + k];
         s7::Pt p = s7::infinity();
         offsets[i] = s7::lift_x(m, p);
-        for (int k = 0; k < 7; k++) { pts[14 * i + k] = p.x.c[k]; pts[14 * i + 7 + k] = p.y.c[k]; }
+        s7::store_point(p, pts + 14 * i);
     }
 }
 void sp1b200_hostcheck_septic_sqrt(const uint32_t* a, uint32_t* out, uint32_t* ok, uint64_t n) {
@@ -219,13 +218,7 @@ void sp1b200_hostcheck_septic_sqrt(const uint32_t* a, uint32_t* out, uint32_t* o
 }
 void sp1b200_hostcheck_curve_add_complete(const uint32_t* p, const uint32_t* q, uint32_t* out, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) {
-        s7::Pt a, b;
-        for (int k = 0; k < 7; k++) {
-            a.x.c[k] = p[14 * i + k]; a.y.c[k] = p[14 * i + 7 + k];
-            b.x.c[k] = q[14 * i + k]; b.y.c[k] = q[14 * i + 7 + k];
-        }
-        const s7::Pt r = s7::add_complete(a, b);
-        for (int k = 0; k < 7; k++) { out[14 * i + k] = r.x.c[k]; out[14 * i + 7 + k] = r.y.c[k]; }
+        s7::store_point(s7::add_complete(s7::load_point(p + 14 * i), s7::load_point(q + 14 * i)), out + 14 * i);
     }
 }
 }

@@ -1,85 +1,34 @@
-// Host-side KoalaBear / ext4 scalar arithmetic used by the library's transcript driver (a few hundred
-// operations per proof: batching coefficients, claimed sums, round-polynomial bookkeeping).  Product code,
-// independent of oracle/.  Same representation as the device code (Montgomery words).
+// Host-side extension-field helpers for the library's transcript drivers (a few hundred operations per proof: batching coefficients,
+// claimed sums, round-polynomial bookkeeping).  The arithmetic itself is the device code's (kb31.cuh, __host__ __device__); this adds
+// host conveniences on top of it.  Product code, independent of oracle/.
 #pragma once
+#include "kb31.cuh"
+#include <cstddef>
 #include <cstdint>
 #include <vector>
 
 namespace hf {
 
-constexpr uint32_t P = 0x7f000001u;
-constexpr uint32_t MPRIME = 0x7effffffu;
-constexpr uint32_t ONE = 0x01fffffeu;
-
-inline uint32_t reduce(uint64_t x) {
-    uint32_t m = (uint32_t)x * MPRIME;
-    uint64_t u = x + (uint64_t)m * P;
-    uint32_t r = (uint32_t)(u >> 32);
-    return r >= P ? r - P : r;
-}
-inline uint32_t add(uint32_t a, uint32_t b) { uint32_t s = a + b; return s >= P ? s - P : s; }
-inline uint32_t sub(uint32_t a, uint32_t b) { return a >= b ? a - b : a + P - b; }
-inline uint32_t neg(uint32_t a) { return a ? P - a : 0; }
-inline uint32_t mul(uint32_t a, uint32_t b) { return reduce((uint64_t)a * b); }
-constexpr uint32_t to_monty(uint64_t c) { return (uint32_t)(((c % P) << 32) % P); }
-inline uint32_t from_monty(uint32_t m) { return reduce(m); }
-inline uint32_t pow(uint32_t b, uint64_t e) {
-    uint32_t r = ONE;
-    while (e) { if (e & 1) r = mul(r, b); b = mul(b, b); e >>= 1; }
-    return r;
-}
-inline uint32_t inv(uint32_t a) { return pow(a, P - 2); }
-
-struct E4 {
-    uint32_t c[4] = {0, 0, 0, 0};
-    static E4 one() { E4 r; r.c[0] = ONE; return r; }
-    static E4 from_base(uint32_t a) { E4 r; r.c[0] = a; return r; }
+// kb::Ext with value semantics for host code: default-constructed to zero, and operators.  Passes wherever a kernel takes a kb::Ext.
+struct E4 : kb::Ext {
+    E4() : kb::Ext{{0, 0, 0, 0}} {}
+    E4(const kb::Ext& e) : kb::Ext(e) {}
+    static E4 one() { return kb::ext_one(); }
+    static E4 from_base(uint32_t a) { return kb::ext_from_base(a); }
+    // word by word: host buffers (caller arrays, proof words at odd offsets) are only 4-byte aligned, and kb::ext_load reads a uint4
     static E4 load(const uint32_t* p) { E4 r; for (int i = 0; i < 4; i++) r.c[i] = p[i]; return r; }
     void store(uint32_t* p) const { for (int i = 0; i < 4; i++) p[i] = c[i]; }
-    bool operator==(const E4& o) const { return c[0] == o.c[0] && c[1] == o.c[1] && c[2] == o.c[2] && c[3] == o.c[3]; }
+    bool operator==(const E4& o) const { return kb::ext_eq(*this, o); }
     bool is_zero() const { return !(c[0] | c[1] | c[2] | c[3]); }
 };
-inline E4 operator+(const E4& a, const E4& b) { E4 r; for (int i = 0; i < 4; i++) r.c[i] = add(a.c[i], b.c[i]); return r; }
-inline E4 operator-(const E4& a, const E4& b) { E4 r; for (int i = 0; i < 4; i++) r.c[i] = sub(a.c[i], b.c[i]); return r; }
-inline E4 operator*(const E4& a, uint32_t s) { E4 r; for (int i = 0; i < 4; i++) r.c[i] = mul(a.c[i], s); return r; }
-// x < 2 p 2^32 (a sum of up to four products of canonical values) -> canonical x 2^-32 mod p; subtractive Montgomery form
-inline uint32_t reduce4(uint64_t x) {
-    uint32_t hi = (uint32_t)(x >> 32);
-    if (hi >= P) hi -= P;
-    const uint32_t m = (uint32_t)x * 0x81000001u;  // lo(x) * p^-1 mod 2^32
-    const uint32_t q = (uint32_t)(((uint64_t)m * P) >> 32);
-    return hi >= q ? hi - q : hi + P - q;
-}
-inline E4 operator*(const E4& a, const E4& b) {
-    // x^4 = 3 folded into b: every coefficient is one sum of four 62-bit products and one reduction (same form as kb::ext_mul)
-    auto tri = [](uint32_t v) { return add(add(v, v), v); };
-    const uint64_t a0 = a.c[0], a1 = a.c[1], a2 = a.c[2], a3 = a.c[3];
-    const uint64_t b0 = b.c[0], b1 = b.c[1], b2 = b.c[2], b3 = b.c[3];
-    const uint64_t t1 = tri(b.c[1]), t2 = tri(b.c[2]), t3 = tri(b.c[3]);
-    E4 r;
-    r.c[0] = reduce4(a0 * b0 + a1 * t3 + a2 * t2 + a3 * t1);
-    r.c[1] = reduce4(a0 * b1 + a1 * b0 + a2 * t3 + a3 * t2);
-    r.c[2] = reduce4(a0 * b2 + a1 * b1 + a2 * b0 + a3 * t3);
-    r.c[3] = reduce4(a0 * b3 + a1 * b2 + a2 * b1 + a3 * b0);
-    return r;
-}
-// the base-field names for E4, so that code templated on the value type (the constraint interpreter, machine.cuh) takes either
-inline E4 add(const E4& a, const E4& b) { return a + b; }
-inline E4 sub(const E4& a, const E4& b) { return a - b; }
-inline E4 mul(const E4& a, const E4& b) { return a * b; }
-inline E4 neg(const E4& a) { return E4() - a; }
-inline E4 inv(const E4& a) {
-    // Frobenius-free inverse via the tower F[y]/(y^2-3) (y = x^2)
-    const uint32_t three = to_monty(3);
-    uint32_t A0 = a.c[0], A1 = a.c[2], B0 = a.c[1], B1 = a.c[3];
-    uint32_t n0 = sub(add(mul(A0, A0), mul(three, mul(A1, A1))), mul(three, add(mul(B0, B1), mul(B0, B1))));
-    uint32_t n1 = sub(add(mul(A0, A1), mul(A0, A1)), add(mul(B0, B0), mul(three, mul(B1, B1))));
-    uint32_t d = inv(sub(mul(n0, n0), mul(three, mul(n1, n1))));
-    uint32_t i0 = mul(n0, d), i1 = neg(mul(n1, d));
-    E4 conj; conj.c[0] = A0; conj.c[1] = neg(B0); conj.c[2] = A1; conj.c[3] = neg(B1);
-    E4 s; s.c[0] = i0; s.c[2] = i1;
-    return conj * s;
-}
+inline E4 operator+(const E4& a, const E4& b) { return kb::ext_add(a, b); }
+inline E4 operator-(const E4& a, const E4& b) { return kb::ext_sub(a, b); }
+inline E4 operator-(const E4& a) { return kb::ext_neg(a); }
+inline E4 operator*(const E4& a, const E4& b) { return kb::ext_mul(a, b); }
+inline E4 operator*(const E4& a, uint32_t s) { return kb::ext_mul_base(a, s); }
+
+// every word is a canonical Montgomery word (< p)
+inline bool canonical(const uint32_t* w, size_t n) { for (size_t i = 0; i < n; i++) if (w[i] >= kb::P) return false; return true; }
 
 // eq(point, i), point[0] <-> MSB of i  (slop/crates/multilinear/src/lagrange.rs:19-45)
 inline std::vector<E4> partial_lagrange(const std::vector<E4>& point) {
@@ -124,7 +73,7 @@ template <int N> inline void lagrange_basis(const E4 (&x)[N], E4 (&L)[N][N]) {
     }
     pre[0] = den[0];
     for (int i = 1; i < N; i++) pre[i] = pre[i - 1] * den[i];
-    E4 acc = inv(pre[N - 1]);
+    E4 acc = kb::ext_inv(pre[N - 1]);
     for (int i = N - 1; i >= 0; i--) {
         const E4 di = i ? acc * pre[i - 1] : acc;  // 1 / den_i
         acc = acc * den[i];

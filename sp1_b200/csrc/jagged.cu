@@ -359,7 +359,7 @@ __global__ void __launch_bounds__(128) bp_update_kernel(const uint8_t* __restric
 
 // p(x) through (0, y0), (1, y1), (1/2, yh): coefficients c0, c1, c2
 inline void interp_0_1_half(const E4& y0, const E4& y1, const E4& yh, E4 c[3]) {
-    const uint32_t two = hf::to_monty(2), three = hf::to_monty(3), four = hf::to_monty(4);
+    const uint32_t two = kb::to_monty_c(2), three = kb::to_monty_c(3), four = kb::to_monty_c(4);
     c[0] = y0;
     c[1] = yh * four - y0 * three - y1;
     c[2] = (y1 + y0) * two - yh * four;
@@ -573,7 +573,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         SP1_TRY(sum_mail_partials(ctx, prev_seq, prev_g, s2));
         E4 e1 = round_claim - e0;
         E4 c[3];
-        interp_0_1_half(e0, e1, eh * hf::inv(hf::to_monty(4)), c);
+        interp_0_1_half(e0, e1, eh * kb::inv(kb::to_monty_c(4)), c);
         for (int i = 0; i < 3; i++) ch.observe_n(c[i].c, 4);
         sc.poly(c, 3);
         E4 alpha; ch.sample_ext(alpha.c);
@@ -587,7 +587,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             for (size_t t = 0; t < m; t++) { w[m + t] = w[t] * alpha; w[t] = w[t] * (E4::one() - alpha); }
             load_weights();
         }
-        SP1_TRY(launch_sums(rd + 1, to_ext(alpha), mail, prev_g));
+        SP1_TRY(launch_sums(rd + 1, alpha, mail, prev_g));
     }
     // component evaluations: base[0] (the dense trace at the sumcheck point), ext[0]
     // (posted by the last fold launch next to its, unused, partial sums: payload EF slot 2)
@@ -635,7 +635,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
         SP1_CUDA(cudaMemcpyAsync(d_zc, zc.data(), (size_t)nk * 16, cudaMemcpyHostToDevice, st));
         std::vector<E4> ones(nk, E4::one());
         SP1_CUDA(cudaMemcpyAsync(d_inter, ones.data(), (size_t)nk * 16, cudaMemcpyHostToDevice, st));
-        const Ext dhalf = to_ext(E4::from_base(hf::inv(hf::to_monty(2))));
+        const Ext dhalf = kb::ext_from_base(kb::inv(kb::to_monty_c(2)));
         // prefix / suffix states (see bp_suffix_kernel): T for the first half now, rebuilt once when the second half starts
         uint32_t *d_T, *d_P, *d_rho_pos;
         SP1_TRY(mem.alloc((void**)&d_T, (size_t)(hl + 2) * nk * 64));
@@ -676,8 +676,7 @@ sp1b200_err sp1b200_jagged_prove(sp1b200_ctx* ctx, sp1b200_jagged_round* const* 
             E4 alpha; ch.sample_ext(alpha.c);
             rhos.insert(rhos.begin(), alpha);
             cl = eval3(c, alpha);
-            const Ext da = to_ext(alpha);
-            SP1_LAUNCH(ctx, bp_update_kernel, blocks_for(nk, 128), 128, 0, d_bits, nk, dim, round, da, d_rho_pos, d_ri, d_inter, d_P);
+            SP1_LAUNCH(ctx, bp_update_kernel, blocks_for(nk, 128), 128, 0, d_bits, nk, dim, round, alpha, d_rho_pos, d_ri, d_inter, d_P);
         }
         je_eval = cl;
         t.stop();

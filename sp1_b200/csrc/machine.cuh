@@ -4,7 +4,6 @@
 #include "hostfield.hpp"
 #include <algorithm>
 #include <cstdint>
-#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -27,22 +26,20 @@ struct HostProg {  // host copy for host_eval_constraints (the prover's all-zero
     std::vector<std::pair<uint32_t, uint32_t>> zc_pieces;
 };
 
-// The host interpreter of a chip's bytecode at one row: Σ powers[assert_alphas[i]] · regs[assert_regs[i]].  R is the register type:
-// the base field's Montgomery word (the prover's all-zero row) or hf::E4 (the verifier's opened values).  leaf(l) is the row's value
-// of leaf l; pv the public values.
-template <class R, class Leaf>
+// The host interpreter of a chip's bytecode at one row of extension values: Σ powers[assert_alphas[i]] · regs[assert_regs[i]].
+// leaf(l) is the row's value of leaf l (the prover's all-zero row, the verifier's opened values); pv the public values.
+template <class Leaf>
 hf::E4 host_eval_constraints(const HostProg& p, uint32_t n_regs, const uint32_t* pv, const std::vector<hf::E4>& powers, Leaf leaf) {
-    const auto base = [](uint32_t x) { if constexpr (std::is_same<R, hf::E4>::value) return hf::E4::from_base(x); else return x; };
-    std::vector<R> regs(std::max<uint32_t>(n_regs, 1));
+    std::vector<hf::E4> regs(std::max<uint32_t>(n_regs, 1));
     for (const DagInstr& in : p.instrs) {
         switch (in.opcode) {
             case BC_LOAD_LEAF: regs[in.out] = leaf(p.leaves[in.a]); break;
-            case BC_LOAD_CONST: regs[in.out] = base(p.consts[in.a]); break;
-            case BC_LOAD_PUBLIC: regs[in.out] = base(pv[p.publics[in.a]]); break;
-            case BC_ADD_F: regs[in.out] = hf::add(regs[in.a], regs[in.b]); break;
-            case BC_SUB_F: regs[in.out] = hf::sub(regs[in.a], regs[in.b]); break;
-            case BC_MUL_F: regs[in.out] = hf::mul(regs[in.a], regs[in.b]); break;
-            case BC_NEG_F: regs[in.out] = hf::neg(regs[in.a]); break;
+            case BC_LOAD_CONST: regs[in.out] = hf::E4::from_base(p.consts[in.a]); break;
+            case BC_LOAD_PUBLIC: regs[in.out] = hf::E4::from_base(pv[p.publics[in.a]]); break;
+            case BC_ADD_F: regs[in.out] = regs[in.a] + regs[in.b]; break;
+            case BC_SUB_F: regs[in.out] = regs[in.a] - regs[in.b]; break;
+            case BC_MUL_F: regs[in.out] = regs[in.a] * regs[in.b]; break;
+            case BC_NEG_F: regs[in.out] = -regs[in.a]; break;
         }
     }
     hf::E4 acc;

@@ -321,11 +321,11 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
     uint32_t* d_trees;
     SP1_TRY(mem.alloc((void**)&d_trees, 2 * M * 32));
 
-    uint32_t d_h = hf::to_monty(log_h);
+    uint32_t d_h = kb::to_monty_c(log_h);
     ch.observe(d_h);
     std::vector<E4> point(log_h);
     for (uint32_t i = 0; i < log_h; i++) point[i] = E4::load(h_point + 4 * (n_point - log_h + i));
-    const uint32_t half = hf::inv(hf::to_monty(2));
+    const uint32_t half = kb::inv(kb::to_monty_c(2));
     std::vector<uint32_t> uni;                      // univariate messages
     std::vector<uint32_t> fri_commits;              // d x 8
     std::vector<uint32_t*> cw_ptr(log_h + 1), tree_ptr(log_h);
@@ -364,7 +364,7 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         E4 zv[1];
         sum_partials(mh + 16, nblk, zv);
         const E4 zero_val = zv[0];
-        E4 one_val = (claim - zero_val) * hf::inv(last) + zero_val;
+        E4 one_val = (claim - zero_val) * kb::ext_inv(last) + zero_val;
         uni.insert(uni.end(), zero_val.c, zero_val.c + 4);
         uni.insert(uni.end(), one_val.c, one_val.c + 4);
         ch.observe_n(zero_val.c, 4); ch.observe_n(one_val.c, 4);
@@ -372,10 +372,9 @@ sp1b200_err sp1b200_stacked_prove(sp1b200_ctx* ctx, sp1b200_commit* const* round
         fri_commits.insert(fri_commits.end(), rc + 8, rc + 16);
         memcpy(fri_roots[r].data(), rc, 32);
         E4 beta; ch.sample_ext(beta.c);
-        const Ext dbeta = to_ext(beta), dbh = to_ext(beta * half);
-        SP1_LAUNCH(ctx, fold_codeword_kernel, blocks_for(m_cur / 2), 256, 0, cw_ptr[r], (int)(log_h + b - r), dbh, half, ctx->d_TH,
+        SP1_LAUNCH(ctx, fold_codeword_kernel, blocks_for(m_cur / 2), 256, 0, cw_ptr[r], (int)(log_h + b - r), beta * half, half, ctx->d_TH,
                    ctx->d_TL, cw_ptr[r + 1]);
-        SP1_LAUNCH(ctx, fold_mle_kernel, blocks_for(n_cur / 2), 256, 0, cur_mle, n_cur / 2, dbeta, nxt_mle);
+        SP1_LAUNCH(ctx, fold_mle_kernel, blocks_for(n_cur / 2), 256, 0, cur_mle, n_cur / 2, beta, nxt_mle);
         std::swap(cur_mle, nxt_mle);
         claim = zero_val + beta * one_val;
     }

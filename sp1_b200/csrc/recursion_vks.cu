@@ -44,7 +44,6 @@ constexpr uint32_t NUM_TO_HASH = at(DIGEST);  // NUM_PV_ELMS_TO_HASH: every word
 static_assert(rpv::NUM_ELTS == 187 && rpv::NUM_TO_HASH == 175 && rpv::at(rpv::PROOF_NONCE) == 183, "recursion public values layout");
 static_assert(rpv::at(rpv::SP1_VK_DIGEST) == 136 && rpv::at(rpv::VK_ROOT) == 144 && rpv::at(rpv::IS_COMPLETE) == 168, "recursion public values layout");
 
-constexpr uint32_t VK_TAIL_WORDS = 24;    // pc_start[3] | initial_global_cumulative_sum x[7] y[7] | enable_untrusted_programs | 6 zeros
 constexpr uint32_t VK_HASHED_TAIL = 18;   // the tail words hash_koalabear reads (the padding is observed, not hashed)
 constexpr uint32_t VK_WORDS = 8 + VK_TAIL_WORDS;
 constexpr uint32_t MAX_PATH = 64;
@@ -59,8 +58,6 @@ const char* const COMPRESSED_NAMES[SP1B200_VERDICT_COMPRESSED_COUNT - SP1B200_VE
     "UninitializedVerificationKey",
 };
 
-bool canonical_words(const uint32_t* w, size_t n) { for (size_t i = 0; i < n; i++) if (w[i] >= hf::P) return false; return true; }
-
 // reverse_bits_len (crates/primitives): the low `bits` bits of x reversed; higher bits are dropped
 uint64_t reverse_bits_len(uint64_t x, uint32_t bits) {
     uint64_t r = 0;
@@ -71,7 +68,7 @@ uint64_t reverse_bits_len(uint64_t x, uint32_t bits) {
 // canonical lexicographic order of two digests (the BTreeMap order of [SP1Field; 8])
 bool key_less(const uint32_t* a, const uint32_t* b) {
     for (int i = 0; i < 8; i++) {
-        const uint32_t x = hf::from_monty(a[i]), y = hf::from_monty(b[i]);
+        const uint32_t x = kb::to_canonical(a[i]), y = kb::to_canonical(b[i]);
         if (x != y) return x < y;
     }
     return false;
@@ -108,7 +105,7 @@ uint32_t check_after_shard(const uint32_t* pv, const uint32_t* key, const sp1b20
         vk_hash(key, key + 8, d);
         if (!merkle_proof_holds(d, index, path, n_path, vks.root)) return SP1B200_VERDICT_INVALID_VERIFICATION_KEY;
     }
-    if (pv[rpv::at(rpv::IS_COMPLETE)] != hf::ONE) return SP1B200_VERDICT_IS_COMPLETE;
+    if (pv[rpv::at(rpv::IS_COMPLETE)] != kb::ONE) return SP1B200_VERDICT_IS_COMPLETE;
     if (memcmp(pv + rpv::at(rpv::SP1_VK_DIGEST), sp1_vk_digest8, 32)) return SP1B200_VERDICT_SP1_VK_DIGEST;
     return SP1B200_VERDICT_ACCEPT;
 }
@@ -126,18 +123,18 @@ sp1b200_err sp1b200_vk_hash(const uint32_t* h_prep_commit8, const uint32_t* h_vk
     if (!h_prep_commit8 || !h_vk_tail || !h_out8) return sp1b200_set_error("vk_hash: NULL argument");
     if (n_vk_tail != VK_TAIL_WORDS)
         return sp1b200_set_error("vk_hash: n_vk_tail is %u; the verifying key without mprotect has %u words after the commitment", n_vk_tail, VK_TAIL_WORDS);
-    if (!canonical_words(h_prep_commit8, 8) || !canonical_words(h_vk_tail, n_vk_tail)) return sp1b200_set_error("vk_hash: a key word is not canonical");
+    if (!hf::canonical(h_prep_commit8, 8) || !hf::canonical(h_vk_tail, n_vk_tail)) return sp1b200_set_error("vk_hash: a key word is not canonical");
     vk_hash(h_prep_commit8, h_vk_tail, h_out8);
     return nullptr;
 }
 
 sp1b200_err sp1b200_digest_bytes32(const uint32_t* h_digest8, uint8_t* h_out32) {
     if (!h_digest8 || !h_out32) return sp1b200_set_error("digest_bytes32: NULL argument");
-    if (!canonical_words(h_digest8, 8)) return sp1b200_set_error("digest_bytes32: a digest word is not canonical");
+    if (!hf::canonical(h_digest8, 8)) return sp1b200_set_error("digest_bytes32: a digest word is not canonical");
     // Σ_i c_i · 2^(31 (7 - i)) < 2^248 < r: no reduction; big-endian, so byte 0 is always zero
     memset(h_out32, 0, 32);
     for (uint32_t i = 0; i < 8; i++) {
-        const uint32_t c = hf::from_monty(h_digest8[i]);
+        const uint32_t c = kb::to_canonical(h_digest8[i]);
         for (uint32_t b = 0; b < 31; b++) {
             const uint32_t pos = 31 * (7 - i) + b;
             h_out32[31 - pos / 8] |= (uint8_t)(((c >> b) & 1) << (pos % 8));
@@ -159,7 +156,7 @@ sp1b200_err sp1b200_recursion_vks_create(sp1b200_ctx* ctx, const uint32_t* h_dig
     *out = nullptr;
     const uint64_t max_keys = (uint64_t)1 << MAX_LOG_KEYS;
     if (n > max_keys || pad_to > max_keys) return sp1b200_set_error("recursion_vks_create: more than 2^%u keys", MAX_LOG_KEYS);
-    if (!canonical_words(h_digests, 8 * n)) return sp1b200_set_error("recursion_vks_create: a digest word is not canonical");
+    if (!hf::canonical(h_digests, 8 * n)) return sp1b200_set_error("recursion_vks_create: a digest word is not canonical");
     // RecursionVks::from_map: the keys, then [i; 8] for every missing index below pad_to, deduplicated and sorted
     std::vector<uint32_t> all(h_digests, h_digests + 8 * n);
     std::vector<uint32_t> order;
@@ -170,7 +167,7 @@ sp1b200_err sp1b200_recursion_vks_create(sp1b200_ctx* ctx, const uint32_t* h_dig
         order.erase(std::unique(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return !memcmp(&all[8 * a], &all[8 * b], 32); }), order.end());
     };
     sort_unique();
-    for (uint64_t i = order.size(); i < pad_to; i++) all.insert(all.end(), 8, hf::to_monty(i));
+    for (uint64_t i = order.size(); i < pad_to; i++) all.insert(all.end(), 8, kb::to_monty_c(i));
     if (pad_to > order.size()) sort_unique();
     const uint64_t nk = order.size();
     if (nk < 2) return sp1b200_set_error("recursion_vks_create: %llu key(s); the tree needs at least two", (unsigned long long)nk);
@@ -211,7 +208,7 @@ uint64_t sp1b200_recursion_vks_num_keys(const sp1b200_recursion_vks* vks) { retu
 sp1b200_err sp1b200_recursion_vks_open(const sp1b200_recursion_vks* vks, const uint32_t* h_digest8, uint64_t* h_index, uint32_t* h_path,
                                        uint32_t path_cap, uint32_t* h_n_path) {
     if (!vks || !h_digest8 || !h_index || !h_n_path) return sp1b200_set_error("recursion_vks_open: NULL argument");
-    if (!canonical_words(h_digest8, 8)) return sp1b200_set_error("recursion_vks_open: a digest word is not canonical");
+    if (!hf::canonical(h_digest8, 8)) return sp1b200_set_error("recursion_vks_open: a digest word is not canonical");
     const uint64_t nk = vks->keys.size() / 8;
     uint64_t lo = 0, hi = nk;
     while (lo < hi) {
@@ -244,7 +241,7 @@ sp1b200_err sp1b200_verify_compressed(sp1b200_ctx* ctx, const sp1b200_machine* m
         return sp1b200_set_error("verify_compressed: NULL argument");
     if (mode != SP1B200_COMPRESSED && mode != SP1B200_SHRINK) return sp1b200_set_error("verify_compressed: mode %u is neither compressed nor shrink", mode);
     if (mode == SP1B200_COMPRESSED && h_shrink_vk) return sp1b200_set_error("verify_compressed: a shrink key in compressed mode");
-    if (h_shrink_vk && !canonical_words(h_shrink_vk, VK_WORDS)) return sp1b200_set_error("verify_compressed: the shrink key is not canonical");
+    if (h_shrink_vk && !hf::canonical(h_shrink_vk, VK_WORDS)) return sp1b200_set_error("verify_compressed: the shrink key is not canonical");
     const auto t0 = std::chrono::steady_clock::now();
     const size_t nch = m->chips.size();
     bool has_prep = false;
@@ -255,11 +252,11 @@ sp1b200_err sp1b200_verify_compressed(sp1b200_ctx* ctx, const sp1b200_machine* m
         const std::string who = "verify_compressed: proof " + std::to_string(s);
         if (!h_proofs[s]) return sp1b200_set_error("%s: NULL proof", who.c_str());
         const uint32_t* key = h_vks + (size_t)VK_WORDS * s;
-        if (!canonical_words(key, VK_WORDS)) return sp1b200_set_error("%s: a verifying-key word is not canonical", who.c_str());
+        if (!hf::canonical(key, VK_WORDS)) return sp1b200_set_error("%s: a verifying-key word is not canonical", who.c_str());
         if (h_vk_path_len[s] > MAX_PATH) return sp1b200_set_error("%s: vk Merkle path of %u digests, more than %u", who.c_str(), h_vk_path_len[s], MAX_PATH);
         if (h_vk_path_len[s] && !h_vk_paths[s]) return sp1b200_set_error("%s: NULL vk Merkle path", who.c_str());
-        if (!canonical_words(h_vk_paths[s], 8 * (size_t)h_vk_path_len[s])) return sp1b200_set_error("%s: a vk Merkle path word is not canonical", who.c_str());
-        if (!canonical_words(h_sp1_vk_digests + 8 * (size_t)s, 8)) return sp1b200_set_error("%s: the SP1 vk digest is not canonical", who.c_str());
+        if (!hf::canonical(h_vk_paths[s], 8 * (size_t)h_vk_path_len[s])) return sp1b200_set_error("%s: a vk Merkle path word is not canonical", who.c_str());
+        if (!hf::canonical(h_sp1_vk_digests + 8 * (size_t)s, 8)) return sp1b200_set_error("%s: the SP1 vk digest is not canonical", who.c_str());
         in.emplace_back(new VerifyShardIn);
         SP1_TRY(verify_parse_shard(ctx, m, has_prep ? key : nullptr, h_heights + (size_t)s * nch, chip_names, h_proofs[s], h_n_words[s], who,
                                    *in.back()));

@@ -1,9 +1,10 @@
-// Septic extension F_p^7 = F_p[z]/(z^7 - 3z - 5) over KoalaBear and the curve y^2 = x^3 + 45x + 41z^3 over it, on the device, for
-// the program setup (setup.cu): the hash-to-curve SepticCurve::lift_x and the complete addition law of SepticCurveComplete
-// (crates/hypercube/src/septic_extension.rs, septic_curve.rs).  Every lift takes a square test and usually a square root, so the
-// Frobenius maps are table-driven (49 products each) and the reciprocal goes through the norm; the host-only septic.hpp serves the
-// verifier's few hundred operations with a Fermat-power inverse instead.  Montgomery words, like kb31.cuh; __host__ __device__ so
-// that the CPU suite runs the same source through libsp1b200_hostcheck.so.
+// Septic extension F_p^7 = F_p[z]/(z^7 - 3z - 5) over KoalaBear and the curve y^2 = x^3 + 45x + 41z^3 over it
+// (crates/hypercube/src/septic_extension.rs, septic_curve.rs, septic_digest.rs): the hash-to-curve SepticCurve::lift_x and the
+// complete addition law of SepticCurveComplete for the program setup (setup.cu), and the incomplete addition law and SepticDigest
+// addition with which the core-proof verifier sums the shards' global cumulative sums (verify_core.cu).  Every lift takes a square
+// test and usually a square root, so the Frobenius maps are table-driven (49 products each) and the reciprocal goes through the
+// norm.  Montgomery words, like kb31.cuh; __host__ __device__ so that the CPU suite runs the same source through
+// libsp1b200_hostcheck.so.
 #pragma once
 #include "kb31.cuh"
 #include "poseidon2.cuh"
@@ -234,13 +235,63 @@ KB_HD Pt add_complete(const Pt& p, const Pt& q) {
     return r;
 }
 
-// SepticDigest::zero() (CURVE_CUMULATIVE_SUM_START), Montgomery words
-KB_HD Pt digest_zero() {
-    constexpr uint32_t x[7] = {0x1414213, 0x5623730, 0x9504880, 0x1688724, 0x2096980, 0x7856967, 0x1875376};
-    constexpr uint32_t y[7] = {2020310104, 1513506566, 1843922297, 2003644209, 805967281, 1882435203, 1623804682};
+// SepticCurve::add_incomplete (septic_curve.rs): the chord through p and q.  Returns false, and leaves r alone, on the exceptional
+// case x_p = x_q, where the reference divides by zero and panics.  r may alias p or q.
+KB_HD bool add_incomplete(const Pt& p, const Pt& q, Pt& r) {
+    const E7 dx = sub(q.x, p.x);
+    if (is_zero(dx)) return false;
+    const E7 slope = mul(sub(q.y, p.y), inv(dx));
+    const E7 x = sub(sub(sqr(slope), p.x), q.x);
+    r = Pt{x, sub(mul(slope, sub(p.x, x)), p.y)};
+    return true;
+}
+KB_HD bool sub_incomplete(const Pt& p, const Pt& q, Pt& r) { return add_incomplete(p, neg(q), r); }
+
+// a point of canonical coordinates, in Montgomery words
+KB_HD Pt point_from_canonical(const uint32_t (&x)[7], const uint32_t (&y)[7]) {
     Pt p;
     for (int i = 0; i < 7; i++) { p.x.c[i] = kb::to_monty_c(x[i]); p.y.c[i] = kb::to_monty_c(y[i]); }
     return p;
+}
+// SepticDigest::zero() (CURVE_CUMULATIVE_SUM_START, from sqrt 2)
+KB_HD Pt digest_zero() {
+    constexpr uint32_t x[7] = {0x1414213, 0x5623730, 0x9504880, 0x1688724, 0x2096980, 0x7856967, 0x1875376};
+    constexpr uint32_t y[7] = {2020310104, 1513506566, 1843922297, 2003644209, 805967281, 1882435203, 1623804682};
+    return point_from_canonical(x, y);
+}
+// SepticDigest::starting_digest() (DIGEST_SUM_START, from sqrt 3)
+KB_HD Pt digest_start() {
+    constexpr uint32_t x[7] = {0x1732050, 0x8075688, 0x7729352, 0x7446341, 0x5058723, 0x6694280, 0x5253810};
+    constexpr uint32_t y[7] = {1095433104, 7540207, 1124564165, 2035506693, 11121645, 102781365, 398772161};
+    return point_from_canonical(x, y);
+}
+// SepticCurve::dummy() (CURVE_WITNESS_DUMMY_POINT, from e)
+KB_HD Pt dummy_point() {
+    constexpr uint32_t x[7] = {0x2718281 + (1 << 24), 0x8284590, 0x4523536, 0x0287471, 0x3526624, 0x9775724, 0x7093699};
+    constexpr uint32_t y[7] = {1250555984, 1592495468, 656721246, 420301347, 2125819749, 819876460, 17687681};
+    return point_from_canonical(x, y);
+}
+KB_HD bool is_zero_digest(const Pt& p) { const Pt z = digest_zero(); return eq(p.x, z.x) && eq(p.y, z.y); }
+
+// SepticDigest + SepticDigest (septic_digest.rs:67-83): start + (a - zero) + (b - zero) + zero - start, one incomplete addition at a
+// time.  Returns false, and leaves r alone, when one of them meets the exceptional case.
+KB_HD bool digest_add(const Pt& a, const Pt& b, Pt& r) {
+    const Pt start = digest_start(), zero = digest_zero();
+    Pt s;
+    return add_incomplete(start, a, s) && sub_incomplete(s, zero, s) && add_incomplete(s, b, s) && sub_incomplete(s, zero, s) &&
+           add_incomplete(s, zero, s) && sub_incomplete(s, start, s) && (r = s, true);
+}
+
+// a point as 14 Montgomery words: x, then y
+KB_HD Pt load_point(const uint32_t* w) {
+    Pt p;
+#pragma unroll
+    for (int i = 0; i < 7; i++) { p.x.c[i] = w[i]; p.y.c[i] = w[7 + i]; }
+    return p;
+}
+KB_HD void store_point(const Pt& p, uint32_t* w) {
+#pragma unroll
+    for (int i = 0; i < 7; i++) { w[i] = p.x.c[i]; w[7 + i] = p.y.c[i]; }
 }
 
 // the lift_x messages of Program::initial_global_cumulative_sum (crates/core/executor/src/program.rs:175-221), Montgomery words.

@@ -3,7 +3,6 @@
 // One thread lifts one image entry onto the septic curve (septic.cuh), a tree of per-thread chunk sums adds the points under the
 // complete law, and a radix sort of the keys finds duplicate addresses and page indices.
 #include "ctx.cuh"
-#include "hostfield.hpp"
 #include "septic.cuh"
 #include "sumcheck.cuh"
 #include <cub/device/device_radix_sort.cuh>
@@ -13,17 +12,6 @@ namespace {
 constexpr uint32_t SUM_CHUNK = 16;   // points per thread and tree level
 constexpr uint64_t NONE = ~0ull;
 
-__device__ __forceinline__ void st_pt(const s7::Pt& p, uint32_t* o) {
-#pragma unroll
-    for (int i = 0; i < 7; i++) { o[i] = p.x.c[i]; o[7 + i] = p.y.c[i]; }
-}
-__device__ __forceinline__ s7::Pt ld_pt(const uint32_t* o) {
-    s7::Pt p;
-#pragma unroll
-    for (int i = 0; i < 7; i++) { p.x.c[i] = o[i]; p.y.c[i] = o[7 + i]; }
-    return p;
-}
-
 // entry i < n_mem: memory entry i; n_mem <= i < n: page entry i - n_mem; i = n: SepticDigest::zero().  pts[i] = -lift_x(message);
 // an entry without a point leaves infinity and records its index in *failed (lowest wins).
 __global__ void __launch_bounds__(128) setup_lift_kernel(const uint64_t* __restrict__ addrs, const uint64_t* __restrict__ words,
@@ -31,7 +19,7 @@ __global__ void __launch_bounds__(128) setup_lift_kernel(const uint64_t* __restr
                                                          uint64_t n, uint32_t* __restrict__ pts, unsigned long long* failed) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n) return;
-    if (i == n) { st_pt(s7::digest_zero(), pts + 14 * i); return; }
+    if (i == n) { s7::store_point(s7::digest_zero(), pts + 14 * i); return; }
     uint32_t m[8];
     if (i < n_mem) s7::memory_message(addrs[i], words[i], m);
     else s7::page_message(pages[i - n_mem], prots[i - n_mem], m);
@@ -42,7 +30,7 @@ __global__ void __launch_bounds__(128) setup_lift_kernel(const uint64_t* __restr
     } else {
         p = s7::neg(p);
     }
-    st_pt(p, pts + 14 * i);
+    s7::store_point(p, pts + 14 * i);
 }
 
 // out[t] = in[t * SUM_CHUNK] + ... + in[min(n, (t + 1) * SUM_CHUNK) - 1] under the complete law
@@ -51,9 +39,9 @@ __global__ void __launch_bounds__(128) setup_sum_kernel(const uint32_t* __restri
     const uint64_t b = t * SUM_CHUNK;
     if (b >= n) return;
     const uint64_t e = b + SUM_CHUNK < n ? b + SUM_CHUNK : n;
-    s7::Pt acc = ld_pt(in + 14 * b);
-    for (uint64_t k = b + 1; k < e; k++) acc = s7::add_complete(acc, ld_pt(in + 14 * k));
-    st_pt(acc, out + 14 * t);
+    s7::Pt acc = s7::load_point(in + 14 * b);
+    for (uint64_t k = b + 1; k < e; k++) acc = s7::add_complete(acc, s7::load_point(in + 14 * k));
+    s7::store_point(acc, out + 14 * t);
 }
 
 // sorted keys: the lowest key that occurs twice
@@ -145,11 +133,11 @@ extern "C" sp1b200_err sp1b200_program_vk_tail(sp1b200_ctx* ctx, uint64_t pc_sta
     bool inf = true;
     for (uint32_t w : sum) inf = inf && w == 0;
     if (inf) return sp1b200_set_error("program_vk_tail: the initial global cumulative sum is the point at infinity");
-    h_vk_tail24[0] = hf::to_monty(pc_start_abs & 0xFFFF);
-    h_vk_tail24[1] = hf::to_monty((pc_start_abs >> 16) & 0xFFFF);
-    h_vk_tail24[2] = hf::to_monty((pc_start_abs >> 32) & 0xFFFF);
+    h_vk_tail24[0] = kb::to_monty_c(pc_start_abs & 0xFFFF);
+    h_vk_tail24[1] = kb::to_monty_c((pc_start_abs >> 16) & 0xFFFF);
+    h_vk_tail24[2] = kb::to_monty_c((pc_start_abs >> 32) & 0xFFFF);
     for (int i = 0; i < 14; i++) h_vk_tail24[3 + i] = sum[i];
-    h_vk_tail24[17] = enable_untrusted_programs ? hf::ONE : 0;
+    h_vk_tail24[17] = enable_untrusted_programs ? kb::ONE : 0;
     for (int i = 18; i < 24; i++) h_vk_tail24[i] = 0;
     SP1_TRY(addrs.finish()); SP1_TRY(words.finish()); SP1_TRY(pages.finish());
     return prots.finish();

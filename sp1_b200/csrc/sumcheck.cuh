@@ -22,8 +22,6 @@ struct DevFree {
 };
 inline unsigned blocks_for(uint64_t n, unsigned bs = 256) { return (unsigned)((n + bs - 1) / bs); }
 
-inline kb::Ext to_ext(const hf::E4& e) { return kb::Ext{{e.c[0], e.c[1], e.c[2], e.c[3]}}; }
-
 // w^e for the two-adic generator w of order 2^24, from the context's tables: TH[e >> 12] * TL[e & 4095]
 __device__ __forceinline__ uint32_t root_pow(const uint32_t* __restrict__ TH, const uint32_t* __restrict__ TL, uint32_t e) {
     uint32_t hi = __ldg(TH + (e >> 12));

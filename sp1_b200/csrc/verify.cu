@@ -32,6 +32,7 @@
 namespace {
 
 using hf::E4;
+using hf::canonical;
 using kb::Ext;
 
 // ---- device part ----------------------------------------------------------------------------------------------------------------
@@ -192,7 +193,7 @@ static_assert(std::size(VERDICT_NAMES) == SP1B200_VERDICT_EMPTY_PROOF, "one name
 inline bool neq(const E4& a, const E4& b) { return !(a == b); }
 inline E4 ld(const uint32_t* p) { return E4::load(p); }
 inline E4 eqf(const E4& a, const E4& b) { return a * b + (E4::one() - a) * (E4::one() - b); }
-inline E4 base(uint64_t canonical) { return E4::from_base(hf::to_monty(canonical)); }
+inline E4 base(uint64_t canonical) { return E4::from_base(kb::to_monty_c(canonical)); }
 
 std::vector<E4> ext_vec(const uint32_t* p, size_t n) { std::vector<E4> v(n); for (size_t i = 0; i < n; i++) v[i] = ld(p + 4 * i); return v; }
 std::vector<E4> point_from_usize(uint64_t x, unsigned dim) {
@@ -278,7 +279,7 @@ struct Verifier {
 
     uint32_t off(const uint32_t* ptr) const { return (uint32_t)(ptr - ev_base); }
     void observe_ext(const E4& e) { ch.observe_n(e.c, 4); }
-    void observe_var_ext(const uint32_t* w, size_t n) { ch.observe(hf::to_monty(n)); ch.observe_n(w, 4 * n); }
+    void observe_var_ext(const uint32_t* w, size_t n) { ch.observe(kb::to_monty_c(n)); ch.observe_n(w, 4 * n); }
     E4 sample_ext() { E4 e; ch.sample_ext(e.c); return e; }
     std::vector<E4> sample_point(size_t n) { std::vector<E4> v(n); for (auto& x : v) x = sample_ext(); return v; }
 
@@ -333,7 +334,7 @@ struct Verifier {
         observe_var_ext(p.out_den, p.n_out);
         const std::vector<E4> num = ext_vec(p.out_num, expected), den = ext_vec(p.out_den, expected);
         E4 cum;
-        for (size_t i = 0; i < expected; i++) { if (den[i].is_zero()) return SP1B200_VERDICT_ZERO_DENOMINATOR; cum = cum + num[i] * hf::inv(den[i]); }
+        for (size_t i = 0; i < expected; i++) { if (den[i].is_zero()) return SP1B200_VERDICT_ZERO_DENOMINATOR; cum = cum + num[i] * kb::ext_inv(den[i]); }
         if (!cum.is_zero()) return SP1B200_VERDICT_CUMULATIVE_SUM_MISMATCH;
         std::vector<E4> point = sample_point(v + 1);
         E4 num_eval = hf::mle_eval(num, point), den_eval = hf::mle_eval(den, point);
@@ -361,7 +362,7 @@ struct Verifier {
         std::vector<E4> pe{E4()};
         pe.insert(pe.end(), tpt.begin(), tpt.end());
         std::vector<E4> nv, dv;
-        ch.observe(hf::to_monty(nch));
+        ch.observe(kb::to_monty_c(nch));
         for (size_t k = 0; k < nch; k++) {
             const ChipProg& c = m->chips[k];
             if (c.prep_w) observe_var_ext(p.gkr_prep[k], c.prep_w);
@@ -370,7 +371,7 @@ struct Verifier {
             const std::vector<E4> mo = ext_vec(p.gkr_main[k], c.main_w), po = ext_vec(p.gkr_prep[k], c.prep_w);
             for (const InterDev& in : H.per_chip[k]) {
                 auto fraction = [&](const E4* prep, const E4* main, E4& n, E4& d) {
-                    d = alpha + betas[0] * hf::to_monty(in.arg_index);
+                    d = alpha + betas[0] * kb::to_monty_c(in.arg_index);
                     for (uint32_t q = 0; q < in.n_values; q++) d = d + betas[q + 1] * vcol(H.vcols[in.vcol_start + 1 + q], prep, main);
                     n = vcol(H.vcols[in.vcol_start], prep, main);
                 };
@@ -391,8 +392,8 @@ struct Verifier {
     // the chip's constraints folded with the reversed α powers (the verifier folder's Horner order) at one row of extension values;
     // null columns: the all-zero row
     E4 eval_air(size_t k, const E4* prep, const E4* main, const std::vector<E4>& powers) const {
-        return host_eval_constraints<E4>(m->host[k], m->chips[k].n_regs, p.pv, powers,
-                                         [&](const LeafRef& l) { return main ? (l.source == LEAF_MAIN ? main : prep)[l.col] : E4(); });
+        return host_eval_constraints(m->host[k], m->chips[k].n_regs, p.pv, powers,
+                                     [&](const LeafRef& l) { return main ? (l.source == LEAF_MAIN ? main : prep)[l.col] : E4(); });
     }
 
     // ShardVerifier::verify_zerocheck (crates/hypercube/src/verifier/shard.rs:288-434)
@@ -426,7 +427,7 @@ struct Verifier {
             mod = lambda * mod + batched_opening_claim(p.gkr_main[k], m->chips[k].main_w, p.gkr_prep[k], m->chips[k].prep_w, gkr_c);
         if (neq(ld(p.zc.claimed_sum), mod)) return SP1B200_VERDICT_CONSTRAINTS_CLAIMED_SUM;
         if (uint32_t e = sumcheck(p.zc, mlr, 4)) return e;
-        ch.observe(hf::to_monty(nch));
+        ch.observe(kb::to_monty_c(nch));
         for (size_t k = 0; k < nch; k++) { observe_var_ext(p.zc_prep[k], m->chips[k].prep_w); observe_var_ext(p.zc_main[k], m->chips[k].main_w); }
         return SP1B200_VERDICT_ACCEPT;
     }
@@ -537,7 +538,7 @@ struct Verifier {
         for (size_t k = 0; k < claims.size(); k++) claim = claim + claims[k] * coeffs[k];
         const size_t len = ls;
         if (point.size() != len || len == 0) { host_fail = SP1B200_VERDICT_FRI_LENGTH; return; }
-        ch.observe(hf::to_monty(len));
+        ch.observe(kb::to_monty_c(len));
         std::vector<E4> betas;
         for (size_t i = 0; i < len; i++) {
             ch.observe_n(p.univariate + 8 * i, 8);
@@ -572,8 +573,8 @@ struct Verifier {
         fa.nq = nq; fa.len = (uint32_t)len; fa.n_comp = (uint32_t)ncomp;
         for (size_t r = 0; r < ncomp; r++) { fa.comp_off[r] = off(p.component[r].values); fa.comp_w[r] = p.component[r].width; }
         fa.log_n = log_n;
-        fa.g = hf::pow(hf::to_monty(3), (uint64_t)127 << (24 - log_n));
-        fa.minus1 = hf::pow(hf::to_monty(3), (uint64_t)127 << 23);
+        fa.g = kb::pow(kb::to_monty_c(3), (uint64_t)127 << (24 - log_n));
+        fa.minus1 = kb::pow(kb::to_monty_c(3), (uint64_t)127 << 23);
         fa.final_off = off(p.final_poly);
         fold = true;
         // the device checks in verify_mle_evaluations' order: component openings round by round, then per fold round the opened value
@@ -673,7 +674,6 @@ struct Verifier {
 };
 
 // every field word of the proof is a canonical Montgomery word
-bool canonical(const uint32_t* w, size_t n) { for (size_t i = 0; i < n; i++) if (w[i] >= hf::P) return false; return true; }
 bool canonical_sumcheck(const layout::Sumcheck& s) {
     for (size_t i = 0; i < s.polys.size(); i++) if (!canonical(s.polys[i], 4 * (size_t)s.n_coeffs[i])) return false;
     return canonical(s.claimed_sum, 4) && canonical(s.point, 4 * s.polys.size()) && canonical(s.eval, 4);

@@ -8,6 +8,10 @@
 #include <string>
 #include <vector>
 
+// the verifying key's words after the preprocessed commitment (without mprotect): pc_start[3] | initial_global_cumulative_sum x[7] y[7] |
+// enable_untrusted_programs | 6 zeros
+constexpr uint32_t VK_TAIL_WORDS = 24;
+
 // one shard's flat proof words, parsed and checked against the machine, its heights and the context's parameters
 struct VerifyShardIn {
     const uint64_t* heights = nullptr;

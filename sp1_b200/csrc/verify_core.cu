@@ -5,7 +5,7 @@
 #include "ctx.cuh"
 #include "challenger.cuh"
 #include "hostfield.hpp"
-#include "septic.hpp"
+#include "septic.cuh"
 #include "verify.cuh"
 #include <chrono>
 #include <cstdlib>
@@ -36,7 +36,6 @@ constexpr uint32_t PROOF_MAX_NUM_PVS = 187;
 }  // namespace pv
 static_assert(pv::PROOF_NONCE + 4 + 4 == pv::NUM_ELTS, "public values layout");
 
-constexpr uint32_t VK_TAIL_WORDS = 24;   // pc_start[3] | initial_global_cumulative_sum x[7] y[7] | enable_untrusted_programs | 6 zeros
 constexpr uint32_t MAX_LOG_NUMBER_OF_SHARDS = 24;
 constexpr uint64_t DEFAULT_BATCH_WORDS = (uint64_t)1 << 26;
 
@@ -81,7 +80,7 @@ bool zerow(const uint32_t* a, size_t n) { for (size_t i = 0; i < n; i++) if (a[i
 // Field elements compare as Montgomery words, which are equal exactly when the canonical values are.
 uint32_t check_public_values(const std::vector<const uint32_t*>& pvs, const std::vector<uint32_t>& n_pv, const uint32_t* vk_tail, uint32_t* shard) {
     const uint32_t n = (uint32_t)pvs.size();
-    const uint32_t ONE = hf::ONE;
+    const uint32_t ONE = kb::ONE;
     *shard = 0;
     if (n == 0) return SP1B200_VERDICT_EMPTY_PROOF;
     auto fail = [&](uint32_t code, uint32_t s) { *shard = s; return code; };
@@ -166,12 +165,10 @@ uint32_t check_public_values(const std::vector<const uint32_t*>& pvs, const std:
     // the global cumulative sum: vk.initial_global_cumulative_sum + every shard's digest, one SepticDigest addition per shard
     // (verify.rs:498-505), must come back to the zero digest.  Where the reference panics on an incomplete addition with a zero
     // denominator, this rejects the proof with its own verdict.
-    sep::Point sum{sep::E7::load(vk_tail + 3), sep::E7::load(vk_tail + 10)};
-    for (uint32_t s = 0; s < n; s++) {
-        const sep::Point d{sep::E7::load(pvs[s] + pv::GLOBAL_CUMULATIVE_SUM), sep::E7::load(pvs[s] + pv::GLOBAL_CUMULATIVE_SUM + 7)};
-        if (!sep::digest_add(sum, d, sum)) return fail(SP1B200_VERDICT_PV_EXCEPTIONAL_ADDITION, s);
-    }
-    if (!sep::is_zero_digest(sum)) return fail(SP1B200_VERDICT_PV_GLOBAL_CUMULATIVE_SUM, n);
+    s7::Pt sum = s7::load_point(vk_tail + 3);
+    for (uint32_t s = 0; s < n; s++)
+        if (!s7::digest_add(sum, s7::load_point(pvs[s] + pv::GLOBAL_CUMULATIVE_SUM), sum)) return fail(SP1B200_VERDICT_PV_EXCEPTIONAL_ADDITION, s);
+    if (!s7::is_zero_digest(sum)) return fail(SP1B200_VERDICT_PV_GLOBAL_CUMULATIVE_SUM, n);
     return SP1B200_VERDICT_ACCEPT;
 }
 
@@ -201,8 +198,8 @@ sp1b200_err sp1b200_verify_core_proof(sp1b200_ctx* ctx, const sp1b200_machine* m
     if (n_shards && (!h_heights || !chip_names || !h_proofs || !h_n_words)) return sp1b200_set_error("verify_core_proof: NULL argument");
     if (n_vk_tail != VK_TAIL_WORDS)
         return sp1b200_set_error("verify_core_proof: n_vk_tail is %u; the verifying key without mprotect has %u words after the commitment", n_vk_tail, VK_TAIL_WORDS);
-    for (uint32_t i = 0; i < 8; i++) if (h_prep_commit8[i] >= hf::P) return sp1b200_set_error("verify_core_proof: the preprocessed commitment is not canonical");
-    for (uint32_t i = 0; i < n_vk_tail; i++) if (h_vk_tail[i] >= hf::P) return sp1b200_set_error("verify_core_proof: vk_tail word %u is not canonical", i);
+    if (!hf::canonical(h_prep_commit8, 8)) return sp1b200_set_error("verify_core_proof: the preprocessed commitment is not canonical");
+    for (uint32_t i = 0; i < n_vk_tail; i++) if (h_vk_tail[i] >= kb::P) return sp1b200_set_error("verify_core_proof: vk_tail word %u is not canonical", i);
     const auto t0 = std::chrono::steady_clock::now();
     const size_t nch = m->chips.size();
     bool has_prep = false;

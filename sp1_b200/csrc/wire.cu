@@ -41,7 +41,7 @@ struct BinWriter {
     void u8(uint8_t v) { b.push_back(v); }
     void u32(uint32_t v) { for (int i = 0; i < 4; i++) b.push_back((uint8_t)(v >> (8 * i))); }
     void u64(uint64_t v) { for (int i = 0; i < 8; i++) b.push_back((uint8_t)(v >> (8 * i))); }
-    void f(uint32_t monty) { u32(hf::from_monty(monty)); }
+    void f(uint32_t monty) { u32(kb::to_canonical(monty)); }
     void fs(const uint32_t* w, size_t n) { for (size_t i = 0; i < n; i++) f(w[i]); }
     void str(const char* s) { const size_t n = strlen(s); u64(n); b.insert(b.end(), s, s + n); }
     void dims(std::initializer_list<uint64_t> d) { u64(d.size()); for (uint64_t x : d) u64(x); }
@@ -83,7 +83,7 @@ struct BinReader {
     uint8_t u8() { if (!need(1)) return 0; return *p++; }
     uint32_t u32() { if (!need(4)) return 0; uint32_t v = 0; for (int i = 0; i < 4; i++) v |= (uint32_t)p[i] << (8 * i); p += 4; return v; }
     uint64_t u64() { if (!need(8)) return 0; uint64_t v = 0; for (int i = 0; i < 8; i++) v |= (uint64_t)p[i] << (8 * i); p += 8; return v; }
-    uint32_t f() { const uint32_t c = u32(); if (c >= hf::P) { ok = false; why = "field element is not canonical (>= p)"; return 0; } return hf::to_monty(c); }
+    uint32_t f() { const uint32_t c = u32(); if (c >= kb::P) { ok = false; why = "field element is not canonical (>= p)"; return 0; } return kb::to_monty_c(c); }
     void fail(const char* m) { if (ok) { ok = false; why = m; } }
     // a length that is about to be used to read at least `unit` bytes per element
     uint64_t len(size_t unit) { const uint64_t n = u64(); if (ok && unit && n > (uint64_t)(end - p) / unit) fail("length prefix exceeds the input"); return ok ? n : 0; }

@@ -583,7 +583,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         all_ap.insert(all_ap.end(), rev.begin(), rev.end());
         if (rev.empty()) all_ap.push_back(E4());
         // the all-zero row (padded_row_adjustment, shard.rs:520-537)
-        s.pra = host_eval_constraints<uint32_t>(m->host[k], p.n_regs, h_pv, rev, [](const LeafRef&) { return 0u; });
+        s.pra = host_eval_constraints(m->host[k], p.n_regs, h_pv, rev, [](const LeafRef&) { return E4(); });
         s.vg.threshold = (uint32_t)s.h; s.vg.geq_c = E4::one();
         const uint64_t nh = (s.h + 1) / 2;
         const size_t w = p.main_w + p.prep_w;
@@ -731,7 +731,7 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
     std::vector<E4> ys((size_t)nchips * 4);  // per chip: round polynomial values at the nodes 0, 1, 2, 4
     std::vector<uint32_t> hs((size_t)max_jobs * 36);
     std::vector<E4> chip_sums(nchips * 9);
-    const E4 two = E4::from_base(hf::to_monty(2)), four = E4::from_base(hf::to_monty(4)), three = E4::from_base(hf::to_monty(3));
+    const E4 two = E4::from_base(kb::to_monty_c(2)), four = E4::from_base(kb::to_monty_c(4)), three = E4::from_base(kb::to_monty_c(3));
     for (uint32_t rd = 0; rd < mlr; rd++) {
         const RoundPlan& R = plan[rd];
         // every chip's partial sums: one launch per register-file tier, one reduction each, one copy back
@@ -757,11 +757,11 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         // Every chip's round polynomial goes through the same five nodes {0, 1, 2, 4, b} (b depends only on the shared point),
         // and interpolation is linear: combine the chips' node values with the lambda powers first, interpolate ONCE.
         const E4 last = gp[mlr - 1 - rd];
-        const E4 bnode = (E4::one() - last) * hf::inv(E4::one() - (last + last));
+        const E4 bnode = (E4::one() - last) * kb::ext_inv(E4::one() - (last + last));
         const E4 nodes[5] = {E4(), E4::one(), two, four, bnode};
         E4 basis[5][5];
         hf::lagrange_basis<5>(nodes, basis);
-        const E4 f0 = E4::one() - last, f2 = last * hf::to_monty(3) - E4::one(), f4 = last * hf::to_monty(7) - three;
+        const E4 f0 = E4::one() - last, f2 = last * kb::to_monty_c(3) - E4::one(), f4 = last * kb::to_monty_c(7) - three;
         E4 Y[4];  // lambda-combined values at nodes 0, 1, 2, 4 (the value at b is zero by construction)
         for (size_t k = 0; k < nchips; k++) {
             St& s = S[k];
@@ -798,12 +798,11 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
         sc.poly(rlc, 5);
         E4 a; ch.sample_ext(a.c);
         point.insert(point.begin(), a);
-        const Ext da = to_ext(a);
         if (R.fix_jobs) {
             if (rd == 0) {
-                SP1_LAUNCH(ctx, zc_fix_kernel<uint32_t>, R.fix_blocks, 256, 0, d_fjobs + R.fix0, (int)R.fix_jobs, da);
-                if (!bjobs.empty()) SP1_LAUNCH(ctx, zc_batch0_kernel, batch_blocks, 256, 0, d_bjobs, (int)bjobs.size(), d_gw, da);
-            } else SP1_LAUNCH(ctx, zc_fix_kernel<Ext>, R.fix_blocks, 256, 0, d_fjobs + R.fix0, (int)R.fix_jobs, da);
+                SP1_LAUNCH(ctx, zc_fix_kernel<uint32_t>, R.fix_blocks, 256, 0, d_fjobs + R.fix0, (int)R.fix_jobs, a);
+                if (!bjobs.empty()) SP1_LAUNCH(ctx, zc_batch0_kernel, batch_blocks, 256, 0, d_bjobs, (int)bjobs.size(), d_gw, a);
+            } else SP1_LAUNCH(ctx, zc_fix_kernel<Ext>, R.fix_blocks, 256, 0, d_fjobs + R.fix0, (int)R.fix_jobs, a);
         }
         E4 La[4];  // L_i(a) for the four non-zero nodes
         for (int i = 0; i < 4; i++) La[i] = hf::eval_poly<5>(basis[i], a);
@@ -832,13 +831,13 @@ sp1b200_err sp1b200_zerocheck(sp1b200_ctx* ctx, const sp1b200_machine* m, const 
     std::vector<uint32_t> fin((wsum ? wsum : 1) * 4);
     SP1_CUDA(cudaMemcpyAsync(fin.data(), d_final, fin.size() * 4, cudaMemcpyDeviceToHost, st));
     SP1_CUDA(cudaStreamSynchronize(st));
-    ch.observe(hf::to_monty(nchips));
+    ch.observe(kb::to_monty_c(nchips));
     for (size_t k = 0; k < nchips; k++) {
         const ChipProg& p = m->chips[k];
         const uint32_t* mv = &fin[4 * woff[k]];
         const uint32_t* pvv = mv + 4 * (size_t)p.main_w;
-        ch.observe(hf::to_monty(p.prep_w)); ch.observe_n(pvv, (size_t)p.prep_w * 4);
-        ch.observe(hf::to_monty(p.main_w)); ch.observe_n(mv, (size_t)p.main_w * 4);
+        ch.observe(kb::to_monty_c(p.prep_w)); ch.observe_n(pvv, (size_t)p.prep_w * 4);
+        ch.observe(kb::to_monty_c(p.main_w)); ch.observe_n(mv, (size_t)p.main_w * 4);
         proof.put(pvv, (size_t)p.prep_w * 4);
         proof.put(mv, (size_t)p.main_w * 4);
     }

@@ -150,7 +150,7 @@ def _ext_eval(coeffs, x):
 
 
 def test_host_transcript_arithmetic_matches_oracle():
-    """hostfield.hpp (the library's host transcript math): ext product / inverse vs the oracle, and the batched-inversion Lagrange
+    """hostfield.hpp's E4 over kb31.cuh (the library's host transcript math): ext product / inverse vs the oracle, and the batched-inversion Lagrange
     interpolation through 3, 4 and 5 nodes reproduces the node values"""
     rng = np.random.default_rng(8)
     n = 200

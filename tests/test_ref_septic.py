@@ -1,6 +1,6 @@
 """The core-proof verifier's septic arithmetic against the reference's own: kb31_septic_extension_t / bb31_septic_curve_t of
 sp1-gpu/crates/sys/include/fields/kb31_septic_extension_t.cuh, compiled unmodified (oracle/ref_septic.mk) and run on seeded inputs.
-Their outputs are stored in tests/golden/ref_septic.json, so this runs on the CPU: the library's host code (sp1_b200/csrc/septic.hpp,
+Their outputs are stored in tests/golden/ref_septic.json, so this runs on the CPU: the library's code (sp1_b200/csrc/septic.cuh,
 through libsp1b200_hostcheck.so) and the oracle's (oracle/core.hpp) must equal them word for word.  Recording needs a GPU and
 oracle/_ref/libsp1ref_septic.so: `SP1B200_RECORD_REF=1 python -m pytest tests/test_ref_septic.py`."""
 import ctypes as C

@@ -1,4 +1,4 @@
-"""CPU tests of the core-proof verifier's host arithmetic (sp1_b200/csrc/septic.hpp, through libsp1b200_hostcheck.so): the septic
+"""CPU tests of the core-proof verifier's arithmetic (sp1_b200/csrc/septic.cuh, through libsp1b200_hostcheck.so): the septic
 extension F_p[z]/(z^7 - 3z - 5), the curve y^2 = x^3 + 45x + 41z^3 and SepticDigest addition, against the Python restatement in
 tests/septic.py; and the PublicValues word offsets of sp1_b200.lib.PV against the struct's field list."""
 import ctypes as C
