@@ -282,6 +282,57 @@ sp1b200_err sp1b200_program_vk_tail(sp1b200_ctx* ctx, uint64_t pc_start_abs, con
                                     uint64_t n_mem, const uint64_t* page_idx_any, const uint8_t* page_prot_any, uint64_t n_pages,
                                     int enable_untrusted_programs, uint32_t* h_vk_tail24);
 
+/* One instruction of a program (Instruction, crates/core/executor/src/instruction.rs:70-83) laid out for C: opcode = the #[repr(u8)]
+ * discriminant of Opcode (crates/core/executor/src/opcode.rs:45-153, ADD = 0 .. UNIMP = 52), op_a a register index, imm_b / imm_c 0 or 1,
+ * op_b / op_c the operands; 24 bytes, pad ignored. */
+typedef struct sp1b200_instruction {
+    uint8_t opcode;
+    uint8_t op_a;
+    uint8_t imm_b;
+    uint8_t imm_c;
+    uint32_t pad;
+    uint64_t op_b;
+    uint64_t op_c;
+} sp1b200_instruction;
+#define SP1B200_MAX_OPCODE 52u       /* Opcode::UNIMP */
+#define SP1B200_BYTE_PREP_COLS 7u    /* BytePreprocessedCols: b, c, and, or, xor, ltu, msb; 2^16 rows */
+#define SP1B200_PROGRAM_PREP_COLS 16u /* ProgramPreprocessedCols: pc[3], opcode, op_a, op_b[4], op_c[4], op_a_0, imm_b, imm_c */
+#define SP1B200_RANGE_PREP_COLS 2u   /* RangePreprocessedCols: a, bits; 2^17 rows */
+
+/* The preprocessed traces of the core machine's three chips with preprocessed columns, generated on the device from the program's
+ * instructions (n_instrs records, host or device memory; instruction i sits at pc_base + 4 i):
+ *   Byte    (crates/core/machine/src/bytes/mod.rs:31-80)      2^16 rows: row 256 b + c = b, c, b & c, b | c, b ^ c, b < c, b >> 7
+ *   Program (crates/core/machine/src/program/trusted.rs:80-127) next_multiple_of_32(n, None) = max(n rounded up to 32, 16) rows: row i =
+ *           the 16-bit limbs 0..16 / 16..32 / 32..48 of pc_base + 4 i, opcode, op_a, the four 16-bit limbs of op_b and of op_c (low
+ *           first), op_a == 0, imm_b, imm_c; every padding row repeats row 0, pc included
+ *   Range   (crates/core/machine/src/range/mod.rs:18-39)      2^17 rows: row 0 = (0, 0), row 2^bits + a = (a, bits) for bits <= 16
+ * in the dense layout sp1b200_jagged_commit / sp1b200_setup_and_prove_shard / sp1b200_debug_* take: the tables back to back in chip-name
+ * order Byte, Program, Range, each column-major, Montgomery words.  Only Program::preprocessed_shape = None is implemented (a program
+ * with fixed preprocessed heights is not).
+ * h_rows3 / h_cols3 / *h_words (each optional) receive the three shapes and the total word count; out_any = NULL only queries them, and a
+ * cap_words below the total is an error.  out_any is host or device memory.  Errors, each naming the offending instruction's index: an
+ * empty program, an opcode above SP1B200_MAX_OPCODE, imm_b or imm_c other than 0 or 1, a pc of 2^48 or more (trusted.rs:118); and a
+ * Program height above 2^max_log_row_count (the shard prover needs preprocessed heights equal to the main heights and within it).  The
+ * context stays usable after an error. */
+sp1b200_err sp1b200_program_preprocessed_traces(sp1b200_ctx* ctx, uint64_t pc_base, const sp1b200_instruction* instrs_any, uint64_t n_instrs,
+                                                uint32_t* out_any, uint64_t cap_words, uint64_t* h_rows3, uint64_t* h_cols3, uint64_t* h_words);
+
+/* AirProver::setup(program) = setup_from_vk(program, None) (crates/hypercube/src/prover/shard.rs:259-290) for a core program in one call:
+ * the preprocessed traces of sp1b200_program_preprocessed_traces, generated on the device and committed with sp1b200_jagged_commit (no
+ * trace crosses the bus; only the instructions do), the vk tail of sp1b200_program_vk_tail (the memory and page image arguments exactly as
+ * there) and the key digest of sp1b200_vk_hash.  The instructions and the image are checked before anything is committed.
+ * h_prep_rows3 (optional): the three table heights (Byte, Program, Range), the preprocessed heights the shards' main heights must equal;
+ * h_prep_commit8: MachineVerifyingKey::preprocessed_commit; h_vk_tail24: the 24 words after it; h_vk_digest8: hash_koalabear of the key
+ * (sp1b200_digest_bytes32 gives vk.bytes32()); *prep_round_out (optional; NULL frees it): the committed round, the device part of the
+ * proving key, for sp1b200_prove_shard / sp1b200_debug_* (free with sp1b200_jagged_round_free).  Device scratch comes from the context's
+ * pool and is returned before the call ends.  Errors: those of both calls above; the context stays usable after one.
+ * Phases: "program_setup", "program_setup.tables", "program_setup.vk_tail", "program_setup.commit". */
+sp1b200_err sp1b200_program_setup(sp1b200_ctx* ctx, uint64_t pc_base, const sp1b200_instruction* instrs_any, uint64_t n_instrs,
+                                  uint64_t pc_start_abs, const uint64_t* mem_addrs_any, const uint64_t* mem_words_any, uint64_t n_mem,
+                                  const uint64_t* page_idx_any, const uint8_t* page_prot_any, uint64_t n_pages, int enable_untrusted_programs,
+                                  int keep_codeword, uint64_t* h_prep_rows3, uint32_t* h_prep_commit8, uint32_t* h_vk_tail24,
+                                  uint32_t* h_vk_digest8, sp1b200_jagged_round** prep_round_out);
+
 /* ---- shard checks (the reference's cfg(sp1_debug_constraints) build; nothing of the transcript is touched) -------------------------
  * Both take the shard inputs of sp1b200_prove_shard (same validation: prep_round = the round committed at setup or NULL, its heights
  * equal to the main heights, every height <= 2^max_log_row_count; main_dense_any = host pointer, device pointer or upload slot), so a

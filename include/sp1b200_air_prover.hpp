@@ -3,7 +3,8 @@
 // Mirrors the trait the reference selects its shard prover through, `sp1_hypercube::prover::AirProver<GC, SC>`
 // (crates/hypercube/src/prover/shard.rs:45-101): same method names, argument meaning and error behaviour
 //   machine()                       -> the chips (name order) this prover was built for
-//   setup(...)                      -> setup_from_vk plus the verifying key's words computed from the program's memory image
+//   setup(...)                      -> setup_from_vk plus the verifying key's words computed from the program's memory image; given the
+//                                      instruction list, the core machine's preprocessed tables are generated on the device too
 //   setup_from_vk(...)              -> commits the preprocessed traces once per program, returns the proving key
 //                                      (`PreprocessedData<ProvingKey>`) and the preprocessed commitment of the verifying key
 //   setup_and_prove_shard(...)      -> setup, observe the verifying key, prove (the vk-less path of the first shard of a program)
@@ -149,6 +150,39 @@ class AirProver {
         ProvingKey pk = setup_from_vk(prep_dense_any, heights);
         vk.preprocessed_commit = pk.commit;
         return {std::move(pk), std::move(vk)};
+    }
+
+    // AirProver::setup(program) for a core program given by its instructions (Program::instructions, pc_base; host or device memory) and
+    // its image: the Byte, Program and Range preprocessed tables are generated and committed on the device (sp1b200_program_setup), so no
+    // trace crosses the bus.  The machine's chips with preprocessed columns must be exactly Byte (7 columns), Program (16) and Range (2).
+    // Only Program::preprocessed_shape = None is implemented.  Returns the proving key, the verifying key words and the key's digest
+    // (MachineVerifyingKey::hash_koalabear; sp1b200_digest_bytes32 of it is vk.bytes32()).
+    struct ProgramSetup {
+        ProvingKey pk;
+        VerifyingKeyWords vk;
+        Digest vk_digest{};
+    };
+    ProgramSetup setup(uint64_t pc_base, const sp1b200_instruction* instrs_any, uint64_t n_instrs, const ProgramImage& image) {
+        static const std::pair<const char*, uint32_t> prep_chips[3] = {
+            {"Byte", SP1B200_BYTE_PREP_COLS}, {"Program", SP1B200_PROGRAM_PREP_COLS}, {"Range", SP1B200_RANGE_PREP_COLS}};
+        size_t t = 0;
+        for (const Chip& c : chips_)
+            if (c.preprocessed_width) {
+                if (t == 3 || c.name != prep_chips[t].first || c.preprocessed_width != prep_chips[t].second)
+                    throw Error("setup(program): the chips with preprocessed columns must be Byte (7), Program (16) and Range (2)");
+                t++;
+            }
+        if (t != 3) throw Error("setup(program): the chips with preprocessed columns must be Byte (7), Program (16) and Range (2)");
+        ProgramSetup out;
+        out.vk.tail.resize(24);
+        uint64_t rows[3];
+        check(sp1b200_program_setup(ctx_, pc_base, instrs_any, n_instrs, image.pc_start_abs, image.mem_addrs, image.mem_words, image.n_mem,
+                                    image.page_idx, image.page_prot, image.n_pages, image.enable_untrusted_programs ? 1 : 0, 1, rows,
+                                    out.pk.commit.data(), out.vk.tail.data(), out.vk_digest.data(), &out.pk.round_));
+        out.pk.ctx_ = ctx_;
+        for (int k = 0; k < 3; k++) out.pk.heights[prep_chips[k].first] = rows[k];
+        out.vk.preprocessed_commit = out.pk.commit;
+        return out;
     }
 
     // AirProver::preprocessed_table_heights

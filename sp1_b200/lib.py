@@ -35,6 +35,23 @@ VK_TAIL_WORDS = 24   # pc_start[3] | initial_global_cumulative_sum x[7] y[7] | e
 RPV = dict(sp1_vk_digest=(136, 8), vk_root=(144, 8), is_complete=(168, 1), digest=(175, 8), proof_nonce=(183, 4))
 RPV_NUM_TO_HASH = 175
 COMPRESSED, SHRINK = 0, 1
+# sp1b200_instruction (include/sp1b200.h): Instruction (crates/core/executor/src/instruction.rs:70-83) laid out for C, 24 bytes
+INSTRUCTION_DTYPE = np.dtype({"names": ["opcode", "op_a", "imm_b", "imm_c", "pad", "op_b", "op_c"],
+                              "formats": [np.uint8, np.uint8, np.uint8, np.uint8, np.uint32, np.uint64, np.uint64],
+                              "offsets": [0, 1, 2, 3, 4, 8, 16], "itemsize": 24})
+MAX_OPCODE = 52   # Opcode::UNIMP
+# preprocessed widths of the core machine's chips with preprocessed columns, in chip-name order
+PREP_CHIP_COLS = dict(Byte=7, Program=16, Range=2)
+
+
+def pack_instructions(opcode, op_a, op_b, op_c, imm_b, imm_c):
+    """parallel arrays (or scalars) of instruction fields -> a contiguous INSTRUCTION_DTYPE array (the records the library reads)"""
+    names = ("opcode", "op_a", "op_b", "op_c", "imm_b", "imm_c")
+    cols = [np.atleast_1d(np.asarray(x, dtype=INSTRUCTION_DTYPE[name])) for name, x in zip(names, (opcode, op_a, op_b, op_c, imm_b, imm_c))]
+    out = np.zeros(max(c.size for c in cols), INSTRUCTION_DTYPE)
+    for name, c in zip(names, cols):
+        out[name] = c
+    return out
 
 
 class Params(C.Structure):
@@ -86,7 +103,7 @@ ERR_FUNCS = [
     "sp1b200_setup_and_prove_shard", "sp1b200_shard_proof_to_bincode", "sp1b200_shard_proof_from_bincode",
     "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard", "sp1b200_verify_core_proof",
     "sp1b200_vk_hash", "sp1b200_digest_bytes32", "sp1b200_recursion_pv_digest", "sp1b200_recursion_vks_create", "sp1b200_recursion_vks_open",
-    "sp1b200_verify_compressed", "sp1b200_program_vk_tail",
+    "sp1b200_verify_compressed", "sp1b200_program_vk_tail", "sp1b200_program_preprocessed_traces", "sp1b200_program_setup",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
@@ -108,6 +125,25 @@ def _ptr(a):
         assert a.is_contiguous() and a.element_size() == 4
         return C.c_void_p(a.data_ptr())
     raise TypeError(type(a))
+
+
+def _image_args(mem_addrs, mem_words, page_idx, page_prot):
+    """a program's memory image (64-bit addresses and words) and page image (64-bit indices, 8-bit protections) as numpy arrays or torch
+    tensors on the host or the device (torch int64 / uint8), None for an absent page image -> (four pointers, n_mem, n_pages, the numpy
+    arrays the pointers point into: keep them alive for the call)"""
+    ptrs, sizes, keep = [], [], []
+    for x, dtype in ((mem_addrs, np.uint64), (mem_words, np.uint64), (page_idx, np.uint64), (page_prot, np.uint8)):
+        if x is None:
+            ptrs.append(None); sizes.append(0)
+        elif hasattr(x, "data_ptr"):
+            assert x.is_contiguous() and x.element_size() == np.dtype(dtype).itemsize
+            ptrs.append(C.c_void_p(x.data_ptr()) if x.numel() else None); sizes.append(x.numel())
+        else:
+            x = np.ascontiguousarray(x, dtype=dtype)
+            keep.append(x)
+            ptrs.append(C.c_void_p(x.ctypes.data) if x.size else None); sizes.append(x.size)
+    assert sizes[0] == sizes[1] and sizes[2] == sizes[3], "one word per address and one protection per page index"
+    return ptrs, sizes[0], sizes[2], keep
 
 
 class Lib:
@@ -411,24 +447,52 @@ class Lib:
         """MachineProgram::pc_start + initial_global_cumulative_sum + untrusted_config of a program's memory image (and page image) ->
         the 24-word vk_tail (Montgomery words).  Addresses, words and page indices are 64-bit, protections 8-bit: numpy arrays or
         torch tensors on the host or the device (torch int64 / uint8)."""
-        def arr(a, dtype):
-            if a is None:
-                return None, 0
-            if hasattr(a, "data_ptr"):
-                assert a.is_contiguous() and a.element_size() == np.dtype(dtype).itemsize
-                return C.c_void_p(a.data_ptr() if a.numel() else None), a.numel()
-            a = np.ascontiguousarray(a, dtype=dtype)
-            return a, a.size
-        a, n_mem = arr(mem_addrs, np.uint64)
-        w, n_w = arr(mem_words, np.uint64)
-        pi, n_pages = arr(page_idx, np.uint64)
-        pp, n_p = arr(page_prot, np.uint8)
-        assert n_mem == n_w and n_pages == n_p, "one word per address and one protection per page index"
-        p = lambda x: x if x is None or isinstance(x, C.c_void_p) else (C.c_void_p(x.ctypes.data) if x.size else None)
+        (a, w, pi, pp), n_mem, n_pages, _keep = _image_args(mem_addrs, mem_words, page_idx, page_prot)
         out = np.zeros(VK_TAIL_WORDS, np.uint32)
-        self._chk(self.L.sp1b200_program_vk_tail(self.ctx, C.c_uint64(pc_start_abs), p(a), p(w), C.c_uint64(n_mem), p(pi), p(pp),
+        self._chk(self.L.sp1b200_program_vk_tail(self.ctx, C.c_uint64(pc_start_abs), a, w, C.c_uint64(n_mem), pi, pp,
                                                  C.c_uint64(n_pages), C.c_int(enable_untrusted_programs), _ptr(out)))
         return out
+
+    @staticmethod
+    def _instructions(instrs):
+        """INSTRUCTION_DTYPE numpy array, or a contiguous torch uint8 tensor of 24-byte records (host or device) -> (pointer, count, the
+        array the pointer points into: keep it alive for the call)"""
+        if hasattr(instrs, "data_ptr"):
+            assert instrs.is_contiguous() and instrs.element_size() == 1 and instrs.numel() % INSTRUCTION_DTYPE.itemsize == 0
+            return C.c_void_p(instrs.data_ptr() if instrs.numel() else None), instrs.numel() // INSTRUCTION_DTYPE.itemsize, instrs
+        a = np.ascontiguousarray(instrs)
+        assert a.dtype == INSTRUCTION_DTYPE, "pack the instructions with pack_instructions"
+        return (C.c_void_p(a.ctypes.data) if a.size else None), a.size, a
+
+    def program_preprocessed_traces(self, pc_base, instrs, out=None):
+        """the Byte, Program and Range preprocessed tables of a program -> (dense words, shapes [(rows, cols)] x 3).  The words are the
+        tables back to back, each column-major (the layout jagged_commit_dense takes).  out: a device tensor (uint32 / int32) to write
+        into instead of a new host array; it is returned as the words."""
+        p, n, _keep_instrs = self._instructions(instrs)
+        R, Cc, nw = (C.c_uint64 * 3)(), (C.c_uint64 * 3)(), C.c_uint64()
+        self._chk(self.L.sp1b200_program_preprocessed_traces(self.ctx, C.c_uint64(pc_base), p, C.c_uint64(n), None, C.c_uint64(0), R, Cc,
+                                                             C.byref(nw)))
+        if out is None:
+            out = np.zeros(nw.value, np.uint32)
+        cap = out.numel() if hasattr(out, "numel") else out.size
+        self._chk(self.L.sp1b200_program_preprocessed_traces(self.ctx, C.c_uint64(pc_base), p, C.c_uint64(n), _ptr(out), C.c_uint64(cap),
+                                                             R, Cc, C.byref(nw)))
+        return out, [(int(R[t]), int(Cc[t])) for t in range(3)]
+
+    def program_setup(self, pc_base, instrs, pc_start_abs, mem_addrs, mem_words, page_idx=None, page_prot=None, enable_untrusted_programs=0,
+                      keep_codeword=True):
+        """AirProver::setup(program): the preprocessed tables generated and committed on the device plus the verifying key ->
+        dict(prep_rows [3], prep_commit [8], vk_tail [24], vk_digest [8], round = the committed round; free it with jagged_round_free).
+        The image arguments are those of program_vk_tail."""
+        p, n, _keep_instrs = self._instructions(instrs)
+        (a, w, pi, pp), n_mem, n_pages, _keep = _image_args(mem_addrs, mem_words, page_idx, page_prot)
+        rows = (C.c_uint64 * 3)()
+        commit, tail, digest = np.zeros(8, np.uint32), np.zeros(VK_TAIL_WORDS, np.uint32), np.zeros(8, np.uint32)
+        h = C.c_void_p()
+        self._chk(self.L.sp1b200_program_setup(self.ctx, C.c_uint64(pc_base), p, C.c_uint64(n), C.c_uint64(pc_start_abs), a, w,
+                                               C.c_uint64(n_mem), pi, pp, C.c_uint64(n_pages), C.c_int(enable_untrusted_programs),
+                                               C.c_int(int(keep_codeword)), rows, _ptr(commit), _ptr(tail), _ptr(digest), C.byref(h)))
+        return dict(prep_rows=[int(rows[t]) for t in range(3)], prep_commit=commit, vk_tail=tail, vk_digest=digest, round=h)
 
     def pack_row_major(self, rows_any, shapes, d_dense_out):
         """tables back to back, each row-major [rows x cols] -> device buffer with each table column-major"""
