@@ -333,6 +333,57 @@ sp1b200_err sp1b200_program_setup(sp1b200_ctx* ctx, uint64_t pc_base, const sp1b
                                   int keep_codeword, uint64_t* h_prep_rows3, uint32_t* h_prep_commit8, uint32_t* h_vk_tail24,
                                   uint32_t* h_vk_digest8, sp1b200_jagged_round** prep_round_out);
 
+/* ---- lookup-table multiplicities of a shard (the main traces of Byte, Program and Range) -------------------------------------------
+ * One byte lookup (ByteLookupEvent, crates/core/executor/src/events/byte.rs:18-27) with a count: a raw executor event has count 1, an
+ * entry of record.byte_lookups has count = its multiplicity.  opcode = the ByteOpcode discriminant (crates/core/executor/src/opcode.rs:
+ * 163-178): AND 0, OR 1, XOR 2, U8Range 3, LTU 4, MSB 5, Range 6.  12 bytes, pad ignored. */
+typedef struct sp1b200_byte_lookup {
+    uint16_t a;
+    uint8_t b;
+    uint8_t c;
+    uint8_t opcode;
+    uint8_t pad[3];
+    uint32_t count;
+} sp1b200_byte_lookup;
+/* One executed pc with the number of times the shard executed it (a raw instruction event has count 1).  16 bytes, pad ignored. */
+typedef struct sp1b200_pc_count {
+    uint64_t pc;
+    uint32_t count;
+    uint32_t pad;
+} sp1b200_pc_count;
+#define SP1B200_BYTE_OPCODE_RANGE 6u /* ByteOpcode::Range; 0 .. 5 are the Byte chip's opcodes */
+#define SP1B200_BYTE_MULT_COLS 6u    /* ByteMultCols: one multiplicity per opcode 0 .. 5; 2^16 rows */
+#define SP1B200_PROGRAM_MULT_COLS 1u /* ProgramMultiplicityCols; next_multiple_of_32(n_instrs) rows */
+#define SP1B200_RANGE_MULT_COLS 1u   /* RangeMultCols; 2^17 rows */
+
+/* The main (multiplicity) traces of the core machine's Byte, Program and Range chips for one shard, generated on the device from its
+ * byte lookups and executed pcs, the halves that go with the preprocessed tables of sp1b200_program_preprocessed_traces:
+ *   Byte    (bytes/trace.rs:68-92)    [6 x 2^16]: each record with opcode 0 .. 5 adds its count at row 256 b + c, column opcode (a is not
+ *                                     read); Range records are skipped
+ *   Range   (range/trace.rs:98-121)   [1 x 2^17]: each record with opcode 6 adds its count at row a + 2^b
+ *   Program (program/trusted.rs:134-292) [1 x next_multiple_of_32(n_instrs)]: each pc record with pc = pc_base + 4 i, i < n_instrs, adds
+ *           its count at row i; a pc below or above the program or not a multiple of 4 past pc_base is dropped without an error (the
+ *           reference's instruction_counts.get(&pc)); rows n_instrs .. are zero
+ * h_public_values (optional; n_public_values = 187 Montgomery words, the public values sp1b200_prove_shard takes): also add the lookups of
+ * ByteChip / RangeChip::generate_dependencies (bytes/trace.rs:50-66, range/trace.rs:54-96, without the mprotect fields): U8Range of the
+ * two timestamps' middle bytes and of the bytes of both committed-value digests, Range (16 bits) of the timestamps' high limbs, Range (13
+ * bits) of (low limb - 1) / 8 as a u16 subtraction (0 wraps to 0xFFFF / 8, as in the release build), Range (16 bits) of the three limbs
+ * of pc_start, next_pc, previous/last_init_addr and previous/last_finalize_addr.
+ * Counts are summed in 64 bits, so the words do not depend on the order of the records and equal keys may come as one counted record or
+ * as many count-1 records.  Outputs: each table column-major, Montgomery words (the chip's slice of the dense main layout of
+ * sp1b200_prove_shard and sp1b200_debug_*), host or device memory, so a caller can write straight into its dense buffer at the chip's
+ * offset; h_rows3 (optional) receives the heights Byte, Program, Range.  The three outputs NULL only report h_rows3 (after the checks
+ * that need no device work); otherwise all three must be set.  The record arrays are host or device memory.
+ * Errors, naming the offending record or key; the context stays usable after one: an opcode above 6, a Range record with b > 16, NULL
+ * arrays with a non-zero count, more than 2^32 records in an array, n_instrs = 0, pc_base + 4 (n_instrs - 1) >= 2^48, a Program height
+ * above 2^max_log_row_count, n_public_values other than 187, a public value >= p or a limb or byte of it out of range, and a total
+ * multiplicity >= p (F::from_canonical_usize).  Device scratch (64-bit counters, 4 MiB + 8 bytes per Program row) comes from the
+ * context's pool and is returned before the call ends.  Phases: "lookup_traces", "lookup_traces.tables", "lookup_traces.write". */
+sp1b200_err sp1b200_lookup_traces(sp1b200_ctx* ctx, uint64_t pc_base, uint64_t n_instrs, const sp1b200_byte_lookup* lookups_any,
+                                  uint64_t n_lookups, const sp1b200_pc_count* pcs_any, uint64_t n_pcs, const uint32_t* h_public_values,
+                                  uint32_t n_public_values, uint32_t* byte_out_any, uint32_t* program_out_any, uint32_t* range_out_any,
+                                  uint64_t* h_rows3);
+
 /* ---- shard checks (the reference's cfg(sp1_debug_constraints) build; nothing of the transcript is touched) -------------------------
  * Both take the shard inputs of sp1b200_prove_shard (same validation: prep_round = the round committed at setup or NULL, its heights
  * equal to the main heights, every height <= 2^max_log_row_count; main_dense_any = host pointer, device pointer or upload slot), so a

@@ -185,6 +185,37 @@ class AirProver {
         return out;
     }
 
+    // The shard's Byte, Program and Range main traces (ByteChip / RangeChip / ProgramChip::generate_trace_into) generated on the device
+    // from record.byte_lookups and the pcs of the shard's instruction events (sp1b200_lookup_traces), written straight into their slices
+    // of main_dense_any: the dense main buffer of prove_shard_with_pk (device memory, or host memory before an upload), laid out for
+    // `heights` in chip order.  public_values non-empty (the 187 words prove_shard_with_pk takes) adds the lookups of the two chips'
+    // generate_dependencies.  The chips must include Byte (6 main columns), Program (1) and Range (1) at the heights the call reports.
+    void lookup_traces(uint32_t* main_dense_any, const std::vector<uint64_t>& heights, uint64_t pc_base, uint64_t n_instrs,
+                       const sp1b200_byte_lookup* lookups_any, uint64_t n_lookups, const sp1b200_pc_count* pcs_any, uint64_t n_pcs,
+                       const std::vector<uint32_t>& public_values) {
+        if (heights.size() != chips_.size()) throw Error("lookup_traces: one height per chip expected");
+        uint64_t rows[3];
+        check(sp1b200_lookup_traces(ctx_, pc_base, n_instrs, lookups_any, n_lookups, pcs_any, n_pcs, nullptr, 0, nullptr, nullptr, nullptr,
+                                    rows));
+        static const std::pair<const char*, uint32_t> chips[3] = {
+            {"Byte", SP1B200_BYTE_MULT_COLS}, {"Program", SP1B200_PROGRAM_MULT_COLS}, {"Range", SP1B200_RANGE_MULT_COLS}};
+        uint32_t* out[3] = {nullptr, nullptr, nullptr};
+        uint64_t off = 0;
+        for (size_t k = 0; k < chips_.size(); k++) {
+            for (int t = 0; t < 3; t++)
+                if (chips_[k].name == chips[t].first) {
+                    if (chips_[k].main_width != chips[t].second || heights[k] != rows[t])
+                        throw Error((std::string("lookup_traces: chip ") + chips[t].first + " has another main width or height").c_str());
+                    out[t] = main_dense_any + off;
+                }
+            off += heights[k] * chips_[k].main_width;
+        }
+        if (!out[0] || !out[1] || !out[2]) throw Error("lookup_traces: the machine lacks one of Byte, Program and Range");
+        check(sp1b200_lookup_traces(ctx_, pc_base, n_instrs, lookups_any, n_lookups, pcs_any, n_pcs,
+                                    public_values.empty() ? nullptr : public_values.data(), (uint32_t)public_values.size(), out[0], out[1],
+                                    out[2], nullptr));
+    }
+
     // AirProver::preprocessed_table_heights
     static const std::map<std::string, uint64_t>& preprocessed_table_heights(const ProvingKey& pk) { return pk.heights; }
 

@@ -2,6 +2,7 @@
 // Program, Range; generate_preprocessed_trace_into exists only in crates/core/machine/src/{bytes/trace.rs, program/trusted.rs,
 // range/trace.rs}), written on the device straight into the dense layout sp1b200_jagged_commit takes, and the whole verifying key built
 // on top of them.  One thread writes one row; the commitment that follows dominates the call.
+#include "core_tables.hpp"
 #include "ctx.cuh"
 #include "sumcheck.cuh"
 #include <algorithm>
@@ -16,8 +17,9 @@ static_assert(offsetof(sp1b200_instruction, opcode) == 0 && offsetof(sp1b200_ins
 
 namespace {
 
-constexpr uint64_t BYTE_ROWS = 1u << 16;    // bytes/trace.rs:15 NUM_ROWS
-constexpr uint64_t RANGE_ROWS = 1u << 17;   // range/trace.rs:15 NUM_ROWS
+using core_tables::BYTE_ROWS;
+using core_tables::RANGE_ROWS;
+using core_tables::program_height;
 constexpr uint32_t BYTE_COLS = SP1B200_BYTE_PREP_COLS, PROGRAM_COLS = SP1B200_PROGRAM_PREP_COLS, RANGE_COLS = SP1B200_RANGE_PREP_COLS;
 constexpr uint64_t NONE = ~0ull;
 
@@ -71,11 +73,6 @@ __global__ void __launch_bounds__(256) program_table_kernel(const sp1b200_instru
     for (uint32_t k = 0; k < PROGRAM_COLS; k++) d_prog[k * h + r] = mont(v[k]);
 }
 
-// next_multiple_of_32(n, None) (hypercube/src/util.rs:50-59): the Program table's height.  Only Program::preprocessed_shape = None is
-// implemented.  For a later fixed-shape path: trusted.rs:91-92 passes `fixed_log2_rows` to next_multiple_of_32 as its fixed *height*;
-// read Shape::log2_height before assuming whether a height or its log is meant.
-uint64_t program_height(uint64_t n) { return std::max<uint64_t>((n + 31) / 32 * 32, 16); }
-
 struct Shapes {
     uint64_t rows[3], cols[3], words;
 };
@@ -90,18 +87,7 @@ sp1b200_err check_program(sp1b200_ctx* ctx, const char* what, uint64_t pc_base, 
     if (!ctx) return sp1b200_set_error("%s: NULL context", what);
     if (n == 0) return sp1b200_set_error("%s: empty program (no instructions)", what);
     if (!instrs_any) return sp1b200_set_error("%s: NULL instruction list with %llu instructions", what, (unsigned long long)n);
-    const uint32_t mlr = ctx->params.max_log_row_count;
-    if (n > ((uint64_t)1 << 40) || program_height(n) > ((uint64_t)1 << mlr))
-        return sp1b200_set_error("%s: %llu instructions give a Program table of %llu rows > 2^%u (max_log_row_count)", what,
-                                 (unsigned long long)n, (unsigned long long)program_height(n), mlr);
-    // trusted.rs:117-118: pc = pc_base + 4 idx < 2^48 for every instruction
-    const uint64_t lim = (uint64_t)1 << 48;
-    if (pc_base >= lim || 4 * (n - 1) >= lim - pc_base) {
-        const uint64_t i = pc_base >= lim ? 0 : (lim - pc_base + 3) / 4;
-        return sp1b200_set_error("%s: instruction %llu has pc 0x%llx + 4 * %llu >= 2^48", what, (unsigned long long)i,
-                                 (unsigned long long)pc_base, (unsigned long long)i);
-    }
-    return nullptr;
+    return core_tables::check_program_window(ctx, what, pc_base, n);
 }
 
 // writes the three tables back to back (Byte, Program, Range; each column-major) into d_out, then reports the lowest malformed instruction

@@ -42,6 +42,16 @@ INSTRUCTION_DTYPE = np.dtype({"names": ["opcode", "op_a", "imm_b", "imm_c", "pad
 MAX_OPCODE = 52   # Opcode::UNIMP
 # preprocessed widths of the core machine's chips with preprocessed columns, in chip-name order
 PREP_CHIP_COLS = dict(Byte=7, Program=16, Range=2)
+# sp1b200_byte_lookup (include/sp1b200.h): ByteLookupEvent (crates/core/executor/src/events/byte.rs:18-27) with a count, 12 bytes
+BYTE_LOOKUP_DTYPE = np.dtype({"names": ["a", "b", "c", "opcode", "pad", "count"],
+                              "formats": [np.uint16, np.uint8, np.uint8, np.uint8, (np.uint8, 3), np.uint32],
+                              "offsets": [0, 2, 3, 4, 5, 8], "itemsize": 12})
+# sp1b200_pc_count: an executed pc with its count, 16 bytes
+PC_COUNT_DTYPE = np.dtype({"names": ["pc", "count", "pad"], "formats": [np.uint64, np.uint32, np.uint32], "offsets": [0, 8, 12],
+                           "itemsize": 16})
+BYTE_OPCODES = dict(AND=0, OR=1, XOR=2, U8Range=3, LTU=4, MSB=5, Range=6)   # ByteOpcode (crates/core/executor/src/opcode.rs:163-178)
+# main widths of the same chips: one multiplicity per Byte opcode 0..5, one for Program and one for Range
+MAIN_CHIP_COLS = dict(Byte=6, Program=1, Range=1)
 
 
 def pack_instructions(opcode, op_a, op_b, op_c, imm_b, imm_c):
@@ -51,6 +61,24 @@ def pack_instructions(opcode, op_a, op_b, op_c, imm_b, imm_c):
     out = np.zeros(max(c.size for c in cols), INSTRUCTION_DTYPE)
     for name, c in zip(names, cols):
         out[name] = c
+    return out
+
+
+def pack_byte_lookups(opcode, a, b, c, count=1):
+    """parallel arrays (or scalars) of byte lookups -> a contiguous BYTE_LOOKUP_DTYPE array (the records the library reads)"""
+    names = ("opcode", "a", "b", "c", "count")
+    cols = [np.atleast_1d(np.asarray(x, dtype=BYTE_LOOKUP_DTYPE[name])) for name, x in zip(names, (opcode, a, b, c, count))]
+    out = np.zeros(max(x.size for x in cols), BYTE_LOOKUP_DTYPE)
+    for name, x in zip(names, cols):
+        out[name] = x
+    return out
+
+
+def pack_pc_counts(pc, count=1):
+    """parallel arrays (or scalars) of executed pcs and their counts -> a contiguous PC_COUNT_DTYPE array"""
+    cols = [np.atleast_1d(np.asarray(x, dtype=PC_COUNT_DTYPE[name])) for name, x in (("pc", pc), ("count", count))]
+    out = np.zeros(max(x.size for x in cols), PC_COUNT_DTYPE)
+    out["pc"], out["count"] = cols
     return out
 
 
@@ -104,6 +132,7 @@ ERR_FUNCS = [
     "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard", "sp1b200_verify_core_proof",
     "sp1b200_vk_hash", "sp1b200_digest_bytes32", "sp1b200_recursion_pv_digest", "sp1b200_recursion_vks_create", "sp1b200_recursion_vks_open",
     "sp1b200_verify_compressed", "sp1b200_program_vk_tail", "sp1b200_program_preprocessed_traces", "sp1b200_program_setup",
+    "sp1b200_lookup_traces",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
@@ -493,6 +522,37 @@ class Lib:
                                                C.c_uint64(n_mem), pi, pp, C.c_uint64(n_pages), C.c_int(enable_untrusted_programs),
                                                C.c_int(int(keep_codeword)), rows, _ptr(commit), _ptr(tail), _ptr(digest), C.byref(h)))
         return dict(prep_rows=[int(rows[t]) for t in range(3)], prep_commit=commit, vk_tail=tail, vk_digest=digest, round=h)
+
+    @staticmethod
+    def _records(recs, dtype):
+        """a contiguous numpy array of `dtype`, or a contiguous torch uint8 tensor of such records (host or device) -> (pointer, count, the
+        object the pointer points into: keep it alive for the call)"""
+        if recs is None:
+            return None, 0, None
+        if hasattr(recs, "data_ptr"):
+            assert recs.is_contiguous() and recs.element_size() == 1 and recs.numel() % dtype.itemsize == 0
+            return C.c_void_p(recs.data_ptr() if recs.numel() else None), recs.numel() // dtype.itemsize, recs
+        a = np.ascontiguousarray(recs)
+        assert a.dtype == dtype, f"pack the records as {dtype}"
+        return (C.c_void_p(a.ctypes.data) if a.size else None), a.size, a
+
+    def lookup_traces(self, pc_base, n_instrs, lookups, pcs, pv=None, out=None):
+        """the Byte, Program and Range main (multiplicity) traces of a shard from its byte lookups (BYTE_LOOKUP_DTYPE, pack_byte_lookups)
+        and executed pcs (PC_COUNT_DTYPE, pack_pc_counts), numpy arrays or torch uint8 tensors of the records on the host or the device;
+        pv: the shard's 187 public values (Montgomery words) to add the public-value lookups, or None.
+        out: None -> three new host arrays [6, 2^16], [1, h], [1, 2^17]; or three uint32 / int32 buffers (numpy arrays or device
+        tensors, e.g. views at the chips' offsets of a dense main buffer) written in place and returned.  -> (byte, program, range)"""
+        lp, nl, _keep_l = self._records(lookups, BYTE_LOOKUP_DTYPE)
+        pp, npc, _keep_p = self._records(pcs, PC_COUNT_DTYPE)
+        pvw = None if pv is None else np.ascontiguousarray(pv, dtype=np.uint32)
+        rows = (C.c_uint64 * 3)()
+        args = (C.c_uint64(pc_base), C.c_uint64(n_instrs), lp, C.c_uint64(nl), pp, C.c_uint64(npc), _ptr(pvw),
+                C.c_uint32(0 if pvw is None else pvw.size))
+        if out is None:
+            self._chk(self.L.sp1b200_lookup_traces(self.ctx, *args, None, None, None, rows))
+            out = tuple(np.zeros((c, int(rows[t])), np.uint32) for t, c in enumerate(MAIN_CHIP_COLS.values()))
+        self._chk(self.L.sp1b200_lookup_traces(self.ctx, *args, _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), rows))
+        return out
 
     def pack_row_major(self, rows_any, shapes, d_dense_out):
         """tables back to back, each row-major [rows x cols] -> device buffer with each table column-major"""
