@@ -57,14 +57,15 @@ class Asm:
     def assert_zero(self, reg):
         self.asserts.append(reg)
 
-    def words(self, main_w, prep_w):
+    def words(self, main_w, prep_w, alphas=None):
+        """the chip's words of the machine blob; alphas[k] = the reversed-powers index of assert k (default: k)"""
         n = len(self.asserts)
         w = [main_w, prep_w, n, self.nreg, len(self.instrs), len(self.leaves), len(self.consts), len(self.publics), n]
         for opc, out, a, b in self.instrs:
             w += [opc | (out << 16), a | (b << 16)]
         for src, col in self.leaves:
             w += [src, col]
-        w += self.consts + self.publics + self.asserts + list(range(n))  # constraint i <-> reversed-powers index i
+        w += self.consts + self.publics + self.asserts + (list(range(n)) if alphas is None else list(alphas))
         return w
 
 

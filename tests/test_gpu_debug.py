@@ -74,6 +74,59 @@ def test_constraint_report_register_tiers(spec, mlr):
     lib.close()
 
 
+def test_constraint_report_random_programs():
+    """random constraint programs (tests/machines.py random_program) in every register-file tier, a chip without constraints and a
+    chip of more than 2^16 main columns: clean -> nothing; one witness cell nudged -> exactly that chip, that row and that constraint's
+    alpha index (twice-asserted registers: both); the zero column of a direct leaf assert nudged -> that assert alone; the constant 0 of
+    a direct constant assert made 1 -> that assert on every row; the zero public value, which every program loads and one assert
+    reads directly, changed -> every row of every constrained chip, with that assert"""
+    spec = [M.prog_chip(300, 81, dup=True), M.prog_chip(77, 82, live=10, prep=2), M.prog_chip(64, 83, live=24, n_asserts=16, n_ops=150),
+            M.prog_chip(40, 84, n_asserts=0), M.prog_chip(129, 85, live=80, dup=True), M.prog_chip(50, 86, live=300, n_asserts=10),
+            M.prog_chip(3, 87, wide=65600, n_asserts=6, n_ops=20), M.prog_chip(0, 88)]
+    rng = np.random.default_rng(1750)
+    blob, heights, mains, preps, pv, _ = M.spec_machine(rng, spec, interactions=False)
+    lib = _lib(9)
+    mach = lib.machine_create(blob)
+    assert {M.zc_tier(lib.machine_chip_regs(mach, k)) for k in range(len(spec))} == set(range(5))
+    pr = GP.commit_prep(lib, preps)[1]
+    assert _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False) == {}
+    for k in (0, 2, 4, 5, 6):
+        rp = M.random_program(spec[k].program)
+        row = int(rng.integers(0, heights[k]))
+        w = min(rp.witness, key=lambda x: (x is None, -rp.witness.count(x), rng.random()))   # a twice-asserted one first
+        mains[k][w, row] = (int(mains[k][w, row]) + 1) % P
+        rep = _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False)
+        alphas = sorted(a for (_, a), w2 in zip(rp.asserts, rp.witness) if w2 == w)
+        assert list(rep) == [k] and rep[k]["n_failing_rows"] == 1 and rep[k]["rows"] == {row: alphas}, (k, w, row, rep)
+        mains[k][w, row] = (int(mains[k][w, row]) - 1) % P
+    # the three direct asserts (leaf, constant 0, zero public value).  On a clean trace each is the zero polynomial, so the zerocheck
+    # cannot see whether the lowering kept them; the report can.  The zero column nudged: the leaf assert alone fails
+    rp = M.random_program(spec[0].program)
+    leaf_alpha, const_alpha, pub_alpha = [a for (_, a), w in zip(rp.asserts, rp.witness) if w is None]
+    mains[0][rp.zero_col, 5] = 1
+    rep = _check(lib, mach, pr, blob, heights, mains, preps, pv, inter=False)
+    assert list(rep) == [0] and rep[0]["rows"] == {5: [leaf_alpha]}, rep
+    mains[0][rp.zero_col, 5] = 0
+    # the constant 0 made 1 in chip 0's constant table (a blob edit): the constant assert fails on every row, next to the constraints
+    # that read the constant elsewhere
+    blob2 = blob.copy()
+    blob2[1 + 9 + 2 * len(rp.instrs) + 2 * len(rp.leaves)] = O.to_monty(np.array([1]))[0]
+    mach2 = lib.machine_create(blob2)
+    rep = _check(lib, mach2, pr, blob2, heights, mains, preps, pv, inter=False)
+    lib.machine_free(mach2)
+    assert list(rep) == [0] and rep[0]["n_failing_rows"] == heights[0] and all(const_alpha in c for c in rep[0]["rows"].values()), rep
+    # the zero public value changed, which every program loads: every row of every constrained chip fails, chip 0's public assert too
+    pv2 = pv.copy(); pv2[4] = (int(pv2[4]) + 1) % P
+    rep = _check(lib, mach, pr, blob, heights, mains, preps, pv2, max_rows=4, inter=False)
+    failing = {k for k, s in enumerate(spec) if heights[k] and s.program.n_asserts}
+    assert set(rep) == failing and all(rep[k]["n_failing_rows"] == heights[k] for k in failing), rep
+    assert all(pub_alpha in c for c in rep[0]["rows"].values()), rep
+    if pr is not None:
+        lib.jagged_round_free(pr)
+    lib.machine_free(mach)
+    lib.close()
+
+
 CALIBRATED = [M.Chip(700, 4, True, 36, 5, 3), M.Chip(96, 14, False, 120, 0, 0, [12, 4, 9, 5]), M.Chip(0, 2, True, 18, 1, 2),
               M.Chip(33, 1, True, 9, 7, 35), M.Chip(2048, 40, False, 360, 2, 0, [9] * 6)]
 

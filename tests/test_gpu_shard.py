@@ -43,7 +43,7 @@ def _run(spec, log_stack, mlr, seed, nq=8, pow_bits=4, batch_bits=2, gkr_bits=3)
     lib.close()
 
 
-@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS + [M.RANDOM_SHARD_SPEC])
 def test_prove_shard_matches_oracle(spec, log_stack, mlr):
     _run(spec, log_stack, mlr, seed=1200 + mlr)
 

@@ -80,11 +80,13 @@ def _agree(c, capfd, words, heights=None, start=None, pc="same", what=""):
     return reason
 
 
-@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS + [M.RANDOM_SHARD_SPEC])
 def test_accepts_small_machines(spec, log_stack, mlr):
-    """max_log_row_count 3 and 7, machines with and without preprocessed columns, absent chips"""
+    """max_log_row_count 3 and 7, machines with and without preprocessed columns, absent chips, random constraint programs (whose
+    constraints the verifier evaluates at the opened point with its own interpreter of the bytecode)"""
     c = _prove(_spec_inp(spec, 2100 + mlr), log_stack, mlr, 2101)
     _accept(c)
+    assert _oracle(c, c["words"]) == 0, "the oracle's verifier rejects the library's proof"
     _close(c)
 
 

@@ -3,7 +3,8 @@
 import numpy as np
 import pytest
 
-from tests.machines import Chip, oracle_zerocheck, product_zerocheck, spec_machine, workload_machine
+from tests.machines import (PROGRAM_ZC_CASES, Chip, lowered_shape, oracle_zerocheck, product_zerocheck, random_program, spec_machine,
+                            workload_machine, zc_tier)
 
 pytestmark = pytest.mark.gpu
 
@@ -23,7 +24,7 @@ pytestmark = pytest.mark.gpu
     # heights on both sides of the "pieces" threshold (<= 16 blocks of 128 row pairs)
     ([Chip(192, 250, False, deep=True), Chip(64, 500, True, deep=True), (8192, 3, True), Chip(96, 1000, False, deep=True),
       Chip(6000, 300, False, deep=True)], 13),
-])
+] + PROGRAM_ZC_CASES)   # and random constraint programs (tests/machines.py random_program)
 def test_zerocheck_matches_oracle(spec, mlr):
     from sp1_b200 import Lib
     rng = np.random.default_rng(900 + mlr)
@@ -33,6 +34,11 @@ def test_zerocheck_matches_oracle(spec, mlr):
     if any(Chip(*s_).deep and s_[1] >= 250 for s_ in spec):
         regs = [lib.machine_chip_regs(mach, k) for k in range(len(spec))]
         assert max(regs) > 900 and sorted(regs)[-2] > 450 and min(regs) <= 32, regs   # the tiers the case is meant to exercise
+    for k, c in enumerate(Chip(*s_) for s_ in spec):
+        if c.program is not None and c.program.n_asserts:
+            # the tier and the path each random chip is meant to exercise: the live set + a few registers; a 150-op body takes pieces
+            assert zc_tier(lib.machine_chip_regs(mach, k)) == zc_tier(c.program.live + 4), (k, lib.machine_chip_regs(mach, k))
+            assert c.program.n_ops < 150 or lowered_shape(random_program(c.program).words)[2], k
     _check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr)
     lib.machine_free(mach)
     lib.close()

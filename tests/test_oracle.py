@@ -242,7 +242,7 @@ def test_jagged_pcs_roundtrip(shapes_rounds, log_stack, max_log_rows):
     ([(5, 1, False), (0, 2, False), (6, 1, True)], 3),     # odd height, empty chip, preprocessed column
     ([(1, 1, False), (2, 1, True)], 4),                    # one real row
     ([(32, 3, True), (96, 2, False), (128, 1, False)], 7),
-])
+] + M.PROGRAM_ZC_CASES)
 def test_zerocheck_roundtrip(spec, mlr):
     """zerocheck over synthetic satisfiable AIRs (reference GPU bytecode format) -> restated verify_zerocheck accepts"""
     rng = np.random.default_rng(41)
@@ -285,7 +285,7 @@ def test_logup_gkr_roundtrip(spec, mlr):
     assert words.size > 50 and (words == words2).all() and (c1.st == c2.st).all()
 
 
-@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS)
+@pytest.mark.parametrize("spec,log_stack,mlr", M.SHARD_SPECS + [M.RANDOM_SHARD_SPEC])
 def test_whole_shard_roundtrip(spec, log_stack, mlr):
     """commit -> LogUp-GKR -> zerocheck -> jagged/stacked/BaseFold open in one transcript; restated verify_shard accepts"""
     blob, heights, mains, preps, pv, names, ch = M.shard_inputs(spec, 61)

@@ -26,7 +26,8 @@ import pytest
 from sp1_b200 import synth_air as SA
 from tests import oracle_lib as O
 from tests.ext_field import EF, ONE, ZERO, efs, eval_at, interpolate, parse_partial_sumcheck
-from tests.machines import Chip, chip_segments, oracle_zerocheck, product_zerocheck, spec_machine, workload_machine
+from tests.machines import (PROG_PV, Chip, chip_segments, lowered_shape, oracle_zerocheck, prog_chip, product_zerocheck, spec_machine,
+                            workload_machine)
 from tests.ref_golden import Ref, Store
 
 STORE = Store("ref_zerocheck", "tests/test_ref_zerocheck.py")
@@ -216,6 +217,14 @@ CASES = [
     # an empty chip between chips
     ("empty_between", "synth", [(16, 1, False, "flat"), (0, 2, True, "flat"), (8, 1, False, "vanishing"), (0, 1, False, "flat"),
                                 (12, 1, True, "flat")], 4),
+    # random constraint programs (tests/machines.py random_program): permuted alpha indices, every public value and constant loaded,
+    # asserts on a leaf, the constant 0 and a public value, a register asserted twice, a program split into pieces, an empty chip
+    ("random_permuted", "random", [prog_chip(64, 4101, dup=True), prog_chip(12, 4102, live=10, prep=2),
+                                   prog_chip(36, 4103, n_asserts=16, n_ops=150), prog_chip(0, 4104)], 7),
+    # random programs with long-lived products: a live set of ~300 registers (the reference's MAX_REGS 512 tier) next to ~30 and ~80
+    ("random_live", "random", [prog_chip(96, 4111, live=300, n_asserts=10), prog_chip(4, 4112, live=24), prog_chip(128, 4113, live=80, dup=True)], 8),
+    # random programs at the smallest max_log_row_count the reference takes, every chip of full height
+    ("random_mlr2", "random", [prog_chip(4, 4121), prog_chip(4, 4122, dup=True, prep=0)], 2),
 ]
 IDS = [c[0] for c in CASES]
 
@@ -226,7 +235,7 @@ def _machine(name):
     seed = 4000 + IDS.index(name)
     if kind == "synth":
         blob, heights, mains, preps, pv = _synth(np.random.default_rng(seed), spec)
-    elif kind == "spec":
+    elif kind in ("spec", "random"):
         blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(seed), spec)
     else:
         blob, heights, mains, preps, pv, _ = workload_machine(kind, seed, max_log_rows=mlr, scale=0.25)
@@ -287,6 +296,19 @@ def _check_case_shape(name, raw):
         assert max(c["prep_w"] for c in chips) == 36 and any(h % 32 for h in heights if h)
     elif name == "empty_between":
         assert 0 in heights[1:-1]
+    elif name == "random_permuted":
+        assert any((c["assert_alphas"] != np.arange(c["assert_alphas"].size)).any() for c in chips), "needs permuted alpha indices"
+        ops = [(c["instrs"].reshape(-1, 2) & 0xffff, c) for c in chips]
+        assert {int(x) for o, _ in ops for x in o[:, 0]} == set(range(7)), "needs every opcode"
+        loaded = {int(c["publics"][a]) for o, c in ops for a in o[o[:, 0] == SA.LOAD_PUBLIC, 1]}
+        assert loaded == set(range(len(PROG_PV))), "needs every public value loaded"
+        assert any(len(set(c["assert_regs"].tolist())) < c["assert_regs"].size for c in chips), "needs a register asserted twice"
+        assert any(lowered_shape(seg[2])[2] for seg in chip_segments(_machine(name)[0])), "needs a program split into pieces"
+        assert 0 in heights
+    elif name == "random_live":
+        assert 256 < max(regs) <= 512 and min(regs) > 16, regs
+    elif name == "random_mlr2":
+        assert mlr == 2 and heights == [4] * len(chips)
 
 
 def _check(name, words, who):
