@@ -384,6 +384,72 @@ sp1b200_err sp1b200_lookup_traces(sp1b200_ctx* ctx, uint64_t pc_base, uint64_t n
                                   uint32_t n_public_values, uint32_t* byte_out_any, uint32_t* program_out_any, uint32_t* range_out_any,
                                   uint64_t* h_rows3);
 
+/* ---- memory chips of a shard (MemoryGlobalInit, MemoryGlobalFinalize, MemoryLocal) ---------------------------------------------------
+ * MemoryInitializeFinalizeEvent (crates/core/executor/src/events/memory.rs:169-176), 24 bytes. */
+typedef struct sp1b200_memory_event {
+    uint64_t addr;
+    uint64_t value;
+    uint64_t timestamp;
+} sp1b200_memory_event;
+/* MemoryLocalEvent (memory.rs:307-314) with its two MemoryRecords (timestamp, value) inlined, 40 bytes. */
+typedef struct sp1b200_memory_local_event {
+    uint64_t addr;
+    uint64_t initial_timestamp;
+    uint64_t initial_value;
+    uint64_t final_timestamp;
+    uint64_t final_value;
+} sp1b200_memory_local_event;
+/* GlobalInteractionEvent (crates/core/executor/src/events/global.rs): is_receive 0 or 1, kind = InteractionKind discriminant (Memory = 1).
+ * 36 bytes, pad written as zero. */
+typedef struct sp1b200_global_event {
+    uint32_t message[8];
+    uint8_t is_receive;
+    uint8_t kind;
+    uint8_t pad[2];
+} sp1b200_global_event;
+#define SP1B200_MEMORY_GLOBAL_COLS 30u    /* MemoryInitCols (memory/global.rs:254-304) */
+#define SP1B200_MEMORY_LOCAL_COLS 20u     /* MemoryLocalCols (memory/local.rs:27-71), one entry per row */
+#define SP1B200_MEMORY_GLOBAL_LOOKUPS 12u /* byte lookup records per init / finalize event */
+#define SP1B200_MEMORY_LOCAL_LOOKUPS 10u  /* byte lookup records per local event */
+
+/* The main traces of the MemoryGlobalInit, MemoryGlobalFinalize and MemoryLocal chips of one shard, generated on the device with the byte
+ * lookups and global interaction events of their generate_dependencies, so that neither the traces nor the dependencies are built on the
+ * host.
+ * Inputs (host or device memory): record.global_memory_initialize_events (n_init), record.global_memory_finalize_events (n_finalize), in
+ * any order, the shard's public values previous_init_addr / previous_finalize_addr, and record.get_local_mem_events() (n_local; precompile
+ * events, then cpu events, the order the rows take).
+ *   MemoryGlobalInit / Finalize (memory/global.rs:155-236): the events sorted by address, one row per event, column order of
+ *     MemoryInitCols with LtOperationUnsigned / U16CompareOperation / IsZeroOperation inlined in field order: clk_high, clk_low, index,
+ *     prev_addr[3], addr[3], lt_cols (bit, u16_flags[4], not_eq_inv, comparison_limbs[2]), value[4], value_lower, value_upper, is_real,
+ *     is_comp, prev_valid, is_prev_addr_zero (inverse, result), is_index_zero (inverse, result).  prev_addr of row 0 is previous_*_addr.
+ *     Height next_multiple_of_32(n) (0 without events: the chip is not included); padding rows are zero.
+ *   MemoryLocal (memory/local.rs:166-238): one row per event in input order: addr[3], initial_clk_high, final_clk_high, initial_clk_low,
+ *     final_clk_low, initial_value[4], final_value[4], initial_value_lower / upper, final_value_lower / upper, is_real; same heights.
+ * Outputs: init_out_any, finalize_out_any, local_out_any: each chip's slice of the dense main layout (column-major Montgomery words),
+ * host or device memory; h_rows3 (optional) receives the heights init, finalize, local.
+ * lookups_out_any (sp1b200_byte_lookup records, count 1 or 0): the lookups of generate_dependencies at a fixed count, *h_n_lookups = 12 n_init
+ * + 12 n_finalize + 10 n_local, in sections init, finalize, local, each in row order.  An init / finalize row gives 4 Range(16) checks of
+ * the value's limbs, 3 of prev_addr's, 3 of addr's, U8Range(value byte 4, byte 5) and the U16CompareOperation's Range(16) check of
+ * (prev limb - addr limb) mod 2^16 at the first differing limb from the top (count 0 on a row that makes no comparison: row 0 with
+ * previous address 0); a local row U8Range and 4 Range(16) checks of the initial value, then the same of the final value.  Give them to
+ * sp1b200_lookup_traces with the shard's other lookups.
+ * globals_out_any: the GlobalInteractionEvents of generate_dependencies, *h_n_globals = n_init + n_finalize + 2 n_local, in sections init
+ * (sorted order; sends with clk 0, 0), finalize (sorted order; receives with the event's clk), local (per event the initial access, a
+ * receive, then the final access, a send).  Messages: clk_high, clk_low, addr limbs [3], value limb 0 + 2^16 byte 4, limb 1 + 2^16 byte 5,
+ * limb 3.  A caller places each section where its machine's dependency order puts that chip's events.
+ * All five outputs NULL only report the sizes; otherwise an output may be NULL only where its size is 0.
+ * Errors, naming the offending event; the context stays usable after one: NULL arrays with a non-zero count, 2^31 or more events in an
+ * array, an address of 2^48 or more (also a previous address), a timestamp of 2^48 or more (clk_high = timestamp >> 24 must fit 24 bits),
+ * and init or finalize addresses that are not strictly increasing after the sort (a duplicate, or an address at or below a non-zero
+ * previous address), which the chip's prev_addr < addr constraint rejects.  Device scratch comes from the context's pool and is
+ * returned before the call ends.  Phases: "memory_traces", "memory_traces.sort", "memory_traces.rows". */
+sp1b200_err sp1b200_memory_traces(sp1b200_ctx* ctx, const sp1b200_memory_event* init_any, uint64_t n_init,
+                                  const sp1b200_memory_event* finalize_any, uint64_t n_finalize, uint64_t previous_init_addr,
+                                  uint64_t previous_finalize_addr, const sp1b200_memory_local_event* local_any, uint64_t n_local,
+                                  uint32_t* init_out_any, uint32_t* finalize_out_any, uint32_t* local_out_any,
+                                  sp1b200_byte_lookup* lookups_out_any, sp1b200_global_event* globals_out_any, uint64_t* h_rows3,
+                                  uint64_t* h_n_lookups, uint64_t* h_n_globals);
+
 /* ---- shard checks (the reference's cfg(sp1_debug_constraints) build; nothing of the transcript is touched) -------------------------
  * Both take the shard inputs of sp1b200_prove_shard (same validation: prep_round = the round committed at setup or NULL, its heights
  * equal to the main heights, every height <= 2^max_log_row_count; main_dense_any = host pointer, device pointer or upload slot), so a

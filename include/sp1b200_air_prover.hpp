@@ -216,6 +216,44 @@ class AirProver {
                                     out[2], nullptr));
     }
 
+    // The shard's MemoryGlobalInit, MemoryGlobalFinalize and MemoryLocal main traces (MemoryGlobalChip / MemoryLocalChip::
+    // generate_trace_into) generated on the device from record.global_memory_initialize_events / _finalize_events and
+    // get_local_mem_events() (sp1b200_memory_traces), written straight into their slices of main_dense_any (laid out for `heights` in chip
+    // order, as for lookup_traces).  previous_*_addr: the shard's public values of those names.  The chips' generate_dependencies go to
+    // lookups_out_any (12 records per init / finalize event + 10 per local event: pass them to lookup_traces with the shard's other
+    // lookups) and globals_out_any (one record per init / finalize event + 2 per local event, in sections init, finalize, local); both host
+    // or device memory.  A chip the machine lacks must have no events; one it has must be at the height the call reports (0 without
+    // events).  Returns {lookup records, global records} written.
+    std::pair<uint64_t, uint64_t> memory_traces(uint32_t* main_dense_any, const std::vector<uint64_t>& heights,
+                                                const sp1b200_memory_event* init_any, uint64_t n_init, const sp1b200_memory_event* finalize_any,
+                                                uint64_t n_finalize, uint64_t previous_init_addr, uint64_t previous_finalize_addr,
+                                                const sp1b200_memory_local_event* local_any, uint64_t n_local,
+                                                sp1b200_byte_lookup* lookups_out_any, sp1b200_global_event* globals_out_any) {
+        if (heights.size() != chips_.size()) throw Error("memory_traces: one height per chip expected");
+        uint64_t rows[3], n_lookups = 0, n_globals = 0;
+        check(sp1b200_memory_traces(ctx_, init_any, n_init, finalize_any, n_finalize, previous_init_addr, previous_finalize_addr, local_any,
+                                    n_local, nullptr, nullptr, nullptr, nullptr, nullptr, rows, &n_lookups, &n_globals));
+        static const std::pair<const char*, uint32_t> chips[3] = {{"MemoryGlobalInit", SP1B200_MEMORY_GLOBAL_COLS},
+                                                                  {"MemoryGlobalFinalize", SP1B200_MEMORY_GLOBAL_COLS},
+                                                                  {"MemoryLocal", SP1B200_MEMORY_LOCAL_COLS}};
+        uint32_t* out[3] = {nullptr, nullptr, nullptr};
+        uint64_t off = 0;
+        for (size_t k = 0; k < chips_.size(); k++) {
+            for (int t = 0; t < 3; t++)
+                if (chips_[k].name == chips[t].first) {
+                    if (chips_[k].main_width != chips[t].second || heights[k] != rows[t])
+                        throw Error((std::string("memory_traces: chip ") + chips[t].first + " has another main width or height").c_str());
+                    out[t] = main_dense_any + off;
+                }
+            off += heights[k] * chips_[k].main_width;
+        }
+        for (int t = 0; t < 3; t++)
+            if (rows[t] && !out[t]) throw Error((std::string("memory_traces: the machine lacks ") + chips[t].first + ", which has events").c_str());
+        check(sp1b200_memory_traces(ctx_, init_any, n_init, finalize_any, n_finalize, previous_init_addr, previous_finalize_addr, local_any,
+                                    n_local, out[0], out[1], out[2], lookups_out_any, globals_out_any, nullptr, nullptr, nullptr));
+        return {n_lookups, n_globals};
+    }
+
     // AirProver::preprocessed_table_heights
     static const std::map<std::string, uint64_t>& preprocessed_table_heights(const ProvingKey& pk) { return pk.heights; }
 

@@ -3,9 +3,9 @@
 // One thread lifts one image entry onto the septic curve (septic.cuh), a tree of per-thread chunk sums adds the points under the
 // complete law, and a radix sort of the keys finds duplicate addresses and page indices.
 #include "ctx.cuh"
+#include "radix_sort.cuh"
 #include "septic.cuh"
 #include "sumcheck.cuh"
-#include <cub/device/device_radix_sort.cuh>
 
 namespace {
 
@@ -54,12 +54,7 @@ sp1b200_err find_duplicate(sp1b200_ctx* ctx, DevFree& mem, const uint64_t* d_key
     if (n < 2) return nullptr;
     uint64_t* d_sorted;
     SP1_TRY(mem.alloc((void**)&d_sorted, n * 8));
-    size_t tb = 0;
-    void* d_tmp = nullptr;
-    SP1_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_keys, d_sorted, (int)n, 0, 64, ctx->stream));
-    SP1_TRY(mem.alloc(&d_tmp, tb));
-    SP1_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp, tb, d_keys, d_sorted, (int)n, 0, 64, ctx->stream));
-    ctx->launches++;
+    SP1_TRY(radix_sort::keys(ctx, mem, d_keys, d_sorted, n, 64));
     SP1_LAUNCH(ctx, setup_dup_kernel, blocks_for(n), 256, 0, d_sorted, n, d_dup);
     return nullptr;
 }

@@ -52,6 +52,17 @@ PC_COUNT_DTYPE = np.dtype({"names": ["pc", "count", "pad"], "formats": [np.uint6
 BYTE_OPCODES = dict(AND=0, OR=1, XOR=2, U8Range=3, LTU=4, MSB=5, Range=6)   # ByteOpcode (crates/core/executor/src/opcode.rs:163-178)
 # main widths of the same chips: one multiplicity per Byte opcode 0..5, one for Program and one for Range
 MAIN_CHIP_COLS = dict(Byte=6, Program=1, Range=1)
+# sp1b200_memory_event: MemoryInitializeFinalizeEvent (crates/core/executor/src/events/memory.rs:169-176), 24 bytes
+MEMORY_EVENT_DTYPE = np.dtype({"names": ["addr", "value", "timestamp"], "formats": [np.uint64] * 3, "offsets": [0, 8, 16], "itemsize": 24})
+# sp1b200_memory_local_event: MemoryLocalEvent (memory.rs:307-314) with its two MemoryRecords inlined, 40 bytes
+MEMORY_LOCAL_EVENT_DTYPE = np.dtype({"names": ["addr", "initial_timestamp", "initial_value", "final_timestamp", "final_value"],
+                                     "formats": [np.uint64] * 5, "offsets": [0, 8, 16, 24, 32], "itemsize": 40})
+# sp1b200_global_event: GlobalInteractionEvent (crates/core/executor/src/events/global.rs), 36 bytes
+GLOBAL_EVENT_DTYPE = np.dtype({"names": ["message", "is_receive", "kind", "pad"], "formats": [(np.uint32, 8), np.uint8, np.uint8, (np.uint8, 2)],
+                               "offsets": [0, 32, 33, 34], "itemsize": 36})
+# main widths of the memory chips, and the byte lookup records sp1b200_memory_traces emits per event
+MEMORY_CHIP_COLS = dict(MemoryGlobalInit=30, MemoryGlobalFinalize=30, MemoryLocal=20)
+MEMORY_GLOBAL_LOOKUPS, MEMORY_LOCAL_LOOKUPS = 12, 10
 
 
 def pack_instructions(opcode, op_a, op_b, op_c, imm_b, imm_c):
@@ -79,6 +90,24 @@ def pack_pc_counts(pc, count=1):
     cols = [np.atleast_1d(np.asarray(x, dtype=PC_COUNT_DTYPE[name])) for name, x in (("pc", pc), ("count", count))]
     out = np.zeros(max(x.size for x in cols), PC_COUNT_DTYPE)
     out["pc"], out["count"] = cols
+    return out
+
+
+def pack_memory_events(addr, value, timestamp):
+    """parallel arrays (or scalars) of init / finalize events -> a contiguous MEMORY_EVENT_DTYPE array"""
+    cols = [x.reshape(-1) for x in np.broadcast_arrays(*[np.asarray(x, dtype=np.uint64) for x in (addr, value, timestamp)])]
+    out = np.zeros(cols[0].size, MEMORY_EVENT_DTYPE)
+    out["addr"], out["value"], out["timestamp"] = cols
+    return out
+
+
+def pack_memory_local_events(addr, initial_timestamp, initial_value, final_timestamp, final_value):
+    """parallel arrays (or scalars) of local memory events -> a contiguous MEMORY_LOCAL_EVENT_DTYPE array"""
+    fields = (addr, initial_timestamp, initial_value, final_timestamp, final_value)
+    cols = [x.reshape(-1) for x in np.broadcast_arrays(*[np.asarray(x, dtype=np.uint64) for x in fields])]
+    out = np.zeros(cols[0].size, MEMORY_LOCAL_EVENT_DTYPE)
+    for name, x in zip(MEMORY_LOCAL_EVENT_DTYPE.names, cols):
+        out[name] = x
     return out
 
 
@@ -132,7 +161,7 @@ ERR_FUNCS = [
     "sp1b200_debug_constraints", "sp1b200_debug_interactions", "sp1b200_verify_shard", "sp1b200_verify_core_proof",
     "sp1b200_vk_hash", "sp1b200_digest_bytes32", "sp1b200_recursion_pv_digest", "sp1b200_recursion_vks_create", "sp1b200_recursion_vks_open",
     "sp1b200_verify_compressed", "sp1b200_program_vk_tail", "sp1b200_program_preprocessed_traces", "sp1b200_program_setup",
-    "sp1b200_lookup_traces",
+    "sp1b200_lookup_traces", "sp1b200_memory_traces",
 ]
 OTHER_FUNCS = ["sp1b200_challenger_init", "sp1b200_challenger_observe", "sp1b200_challenger_sample",
                "sp1b200_challenger_sample_bits", "sp1b200_challenger_check_witness", "sp1b200_ctx_destroy", "sp1b200_default_core_params", "sp1b200_version", "sp1b200_ctx_stream",
@@ -552,6 +581,34 @@ class Lib:
             self._chk(self.L.sp1b200_lookup_traces(self.ctx, *args, None, None, None, rows))
             out = tuple(np.zeros((c, int(rows[t])), np.uint32) for t, c in enumerate(MAIN_CHIP_COLS.values()))
         self._chk(self.L.sp1b200_lookup_traces(self.ctx, *args, _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), rows))
+        return out
+
+    def memory_traces(self, init, finalize, previous_init_addr, previous_finalize_addr, local, out=None):
+        """the MemoryGlobalInit, MemoryGlobalFinalize and MemoryLocal main traces of a shard with their byte lookups and global interaction
+        events, from its init and finalize events (MEMORY_EVENT_DTYPE, pack_memory_events; any order) and local events
+        (MEMORY_LOCAL_EVENT_DTYPE, pack_memory_local_events; record.get_local_mem_events() order): numpy arrays or torch uint8 tensors of
+        the records on the host or the device, None for none.
+        out: None -> new host arrays; or five buffers written in place and returned: three uint32 / int32 traces (numpy arrays or device
+        tensors, e.g. views at the chips' offsets of a dense main buffer), the lookups (BYTE_LOOKUP_DTYPE array or uint8 tensor) and the
+        global events (GLOBAL_EVENT_DTYPE array or uint8 tensor).  -> (init [30, h], finalize [30, h], local [20, h], lookups, globals)"""
+        ip, ni, _keep_i = self._records(init, MEMORY_EVENT_DTYPE)
+        fp, nf, _keep_f = self._records(finalize, MEMORY_EVENT_DTYPE)
+        lp, nl, _keep_l = self._records(local, MEMORY_LOCAL_EVENT_DTYPE)
+        rows, n_lk, n_ge = (C.c_uint64 * 3)(), C.c_uint64(), C.c_uint64()
+        args = (ip, C.c_uint64(ni), fp, C.c_uint64(nf), C.c_uint64(previous_init_addr), C.c_uint64(previous_finalize_addr), lp, C.c_uint64(nl))
+        if out is None:
+            self._chk(self.L.sp1b200_memory_traces(self.ctx, *args, None, None, None, None, None, rows, C.byref(n_lk), C.byref(n_ge)))
+            out = tuple(np.zeros((c, int(rows[t])), np.uint32) for t, c in enumerate(MEMORY_CHIP_COLS.values())) + \
+                (np.zeros(n_lk.value, BYTE_LOOKUP_DTYPE), np.zeros(n_ge.value, GLOBAL_EVENT_DTYPE))
+
+        def rec_ptr(x):   # a record array or a uint8 tensor, written in place
+            if hasattr(x, "data_ptr"):
+                assert x.is_contiguous()
+                return C.c_void_p(x.data_ptr() or None)
+            assert x.flags["C_CONTIGUOUS"]
+            return C.c_void_p(x.ctypes.data)
+        self._chk(self.L.sp1b200_memory_traces(self.ctx, *args, _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), rec_ptr(out[3]), rec_ptr(out[4]),
+                                               rows, C.byref(n_lk), C.byref(n_ge)))
         return out
 
     def pack_row_major(self, rows_any, shapes, d_dense_out):
