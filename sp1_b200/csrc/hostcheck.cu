@@ -59,6 +59,17 @@ uint32_t sp1b200_hostcheck_rs_tw8(uint32_t* out) {
 void sp1b200_hostcheck_field(const uint32_t* a, const uint32_t* b, uint32_t* add, uint32_t* sub, uint32_t* mul, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) { add[i] = kb::add(a[i], b[i]); sub[i] = kb::sub(a[i], b[i]); mul[i] = kb::mul(a[i], b[i]); }
 }
+// The three Montgomery reductions of kb31.cuh on n 64-bit inputs: monty_reduce, monty_reduce2 and monty_reduce_lazy of each x[i]
+// (the caller judges each result only inside that reduction's domain)
+void sp1b200_hostcheck_reduce(const uint64_t* x, uint32_t* r, uint32_t* r2, uint32_t* r_lazy, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) { r[i] = kb::monty_reduce(x[i]); r2[i] = kb::monty_reduce2(x[i]); r_lazy[i] = kb::monty_reduce_lazy(x[i]); }
+}
+// The Poseidon2 s-box's products (poseidon2.cuh): mont_lazy(a, b), mont_wide_lazy(a, b) and sbox(a, b) (b as the round constant)
+void sp1b200_hostcheck_p2_products(const uint32_t* a, const uint32_t* b, uint32_t* lazy, uint32_t* wide_lazy, uint32_t* sbox, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        lazy[i] = p2::mont_lazy(a[i], b[i]); wide_lazy[i] = p2::mont_wide_lazy(a[i], b[i]); sbox[i] = p2::sbox(a[i], b[i]);
+    }
+}
 
 // Evaluate ONE chip's constraint program on one row (base-field values) two ways: the bytecode as given, and the stream
 // produced by zc_lower (what the zerocheck kernels interpret).  chip = the per-chip words of the machine blob
@@ -174,6 +185,15 @@ void sp1b200_hostcheck_septic(const uint32_t* a, const uint32_t* b, uint32_t* mu
         for (int k = 0; k < 7; k++) { x.c[k] = a[7 * i + k]; y.c[k] = b[7 * i + k]; }
         const s7::E7 m = s7::mul(x, y), v = s7::inv(x);
         for (int k = 0; k < 7; k++) { mul_out[7 * i + k] = m.c[k]; inv_out[7 * i + k] = v.c[k]; }
+    }
+}
+// frobenius and double_frobenius of n septic elements (septic.cuh, the lazily reduced table products of `lin`)
+void sp1b200_hostcheck_septic_frobenius(const uint32_t* a, uint32_t* frob_out, uint32_t* dfrob_out, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        s7::E7 x;
+        for (int k = 0; k < 7; k++) x.c[k] = a[7 * i + k];
+        const s7::E7 f = s7::frobenius(x), d = s7::double_frobenius(x);
+        for (int k = 0; k < 7; k++) { frob_out[7 * i + k] = f.c[k]; dfrob_out[7 * i + k] = d.c[k]; }
     }
 }
 void sp1b200_hostcheck_septic_curve_add(const uint32_t* p, const uint32_t* q, uint32_t* out, uint32_t* ok, uint64_t n) {

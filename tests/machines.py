@@ -38,12 +38,14 @@ Chip = collections.namedtuple("Chip", "h g wp n_constraints extra extra_prep vps
 #   direct     one assert each on a leaf (a main column that is zero on every row), on the constant 0 and on a public value that is 0;
 #   dup        one register asserted under two alpha indices;
 #   max_deg    the highest degree of any value (1, 2 or 3);
+#   max_word   the constant table also holds the canonical value 0x3FFF0001, whose Montgomery word is p - 1 (the largest word)
 #   sat        False: a program no trace needs to satisfy (the host lowering checks): asserts name any register at any point of the
 #              body, which later instructions may still read or overwrite, direct asserts land on loads that ops also read, there is
 #              no sum over the constants and public values, the register file can be as small as one register, and n_asserts is
 #              what the body asserts besides the live sum, the direct asserts and the duplicate.
-Prog = collections.namedtuple("Prog", "seed n_asserts live cols prep n_ops wide direct dup max_deg sat",
-                              defaults=(8, 0, 6, 1, 40, 0, True, False, 3, True))
+Prog = collections.namedtuple("Prog", "seed n_asserts live cols prep n_ops wide direct dup max_deg sat max_word",
+                              defaults=(8, 0, 6, 1, 40, 0, True, False, 3, True, False))
+MAX_WORD_VALUE = 0x3FFF0001     # the canonical value whose Montgomery word is p - 1
 
 # the public values of a machine with random-program chips: every program loads each of them; index 4 is 0 (the public assert)
 PROG_PV_CANONICAL = [PV0, 5, 6, 7, 0, O.P - 1, 1, 987654321]
@@ -64,12 +66,16 @@ class RandomProgram(collections.namedtuple("RandomProgram", "words main_w prep_w
     "assert_leaf", "assert_const", "assert_public", "alpha_permuted", "dup_assert", "cube", "alias", "overwrite", "dead_code",
     "high_column", and "degree_d" for the highest degree d of its constraints)."""
 
-    def trace(self, rng, h, pv):
+    def trace(self, rng, h, pv, kind=None):
         """a main and preprocessed trace of height h (Montgomery, [w, h]) that satisfies every constraint under the canonical public
-        values pv: random free and preprocessed columns, the zero column, and each witness column filled with its asserted
-        expression evaluated row by row mod p"""
-        main = rng.integers(0, O.P, (self.main_w, h), dtype=np.uint64)
-        prep = rng.integers(0, O.P, (self.prep_w, h), dtype=np.uint64)
+        values pv: free and preprocessed columns of Montgomery words of the given kind (O.words; None: uniform values), the zero
+        column, and each witness column filled with its asserted expression evaluated row by row mod p"""
+        if kind is None:
+            main = rng.integers(0, O.P, (self.main_w, h), dtype=np.uint64)
+            prep = rng.integers(0, O.P, (self.prep_w, h), dtype=np.uint64)
+        else:
+            main = O.from_monty(O.words(rng, (self.main_w, h), kind)).astype(np.uint64)
+            prep = O.from_monty(O.words(rng, (self.prep_w, h), kind)).astype(np.uint64)
         if self.asserts:                                      # the zero column and the witness columns close the main trace
             main[self.zero_col:] = 0
         regs = self._eval(main, prep, pv, h)
@@ -117,7 +123,7 @@ def random_program(prog):
     n_a, n_pv, sat = prog.n_asserts, len(PROG_PV_CANONICAL), prog.sat
     free = list(range(prog.cols)) + (list(range(prog.cols + prog.wide, 2 * prog.cols + prog.wide)) if prog.wide else [])
     zero_col = free[-1] + 1 if free else 0
-    consts = [0, 1, O.P - 1] + [int(x) for x in rng.integers(2, O.P - 1, 3)]
+    consts = [0, 1, O.P - 1] + ([MAX_WORD_VALUE] if prog.max_word else []) + [int(x) for x in rng.integers(2, O.P - 1, 3)]
     publics = [int(x) for x in rng.permutation(n_pv)] + [int(x) for x in rng.integers(0, n_pv, 2)]
     zero_pub = [j for j, i in enumerate(publics) if PROG_PV_CANONICAL[i] == 0]
     instrs, leaves, asserts, witness = [], [], [], []
@@ -333,20 +339,46 @@ def lowered_shape(words):
     return regs, nl.value, int(cw[8]) >= 8 and nl.value >= 128
 
 
-def traces(specs, seed, pv0=PV0):
+def traces(specs, seed, pv0=PV0, kind=None):
     """numpy traces of chips with fields h, g, wp, extra, extra_prep (Chip, or the specs of sp1_b200.workload.synthetic_machine)
     drawn from `seed` (an int or a numpy Generator, which is drawn from in place) -> (mains, preps).  A multi-shard test calls this
     with the same seed for every shard, so that the preprocessed tables agree, and each shard's own public value 0.  A random-program
-    chip's trace satisfies its program under PROG_PV with public value 0 replaced by pv0."""
+    chip's trace satisfies its program under PROG_PV with public value 0 replaced by pv0.  kind: the word kind of the free columns
+    (O.words); None keeps the uniform draws, so that a seed gives the same traces as before the argument existed."""
     rng = np.random.default_rng(seed)
     mains, preps = [], []
     for c in specs:
         if getattr(c, "program", None) is not None:
-            m, p = random_program(c.program).trace(rng, c.h, [pv0] + PROG_PV_CANONICAL[1:])
+            m, p = random_program(c.program).trace(rng, c.h, [pv0] + PROG_PV_CANONICAL[1:], kind=kind)
         else:
             m, p = SA.synth_trace(rng, c.h, c.g, c.wp, pv0, extra_cols=c.extra, extra_prep=c.extra_prep)
+            if kind is not None:
+                m, p = refill_template_trace(rng, m, p, c.g, c.wp, pv0, kind)
         mains.append(m); preps.append(p)
     return mains, preps
+
+
+def refill_template_trace(rng, main, prep, groups, with_prep, pv0, kind, kconst=7):
+    """a synth_air.synth_trace trace (main [6 groups + with_prep + extra, h], prep [1 + extra_prep, h] or None) with its free columns
+    redrawn as words of the given kind (O.words): per group a and b, the filler columns, and the preprocessed columns; then the
+    constrained columns recomputed mod p from them: c = a b, e = c d, f = a + kconst pv0, and the product g a_0 of the first
+    preprocessed column with group 0's a.  The boolean column d is kept."""
+    h = main.shape[1]
+    if not h:
+        return main, prep
+    cols = O.from_monty(main).astype(np.uint64)
+    P = np.uint64(O.P)
+    free = [6 * g + k for g in range(groups) for k in (0, 1)] + list(range(6 * groups + (1 if with_prep else 0), main.shape[0]))
+    cols[free] = O.from_monty(O.words(rng, (len(free), h), kind))
+    for g in range(groups):
+        a, b, d = cols[6 * g], cols[6 * g + 1], cols[6 * g + 3]
+        cols[6 * g + 2] = a * b % P
+        cols[6 * g + 4] = cols[6 * g + 2] * d % P
+        cols[6 * g + 5] = (a + np.uint64(kconst * pv0 % O.P)) % P
+    if with_prep:
+        prep = O.words(rng, prep.shape, kind)
+        cols[6 * groups] = O.from_monty(prep[0]).astype(np.uint64) * cols[0] % P
+    return O.to_monty(cols), prep
 
 
 def workload_machine(workload, seed, max_log_rows=22, scale=1.0, machine_seed=42):
@@ -358,10 +390,10 @@ def workload_machine(workload, seed, max_log_rows=22, scale=1.0, machine_seed=42
     return mach["blob"], [sp.h for sp in mach["specs"]], mains, preps, PV.copy(), list(mach["names"])
 
 
-def spec_machine(rng, chips, interactions=True, names="Chip{:03d}"):
+def spec_machine(rng, chips, interactions=True, names="Chip{:03d}", kind=None):
     """chips: list of Chip (or plain tuples in Chip's field order).  interactions=False builds the blob without an interaction
     section (synth_air.machine_blob).  names: the chip-name format; the names are observed into the transcript.  The public values are
-    PV, or PROG_PV when a chip has a random program."""
+    PV, or PROG_PV when a chip has a random program.  kind: the word kind of the traces' free columns (traces)."""
     chips = [Chip(*c) for c in chips]
     words, iwords = [], []
     for c in chips:
@@ -376,17 +408,18 @@ def spec_machine(rng, chips, interactions=True, names="Chip{:03d}"):
             iwords.append([0])
         else:
             iwords.append(SA.synth_interactions_calibrated(c.g, c.wp, list(c.vps)))
-    mains, preps = traces(chips, rng)
+    mains, preps = traces(chips, rng, kind=kind)
     blob = SA.machine_blob_with_interactions(words, iwords) if interactions else SA.machine_blob(words)
     pv = PROG_PV if any(c.program is not None for c in chips) else PV
     return blob, [c.h for c in chips], mains, preps, pv.copy(), [names.format(i) for i in range(len(chips))]
 
 
-def shard_inputs(spec, seed):
-    """the seeded whole-shard inputs of the golden fixtures and the shard tests: spec_machine with names Chip00, Chip01, ..., then a
-    challenger that has observed 9 random words from the same generator -> (blob, heights, mains, preps, pv, names, challenger)"""
+def shard_inputs(spec, seed, kind=None):
+    """the seeded whole-shard inputs of the golden fixtures and the shard tests: spec_machine with names Chip00, Chip01, ... (traces of
+    the word kind `kind`), then a challenger that has observed 9 random words from the same generator -> (blob, heights, mains, preps,
+    pv, names, challenger)"""
     rng = np.random.default_rng(seed)
-    inp = spec_machine(rng, spec, names="Chip{:02d}")
+    inp = spec_machine(rng, spec, names="Chip{:02d}", kind=kind)
     ch = O.Challenger(); ch.observe(O.rand_field(rng, 9))
     return inp + (ch,)
 

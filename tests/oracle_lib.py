@@ -63,6 +63,40 @@ def rand_field(rng, shape):
     return to_monty(rng.integers(0, P, size=shape, dtype=np.uint64))
 
 
+ONE = (1 << 32) % P                    # the Montgomery word of 1
+WORD_KINDS = ("max", "zero", "one", "minus_one", "mixed")
+# the words of the `mixed` kind besides uniform ones: the ends of [0, p), 1 and -1 in Montgomery form, and 2^30 (p - 1 is also
+# 2^31 - 2^24, so it appears once)
+SPECIAL_WORDS = np.array([0, 1, 2, P - 2, P - 1, ONE, P - ONE, 1 << 30], np.uint32)
+
+
+def words(rng, shape, kind=None):
+    """Montgomery WORDS of a given kind (the canonical values follow through from_monty).  The lazily reducing kernels see words, and
+    only words near p - 1 bring their 64-bit accumulators close to the reduction's bound:
+      None       uniform canonical values (rand_field; the same draws, so a seed gives the same words as rand_field)
+      "max"      every word p - 1 (the canonical value 0x3FFF0001)
+      "zero"     every word 0
+      "one"      every word ONE (the value 1)
+      "minus_one" every word p - ONE (the value p - 1)
+      "mixed"    blocks of 16 words: uniform words, one special word (SPECIAL_WORDS) repeated, or specials and uniform words alternating
+                 at random"""
+    if kind is None:
+        return rand_field(rng, shape)
+    fill = {"max": P - 1, "zero": 0, "one": ONE, "minus_one": P - ONE}
+    if kind in fill:
+        return np.full(shape, fill[kind], np.uint32)
+    assert kind == "mixed", f"unknown word kind {kind!r}"
+    n = int(np.prod(shape, dtype=np.int64))
+    nb = (n + 15) // 16
+    u = rand_field(rng, nb * 16).reshape(nb, 16)
+    spec = SPECIAL_WORDS[rng.integers(0, SPECIAL_WORDS.size, (nb, 16))]
+    mode = rng.integers(0, 4, nb)                                # 0, 1: uniform, 2: a run of one special word, 3: singletons
+    pick = rng.integers(0, 2, (nb, 16)).astype(bool) & (mode == 3)[:, None]
+    out = np.where(pick, spec, u)
+    out = np.where((mode == 2)[:, None], spec[:, :1], out)
+    return np.ascontiguousarray(out.reshape(-1)[:n].reshape(shape))
+
+
 def permute(state):
     s = np.ascontiguousarray(state, dtype=np.uint32).copy()
     lib().orc_poseidon2_permute(ptr(s))
@@ -207,9 +241,9 @@ def jagged_prove_verify(rounds_tables, log_stack, max_log_rows, z_row, challenge
     return commits, claims, proof[:nwords].copy()
 
 
-def random_tables(rng, shapes):
-    """shapes: list of (rows, cols) -> list of [cols, rows] Montgomery arrays"""
-    return [rand_field(rng, (c, r)) if r else np.zeros((c, 0), np.uint32) for r, c in shapes]
+def random_tables(rng, shapes, kind=None):
+    """shapes: list of (rows, cols) -> list of [cols, rows] Montgomery arrays of the given word kind (words; None: uniform)"""
+    return [words(rng, (c, r), kind) if r else np.zeros((c, 0), np.uint32) for r, c in shapes]
 
 
 def zerocheck_prove_verify(blob, heights, mains, preps, pv, max_log_rows, gkr_point, challenger):

@@ -6,7 +6,7 @@ import pytest
 from tests import gpu_prove as GP
 from tests import machines as M
 from tests import oracle_lib as O
-from tests.machines import Chip, first_diff, full_table_spec, n_interactions, shard_diff, spec_machine
+from tests.machines import Chip, full_table_spec, n_interactions, shard_diff, spec_machine
 
 pytestmark = pytest.mark.gpu
 
@@ -27,7 +27,7 @@ def test_logup_gkr_matches_oracle(spec, mlr):
     owords = O.gkr_prove_verify(blob, heights, mains, preps, mlr, och, gkr_pow_bits=6)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21), gkr_pow_bits=6)
     mach = lib.machine_create(blob)
-    d_mains, d_preps = _upload(mains, preps)
+    d_mains, d_preps = GP.upload(mains, preps)
     st = ch.st.copy()
     words = lib.logup_gkr(mach, heights, d_mains, d_preps, st)
     assert words.size == owords.size, (words.size, owords.size)
@@ -50,7 +50,7 @@ def test_logup_gkr_and_whole_shard_with_silent_chips():
         log_stack = min(mlr, 4)
         lib = Lib(0, max_log_row_count=mlr, log_stacking_height=log_stack, gkr_pow_bits=4, num_queries=4, pow_bits=3, batch_pow_bits=2)
         mach = lib.machine_create(blob)
-        d_mains, d_preps = _upload(mains, preps)
+        d_mains, d_preps = GP.upload(mains, preps)
         st = ch.st.copy()
         words = lib.logup_gkr(mach, heights, d_mains, d_preps, st)
         assert words.size == owords.size and (words == owords).all()
@@ -78,32 +78,12 @@ SUM2_THREADS_TOTAL = 396 * 128    # gkr_sum2_kernel: at most 396 blocks of 128 t
 FIX_THREADS_TOTAL = 528 * 256     # gkr_fix2_kernel / gkr_fix_sum_kernel: at most 528 blocks of 256 threads
 
 
-def _upload(mains, preps):
-    import torch
-    d_mains = [torch.from_numpy(np.ascontiguousarray(m).view(np.int32)).cuda() for m in mains]
-    d_preps = [torch.from_numpy(np.ascontiguousarray(p).view(np.int32)).cuda() if p is not None else None for p in preps]
-    torch.cuda.synchronize()
-    return d_mains, d_preps
-
-
-def _check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed, pow_bits=4):
-    rng = np.random.default_rng(seed)
-    ch = O.Challenger(); ch.observe(O.rand_field(rng, 4))
-    och = ch.clone()
-    owords = O.gkr_prove_verify(blob, heights, mains, preps, mlr, och, gkr_pow_bits=pow_bits)
-    d_mains, d_preps = _upload(mains, preps)
-    st = ch.st.copy()
-    words = lib.logup_gkr(mach, heights, d_mains, d_preps, st)
-    assert words.size == owords.size and (words == owords).all(), first_diff(words, owords, "LogUp-GKR proof")
-    assert (st == och.st).all(), "final challenger state differs from the oracle"
-
-
 def _gkr_case(spec, mlr, seed):
     from sp1_b200 import Lib
     blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(seed), spec)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21), gkr_pow_bits=4)
     mach = lib.machine_create(blob)
-    _check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed + 1)
+    GP.check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed + 1)
     lib.machine_free(mach)
     lib.close()
     return blob, heights
@@ -163,7 +143,7 @@ def test_logup_gkr_and_whole_shard_two_row_variables(case):
     prm = dict(num_queries=4, pow_bits=3, batch_pow_bits=2, gkr_pow_bits=4)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=log_stack, **prm)
     mach = lib.machine_create(blob)
-    _check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed + 1)
+    GP.check_gkr(lib, mach, blob, heights, mains, preps, mlr, seed + 1)
     ch = O.Challenger(); ch.observe(O.rand_field(np.random.default_rng(seed + 2), 9))
     och = ch.clone()
     opc, owords = O.prove_shard_verify(blob, heights, mains, preps, names, pv, log_stack, mlr, och, **prm)
@@ -187,13 +167,13 @@ def test_logup_gkr_full_batch_table_then_one_chip_too_many():
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=mlr, gkr_pow_bits=4)
     blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(1001), full_table_spec(97, 1000))
     mach = lib.machine_create(blob)
-    d_mains, d_preps = _upload(mains, preps)
+    d_mains, d_preps = GP.upload(mains, preps)
     with pytest.raises(Sp1B200Error, match="batch table"):
         lib.logup_gkr(mach, heights, d_mains, d_preps, O.Challenger().st.copy())
     lib.machine_free(mach)
     for k, absent in enumerate((False, True)):
         blob, heights, mains, preps, pv, _ = spec_machine(np.random.default_rng(1002 + k), full_table_spec(96, 1010 + k, absent))
         mach = lib.machine_create(blob)
-        _check_gkr(lib, mach, blob, heights, mains, preps, mlr, 1020 + k)
+        GP.check_gkr(lib, mach, blob, heights, mains, preps, mlr, 1020 + k)
         lib.machine_free(mach)
     lib.close()

@@ -5,36 +5,9 @@ rounds: the fold pass to level 0 sums round 0.  Each case names the K it reaches
 oracle through the same harness as tests/test_gpu_jagged.py (gpu_prove.check_jagged)."""
 import pytest
 
-from tests.gpu_prove import check_jagged
+from tests.gpu_prove import check_jagged, trace_rounds_k
 
 pytestmark = pytest.mark.gpu
-
-JK_MAX = 5
-
-
-def trace_rounds_k(shapes_rounds, log_stack, mlr):
-    """K as sp1b200_jagged_prove picks it: the column heights of all rounds, dummy padding columns included (jagged_commit)"""
-    heights, S, R = [], 1 << log_stack, 1 << mlr
-    for shapes in shapes_rounds:
-        area = 0
-        for rows, cols in shapes:
-            heights += [rows] * cols
-            area += rows * cols
-        padded = max(-(-area // S) * S, S)
-        added = padded - area
-        added_cols = max(-(-added // R), 1)
-        heights += [R] * (added_cols - 1) + [added - (added_cols - 1) * R]
-    prefix, s = [], 0
-    for h in heights:
-        s += h
-        prefix.append(s)
-    lm = (s - 1).bit_length()
-    k = min(JK_MAX, log_stack, lm - 1, min(10, mlr))
-    for p in prefix:
-        if p:
-            k = min(k, (p & -p).bit_length() - 1)
-    return k
-
 
 CASES = [
     # column starts aligned exactly to 2, 4, 8, 16 and 32 (K = 1 .. 5), empty chips in between

@@ -1,72 +1,27 @@
 """GPU parity tests (PCS level): stacked commit + BaseFold evaluation proof through the C ABI vs the oracle.
 Bit-exact: commitments, every proof word, and the post-proof challenger state.  The oracle also runs the restated
 reference verifier on its own proof, so equality here implies the CUDA proof verifies."""
-import numpy as np
 import pytest
 
-from tests import oracle_lib as O
+from tests.gpu_prove import check_stacked
 
 pytestmark = pytest.mark.gpu
 
 
-def _run(ncols_rounds, log_h, nq, pow_bits, batch_bits, seed, keep_codeword=True, device_input=False):
-    from sp1_b200 import Lib
-    rng = np.random.default_rng(seed)
-    rounds = [O.rand_field(rng, (c, 1 << log_h)) for c in ncols_rounds]
-    extra = max(1, int(np.ceil(np.log2(sum(ncols_rounds)))))
-    point = O.rand_field(rng, (extra + log_h, 4))
-    ch = O.Challenger()
-    ch.observe(O.rand_field(rng, 5))
-    och = ch.clone()
-    ocommits, oproof = O.stacked_prove_verify(rounds, log_h, point, och, num_queries=nq, pow_bits=pow_bits,
-                                              batch_pow_bits=batch_bits)
-    lib = Lib(0, log_stacking_height=log_h, num_queries=nq, pow_bits=pow_bits, batch_pow_bits=batch_bits)
-    handles, keep = [], []
-    for i, r in enumerate(rounds):
-        src = r
-        if device_input:
-            import torch
-            src = torch.from_numpy(r.view(np.int32)).cuda()
-            torch.cuda.synchronize()
-            keep.append(src)
-        commit, h = lib.stacked_commit(src, r.shape[0], keep_codeword=keep_codeword)
-        assert (commit == ocommits[i]).all(), f"round {i} commitment differs"
-        handles.append(h)
-    st = ch.st.copy()
-    proof = lib.stacked_prove(handles, point, st)
-    assert proof.size == oproof.size, (proof.size, oproof.size)
-    bad = np.nonzero(proof != oproof)[0]
-    assert bad.size == 0, f"first differing proof word {bad[:5]} of {proof.size}"
-    assert (st == och.st).all()
-    # replay mode: same witnesses -> same proof
-    nev = sum(ncols_rounds) * 4
-    pow_w, batch_w = proof[-nev - 2], proof[-nev - 1]
-    lib2 = Lib(0, log_stacking_height=log_h, num_queries=nq, pow_bits=pow_bits, batch_pow_bits=batch_bits, grind_mode=1)
-    hs2 = [lib2.stacked_commit(r, r.shape[0])[1] for r in rounds]
-    st2 = ch.st.copy()
-    proof2 = lib2.stacked_prove(hs2, point, st2, replay=[batch_w, pow_w])
-    assert (proof2 == oproof).all() and (st2 == och.st).all()
-    for h in handles:
-        lib.commit_free(h)
-    for h in hs2:
-        lib2.commit_free(h)
-    lib.close(); lib2.close()
-
-
 @pytest.mark.parametrize("ncols,log_h", [([1], 1), ([3], 4), ([2, 5], 5), ([9, 17], 8), ([33], 10)])
 def test_stacked_basefold_matches_oracle(ncols, log_h):
-    _run(ncols, log_h, nq=10, pow_bits=6, batch_bits=3, seed=1000 + log_h)
+    check_stacked(ncols, log_h, nq=10, pow_bits=6, batch_bits=3, seed=1000 + log_h)
 
 
 def test_stacked_basefold_two_step_ntt_sizes():
     # log_h = 13 exercises the strided (step A) + contiguous (step B) split of the RS-encode kernels
-    _run([3, 2], 13, nq=16, pow_bits=8, batch_bits=5, seed=77)
+    check_stacked([3, 2], 13, nq=16, pow_bits=8, batch_bits=5, seed=77)
 
 
 def test_recomputed_codeword_and_device_input():
-    _run([4, 3], 9, nq=12, pow_bits=5, batch_bits=2, seed=78, keep_codeword=False, device_input=True)
+    check_stacked([4, 3], 9, nq=12, pow_bits=5, batch_bits=2, seed=78, keep_codeword=False, device_input=True)
 
 
 def test_core_parameters_small_trace():
     # real FRI parameters (124 queries, 16 + 5 PoW bits) on a reduced stacking height
-    _run([5, 11], 12, nq=124, pow_bits=16, batch_bits=5, seed=79)
+    check_stacked([5, 11], 12, nq=124, pow_bits=16, batch_bits=5, seed=79)

@@ -3,8 +3,8 @@
 import numpy as np
 import pytest
 
-from tests.machines import (PROGRAM_ZC_CASES, Chip, lowered_shape, oracle_zerocheck, product_zerocheck, random_program, spec_machine,
-                            workload_machine, zc_tier)
+from tests import gpu_prove as GP
+from tests.machines import PROGRAM_ZC_CASES, Chip, lowered_shape, random_program, spec_machine, workload_machine, zc_tier
 
 pytestmark = pytest.mark.gpu
 
@@ -39,18 +39,9 @@ def test_zerocheck_matches_oracle(spec, mlr):
             # the tier and the path each random chip is meant to exercise: the live set + a few registers; a 150-op body takes pieces
             assert zc_tier(lib.machine_chip_regs(mach, k)) == zc_tier(c.program.live + 4), (k, lib.machine_chip_regs(mach, k))
             assert c.program.n_ops < 150 or lowered_shape(random_program(c.program).words)[2], k
-    _check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr)
+    GP.check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr)
     lib.machine_free(mach)
     lib.close()
-
-
-def _check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr):
-    gp, st0, openings, owords, ost = oracle_zerocheck(rng, blob, heights, mains, preps, pv, mlr)
-    words, st = product_zerocheck(lib, mach, heights, mains, preps, pv, gp, st0, openings)
-    assert words.size == owords.size, (words.size, owords.size)
-    bad = np.nonzero(words != owords)[0]
-    assert bad.size == 0, f"first differing words {bad[:8]} of {words.size}"
-    assert (st == ost).all()
 
 
 # calibrated chips: constraint counts from the workloads' chip_stats.json range (up to 9 per group), filler main columns, several
@@ -70,7 +61,7 @@ def test_zerocheck_calibrated_chips_match_oracle(case):
     blob, heights, mains, preps, pv, _ = spec_machine(rng, spec)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21))
     mach = lib.machine_create(blob)
-    _check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr)
+    GP.check_zerocheck(lib, mach, rng, blob, heights, mains, preps, pv, mlr)
     lib.machine_free(mach)
     lib.close()
 
@@ -82,6 +73,6 @@ def test_zerocheck_workload_machines_match_oracle(workload, mlr):
     blob, heights, mains, preps, pv, _ = workload_machine(workload, seed=1110, max_log_rows=mlr, scale=0.25)
     lib = Lib(0, max_log_row_count=mlr, log_stacking_height=min(mlr, 21))
     mach = lib.machine_create(blob)
-    _check_zerocheck(lib, mach, np.random.default_rng(1111), blob, heights, mains, preps, pv, mlr)
+    GP.check_zerocheck(lib, mach, np.random.default_rng(1111), blob, heights, mains, preps, pv, mlr)
     lib.machine_free(mach)
     lib.close()
