@@ -307,6 +307,14 @@ uint32_t orc_jagged_last_inputs(uint32_t* z_col_out, uint32_t cap, uint32_t* cla
     return (uint32_t)in.z_col.size();
 }
 
+// tests only: the challenger (34 words each) just before the evaluation sumcheck of this thread's last jagged prove observes its claimed
+// sum, and just after the sumcheck's last sample
+void orc_jagged_eval_states(uint32_t* before34, uint32_t* after34) {
+    const JaggedProveInputs& in = jagged_last_inputs();
+    chal_store(in.eval_before, before34);
+    chal_store(in.eval_after, after34);
+}
+
 
 }  // extern "C"
 

@@ -293,9 +293,10 @@ struct JaggedProof {
     unsigned max_log_rows = 0, log_m = 0;
 };
 
-// The transcript-derived inputs of the last jagged_prove on this thread: z_col and the Hadamard sumcheck's claim.  Tests read them to
-// rerun the sumcheck rounds on the reference's own kernels.
-struct JaggedProveInputs { std::vector<EF> z_col; EF claim; };
+// The transcript-derived inputs of the last jagged_prove on this thread: z_col, the Hadamard sumcheck's claim, and the challenger just
+// before the evaluation sumcheck observes its claimed sum and just after its last sample.  Tests read them to rerun both sumchecks on
+// the reference's own kernels.
+struct JaggedProveInputs { std::vector<EF> z_col; EF claim; Challenger eval_before, eval_after; };
 static inline JaggedProveInputs& jagged_last_inputs() { static thread_local JaggedProveInputs v; return v; }
 
 // JaggedProver::prove_trusted_evaluations (jagged/src/prover.rs:162-328).  claims[r] = per-column evaluations at
@@ -339,7 +340,8 @@ static inline JaggedProof jagged_prove(const std::vector<EF>& z_row, const std::
         return col_eq[c] * row_eq[idx - jp.prefix[c]];
     };
     EF claim = mle_eval(column_claims.data(), column_claims.size(), z_col);
-    jagged_last_inputs() = {z_col, claim};
+    jagged_last_inputs().z_col = z_col;
+    jagged_last_inputs().claim = claim;
     JaggedProof pf;
     pf.sumcheck.claimed_sum = claim;
     EF half = EF(F::two().inv()), quarter = EF(F::from_canonical(4).inv());
@@ -418,7 +420,12 @@ static inline JaggedProof jagged_prove(const std::vector<EF>& z_row, const std::
     pf.sumcheck.eval = round_claim;
     delete t_sc;
     EF base_eval = base[0];
-    { OrcTrace t("jagged.eval_sumcheck"); pf.jagged_eval = jagged_eval_prove(jp, z_row, z_col, point, ch); }
+    {
+        OrcTrace t("jagged.eval_sumcheck");
+        jagged_last_inputs().eval_before = ch;   // jagged_eval_prove's first transcript step is observe_ext(expected_sum)
+        pf.jagged_eval = jagged_eval_prove(jp, z_row, z_col, point, ch);
+        jagged_last_inputs().eval_after = ch;    // and its last the sample of the final round
+    }
     std::vector<std::shared_ptr<StackedRound>> srounds;
     for (auto& r : rounds) {
         srounds.push_back(r.stacked);

@@ -727,6 +727,138 @@ const char* ref_jagged_sumcheck(const uint32_t* h_dense, uint64_t dense_len, con
     return nullptr;
 }
 
+// ---- jagged evaluation (branching-program) sumcheck: the reference's jagged_assist kernels ------------------------------------------
+extern "C" void* branching_program_kernel();
+extern "C" void* transition_kernel();
+extern "C" void* interpolateAndObserve_kernel_duplex();
+extern "C" void* fixLastVariable_kernel();
+
+// the device constants JaggedAssistSumAsPolyGPUImpl::new and new_jagged_eval_sumcheck_poly_sync upload (sumcheck_sum_as_poly.rs:74-78,
+// sync_eval_sumcheck.rs:121-124): lambdas = [0, EF::two().inverse()], intermediate_eq_full_evals = [1; n]
+__global__ void ref_jagged_eval_init_kernel(kb31_extension_t* lambdas, kb31_extension_t* inter, uint32_t n) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        lambdas[0] = kb31_extension_t::zero();
+        lambdas[1] = kb31_extension_t::two().reciprocal();
+    }
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += blockDim.x * gridDim.x) inter[i] = kb31_extension_t::one();
+}
+
+// challenger.observe_ext_element(expected_sum) (sync_eval_sumcheck.rs:277), on the device challenger the Rust builds right after it
+__global__ void ref_observe_ext_kernel(DuplexChallenger ch, kb31_extension_t* v) {
+    if (blockIdx.x || threadIdx.x) return;
+    ch.observe_ext(v);
+}
+
+// The 16 x 5 TRANSITIONS table of jagged_assist/branching_program.cuh as transition_kernel writes it (branching_program.rs:254-279: one
+// thread): out[bit_state * 5 + input memory state] = output memory state, FAIL = 4.
+const char* ref_bp_transitions(uint64_t* out80) {
+    DevScope mem;
+    void* d_out;
+    RCHK(mem.alloc(&d_out, 80 * sizeof(size_t)));
+    void* args[] = {&d_out};
+    RCHK(cudaLaunchKernel(transition_kernel(), dim3(1), dim3(1), args, 0, 0));
+    RCHK(cudaMemcpy(out80, d_out, 80 * sizeof(size_t), cudaMemcpyDeviceToHost));
+    return nullptr;
+}
+
+// prove_jagged_eval_sumcheck_sync (jagged_assist/src/sync_eval_sumcheck.rs:141-239) with the device state that
+// new_jagged_eval_sumcheck_poly_sync (:36-137) and JaggedAssistSumAsPolyGPUImpl::new (sumcheck_sum_as_poly.rs:34-90) build, each round
+// one sum_as_poly_and_sample_into_point (sumcheck_sum_as_poly.rs:93-162 -> branching_program.rs:89-195) and one fix_last_variable_kernel
+// (sumcheck_sum_as_poly.rs:164-201).  Inputs, as the Rust has them after condensing (sync_eval_sumcheck.rs:77-87):
+//   merged   [nk][2 (log_m + 1)] field words: merged prefix sum k = (bits of t_k || bits of t_{k+1}), most significant bit first
+//   zc       [nk] ext: the condensed z_col eq values;  z_row [z_row_len], z_index [z_index_len] ext (z_index = the Hadamard sumcheck point)
+//   claim4   the claimed sum;  st34: the challenger before the claim is observed (prove_jagged_evaluation_sync, :277-280), updated in place
+// Outputs: out_bp [2][nk] ext: one branchingProgram launch with round_num = -1 (no substitution: the program at the boolean prefix
+// sums, both rows); out_sum_values [2 (log_m + 1)][3] ext: (y_0, y_1/2, y_1) per round as interpolateAndObserve stores them;
+// out_point [2 (log_m + 1)] ext: the sampled point, most recent first (branching_program.rs:192 prepends every new sample).
+const char* ref_jagged_eval(const uint32_t* merged, uint32_t nk, uint32_t log_m, const uint32_t* zc, const uint32_t* z_row, uint32_t z_row_len,
+                            const uint32_t* z_index, uint32_t z_index_len, const uint32_t* claim4, uint32_t* st34, uint32_t* out_bp,
+                            uint32_t* out_sum_values, uint32_t* out_point) {
+    // round_num is an int8_t kernel argument (branching_program.cu:320), so the last round, 2 (log_m + 1) - 1, must fit in it
+    if (nk == 0) return "ref_jagged_eval: need at least one merged prefix sum";
+    if (2 * ((uint64_t)log_m + 1) > 127) return "ref_jagged_eval: 2 (log_m + 1) rounds do not fit the kernels' int8_t round_num";
+    const size_t psl = log_m + 1, dim = 2 * psl, E = sizeof(kb31_extension_t);
+    // JaggedAssistSumAsPolyGPUImpl::new: split each merged prefix sum into current | next and transpose each [nk, psl] tensor to [psl, nk]
+    std::vector<uint32_t> cur_t(psl * nk), next_t(psl * nk);
+    for (size_t k = 0; k < nk; k++)
+        for (size_t i = 0; i < psl; i++) {
+            cur_t[i * nk + k] = merged[k * dim + i];
+            next_t[i * nk + k] = merged[k * dim + psl + i];
+        }
+    DevScope mem;
+    void *d_cur, *d_next, *d_merged, *d_zc, *d_zrow, *d_zindex, *d_claim, *d_lambdas, *d_inter, *d_bp, *d_results, *d_sum_values, *d_rho, *d_new;
+    RCHK(dev_upload(mem, cur_t.data(), cur_t.size() * 4, &d_cur));
+    RCHK(dev_upload(mem, next_t.data(), next_t.size() * 4, &d_next));
+    RCHK(dev_upload(mem, merged, (size_t)nk * dim * 4, &d_merged));
+    RCHK(dev_upload(mem, zc, (size_t)nk * E, &d_zc));
+    RCHK(dev_upload(mem, z_row, (size_t)z_row_len * E, &d_zrow));
+    RCHK(dev_upload(mem, z_index, (size_t)z_index_len * E, &d_zindex));
+    RCHK(dev_upload(mem, claim4, E, &d_claim));
+    RCHK(mem.alloc(&d_lambdas, 2 * E));
+    RCHK(mem.alloc(&d_inter, (size_t)nk * E));
+    RCHK(mem.alloc(&d_bp, 2 * (size_t)nk * E));
+    RCHK(mem.alloc(&d_results, 2 * E));
+    RCHK(mem.alloc(&d_sum_values, 3 * dim * E));
+    RCHK(cudaMemset(d_sum_values, 0, 3 * dim * E));   // Tensor::zeros_in([3, 2 (log_m + 1)]) (sync_eval_sumcheck.rs:275)
+    RCHK(mem.alloc(&d_rho, dim * E));
+    RCHK(mem.alloc(&d_new, dim * E));
+    ref_jagged_eval_init_kernel<<<(nk + 255) / 256, 256>>>((kb31_extension_t*)d_lambdas, (kb31_extension_t*)d_inter, nk);
+    RCHK(cudaGetLastError());
+    const size_t BLOCK = 256;   // branching_program.rs:119-122: block 256, grid (ceil(nk / 256), 2)
+    const dim3 bp_grid((unsigned)((nk + BLOCK - 1) / BLOCK), 2);
+    size_t z_row_n = z_row_len, z_index_n = z_index_len, n_cols = nk, psl_arg = psl;
+    auto launch_bp = [&](int8_t round_num, void* cur_rho, size_t cur_rho_len, void* next_rho, size_t next_rho_len) -> cudaError_t {
+        void* args[] = {&d_cur, &d_next, &psl_arg, &d_zrow, &z_row_n, &d_zindex, &z_index_n, &cur_rho, &cur_rho_len, &next_rho,
+                        &next_rho_len, &n_cols, &round_num, &d_lambdas, &d_zc, &d_inter, &d_bp};
+        return cudaLaunchKernel(branching_program_kernel(), bp_grid, dim3((unsigned)BLOCK), args, 0, 0);
+    };
+    // round_num = -1: the per-column program values at the boolean prefix sums, which the claimed sum is made of
+    RCHK(launch_bp(-1, d_rho, 0, d_rho, 0));
+    RCHK(cudaMemcpy(out_bp, d_bp, 2 * (size_t)nk * E, cudaMemcpyDeviceToHost));
+    DevChallenger ch;
+    if (const char* e = ch.init(st34)) return e;
+    {
+        void* args[] = {&ch.raw, &d_claim};
+        RCHK(cudaLaunchKernel((void*)ref_observe_ext_kernel, dim3(1), dim3(1), args, 0, 0));
+    }
+    Ext4Raw claim;
+    memcpy(&claim, claim4, 16);
+    for (size_t r = 0; r < dim; r++) {
+        // sumcheck_sum_as_poly.rs:106-135: rounds < psl bind next-prefix-sum bits (current rho empty, next rho = the whole point);
+        // later rounds split the point after its first r - psl entries
+        void *cur_rho = d_rho, *next_rho = d_rho;
+        size_t cur_len = 0, next_len = r;
+        if (r >= psl) {
+            cur_len = r - psl;
+            next_rho = (char*)d_rho + cur_len * E;
+            next_len = r - cur_len;
+        }
+        int8_t round_num = (int8_t)r;
+        RCHK(launch_bp(round_num, cur_rho, cur_len, next_rho, next_len));
+        ref_sum_rows_kernel<<<1, 32>>>((const kb31_extension_t*)d_bp, 2, nk, (kb31_extension_t*)d_results);   // sum_dim(1)
+        RCHK(cudaGetLastError());
+        {
+            void* args[] = {&d_results, &ch.raw, &d_new, &round_num, &d_sum_values, &claim};
+            RCHK(cudaLaunchKernel(interpolateAndObserve_kernel_duplex(), dim3(1), dim3((unsigned)BLOCK), args, 0, 0));
+        }
+        // the new point = [alpha] ++ the old point (branching_program.rs:163-192)
+        if (r) RCHK(cudaMemcpy((char*)d_new + E, d_rho, r * E, cudaMemcpyDeviceToDevice));
+        std::swap(d_rho, d_new);
+        // the next round's claim: bp_results[0], read back to the host (sumcheck_sum_as_poly.rs:156-161)
+        RCHK(cudaMemcpy(&claim, d_results, E, cudaMemcpyDeviceToHost));
+        {
+            // fix_last_variable_kernel: block 512, grid ceil(merged_prefix_sums.len() / 512) over the flat nk x dim words
+            size_t mdim = dim, rn = r, rho_len = r + 1;
+            void* args[] = {&d_merged, &d_inter, &d_rho, &mdim, &n_cols, &rn, &rho_len};
+            RCHK(cudaLaunchKernel(fixLastVariable_kernel(), dim3((unsigned)((nk * dim + 511) / 512)), dim3(512), args, 0, 0));
+        }
+    }
+    RCHK(cudaDeviceSynchronize());
+    RCHK(cudaMemcpy(out_sum_values, d_sum_values, 3 * dim * E, cudaMemcpyDeviceToHost));
+    RCHK(cudaMemcpy(out_point, d_rho, dim * E, cudaMemcpyDeviceToHost));
+    return ch.read(st34);
+}
+
 // ---- LogUp-GKR: the reference's circuit and round kernels -----------------------------------------------------------------------------
 extern "C" void* logup_gkr_first_sum_as_poly_circuit_layer();
 extern "C" void* logup_gkr_fix_and_sum_circuit_layer();

@@ -6,6 +6,7 @@
 #include "debug_fp.cuh"
 #include "hostfield.hpp"
 #include "septic.cuh"
+#include "sumcheck.cuh"
 #include "zc_lower.hpp"
 #include <cstring>
 #include <type_traits>
@@ -235,6 +236,13 @@ void sp1b200_hostcheck_septic_sqrt(const uint32_t* a, uint32_t* out, uint32_t* o
         const s7::E7 r = ok[i] ? s7::sqrt(x, nrm) : s7::zero();
         for (int k = 0; k < 7; k++) out[7 * i + k] = r.c[k];
     }
+}
+// the jagged branching program's one-layer transition (bp_transition, shared by the prover's kernels and the verifier) on every
+// (bit state, memory state) pair: out[bit_state * 4 + state], bit_state = row * 8 + index * 4 + current bit * 2 + next bit,
+// state = carry + 2 * comparison_so_far; -1 on failure
+void sp1b200_hostcheck_bp_transitions(int32_t* out64) {
+    for (int b = 0; b < 16; b++)
+        for (int st = 0; st < 4; st++) out64[b * 4 + st] = bp_transition(b >> 3, (b >> 2) & 1, (b >> 1) & 1, b & 1, st);
 }
 void sp1b200_hostcheck_curve_add_complete(const uint32_t* p, const uint32_t* q, uint32_t* out, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) {

@@ -359,6 +359,14 @@ def jagged_last_inputs():
     return z_col, claim
 
 
+def jagged_eval_states():
+    """the challenger states [34] just before the evaluation sumcheck of this thread's last oracle jagged proof observes its claimed sum
+    and just after the sumcheck's last sample"""
+    before, after = np.zeros(34, np.uint32), np.zeros(34, np.uint32)
+    lib().orc_jagged_eval_states(ptr(before), ptr(after))
+    return before, after
+
+
 def gkr_last_inputs():
     """the inputs of this thread's last oracle LogUp-GKR prove that the proof does not carry:
     -> (alpha [4], beta_seed [n, 4], per GKR layer in proof order (lambda [4], claim [4], evaluation point [m, 4]))"""

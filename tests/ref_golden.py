@@ -1,7 +1,8 @@
 """Stored outputs of the reference's own CUDA kernels (oracle/_ref/libsp1ref.so) on seeded inputs, kept under tests/golden/ so that the
 comparison with the reference runs from this repository alone.  Each test module that pins kernels to the reference owns one `Store` (one
 JSON file): tests/test_gpu_ref_kernels.py writes tests/golden/ref_kernels.json, tests/test_ref_sumcheck.py tests/golden/ref_sumcheck.json,
-tests/test_ref_gkr.py tests/golden/ref_gkr.json, tests/test_ref_zerocheck.py tests/golden/ref_zerocheck.json.
+tests/test_ref_gkr.py tests/golden/ref_gkr.json, tests/test_ref_zerocheck.py tests/golden/ref_zerocheck.json, tests/test_ref_jagged_eval.py
+tests/golden/ref_jagged_eval.json.
 
 Every entry holds the SHA-256 of an output's little-endian u32 words, and the words themselves for the outputs a test reads (keep=True).
 With SP1B200_RECORD_REF=1 (and oracle/_ref built) the tests run the reference kernels instead, compare against them directly, and

@@ -34,7 +34,7 @@ def lib():
         for n in ("ref_init", "ref_malloc", "ref_free", "ref_h2d", "ref_d2h", "ref_field_op", "ref_ext_op", "ref_permute", "ref_hash",
                   "ref_compress", "ref_merkle_tree", "ref_batch_coset_dft", "ref_batch", "ref_fold_mle_ext", "ref_fix_last_variable_ext",
                   "ref_partial_lagrange_ext", "ref_grind", "ref_challenger_script", "ref_gkr_populate", "ref_zerocheck_node_sums",
-                  "ref_jagged_sumcheck", "ref_logup_gkr", "ref_zerocheck"):
+                  "ref_jagged_sumcheck", "ref_logup_gkr", "ref_zerocheck", "ref_bp_transitions", "ref_jagged_eval"):
             getattr(L, n).restype = C.c_char_p
         _chk(L.ref_init())
         _lib = L
@@ -462,3 +462,34 @@ def jagged_sumcheck(dense, col_heights, eq_row, eq_col, challenges, log_stacking
                                    _p(ch.reshape(-1)), C.c_uint32(log_m), C.c_uint32(log_stacking_height), _p(grid8), _p(r2), _p(rounds), _p(pq),
                                    _p(stacked)))
     return np.concatenate([grid8, r2, rounds[:8 * (log_m - 3)], pq, stacked])
+
+
+def bp_transitions():
+    """the reference's TRANSITIONS table as its transition_kernel writes it (ref_bp_transitions): [16 bit states, 5 input memory states]
+    -> output memory state, FAIL = 4; bit state = row * 8 + index * 4 + current prefix-sum bit * 2 + next prefix-sum bit, memory state =
+    comparison_so_far * 2 + carry"""
+    out = np.zeros(80, np.uint64)
+    _chk(lib().ref_bp_transitions(out.ctypes.data_as(C.POINTER(C.c_uint64))))
+    return out.reshape(16, 5)
+
+
+def jagged_eval(merged, zc, z_row, z_index, claim, st34):
+    """the reference's jagged evaluation sumcheck kernels (ref_jagged_eval) on the condensed merged prefix sums [nk, 2 (log_m + 1)] (field
+    words), the condensed z_col eq values [nk, 4], z_row, z_index (the Hadamard sumcheck point) and the claimed sum, from the challenger
+    state before the claim is observed.  -> (the round_num = -1 program values [2, nk, 4], sum values [2 (log_m + 1), 3, 4] = (y_0, y_1/2,
+    y_1) per round, the sampled point [2 (log_m + 1), 4] most recent first, the final challenger state [34])"""
+    merged = np.ascontiguousarray(merged, np.uint32)
+    nk, dim = merged.shape
+    zc = np.ascontiguousarray(zc, np.uint32).reshape(-1)
+    z_row = np.ascontiguousarray(z_row, np.uint32).reshape(-1, 4)
+    z_index = np.ascontiguousarray(z_index, np.uint32).reshape(-1, 4)
+    claim = np.ascontiguousarray(claim, np.uint32).reshape(4)
+    st = np.ascontiguousarray(st34, np.uint32).copy()
+    bp = np.zeros((2, nk, 4), np.uint32)
+    sums = np.zeros((dim, 3, 4), np.uint32)
+    point = np.zeros((dim, 4), np.uint32)
+    z = lambda a: a if a.size else np.zeros(4, np.uint32)
+    _chk(lib().ref_jagged_eval(_p(merged.reshape(-1)), C.c_uint32(nk), C.c_uint32(dim // 2 - 1), _p(zc), _p(z(z_row).reshape(-1)),
+                               C.c_uint32(z_row.shape[0]), _p(z(z_index).reshape(-1)), C.c_uint32(z_index.shape[0]), _p(claim), _p(st),
+                               _p(bp.reshape(-1)), _p(sums.reshape(-1)), _p(point.reshape(-1))))
+    return bp, sums, point, st

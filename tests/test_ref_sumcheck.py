@@ -17,7 +17,8 @@ import numpy as np
 import pytest
 
 from tests import oracle_lib as O
-from tests.ext_field import EF, HALF, ONE, QUARTER, ZERO, efs as _efs, eval_at, interpolate, parse_partial_sumcheck
+from tests.ext_field import EF, HALF, ONE, QUARTER, ZERO, efs as _efs, eval_at, interpolate
+from tests.jagged_layout import column_heights, dense, parse_jagged_proof, stacked_cols
 from tests.ref_golden import Ref, Store
 
 STORE = Store("ref_sumcheck", "tests/test_ref_sumcheck.py")
@@ -57,33 +58,6 @@ def reference_round_polys(raw, claim, challenges):
     return polys, claim_r, p_eval, q_eval, v[12 + 2 * (log_m - 3):]
 
 
-# ---- the jagged PCS proof words (oracle/capi.cpp put(JaggedProof)) -------------------------------------------------------------------
-def parse_jagged_proof(w, stacked_cols, log_stack):
-    """-> dict(batch_evals, sumcheck, rc_cc, expected_eval, log_m); stacked_cols: the stacked columns of each commitment round"""
-    w = np.asarray(w, np.uint32)
-    lh = log_stack + LOG_BLOWUP
-    o = 2 * 4 * log_stack + 8 * log_stack                                 # univariate messages, FRI commitments
-    for width in stacked_cols:                                            # component openings
-        o += NQ * width + 8 + 2 + NQ * lh * 8
-    for q in range(log_stack):                                            # query phase
-        o += NQ * 8 + 8 + 2 + NQ * (lh - q - 1) * 8
-    o += 4 + 1 + 1                                                        # final poly, two witnesses
-    batch = []
-    for width in stacked_cols:
-        batch += _efs(w[o:o + 4 * width]); o += 4 * width
-    sc, o = parse_partial_sumcheck(w, o)
-    _, o = parse_partial_sumcheck(w, o)                                                # jagged evaluation sumcheck
-    rc_cc = []
-    for _ in stacked_cols:
-        cnt = int(w[o]); o += 1
-        rc_cc.append([(int(w[o + 2 * i]), int(w[o + 2 * i + 1])) for i in range(cnt)]); o += 2 * cnt
-    o += 8 * len(stacked_cols)
-    expected = EF(w[o:o + 4]); o += 4
-    log_m = int(w[o + 1]); o += 2
-    assert o == w.size, (o, w.size)
-    return dict(batch_evals=batch, sumcheck=sc, rc_cc=rc_cc, expected_eval=expected, log_m=log_m)
-
-
 # ---- cases --------------------------------------------------------------------------------------------------------------------------
 # (name, tables per commitment round as (rows, cols), log_stacking_height, max_log_row_count).  Heights are multiples of 16, the dense
 # length a multiple of 8: the preconditions of the reference's fused kernels (sumcheck.rs:107, 150).  K = the product's number of rounds
@@ -107,11 +81,6 @@ CASES = [
 IDS = [c[0] for c in CASES]
 
 
-def _stacked_cols(shapes_rounds, log_stack):
-    S = 1 << log_stack
-    return [max(-(-sum(r * c for r, c in shapes) // S), 1) for shapes in shapes_rounds]
-
-
 @functools.lru_cache(maxsize=None)
 def _oracle(name):
     """the case's tables and the oracle's proof: (rounds, z_row, challenger state before the proof, proof words, z_col, claim)"""
@@ -128,16 +97,6 @@ def _oracle(name):
     return rounds, z_row, st0, proof, z_col, claim
 
 
-def _dense(rounds, log_stack):
-    """the committed words of all rounds back to back, each round zero-padded to a multiple of 2^log_stack (jagged_commit)"""
-    parts = []
-    S = 1 << log_stack
-    for tabs in rounds:
-        d = np.concatenate([t.reshape(-1) for t in tabs if t.size] or [np.zeros(0, np.uint32)])
-        parts += [d, np.zeros(max(-(-d.size // S) * S, S) - d.size, np.uint32)]
-    return np.concatenate(parts)
-
-
 def _reference(name, pf):
     """the reference kernels' raw sums on the case (stored words; run live while recording)"""
     _, shapes_rounds, log_stack, mlr = CASES[IDS.index(name)]
@@ -146,10 +105,9 @@ def _reference(name, pf):
     def run():
         from tests import ref_lib as R
         rounds, z_row, _, _, z_col, _ = _oracle(name)
-        # the columns of the jagged layout, dummy padding tables included, as the proof's table sizes record them
-        heights = [rows for rc in pf["rc_cc"] for rows, cols in rc for _ in range(cols)]
+        heights = column_heights(pf["rc_cc"])
         challenges = np.stack([p.w for p in reversed(pf["sumcheck"]["point"])])
-        return R.jagged_sumcheck(_dense(rounds, log_stack), heights, O.partial_lagrange(z_row), O.partial_lagrange(z_col), challenges,
+        return R.jagged_sumcheck(dense(rounds, log_stack), heights, O.partial_lagrange(z_row), O.partial_lagrange(z_col), challenges,
                                  log_stack)
     n_rounds = 12 + 2 * (pf["log_m"] - 3)
     sums = Ref(f"jagged.{name}.rounds", lambda: run()[:4 * n_rounds], keep=True, store=STORE)
@@ -160,7 +118,7 @@ def _reference(name, pf):
 def _check(name, words, who):
     _, shapes_rounds, log_stack, _ = CASES[IDS.index(name)]
     _, _, _, _, z_col, claim = _oracle(name)
-    pf = parse_jagged_proof(words, _stacked_cols(shapes_rounds, log_stack), log_stack)
+    pf = parse_jagged_proof(words, stacked_cols(shapes_rounds, log_stack), log_stack, NQ, LOG_BLOWUP)
     sc = pf["sumcheck"]
     assert sc["claim"] == EF(claim), f"{who}: Hadamard sumcheck claim differs from the oracle's z_col claim"
     sums, stacked = _reference(name, pf)
